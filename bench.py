@@ -2,6 +2,7 @@
 """Benchmark of the rigid-ICP hot path (BASELINE.json metric: ICP iterations/s and correspondences/s).
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--no-secondary]
+                    [--dump-outputs DIR]
 
 A "step" is one full ICP iteration (transform + radius-bounded 1-NN of every source point + moment accumulation +
 reduction (+ all-reduce) + solve) on the named workload.
@@ -23,13 +24,16 @@ Timing: W untimed warm-up iterations (a separate estimate() call), then ONE esti
 the iteration's kernels, with an L2 flush (256 MiB memset) before every iteration OUTSIDE the event bracket; max over
 ranks. The timed call starts like every ICP run: its first iteration searches every query (nothing cached), later
 iterations re-search only the queries whose cached match cannot be proven to still be the nearest neighbour
-(icp_loop.cu) - `roofline` reports the mean and both regimes.
+(icp_loop.cu) - `roofline` reports the mean and both regimes. Every timed leg, the `secondary` ones included, times
+K steps.
+--dump-outputs DIR: after the timed call, rank 0 writes what it returned and the correspondence list of its last
+iteration to DIR/*.npy (dump_outputs); the inputs are seeded, so two builds can be compared output for output.
 Parity inside the bench: the GPU transform is compared with the CPU arm's (same inputs, same iteration count), the
 correspondence counts must be equal, all ranks must hold bit-identical transforms, and at N > 1 the sharded result
 is compared with a single-GPU run of the whole problem on rank 0.
 The reference arm (--impl reference) times cilantro's own CPU path: the reference's vendored nanoflann compiled in
 place (oracle/_ref) driving the Eigen-free restatement of its ICP loop (oracle/), on all host cores. Nothing here
-reads /root/reference at run time.
+reads the reference checkout at run time.
 """
 import argparse
 import hashlib
@@ -63,7 +67,7 @@ def load_peaks():
         with open(path) as f:
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 def load_traffic(workload):
@@ -76,7 +80,7 @@ def load_traffic(workload):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -168,9 +172,9 @@ def cpu_reference_run(w, steps, warmup, dst, src, nrm, build_in_timed_region):
     t0 = time.perf_counter()
     knn = mk()
     t_build = time.perf_counter() - t0
-    # "all the host threads it can use": the kd-tree sweep is latency-bound and was measured 3x slower
-    # with every hyper-thread (128) than with one thread per core (64) on the B200 host, so probe both
-    # on one iteration and give the reference the better setting
+    # "all the host threads it can use": the kd-tree sweep is latency-bound and can be slower with every
+    # hyper-thread than with one thread per core, so probe both on one iteration and give the reference the
+    # better setting
     ncpu = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     best = None
     for nt in sorted({ncpu, max(1, ncpu // 2)}):
@@ -273,8 +277,27 @@ def t_hash(T):
     return hashlib.sha1(np.ascontiguousarray(T, np.float32).tobytes()).hexdigest()[:16]
 
 
+DUMP_MAX_PAIRS = 1 << 20  # 28 B per dumped pair: at most 28 MiB of correspondences
+
+
+def dump_outputs(out_dir, res, icp):
+    """What the timed estimate() returned (transform, correspondence count) and the engine's correspondence list
+    after its last iteration (getCorrespondences()), as float32 / float64 .npy files. A list longer than
+    DUMP_MAX_PAIRS is cut to a fixed, seeded sample of its positions (corr_position)."""
+    os.makedirs(out_dir, exist_ok=True)
+    first, second, value = icp.correspondences()
+    pos = np.arange(first.size)
+    if first.size > DUMP_MAX_PAIRS:
+        pos = np.sort(np.random.default_rng(0).choice(first.size, DUMP_MAX_PAIRS, replace=False))
+    arrays = {"transform": res["T"].astype(np.float64), "num_corr": np.float64(res["num_corr"]),
+              "corr_position": pos.astype(np.float64), "corr_first": first[pos].astype(np.float64),
+              "corr_second": second[pos].astype(np.float64), "corr_value": value[pos]}
+    for key, a in arrays.items():
+        np.save(os.path.join(out_dir, key + ".npy"), np.asarray(a))
+
+
 def icp_bench(args, name, w, scaling, ctx, rank, world, local, with_e2e=True, with_cpu=True, with_survey=True,
-              clocks_wanted=True):
+              clocks_wanted=True, dump_dir=None):
     """The ICP legs on `ctx` (all ranks call it); rank 0 gets the JSON-able dict, the others None."""
     from cilantro_b200 import capi, dist as cdist, synth
 
@@ -296,6 +319,8 @@ def icp_bench(args, name, w, scaling, ctx, rank, world, local, with_e2e=True, wi
     if rank == 0 and clocks_wanted:
         sampler.start()
     res, ms_per_step, wall = timed_estimate(icp, ctx, cdist, world, args.steps, args.warmup, flush, kw)
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, res, icp)
     launches = res["kernel_launches"]  # this library's kernels launched by the timed estimate() call (not the warm-up)
     iter_ms = np.array([cdist.max_over_ranks(x) for x in res["iter_ms"]])
     clocks = None
@@ -500,7 +525,8 @@ def run_ours(args):
     cdist.attach_comm(ctx)
     name, scaling = pick_workload(args)
     w = WORKLOADS[name]
-    main = icp_bench(args, name, w, scaling, ctx, rank, world, local, with_cpu=not args.no_cpu_baseline)
+    main = icp_bench(args, name, w, scaling, ctx, rank, world, local, with_cpu=not args.no_cpu_baseline,
+                     dump_dir=args.dump_outputs)
 
     # ---- secondary workloads ------------------------------------------------------------------------------------
     secondary = {}
@@ -510,22 +536,21 @@ def run_ours(args):
         if world == 1:
             if name != "icp_combined_10m":
                 sub = argparse.Namespace(**vars(args))
-                sub.steps, sub.warmup = WORKLOADS["icp_combined_10m"]["iters"], 3
+                sub.warmup = 3
                 r = icp_bench(sub, "icp_combined_10m", WORKLOADS["icp_combined_10m"], "weak", ctx, rank, world, local,
                               with_cpu=not args.no_cpu_baseline, clocks_wanted=False)
                 r["steps"], r["warmup"] = sub.steps, sub.warmup
                 secondary["icp_combined_10m"] = r
             aux = argparse.Namespace(**vars(args))
-            for key, fn, steps in (("kmeans_50m", bench_aux.kmeans, 5), ("ransac_5m", bench_aux.ransac, 3),
-                                   ("pca_50m", bench_aux.pca, 5)):
-                aux.steps, aux.warmup = steps, 1
+            aux.warmup = 1
+            for key, fn in (("kmeans_50m", bench_aux.kmeans), ("ransac_5m", bench_aux.ransac), ("pca_50m", bench_aux.pca)):
                 try:
                     secondary[key] = bench_aux.brief(fn(aux, ctx=ctx))
                 except Exception as e:  # a secondary workload must not take the headline down with it
                     secondary[key] = {"error": f"{type(e).__name__}: {e}"}
         else:
             aux = argparse.Namespace(**vars(args))
-            aux.steps, aux.warmup = 5, 1
+            aux.warmup = 1
             try:
                 r = bench_aux.kmeans(aux, ctx=ctx, rank=rank, world=world)
                 if rank == 0:
@@ -570,6 +595,8 @@ def main():
     ap.add_argument("--no-secondary", action="store_true", help="skip the `secondary` block (other BASELINE configs)")
     ap.add_argument("--no-flush", action="store_true",
                     help="experiments only: skip the L2 flush between timed iterations (the reported config says so)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed call's outputs of its last step to DIR/*.npy (ICP workloads)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
     if args.workload in AUX:  # secondary single-GPU workloads (k-means, RANSAC, PCA, ...) on their own: bench_aux.py

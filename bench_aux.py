@@ -12,7 +12,7 @@ import time
 
 import numpy as np
 
-FP32_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12  # nominal FMA rate of the FP32 pipe (SMs x lanes x 2 x max clock)
+FP32_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12  # H100 SXM nominal FMA rate of the FP32 pipe (SMs x lanes x 2 x max clock)
 
 
 def _ctx(ctx=None):
@@ -87,7 +87,7 @@ def kmeans(args, n=50_000_000, k=1024, ctx=None, rank=0, world=1):
         "gpu_launches": int(launches),
         "roofline": {"bound": "fp32", "achieved": flop / (ms * 1e-3) / 1e12 / world, "peak": FP32_PEAK_TFLOPS, "unit": "TFLOP/s",
                      "frac": flop / (ms * 1e-3) / 1e12 / world / FP32_PEAK_TFLOPS, "traffic": None,
-                     "kernel": "kmeans_assign_kernel", "peak_source": "nominal: 148 SMs x 128 lanes x 2 x 1.965 GHz (MEASURED_PEAKS.json has no FP32 figure)",
+                     "kernel": "kmeans_assign_kernel", "peak_source": "nominal: 132 SMs x 128 lanes x 2 x 1.98 GHz (H100 SXM)",
                      "note": "per GPU; 8 N K flop per iteration (3 sub, 3 mul, 2 add; the "
                      "arithmetic contract forbids FMA, so the attainable rate is half the FMA peak)"},
         "cpu_baseline": {"value": sample / cpu_s, "unit": "points/s", "cores": oracle.num_threads(), "kind": "port",
@@ -142,7 +142,7 @@ def ransac(args, n=5_000_000, batch=1000, ctx=None):
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": f"RigidTransformRANSACEstimator3f scoring: {n} correspondences (30 % inliers), {batch} hypotheses per step, thresh 0.01",
-                   "l2": "inputs (120 MB) comparable to L2; the pairs are read once per batch"},
+                   "l2": "inputs (120 MB) larger than L2; the pairs are read once per batch"},
         "e2e": {"value": full["iterations"] / full_s, "unit": "hypotheses/s", "h2d_bytes_per_step": 48.0 * 1000, "d2h_bytes_per_step": 4.0 * 1000,
                 "what": f"cb_ransac_rigid: 10000 hypotheses (sample on host, Kabsch-of-3 on host, batches of 1024 scored on the "
                         f"device, re-estimation) in {full_s:.3f} s; |T - T_ref|_F = {err:.2e}; inliers {full['num_inliers']}"},

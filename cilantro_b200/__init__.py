@@ -1,4 +1,4 @@
-"""cilantro_b200 — B200-native (sm_100a) rigid-ICP / k-means / RANSAC / PCA hot path of cilantro.
+"""cilantro_b200 — H100-native (sm_90a) rigid-ICP / k-means / RANSAC / PCA hot path of cilantro.
 
 The product is the shared library cilantro_b200/libcilantro_b200.so (hand-written CUDA behind the
 C ABI of include/cilantro_b200.h) plus the C++ header shims in include/cilantro/. This Python

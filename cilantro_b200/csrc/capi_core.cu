@@ -163,7 +163,7 @@ using namespace cb;
 extern "C" {
 
 const char* cb_last_error(void) { return cb::g_err.c_str(); }
-const char* cb_version(void) { return "cilantro_b200 0.1 (sm_100a)"; }
+const char* cb_version(void) { return "cilantro_b200 0.1 (sm_90a)"; }
 
 // ---- context ------------------------------------------------------------------------------------
 int cb_context_create(int device, cb_context** out) {
@@ -190,7 +190,7 @@ int cb_context_create(int device, cb_context** out) {
   {
     // All cloud / index / scratch buffers come from the stream-ordered pool. Keep freed memory in the
     // pool (default: returned to the OS at every synchronise, which made repeated cloud creation pay
-    // page allocation again each time: 30-400 ms outliers in the end-to-end call).
+    // page allocation again each time: large outliers in the end-to-end call).
     cudaMemPool_t pool;
     CB_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
     uint64_t keep = UINT64_MAX;
@@ -859,8 +859,8 @@ int cb_icp_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res) {
   const int max_iter = std::max(prm->max_iter, 0);
   // Optional CUDA-event instrumentation, ONE bracket (2 events) per iteration: timing 1 = whole
   // iteration, timing 2 = the search kernel only. Every cudaEventRecord costs the device front end a
-  // few microseconds — measured with %globaltimer: 4 records per iteration inflated a 103 us period to
-  // 147 us — so production runs (timing 0) record nothing. Elapsed times are read after the final
+  // few microseconds (visible in a %globaltimer trace of the iteration period), so production runs
+  // (timing 0) record nothing. Elapsed times are read after the final
   // synchronise: with the fused exchange the host never waits on the stream inside the loop.
   const int timing = prm->timing;
   while (timing != 0 && (int)icp->events.size() < 2 * max_iter) {

@@ -1,4 +1,4 @@
-// Voxel-grid downsampling (product code, sm_100a) — §8(f) rank 2.
+// Voxel-grid downsampling (product code, sm_90a) — §8(f) rank 2.
 // Replaces GridAccumulator::build_index_ (core/grid_accumulator.hpp:146-199) + Points[Normals][Colors]
 // GridDownsampler::getDownsampled* (core/grid_downsampler.hpp) behind PointCloud::gridDownsample
 // (utilities/point_cloud.hpp:246-290).

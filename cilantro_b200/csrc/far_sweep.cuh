@@ -1,4 +1,4 @@
-// Far-query path of the grid searches (product code, sm_100a).
+// Far-query path of the grid searches (product code, sm_90a).
 // The shell sweeps of nn_search.cuh / grid_sweep.cuh cost O(k^2) row tests for shell k whether or not the
 // shell holds points, so a query that has to cross a lot of empty space (a point far outside the cloud, the
 // centre of a hollow scan, an isolated outlier asking for k neighbours) would spend O(k^3) on nothing. Once a

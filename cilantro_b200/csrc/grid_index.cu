@@ -1,4 +1,4 @@
-// Uniform-grid index build (product code, sm_100a). One-time per cloud; the GPU counterpart of the
+// Uniform-grid index build (product code, sm_90a). One-time per cloud; the GPU counterpart of the
 // reference's single-threaded kd-tree build (core/kd_tree.hpp:162-170 ->
 // 3rd_party/nanoflann/nanoflann.hpp:1661-1687 buildIndex / :1150-1212 divideTree).
 //

@@ -1,4 +1,4 @@
-// Generic shell sweep over the uniform grid (product code, sm_100a): visits, for one query, every cell
+// Generic shell sweep over the uniform grid (product code, sm_90a): visits, for one query, every cell
 // range that can still hold a point closer than bound(), in growing Chebyshev shells around the query's
 // cell, with the same conservative pruning as nn_search.cuh (2^-10 cell margin, h_safe). bound() may
 // shrink while scanning (k-best lists) or stay constant (radius neighbourhoods).

@@ -1,4 +1,4 @@
-// Per-correspondence accumulation of the ICP estimators (product code, sm_100a), shared by the fused
+// Per-correspondence accumulation of the ICP estimators (product code, sm_90a), shared by the fused
 // search+accumulate kernel (icp_kernels.cu) and the pair-list kernel of the non-default correspondence
 // engine modes (icp_engine.cu).
 //   kModeP2P      Kabsch moments  n, sum d, sum q, sum d q^T          transform_estimation.hpp:25-34

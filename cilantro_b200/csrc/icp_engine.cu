@@ -1,4 +1,4 @@
-// Non-default correspondence-engine modes of the ICP path (product code, sm_100a) — §8(f) rank 3.
+// Non-default correspondence-engine modes of the ICP path (product code, sm_90a) — §8(f) rank 3.
 // Replaces CorrespondenceSearchKDTree::findCorrespondences(tform) (correspondence_search/
 // correspondence_search_kd_tree.hpp:107-229) for search directions FIRST_TO_SECOND / BOTH, reciprocity,
 // inlier_fraction < 1 and one_to_one; the default configuration keeps the fused single-kernel path

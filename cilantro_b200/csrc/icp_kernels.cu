@@ -1,4 +1,4 @@
-// Fused ICP iteration kernels (product code, sm_100a).
+// Fused ICP iteration kernels (product code, sm_90a).
 //
 // One launch per ICP iteration does, for every source point s_i:
 //   q_i = T s_i                               transformFeatures + transformPoints

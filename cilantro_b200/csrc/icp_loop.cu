@@ -1,4 +1,4 @@
-// Device-resident rigid ICP loop (product code, sm_100a).
+// Device-resident rigid ICP loop (product code, sm_90a).
 //
 // IterativeClosestPointBase::estimate() (registration/icp_base.hpp:68-87) for the default correspondence engine:
 // ONE kernel per ICP iteration and NO host round trip between iterations. The kernel of iteration k
@@ -45,10 +45,9 @@ constexpr int kBlock = kReduceBlock;
 // queries an iteration will have to search again, but the sequence is predictable for a converging run (10^6, 19 %, 7 %,
 // 0.07 %, then a few dozen queries at 1 M): the first kDenseIters warm iteration(s) use small tiles (a tile's first 256
 // flagged queries are searched by the inline body, only the rest by the slower out-of-line copy), later iterations
-// large ones (a tile without flagged queries costs its block ~3 us of latency, so fewer, larger tiles). Either
-// variant is correct for any number of flagged queries. Measured (B200): small tiles for iterations 1-3 made iteration 1
-// 20 % faster and iterations 2-3 up to 50 % slower (mostly empty tiles already); small tiles for iteration 1 only, 8192-query
-// tiles afterwards: 1 M p2p 0.89 -> 0.87 ms per 15 iterations, 10 M combined 5.98 -> 5.7 ms per 10.
+// large ones (a tile without flagged queries still costs its block a few microseconds of latency, so fewer, larger
+// tiles). Either variant is correct for any number of flagged queries. Small tiles pay off in the first warm iteration
+// only (later ones search mostly empty tiles already); the two sizes are timing choices (bench.py, DESIGN §4.2).
 #ifndef CB_LOOP_QPT_DENSE
 #define CB_LOOP_QPT_DENSE 4
 #endif
@@ -104,8 +103,7 @@ __device__ __forceinline__ Rigid rigid_from_t12_dev(const float* T12) {
 // The serial epilogue of an iteration (one thread): totals -> update -> new state. It runs in a kernel of its own
 // (icp_finish_kernel, one warp): inside the search kernel its temporaries were spilled at that kernel's register
 // budget, and a spilled word of ONE thread lives in its own 128-byte line of local memory - after a 10 M-point pass
-// every one of them was a cold DRAM miss (%globaltimer trace: 47 us per solve at 10 M, 12 us at 1 M, for ~2 us of
-// arithmetic).
+// every one of them was a cold DRAM miss (in a %globaltimer trace the solve took many times its arithmetic).
 template <int MODE>
 __device__ __forceinline__ void loop_solve(const LoopArgs* ap, const BlockCtx* cxp, const double* s, int late,
                                         unsigned long long seq) {
@@ -343,9 +341,8 @@ __global__ void __launch_bounds__(kBlock, CB_WARM_MIN_BLOCKS) icp_cached_kernel(
 
 // ---- the cached pass, asynchronous-copy pipeline (the shipped version) ---------------------------------------------------
 // Same arithmetic, same tile walk, same flags and sums as icp_cached_kernel above; what changes is how the data gets
-// to the thread. ncu on the register version (an early round-2 capture; DESIGN.md 4.2): 128 registers -> 2 blocks/SM, 24 %
-// of the warp slots occupied, long-scoreboard the top stall, 27 % of the DRAM bandwidth - each thread can only keep
-// the loads in flight that it has registers for. Here every thread runs a private three-deep pipeline of
+// to the thread. The register version needs 128 registers -> 2 blocks/SM, few warp slots occupied, long-scoreboard
+// stalls on top - each thread can only keep the loads in flight that it has registers for. Here every thread runs a private three-deep pipeline of
 // cp.async copies into shared memory (LDGSTS: no destination register, no scoreboard slot):
 //   stage A (tile k+2)  the streamed arrays: its queries' point (16 B), exclusion radius (4 B), cached match (4 B)
 //   stage B (tile k+1)  the gathers, once A has landed: the matched destination point (+ normal for the plane term)
@@ -803,7 +800,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   constexpr int kBridgeBatch = 2;  // enqueued behind the first batch: covers the host's look at the first batch's state
   constexpr double kGiveUpShare = 0.15;
   // Batches are enqueued ONE AHEAD of the batch whose state the host is looking at: the device never waits for the host
-  // between batches (with several ranks such a gap showed up as a 1.8 ms peer wait in the next iteration), and the
+  // between batches (with several ranks such a gap shows up as a peer wait in the next iteration), and the
   // hand-over / convergence decisions lag by at most one batch. Two pinned copies of LoopState alternate.
   if (!icp->h_state2) CB_CUDA(cudaMallocHost(&icp->h_state2, sizeof(LoopState)));
   for (int e = 0; e < 2; ++e)

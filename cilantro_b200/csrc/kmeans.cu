@@ -1,4 +1,4 @@
-// k-means: fused assignment + centroid-sum kernel and the Lloyd loop (product code, sm_100a).
+// k-means: fused assignment + centroid-sum kernel and the Lloyd loop (product code, sm_90a).
 //
 // Replaces KMeans<float,3>::cluster_ (clustering/kmeans.hpp:67-194), brute-force branch:
 //   assignment  :100-119  argmin_j |c_j - p_i|^2, strict '<' scanning j ascending (lowest j wins ties)
@@ -136,7 +136,7 @@ int kmeans_step(cb_context* ctx, const cb_cloud* pts, const KMeansBuffers& b, co
   const bool use_smem = smem_sums + kChunk * sizeof(float4) <= 200 * 1024;
   const size_t smem = kChunk * sizeof(float4) + (use_smem ? smem_sums : 0);
   // persistent grid = SMs x resident blocks per SM (occupancy API with this launch's dynamic smem);
-  // ncu showed 22 % occupancy and 0.74 issue utilisation with a fixed 2 blocks/SM
+  // a fixed 2 blocks/SM left most warp slots empty
   int per_sm = 0;
   if (use_smem) {
     CB_CUDA(cudaFuncSetAttribute(kmeans_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

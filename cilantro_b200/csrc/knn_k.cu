@@ -1,4 +1,4 @@
-// General-k nearest neighbours over the grid (product code, sm_100a).
+// General-k nearest neighbours over the grid (product code, sm_90a).
 // Replaces the batched KDTree::kNNInRadiusSearch / kNNSearch (core/kd_tree.hpp:215-318) for k <= 256 (the k-best list is a
 // per-thread array: registers for small k, L1-resident local memory for large k; the reference is unbounded in k):
 // same shell sweep as nn_search.cuh, with a per-thread sorted list of the k best (d2, index) pairs

@@ -1,4 +1,4 @@
-// Device-side exact nearest-neighbour search over the uniform grid (product code, sm_100a).
+// Device-side exact nearest-neighbour search over the uniform grid (product code, sm_90a).
 //
 // Replaces the nanoflann kd-tree descent the reference runs per query
 // (core/kd_tree.hpp:284-291 -> 3rd_party/nanoflann/nanoflann.hpp:1709-1732,1886-1961) with a
@@ -100,9 +100,8 @@ __device__ __forceinline__ void scan_range(const float4* __restrict__ pts, uint3
       }
     }
   } else {
-    // The scan is a chain of load -> use steps; ncu showed ~25 such waits per warp at ~900 cycles
-    // each (long scoreboard = 64 % of warp residency). Batches of kW candidates put kW loads in
-    // flight per wait; slots past the end of the range are predicated off (no padded arithmetic —
+    // The scan is a chain of load -> use steps, and the warps mostly wait on those loads (long
+    // scoreboard). Batches of kW candidates put kW loads in flight per wait; slots past the end of the range are predicated off (no padded arithmetic —
     // a padded variant doubled the instruction count and was slower).
     constexpr int kW = 4;
     auto eval = [&](const float4& p, uint32_t j) {

@@ -1,4 +1,4 @@
-// Per-point normal and curvature estimation (product code, sm_100a).
+// Per-point normal and curvature estimation (product code, sm_90a).
 // Replaces NormalEstimation::compute_normals_*/compute_normals_curvature_* (core/normal_estimation.hpp:
 // 279-332, 357-421) behind PointCloud::estimateNormals{KNN,Radius,KNNInRadius} (utilities/point_cloud.hpp:
 // 294-420): one thread per point of the (cell-sorted) cloud runs the neighbourhood search over the

@@ -1,4 +1,4 @@
-// Stable LSD radix sort of (uint64 key, uint32 value) pairs, 8 bits per pass (product code, sm_100a).
+// Stable LSD radix sort of (uint64 key, uint32 value) pairs, 8 bits per pass (product code, sm_90a).
 // Used by the voxel-grid downsampler (bin key -> point index) where the number of bins is unbounded and a
 // dense counter table (grid_index.cu) is not an option. HBM-bound integer work: per pass one histogram
 // read (8 B/elem) and one scatter pass (12 B read + 12 B written per element); only the passes the key

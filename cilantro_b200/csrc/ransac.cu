@@ -1,4 +1,4 @@
-// RANSAC hypothesis scoring for rigid transforms (product code, sm_100a).
+// RANSAC hypothesis scoring for rigid transforms (product code, sm_90a).
 //
 // Replaces, for H hypotheses at once, TransformRANSACEstimator::computeResiduals
 // (model_estimation/ransac_transform_estimator.hpp:90-98) followed by the serial inlier scan of
@@ -173,7 +173,7 @@ int score_batch(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const
   const size_t smem = (size_t)kHypChunk * 12 * sizeof(float) + (size_t)H * sizeof(uint32_t);
   CB_CUDA(cudaFuncSetAttribute(ransac_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const size_t tile = (size_t)kBlock * kPairs;
-  int per_sm = 0;  // resident blocks per SM for this launch's dynamic shared memory (was a fixed 2: 22 % occupancy)
+  int per_sm = 0;  // resident blocks per SM for this launch's dynamic shared memory (a fixed 2 left most warp slots empty)
   CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ransac_score_kernel, kBlock, smem));
   per_sm = std::max(1, std::min(per_sm, 6));
   const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (dst->n + tile - 1) / tile));

@@ -30,8 +30,8 @@ __device__ __forceinline__ void block_sum_rows(const double* __restrict__ table,
 
 // warp shuffle -> shared -> one row per block; the last block of each group of kReduceGroup blocks
 // folds the group's rows into one group row; the last group folds the group rows into `result`.
-// Two levels keep the serial tail short (a single last block summing thousands of rows was measured
-// at ~30 us of a 100 us kernel). Summation order is fixed, so the result does not depend on block
+// Two levels keep the serial tail short (a single last block summing thousands of rows is a long
+// serial tail). Summation order is fixed, so the result does not depend on block
 // scheduling. All counters are zero on entry and are left zero.
 template <int NV>
 __device__ __forceinline__ void grid_reduce(double (&acc)[NV], const ReduceScratch& rs) {
@@ -77,8 +77,8 @@ __device__ __forceinline__ void grid_reduce(double (&acc)[NV], const ReduceScrat
 // Same result and the same fixed summation order, but no warp ever WAITS for another: each warp
 // parks its 32-lane sum in its own shared slot and takes a ticket; the warp that arrives last folds
 // the block's slots, writes the block row and carries on alone through the group / grid levels.
-// Used by the ICP search kernel, whose warps finish at very different times (ncu: a third of the
-// warp residency was spent at the __syncthreads of the barrier version).
+// Used by the ICP search kernel, whose warps finish at very different times (the barrier version kept
+// warps parked at __syncthreads).
 template <int NV>
 struct AsyncReduceSmem {
   double slot[kReduceBlock / 32][NV];

@@ -1,8 +1,8 @@
-// Warp-cooperative 6x6 solve of the Gauss-Newton normal equations (product code, sm_100a): the same elimination as
+// Warp-cooperative 6x6 solve of the Gauss-Newton normal equations (product code, sm_90a): the same elimination as
 // la::solve6 (solve_core.hpp: partial pivoting, one reciprocal per pivot, back substitution in the same order) with
 // the augmented matrix spread over the lanes of ONE warp instead of a local-memory array of one thread. In the
-// single-thread epilogue of a device-resident ICP iteration the serial version cost ~10 us of dependent
-// local-memory accesses (%globaltimer trace: 19 us per combined-metric solve); here every step is a handful of
+// single-thread epilogue of a device-resident ICP iteration the serial version was a chain of dependent
+// local-memory accesses; here every step is a handful of
 // shuffles and the six divisions are the critical path.
 #pragma once
 #include "cb_internal.hpp"

@@ -1,4 +1,4 @@
-// First and second moments of a point set (product code, sm_100a).
+// First and second moments of a point set (product code, sm_90a).
 // Replaces the two serial passes of Covariance::operator() (core/covariance.hpp:64-76) and the
 // rowwise().mean() of the ICP constructors (icp_single_transform_combined_metric.hpp:51-58) with one
 // streaming pass over the packed xyz array: HBM-bound, 12 B/point.

@@ -1,10 +1,9 @@
-// Warp-cooperative exact nearest neighbour over the grid (product code, sm_100a).
+// Warp-cooperative exact nearest neighbour over the grid (product code, sm_90a).
 //
 // Why: in the per-lane search (nn_search.cuh) each of the 10 "residual" regions around a query — the
 // two x-neighbour cells and the 8 neighbour rows of shells 0-1 — is needed by only ~5-15 % of the
 // lanes once the own cell has been scanned (the match is usually there), but a warp executes a
-// region's scan loop if ANY lane needs it, so >60 % of the issued instructions were spent at <15 %
-// lane utilisation (ncu, profiles/r01_icp_pass_kernel.md: 79 M warp-instructions per 1 M queries).
+// region's scan loop if ANY lane needs it, so most of the issued instructions ran at low lane utilisation.
 //
 // Here the warp pools that work:
 //   phase A (per lane)   own-cell scan; decide which of the 10 regions can still hold a closer point;

@@ -1,4 +1,4 @@
-// Warp-cooperative exact nearest neighbour WITH an exclusion bound (product code, sm_100a).
+// Warp-cooperative exact nearest neighbour WITH an exclusion bound (product code, sm_90a).
 //
 // Same search as warp_grid_nearest() (warp_search.cuh) — same candidates' arithmetic, same conservative
 // region bounds, same tie rule, hence the same (index, d2) bit for bit — plus one more output:
@@ -126,7 +126,7 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
     constexpr int kDy[8] = {-1, 1, 0, 0, -1, 1, -1, 1};
     constexpr int kDz[8] = {0, 0, -1, 1, -1, -1, 1, 1};
     // (Tried: a 10-bit need mask per lane, ONE warp scan and lane-major item order instead of a ballot per region -
-    // fewer instructions (this loop is 21 % of the cold kernel's, ncu source page) but 8 % slower: region-major order
+    // fewer instructions but slower: region-major order
     // makes neighbouring lanes of the pooled scan read neighbouring rows of the sorted array.)
 #pragma unroll
     for (int t = 0; t < 10; ++t) {

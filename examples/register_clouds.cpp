@@ -1,6 +1,6 @@
 // Example: the flow of cilantro's examples/rigid_icp.cpp and examples/normal_estimation.cpp — load, voxel-grid
 // downsample, estimate normals, register with the combined-metric ICP, save — written against the cilantro names and
-// running on a B200 through libcilantro_b200.so (no Eigen, no visualisation).
+// running on an H100 through libcilantro_b200.so (no Eigen, no visualisation).
 //
 //   make -C examples && ./examples/register_clouds dst.ply src.ply [bin_size] [max_correspondence_distance]
 //

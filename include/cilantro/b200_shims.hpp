@@ -1,8 +1,8 @@
 // cilantro_b200 — header-only C++ mirror of the cilantro types on the rigid-ICP / k-means / RANSAC /
 // PCA hot path, forwarding to the C ABI of libcilantro_b200.so (include/cilantro_b200.h).
 //
-// Same names, argument meaning and error behaviour as the reference (paths relative to
-// /root/reference/include/cilantro/):
+// Same names, argument meaning and error behaviour as the reference (paths relative to its
+// include/cilantro/):
 //   VectorSet3f / ConstVectorSetMatrixMap3f / Vector3f      core/data_containers.hpp:73-156
 //   RigidTransform3f                                        core/space_transformations.hpp:54-57
 //   Neighbor / NeighborSet                                  core/nearest_neighbors.hpp

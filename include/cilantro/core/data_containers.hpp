@@ -1,3 +1,3 @@
-// Same include path as cilantro's core/data_containers.hpp; the B200-native drop-in lives in b200_shims.hpp.
+// Same include path as cilantro's core/data_containers.hpp; the GPU-native drop-in lives in b200_shims.hpp.
 #pragma once
 #include "../b200_shims.hpp"

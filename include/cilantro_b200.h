@@ -1,9 +1,9 @@
 /*
- * cilantro_b200 — C ABI of the B200-native (sm_100a) rigid-ICP / k-means / RANSAC / PCA hot path.
+ * cilantro_b200 — C ABI of the H100-native (sm_90a) rigid-ICP / k-means / RANSAC / PCA hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b). cilantro itself has no FFI: its "interface" for this
  * path is a set of C++ templates over Eigen types. Each entry point below names the reference
- * function(s) it replaces (paths relative to /root/reference/include/cilantro/). The header-only C++
+ * function(s) it replaces (paths relative to the reference's include/cilantro/). The header-only C++
  * shims in include/cilantro/ re-create the reference's class names on top of these calls; see
  * INTEGRATION.md for the binding a cilantro maintainer would add.
  *

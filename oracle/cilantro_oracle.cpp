@@ -2,7 +2,7 @@
 //
 // CPU restatement (no Eigen, no CUDA) of the rigid-ICP / k-means / RANSAC / PCA hot path of
 // kzampog/cilantro, written from the reference's behaviour; every function cites the
-// reference file:line it follows (paths relative to /root/reference/include/cilantro/).
+// reference file:line it follows (paths relative to the reference's include/cilantro/).
 // Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
 // load this library, and only as the checker / CPU baseline. The product
 // (cilantro_b200/csrc) never links, includes or calls anything in oracle/.

@@ -1,5 +1,5 @@
 """Registers / stack / shared memory per kernel of the built library, from `cuobjdump --dump-resource-usage`
-(no GPU needed). Writes profiles/r02_resource_usage.md.   python profiles/resource_usage.py"""
+(no GPU needed). Writes profiles/resource_usage.md.   python profiles/resource_usage.py"""
 import os
 import re
 import subprocess
@@ -28,15 +28,15 @@ def main():
                 rows.append((short, *map(int, m.groups())))
             fn = None
     rows.sort()
-    out = ["# Kernel resources (round 2 build; `cuobjdump --dump-resource-usage`, sm_100a)", "",
+    out = ["# Kernel resources (`cuobjdump --dump-resource-usage`, sm_90a)", "",
            "STACK is per-thread local memory the kernel reserves: call frames of the out-of-line far-chunk search",
            "(`search_chunk_far`, DESIGN §4.2), the k-best arrays of the general-k search, and spills. The loop's cached pass",
-           "(`icp_cached_pipe_kernel`, 40 B in the combined-metric variant at 3 blocks per SM) and the k-means / RANSAC kernels",
-           "stay in registers. `MODE` template values: 0 correspondences only, 1 p2p raw moments, 2 combined, 3 p2p pivoted moments.", "",
+           "(`icp_cached_pipe_kernel`) and the k-means / RANSAC kernels stay (almost) in registers.",
+           "`MODE` template values: 0 correspondences only, 1 p2p raw moments, 2 combined, 3 p2p pivoted moments.", "",
            "| kernel | registers | stack B | static smem B |", "|---|---:|---:|---:|"]
     for name, reg, stack, smem, _local in rows:
         out.append(f"| `{name}` | {reg} | {stack} | {smem} |")
-    path = os.path.join(ROOT, "profiles", "r02_resource_usage.md")
+    path = os.path.join(ROOT, "profiles", "resource_usage.md")
     with open(path, "w") as f:
         f.write("\n".join(out) + "\n")
     print(path, len(rows), "kernels")

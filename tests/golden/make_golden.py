@@ -1,6 +1,6 @@
 """Generate tests/golden/oracle_golden.json (committed fixture).
 
-Run in the build container, where /root/reference exists and oracle/_ref has been built from the
+Run where a reference checkout exists and oracle/_ref has been built from the
 reference's own nanoflann:   python tests/golden/make_golden.py
 The kNN entries are produced with the REFERENCE kd-tree (oracle.RefKnn) when available, so the
 fixture pins the brute-force restatement to the reference's own code on a case without exact ties.

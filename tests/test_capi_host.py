@@ -31,7 +31,7 @@ def test_library_exports_every_declared_symbol(cb):
     missing = [s for s in declared if not hasattr(lib, s)]
     assert not missing, f"declared in include/cilantro_b200.h but not exported: {missing}"
     assert sorted(cb.EXPORTED) == declared, "capi.EXPORTED is out of sync with the header"
-    assert b"sm_100a" in lib.cb_version()
+    assert b"sm_90a" in lib.cb_version()
 
 
 def test_integration_guide_names_every_entry_point():
@@ -172,8 +172,8 @@ def test_product_never_touches_the_oracle():
     assert "oracle" not in needed and "ref_knn" not in needed
 
 
-def test_library_carries_only_sm_100a_code():
-    """Built for B200 and nothing else: every embedded cubin is sm_100a (no multi-arch fat binary, no PTX-only JIT
+def test_library_carries_only_sm_90a_code():
+    """Built for H100 and nothing else: every embedded cubin is sm_90a (no multi-arch fat binary, no PTX-only JIT
     path), and the hot kernels are in it."""
     import shutil
     import subprocess
@@ -183,7 +183,7 @@ def test_library_carries_only_sm_100a_code():
     lib = os.path.join(ROOT, "cilantro_b200", "libcilantro_b200.so")
     elfs = [ln for ln in subprocess.run(["cuobjdump", "-lelf", lib], capture_output=True, text=True).stdout.splitlines()
             if ln.startswith("ELF file")]
-    assert elfs and all(".sm_100a.cubin" in ln for ln in elfs), elfs
+    assert elfs and all(".sm_90a.cubin" in ln for ln in elfs), elfs
     syms = subprocess.run(["cuobjdump", "-symbols", lib], capture_output=True, text=True).stdout
     for kernel in ("icp_pass_kernel", "icp_search_kernel", "icp_cached_pipe_kernel", "icp_finish_kernel",
                    "kmeans_assign_kernel", "ransac_score_kernel", "moments_kernel", "normals_knn_kernel",

@@ -3,7 +3,8 @@ examples/test_clouds/test.ply) — on the committed fixture tests/golden/config1
 at 12 mm by the oracle; tests/golden/make_config1_fixture.py).
 
 CPU part: the oracle runs the example's recipe (rigid_icp.cpp:25-65, settings :119-123) and recovers tf_ref^-1 — the
-self-checking property the example prints; where /root/reference exists the fixture is regenerated and compared.
+self-checking property the example prints; the fixture is checked against an excerpt of the scan
+(tests/golden/scan_excerpt.ply).
 GPU part: the same recipe through the C ABI against the oracle: transforms within 1e-5, neighbour indices and residuals
 bit-exact, plus downsampling and normal estimation on real scan data.
 """
@@ -30,16 +31,16 @@ def test_fixture_matches_the_reference_scan(orc):
     pts, nrm, n_source, n5 = _scan()
     assert pts.shape == nrm.shape and pts.shape[0] > 40000 and n_source == 573663
     assert np.all(np.abs(np.linalg.norm(nrm, axis=1) - 1) < 1e-4)
-    if not os.path.exists("/root/reference/examples/test_clouds/test.ply"):
-        pytest.skip("no /root/reference on this machine: fixture content checked where it was made")
-    from golden.make_config1_fixture import read_test_ply
+    assert pts.shape[0] < n5 < n_source
+    from golden.make_config1_fixture import EXCERPT, read_test_ply
 
-    p, n, c = read_test_ply()
-    assert p.shape[0] == n_source
-    assert orc.grid_downsample(p, 0.005, normals=n, colors=c)[0].shape[0] == n5
+    # the excerpt holds every scan vertex of some 12 mm bins: their averages are those bins of the fixture, bit for bit
+    p, n, _ = read_test_ply(EXCERPT)
     p12, n12, _ = orc.grid_downsample(p, 0.012, normals=n)
-    assert np.array_equal(p12.view(np.uint32), pts.view(np.uint32))
-    assert np.array_equal(n12.view(np.uint32), nrm.view(np.uint32))
+    row = {r.tobytes(): i for i, r in enumerate(pts.view(np.uint32))}
+    at = [row.get(r.tobytes()) for r in p12.view(np.uint32)]
+    assert p12.shape[0] > 100 and None not in at
+    assert np.array_equal(n12.view(np.uint32), nrm[at].view(np.uint32))
 
 
 def test_oracle_runs_the_example_recipe(orc):
