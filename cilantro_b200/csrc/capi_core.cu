@@ -615,10 +615,12 @@ void cb_icp_default_params(cb_icp_params* p) {
   p->inlier_fraction = 1.0;
 }
 
-// mean of a cloud over all ranks (rowwise().mean(), icp_single_transform_combined_metric.hpp:51-58)
+// mean of the finite points of a cloud over all ranks (rowwise().mean(), icp_single_transform_combined_metric.hpp:51-58,
+// on the cloud without its NaN / Inf points): the pivots of every ICP metric. The searches never match a non-finite
+// point, so skipping them keeps the pivots, and with them the transform, finite (DESIGN §6).
 static int global_mean(cb_context* ctx, const cb_cloud* c, bool allreduce, float* mean3) {
   const float zero[3] = {0, 0, 0};
-  CB_TRY(launch_moments(ctx, c->d_raw, c->n, zero));
+  CB_TRY(launch_moments(ctx, c->d_raw, c->n, zero, /*finite_only=*/true));
   double m[kMomentValues];
   CB_TRY(fetch_result(ctx, kMomentValues, allreduce, m));
   for (int r = 0; r < 3; r++) mean3[r] = (m[0] > 0) ? (float)(m[1 + r] / m[0]) : 0.f;

@@ -11,13 +11,17 @@ namespace cb {
 
 namespace {
 
-// result[0] = n, [1..3] = sum (p - c), [4..9] = sum (p - c)(p - c)^T upper triangle (xx xy xz yy yz zz)
+// result[0] = n, [1..3] = sum (p - c), [4..9] = sum (p - c)(p - c)^T upper triangle (xx xy xz yy yz zz).
+// kFiniteOnly: points with a NaN / Inf coordinate are skipped (n counts the finite ones) - the ICP pivots, which must
+// stay finite whatever the cloud holds; otherwise every point counts, as in Covariance::operator().
+template <bool kFiniteOnly>
 __global__ void __launch_bounds__(kReduceBlock) moments_kernel(const float* __restrict__ raw, size_t n, float cx,
                                                                float cy, float cz, const ReduceScratch rs) {
   double acc[kMomentValues];
 #pragma unroll
   for (int i = 0; i < kMomentValues; i++) acc[i] = 0.0;
   auto add = [&](float px, float py, float pz) {
+    if (kFiniteOnly && !(isfinite(px) && isfinite(py) && isfinite(pz))) return;
     const double x = (double)px - (double)cx, y = (double)py - (double)cy, z = (double)pz - (double)cz;
     acc[0] += 1.0;
     acc[1] += x;
@@ -55,19 +59,25 @@ __global__ void __launch_bounds__(kReduceBlock) moments_kernel(const float* __re
 
 }  // namespace
 
-int launch_moments(cb_context* ctx, const float* d_raw, size_t n, const float* shift3) {
+int launch_moments(cb_context* ctx, const float* d_raw, size_t n, const float* shift3, bool finite_only) {
   // persistent grid: a whole number of resident blocks per SM (occupancy API), 8 points per thread and trip
-  static int per_sm = 0;
-  if (per_sm == 0) {
+  static int per_sm[2] = {0, 0};
+  int& psm = per_sm[finite_only ? 1 : 0];
+  if (psm == 0) {
     int v = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, moments_kernel, kReduceBlock, 0) != cudaSuccess || v < 1) v = 4;
-    per_sm = v;
+    const cudaError_t e = finite_only ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, moments_kernel<true>, kReduceBlock, 0)
+                                      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, moments_kernel<false>, kReduceBlock, 0);
+    if (e != cudaSuccess || v < 1) v = 4;
+    psm = v;
   }
   int blocks = (int)std::max<size_t>(
-      1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (n / 8 + kReduceBlock - 1) / kReduceBlock + 1));
+      1, std::min<size_t>((size_t)ctx->sm_count * psm, (n / 8 + kReduceBlock - 1) / kReduceBlock + 1));
   ReduceScratch rs;
   CB_TRY(get_reduce_scratch(ctx, blocks, kMomentValues, &rs));
-  moments_kernel<<<blocks, kReduceBlock, 0, ctx->stream>>>(d_raw, n, shift3[0], shift3[1], shift3[2], rs);
+  if (finite_only)
+    moments_kernel<true><<<blocks, kReduceBlock, 0, ctx->stream>>>(d_raw, n, shift3[0], shift3[1], shift3[2], rs);
+  else
+    moments_kernel<false><<<blocks, kReduceBlock, 0, ctx->stream>>>(d_raw, n, shift3[0], shift3[1], shift3[2], rs);
   ctx->launches += 1;
   CB_CUDA(cudaGetLastError());
   return CB_OK;
