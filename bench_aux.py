@@ -5,6 +5,7 @@
     python bench.py --workload pca_50m      [--steps K --warmup W]     step = one mean+covariance pass
     python bench.py --workload segment_1m   [--steps K --warmup W]     step = one all-seeds segmentation (radius)
     python bench.py --workload segment_knn_1m                           step = one all-seeds segmentation (kNN 10)
+    python bench.py --workload meanshift_1m [--steps K --warmup W]     step = one all-seeds mean-shift call
 
 Same timing hygiene as the ICP workload (CUDA events inside the library, inputs larger than L2 or an L2
 flush, CPU baseline = the oracle on a bounded sample of the same workload).
@@ -460,9 +461,90 @@ def _pca_parity(g, o, sample):
     return out
 
 
+def meanshift(args, blobs=1000, per_blob=1000, ctx=None):
+    """MeanShift3f::cluster on synth.mean_shift_scene(blobs, per_blob, sigma=1), every point a seed, the reference
+    example's recipe (kernel radius 2 sigma, cluster tol 0.2 sigma, flat kernel), max_iter 100. One step = one call."""
+    import oracle
+    from oracle import mean_shift as oms
+    from cilantro_b200 import synth
+
+    capi, ctx = _ctx(ctx)
+    sc = synth.mean_shift_scene(blobs, per_blob, sigma=1.0, seed=1)
+    pts = sc["points"]
+    n = pts.shape[0]
+    radius, max_iter, ctol = 2.0, 100, 0.2
+    cloud = capi.Cloud(ctx, pts)
+    for _ in range(max(args.warmup, 1)):
+        cloud.mean_shift(radius, max_iter, ctol)
+    l0 = ctx.kernel_launches()
+    ms_list, shift_list = [], []
+    for _ in range(args.steps):
+        ctx.flush_l2()
+        r = cloud.mean_shift(radius, max_iter, ctol)
+        ms_list.append(r["gpu_ms"])
+        shift_list.append(r["gpu_ms_shift"])
+    launches = (ctx.kernel_launches() - l0) // max(args.steps, 1)
+    ms, ms_shift = float(np.mean(ms_list)), float(np.mean(shift_list))
+    r2 = float(np.float32(radius) * np.float32(radius))
+    count_ms, pairs = _radius_count_ms(capi, ctx, cloud, r2)
+    # device time per kernel of one call (torch.profiler, CUDA activities, in a run of its own)
+    kernels = None
+    try:
+        import torch
+        from torch.profiler import ProfilerActivity, profile
+
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            cloud.mean_shift(radius, max_iter, ctol)
+            torch.cuda.synchronize()
+        acc = {}
+        for e in prof.events():
+            if e.device_type == torch.autograd.DeviceType.CUDA:
+                name = e.name.replace("(anonymous namespace)::", "").replace("void ", "").split("(")[0]
+                acc[name] = acc.get(name, 0.0) + e.device_time_total / 1e3
+        kernels = {k: round(v, 3) for k, v in sorted(acc.items(), key=lambda kv: -kv[1])[:12]}
+    except Exception as exc:  # the profiler is diagnostic only: the timed numbers above do not depend on it
+        kernels = {"error": repr(exc)}
+    # CPU arm: one reference nanoflann radius pass (OpenMP) over a seeded 1 % sample of the seeds at the first
+    # iteration's positions; the seeds are independent, so this is the per-seed rate of one full shift iteration.
+    rng = np.random.default_rng(7)
+    sample = np.sort(rng.choice(n, n // 100, replace=False))
+    knn = oracle.make_knn(pts)
+    _, _, cnt = knn.neighborhoods(pts[sample], 0, r2, stride=1)
+    stride = max(1, int(cnt.max()))
+    t0 = time.perf_counter()
+    knn.neighborhoods(pts[sample], 0, r2, stride=stride)
+    t_sample = time.perf_counter() - t0
+    cpu_iter_ms = t_sample * 1e3 * n / sample.size
+    # parity inside the run: the oracle's shift of 200 sampled seeds (bit for bit) and the oracle's clustering of the
+    # device's shifted seeds (labels, CSR and modes)
+    few = np.sort(rng.choice(n, 200, replace=False))
+    want = oms.mean_shift(pts, radius, r["iterations"], ctol, seeds=pts[few])
+    shift_ok = bool(np.array_equal(want["shifted_seeds"].view(np.uint32), r["shifted_seeds"][few].view(np.uint32)))
+    wc = oms.mean_shift(pts, radius, 0, ctol, seeds=r["shifted_seeds"])
+    cluster_ok = bool(all(np.array_equal(wc[k], r[k]) for k in ("offsets", "points", "point_to_cluster")) and
+                      np.array_equal(wc["modes"].view(np.uint32), r["modes"].view(np.uint32)))
+    return {
+        "metric": "meanshift_ms_per_call", "value": ms, "unit": "ms", "n_gpus": 1, "steps": args.steps,
+        "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": False, "dtype": "f32", "data": "synthetic",
+        "config": {"workload": f"MeanShift3f::cluster on synth.mean_shift_scene({blobs}, {per_blob}, sigma 1): {n} seeds, "
+                               f"kernel radius {radius}, cluster tol {ctol}, flat kernel, max_iter {max_iter}",
+                   "l2": "flushed before every timed call"},
+        "iterations": r["iterations"], "clusters": r["num_clusters"], "gpu_launches": int(launches),
+        "ms_shift": ms_shift, "ms_cluster": ms - ms_shift, "ms_per_iteration": ms_shift / max(r["iterations"], 1),
+        "kernel_ms_one_call": kernels,
+        "sweep_yardstick": {"radius_count_ms": count_ms, "pairs": pairs,
+                            "what": "one cb_radius_search sizing call on the same cloud at the kernel radius"},
+        "cpu_baseline": {"ms_per_full_iteration": cpu_iter_ms, "sample_seeds": int(sample.size), "sample_s": t_sample,
+                         "impl": knn.kind, "threads": oracle.num_threads(),
+                         "what": "reference nanoflann radiusSearch over a 1 % seed sample at the starting positions, "
+                                 "scaled to all seeds (one shift iteration; the weighted sums are not timed)"},
+        "parity": {"sampled_shifted_seeds_bit_exact": shift_ok, "oracle_clustering_of_gpu_seeds_identical": cluster_ok},
+    }
+
+
 AUX = {"downsample_10m": downsample, "downsample_1m": lambda a: downsample(a, n=1_000_000, bin_size=0.02),
        "normals_5m": normals, "normals_1m": lambda a: normals(a, n=1_000_000),
        "kmeans_50m": kmeans, "ransac_5m": ransac, "pca_50m": pca,
        "kmeans_5m": lambda a: kmeans(a, n=5_000_000, k=256), "ransac_500k": lambda a: ransac(a, n=500_000, batch=256),
        "pca_5m": lambda a: pca(a, n=5_000_000),
-       "segment_1m": segment, "segment_knn_1m": lambda a: segment(a, k=10)}
+       "segment_1m": segment, "segment_knn_1m": lambda a: segment(a, k=10), "meanshift_1m": meanshift}

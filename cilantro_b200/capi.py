@@ -101,6 +101,21 @@ class SegmentParams(C.Structure):
 SEG_POINTS, SEG_NORMALS, SEG_COLORS = 1, 2, 4
 
 
+class MeanShiftParams(C.Structure):
+    _fields_ = [
+        ("kernel_radius", C.c_float),
+        ("weight_kind", C.c_int32),
+        ("max_iter", C.c_uint64),
+        ("cluster_tol", C.c_float),
+        ("convergence_tol", C.c_float),
+        ("weight_coeff", C.c_float),
+        ("reserved_", C.c_int32),
+    ]
+
+
+FLT_EPSILON = float(np.finfo(np.float32).eps)
+
+
 # every symbol include/cilantro_b200.h declares (tests/test_capi_host.py checks that the .so exports them and that this list matches the header)
 EXPORTED = [
     "cb_last_error", "cb_version",
@@ -110,6 +125,7 @@ EXPORTED = [
     "cb_comm_ipc_detach",
     "cb_cloud_create", "cb_cloud_create_pair", "cb_cloud_create_from_device", "cb_cloud_create_replicated", "cb_cloud_destroy", "cb_cloud_size", "cb_cloud_grid_info",
     "cb_cloud_estimate_normals", "cb_grid_downsample", "cb_cloud_grid_downsample", "cb_cloud_download", "cb_cloud_segment",
+    "cb_cloud_mean_shift",
     "cb_knn1_radius", "cb_knn_radius", "cb_radius_search", "cb_find_correspondences",
     "cb_icp_default_params", "cb_icp_create", "cb_icp_destroy", "cb_icp_estimate", "cb_icp_iteration_times",
     "cb_icp_correspondences", "cb_icp_residuals", "cb_icp_accumulate", "cb_icp_loop_cache",
@@ -341,6 +357,41 @@ class Cloud:
         off = off[:m + 1].astype(np.int64)
         return {"offsets": off, "points": pts[:off[-1]].astype(np.int64), "point_to_cluster": p2c.astype(np.int64),
                 "num_clusters": m, "gpu_ms": ms.value}
+
+    def mean_shift(self, kernel_radius, max_iter, cluster_tol, convergence_tol=FLT_EPSILON, seeds=None, weight="unity"):
+        """cb_cloud_mean_shift (MeanShift3f::cluster). seeds None = the cloud's own points; weight "unity" or
+        ("rbf", sigma) (RBFKernelWeightEvaluator<float, float, true>). Returns dict(offsets, points, point_to_cluster,
+        num_clusters, gpu_ms) laid out like segment()'s, indexed by seed, plus shifted_seeds, modes, iterations and
+        gpu_ms_shift (the shift loop's part of gpu_ms)."""
+        p = MeanShiftParams()
+        p.kernel_radius, p.max_iter = float(kernel_radius), int(max_iter)
+        p.cluster_tol, p.convergence_tol = float(cluster_tol), float(convergence_tol)
+        if weight == "unity":
+            p.weight_kind = 0
+        else:
+            kind, sigma = weight
+            assert kind == "rbf", weight
+            p.weight_kind, p.weight_coeff = 1, rbf_coeff(sigma)
+        sd = _f32(seeds) if seeds is not None else None
+        ns = self.n if sd is None else sd.shape[0]
+        if sd is not None and ns == 0:
+            sd = np.empty((1, 3), np.float32)
+        shifted = np.empty((max(ns, 1), 3), np.float32)
+        modes = np.empty((max(ns, 1), 3), np.float32)
+        p2c = np.empty(max(ns, 1), np.uint64)
+        off = np.empty(ns + 1, np.uint64)
+        pts = np.empty(max(ns, 1), np.uint64)
+        m = C.c_size_t()
+        it = C.c_uint64()
+        ms, ms_shift = C.c_float(), C.c_float()
+        _check(lib().cb_cloud_mean_shift(self.ctx.h, self.h, C.byref(p), _p(sd), C.c_size_t(ns), _p(shifted), _p(p2c),
+                                         _p(off), _p(pts), _p(modes), C.byref(m), C.byref(it), C.byref(ms),
+                                         C.byref(ms_shift)))
+        m = m.value
+        off = off[:m + 1].astype(np.int64)
+        return {"offsets": off, "points": pts[:off[-1]].astype(np.int64), "point_to_cluster": p2c[:ns].astype(np.int64),
+                "num_clusters": m, "shifted_seeds": shifted[:ns].copy(), "modes": modes[:m].copy(),
+                "iterations": int(it.value), "gpu_ms": ms.value, "gpu_ms_shift": ms_shift.value}
 
     def download(self, normals=False):
         xyz = np.empty((self.n, 3), np.float32)

@@ -187,3 +187,25 @@ def segment_far_scene(seed=1, outliers=0):
     nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
     perm = rng.permutation(pts.shape[0])
     return pts[perm].astype(np.float32), nrm[perm].astype(np.float32)
+
+
+def mean_shift_scene(blobs, per_blob, sigma=1.0, seed=1):
+    """Truncated-Gaussian blobs for mean-shift: per_blob points around each centre, N(0, sigma^2) per axis, cut at
+    4 sigma from the centre, point-symmetric about it (every offset d comes with -d), so the centre is the blob's
+    centroid. Centres sit on a lattice of pitch 16 sigma around the origin with +-2 sigma jitter, hence >= 12 sigma
+    apart. With the reference example's recipe (kernel radius 2 sigma, cluster tol 0.2 sigma) the answer is one
+    cluster per blob. Returns dict(points (n,3) float32 in random order, blob (n,) blob id per point, centres
+    (blobs,3) float64, sigma)."""
+    rng = np.random.default_rng(seed)
+    side = int(np.ceil(blobs ** (1.0 / 3.0)))
+    lat = np.stack(np.meshgrid(*(np.arange(side),) * 3, indexing="ij"), axis=-1).reshape(-1, 3)[:blobs]
+    centres = (lat - (side - 1) / 2.0) * 16.0 * sigma + rng.uniform(-2.0, 2.0, (blobs, 3)) * sigma
+    half = (per_blob + 1) // 2
+    off = rng.standard_normal((blobs, 4 * half, 3))
+    keep = np.linalg.norm(off, axis=2) <= 4.0
+    d = np.stack([o[k][:half] for o, k in zip(off, keep)]) * sigma  # (>= half of 4 * half survive the cut)
+    pts = np.concatenate([centres[:, None, :] + d, centres[:, None, :] - d], axis=1)[:, :per_blob]
+    blob = np.repeat(np.arange(blobs), per_blob)
+    perm = rng.permutation(blobs * per_blob)
+    return {"points": np.ascontiguousarray(pts.reshape(-1, 3)[perm], np.float32), "blob": blob[perm],
+            "centres": centres, "sigma": float(sigma)}

@@ -603,6 +603,8 @@ public:
   using InputScalar = ValueT;
   using OutputScalar = WeightT;
   constexpr WeightT operator()(ValueT) const { return (WeightT)1; }
+  template <class PointT>
+  constexpr WeightT operator()(const PointT&, const PointT&, ValueT) const { return (WeightT)1; }
   constexpr WeightT operator()(size_t, size_t, ValueT) const { return (WeightT)1; }
   static constexpr int b200_kind() { return CB_WEIGHT_UNITY; }
   float b200_coeff() const { return 0.f; }
@@ -622,6 +624,8 @@ public:
     return *this;
   }
   WeightT operator()(ValueT dist) const { return std::exp(coeff_ * static_cast<WeightT>(dist)); }
+  template <class PointT>
+  WeightT operator()(const PointT&, const PointT&, ValueT dist) const { return std::exp(coeff_ * static_cast<WeightT>(dist)); }
   WeightT operator()(size_t, size_t, ValueT dist) const { return std::exp(coeff_ * static_cast<WeightT>(dist)); }
   static constexpr int b200_kind() { return CB_WEIGHT_RBF; }
   float b200_coeff() const { return (float)coeff_; }

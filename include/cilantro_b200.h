@@ -208,6 +208,39 @@ typedef struct cb_segment_params {
 int cb_cloud_segment(cb_context* ctx, cb_cloud* cloud, const cb_segment_params* params, const float* normals,
                      const float* colors, const uint64_t* seeds, size_t n_seeds, uint64_t* point_to_cluster,
                      uint64_t* cluster_offsets, uint64_t* cluster_points, size_t* num_clusters, float* gpu_ms);
+/* ---- mean-shift clustering ---------------------------------------------------------------------
+ * Replaces MeanShift3f::cluster(seeds, kernel_radius, max_iter, cluster_tol, convergence_tol, evaluator)
+ * (clustering/mean_shift.hpp:37-115) and the all-points overload (:118-124, seeds == NULL: the cloud's own points).
+ * Shift (:45-82): r2 = kernel_radius^2 (kernel_radius is a distance, not a squared one), tol2 = convergence_tol^2;
+ * every iteration, every seed not yet converged takes N = the cloud points with d2 < r2, ascending (d2, index) (the
+ * reference leaves equal distances to std::sort), sums acc += w p_j and W += w in that order in fp32,
+ * m = acc * (1 / W), is marked converged when |seed - m|^2 < tol2, and becomes m. The loop stops after the first
+ * iteration whose processed seeds all converged, or at max_iter (zero seeds: 1 iteration). A seed without
+ * neighbours becomes NaN (0 * inf) and never converges. Cluster (:84-100): seed i joins the first cluster, in
+ * creation order, whose first seed is within |.|^2 < cluster_tol^2, else starts one. Modes (:102-112): the fp32 sum
+ * of the members' shifted seeds in member order times 1 / size.
+ * Weight (cb_weight_kind): CB_WEIGHT_UNITY (UnityWeightEvaluator, the default) or CB_WEIGHT_RBF
+ * (RBFKernelWeightEvaluator<float, float, true>: exp(weight_coeff * d2), weight_coeff = -0.5f / (sigma * sigma)).
+ * Outputs, sized by n_seeds: shifted_seeds[3 n_seeds], point_to_cluster[n_seeds] (indexed by SEED),
+ * cluster_offsets[n_seeds + 1], cluster_points[n_seeds] (CSR of getClusterToPointIndicesMap, seeds ascending),
+ * modes[3 n_seeds] (the first *num_clusters rows are written); *iterations = getNumberOfPerformedIterations().
+ * A cloud with index_offset != 0 or more than 2^31 - 1 seeds: CB_ERR_UNSUPPORTED; an empty cloud with seeds:
+ * CB_ERR_INVALID (the reference's kd-tree throws on an empty index); the seed limit is 2^31 - 1 because seed ids travel as
+ * 32-bit signed slots through the radius-list kernels. gpu_ms (may be NULL) = device time of the call, gpu_ms_shift
+ * (may be NULL) = the part spent in the shift loop (the rest is the clustering and the modes). */
+typedef struct cb_mean_shift_params {
+  float kernel_radius;
+  int32_t weight_kind;   /* cb_weight_kind */
+  uint64_t max_iter;
+  float cluster_tol;
+  float convergence_tol; /* FLT_EPSILON in the reference's signature */
+  float weight_coeff;    /* CB_WEIGHT_RBF only */
+  int32_t reserved_;
+} cb_mean_shift_params;
+int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_mean_shift_params* params, const float* seeds,
+                        size_t n_seeds, float* shifted_seeds, uint64_t* point_to_cluster, uint64_t* cluster_offsets,
+                        uint64_t* cluster_points, float* modes, size_t* num_clusters, uint64_t* iterations,
+                        float* gpu_ms, float* gpu_ms_shift);
 /* Copies a cloud's points (and normals, if normals != NULL and the cloud has them) back to the host in
  * original order. */
 int cb_cloud_download(cb_context* ctx, const cb_cloud* cloud, float* xyz, float* normals);

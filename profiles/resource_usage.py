@@ -9,7 +9,7 @@ LIB = os.path.join(ROOT, "cilantro_b200", "libcilantro_b200.so")
 HOT = ("icp_search_kernel", "icp_cached_pipe_kernel", "icp_cached_kernel", "icp_finish_kernel", "icp_pass_kernel",
        "pairs_pass_kernel", "kmeans_assign_kernel", "ransac_score_kernel", "inlier_moments_kernel", "moments_kernel",
        "normals_knn_kernel", "normals_radius_kernel", "knn_k_kernel", "radius_kernel", "residual_kernel",
-       "segment_kernel")
+       "segment_kernel", "shift_kernel", "round_kernel", "rep_kernel")
 
 
 def main():
@@ -28,7 +28,7 @@ def main():
             if any(h in short for h in HOT):
                 rows.append((short, *map(int, m.groups())))
             fn = None
-    rows.sort()
+    rows = sorted(set(rows))  # kernels of a shared header (radius_lists.cuh) appear once per translation unit
     out = ["# Kernel resources (`cuobjdump --dump-resource-usage`, sm_90a)", "",
            "STACK is per-thread local memory the kernel reserves: call frames of the out-of-line far-chunk search",
            "(`search_chunk_far`, DESIGN §4.2), the k-best arrays of the general-k search, and spills. The loop's cached pass",

@@ -60,6 +60,15 @@ def main():
                 colors=np.abs(sheet_n), seeds=[0, 5, 5, N - 1])
     seg.segment(k=8, seeds=[3, 4])
     seg.segment(k=8, radius2=0.02 ** 2, max_size=50)
+    # mean-shift: all points, a seed list with a far and a NaN seed, RBF weights, and many small batches
+    ms = synth.mean_shift_scene(4, 200, sigma=0.05, seed=1)
+    msc = capi.Cloud(ctx, ms["points"])
+    msc.mean_shift(0.1, 20, 0.01)
+    msc.mean_shift(0.1, 5, 0.01, seeds=np.concatenate([ms["points"][:50], [[9.0, 9.0, 9.0], [np.nan, 0.0, 0.0]]]))
+    msc.mean_shift(0.1, 5, 0.01, weight=("rbf", 0.05))
+    os.environ["CB_MEAN_SHIFT_PAIR_BUDGET"] = "500"
+    msc.mean_shift(0.1, 3, 0.01)
+    del os.environ["CB_MEAN_SHIFT_PAIR_BUDGET"]
     # k-means, RANSAC, PCA
     pts, cent = synth.kmeans_data(N, 16, seed=1)
     capi.kmeans_cluster(ctx, capi.Cloud(ctx, pts), cent, max_iter=3, tol=0.0)
