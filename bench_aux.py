@@ -6,6 +6,7 @@
     python bench.py --workload segment_1m   [--steps K --warmup W]     step = one all-seeds segmentation (radius)
     python bench.py --workload segment_knn_1m                           step = one all-seeds segmentation (kNN 10)
     python bench.py --workload meanshift_1m [--steps K --warmup W]     step = one all-seeds mean-shift call
+    python bench.py --workload ransac_plane_5m [--steps K --warmup W]  step = one batch of 1000 plane hypotheses
 
 Same timing hygiene as the ICP workload (CUDA events inside the library, inputs larger than L2 or an L2
 flush, CPU baseline = the oracle on a bounded sample of the same workload).
@@ -439,6 +440,95 @@ def segment(args, n=1_000_000, k=0, ctx=None):
     return line
 
 
+# SASS of plane_score_kernel's plane loop (cuobjdump -sass; two planes per trip of 8 points per thread): 48 FMUL,
+# 48 FADD, 16 FSETP, 16 SEL, 8 IADD3 and 18 shared-memory, vote and loop instructions = 154 per 16 point-hypotheses
+PLANE_INSTR_PER_POINT_HYP = 154 / 16
+
+
+def _gpu_facts():
+    """Name, power limit and maximum SM clock of GPU 0, read with nvidia-smi (queries only)."""
+    import subprocess
+
+    q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                       capture_output=True, text=True).stdout.strip().split(", ")
+    return {"name": q[0], "power_limit_w": float(q[1]), "max_sm_clock_mhz": float(q[2])}
+
+
+def ransac_plane(args, n=5_000_000, batch=1000, ctx=None):
+    """PlaneRANSACEstimator3f on a 5 M-point synth.plane_scene: the step is one batch of 1000 hypotheses through
+    cb_plane_score; also a full cb_ransac_plane with an unreachable target (phase split), the reference example's
+    recipe end to end, the FP32 issue share, the serial CPU computeResiduals + scan and parity with the oracle."""
+    import oracle
+    from cilantro_b200 import synth
+    from oracle import ransac_plane as orp
+
+    capi, ctx = _ctx(ctx)
+    gpu = _gpu_facts()
+    sc = synth.plane_scene(n, seed=1)
+    pts = sc["points"]
+    cloud = capi.Cloud(ctx, pts)
+    _, planes = orp.hypotheses(pts, 7, batch)  # the loop's own hypotheses (sample -> closed-form fit)
+    for _ in range(max(args.warmup, 1)):
+        capi.plane_score(ctx, cloud, planes, 0.01)
+    l0 = ctx.kernel_launches()
+    times = []
+    for _ in range(args.steps):
+        ctx.synchronize()
+        t0 = time.perf_counter()
+        counts = capi.plane_score(ctx, cloud, planes, 0.01)
+        times.append(time.perf_counter() - t0)
+    launches = ctx.kernel_launches() - l0
+    ms = 1e3 * float(np.median(times))
+    sms = ctx.device_info()["sm_count"]
+    issue_peak = sms * 4 * 32 * gpu["max_sm_clock_mhz"] * 1e6  # thread-instructions per second (4 schedulers per SM)
+    instr = PLANE_INSTR_PER_POINT_HYP * n * batch
+    # full loop, early exit disabled, and the reference example's recipe (examples/ransac_plane_estimator.cpp)
+    full = capi.ransac_plane(ctx, cloud, 11, max_iter=1000, thresh=0.01, inlier_count_thresh=n + 1)
+    recipe_kw = dict(max_iter=250, thresh=0.01, inlier_count_thresh=int(0.15 * n))
+    capi.ransac_plane(ctx, cloud, 3, **recipe_kw)
+    t0 = time.perf_counter()
+    recipe = capi.ransac_plane(ctx, cloud, 3, **recipe_kw)
+    recipe_s = time.perf_counter() - t0
+    # CPU arm: the reference's serial computeResiduals + inlier scan, one hypothesis at a time
+    hyp_cpu = 4
+    t0 = time.perf_counter()
+    oc = [orp.residuals(pts, planes[h], 0.01)[1].size for h in range(hyp_cpu)]
+    cpu_s = (time.perf_counter() - t0) / hyp_cpu
+    want = orp.ransac_plane(pts, 3, accum_double=True, **recipe_kw)
+    parity = {"counts_equal": bool(np.array_equal(oc, counts[:hyp_cpu])), "hypotheses_compared": hyp_cpu,
+              "recipe_iterations_equal": recipe["iterations"] == want["iterations"],
+              "recipe_best_iteration_equal": recipe["best_iteration"] == want["best_iteration"],
+              "recipe_hyp_plane_bits_equal": bool(np.array_equal(recipe["hyp_plane"].view(np.uint32),
+                                                                 want["hyp_plane"].view(np.uint32)))}
+    parity["all"] = all(v for k, v in parity.items() if k != "hypotheses_compared")
+    return {
+        "metric": "plane_ransac_hypotheses_per_sec", "value": batch * 1e3 / ms, "unit": "hypotheses/s", "n_gpus": 1,
+        "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
+        "vs_baseline": None, "dtype": "f32", "data": "synthetic", "gpu": gpu,
+        "config": {"workload": f"PlaneRANSACEstimator3f scoring: synth.plane_scene({n}) (floor 45 %, wall 25 %, clutter 30 %), "
+                               f"{batch} hypotheses per step, thresh 0.01",
+                   "l2": "inputs (60 MB) larger than L2; the points are read once per batch"},
+        "full_loop": {"iterations": full["iterations"], "ms": full["gpu_ms_total"], "ms_fit": full["gpu_ms_fit"],
+                      "ms_score": full["gpu_ms_score"], "ms_reestimate": full["gpu_ms_reestimate"],
+                      "ms_final": full["gpu_ms_final"], "num_inliers": full["num_inliers"],
+                      "what": "cb_ransac_plane, target n + 1 (no early exit), re-estimation on; device time per phase"},
+        "e2e": {"value": recipe["iterations"] / recipe_s, "unit": "hypotheses/s",
+                "what": f"the reference example's recipe (thresh 0.01, target 15 %, 250 iterations, re-estimation): "
+                        f"{recipe['iterations']} iterations, {recipe['num_inliers']} inliers, {1e3 * recipe_s:.2f} ms host "
+                        f"wall clock, {recipe['gpu_ms_total']:.2f} ms device"},
+        "gpu_launches": int(launches),
+        "roofline": {"bound": "fp32 issue", "achieved": instr / (ms * 1e-3), "peak": issue_peak, "unit": "thread-instr/s",
+                     "frac": instr / (ms * 1e-3) / issue_peak, "traffic": None, "kernel": "plane_score_kernel",
+                     "peak_source": f"{sms} SMs x 4 warp-instructions x 32 lanes per clock at {gpu['max_sm_clock_mhz']:.0f} MHz",
+                     "note": f"{PLANE_INSTR_PER_POINT_HYP:.2f} instructions per point-hypothesis counted in the SASS; "
+                             "wall-clock per call incl. 16 KB H2D + 4 KB D2H"},
+        "cpu_baseline": {"value": 1.0 / cpu_s, "unit": "hypotheses/s", "cores": 1, "kind": "port",
+                         "sample": f"serial computeResiduals + scan over all {n} points, {hyp_cpu} hypotheses "
+                                   f"({1e3 * cpu_s:.1f} ms each; {batch} would take {batch * cpu_s:.1f} s)"},
+        "parity": parity,
+    }
+
+
 def _pca_parity(g, o, sample):
     def get(d, *names):
         for nm in names:
@@ -547,4 +637,5 @@ AUX = {"downsample_10m": downsample, "downsample_1m": lambda a: downsample(a, n=
        "kmeans_50m": kmeans, "ransac_5m": ransac, "pca_50m": pca,
        "kmeans_5m": lambda a: kmeans(a, n=5_000_000, k=256), "ransac_500k": lambda a: ransac(a, n=500_000, batch=256),
        "pca_5m": lambda a: pca(a, n=5_000_000),
-       "segment_1m": segment, "segment_knn_1m": lambda a: segment(a, k=10), "meanshift_1m": meanshift}
+       "segment_1m": segment, "segment_knn_1m": lambda a: segment(a, k=10), "meanshift_1m": meanshift,
+       "ransac_plane_5m": ransac_plane}

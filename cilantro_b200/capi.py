@@ -83,6 +83,22 @@ class RansacResult(C.Structure):
     ]
 
 
+class RansacPlaneResult(C.Structure):
+    _fields_ = [
+        ("plane", C.c_float * 4),
+        ("hyp_plane", C.c_float * 4),
+        ("iterations", C.c_uint64),
+        ("best_iteration", C.c_uint64),
+        ("num_inliers", C.c_uint64),
+        ("gpu_ms_total", C.c_double),
+        ("gpu_ms_fit", C.c_double),
+        ("gpu_ms_score", C.c_double),
+        ("gpu_ms_reestimate", C.c_double),
+        ("gpu_ms_final", C.c_double),
+        ("kernel_launches", C.c_uint64),
+    ]
+
+
 class SegmentParams(C.Structure):
     _fields_ = [
         ("k", C.c_int32),
@@ -132,6 +148,7 @@ EXPORTED = [
     "cb_solve_kabsch_moments", "cb_solve_gauss_newton", "cb_solve_rotation", "cb_compose",
     "cb_kmeans_cluster", "cb_kmeans_assign", "cb_kmeans_seed_indices",
     "cb_ransac_score", "cb_ransac_residuals", "cb_ransac_rigid",
+    "cb_plane_score", "cb_plane_residuals", "cb_ransac_plane",
     "cb_mean_cov", "cb_pca", "cb_transform_points",
 ]
 
@@ -682,6 +699,46 @@ def ransac_rigid(ctx, dst: Cloud, src: Cloud, seed, max_iter=100, thresh=0.01, i
         "gpu_ms_total": float(res.gpu_ms_total),
         "kernel_launches": int(res.kernel_launches),
     }
+
+
+def plane_score(ctx, cloud: Cloud, planes, thresh):
+    """cb_plane_score: inlier counts of H planes (H x 4: n0, n1, n2, d) over the cloud."""
+    planes = np.ascontiguousarray(planes, np.float32).reshape(-1, 4)
+    counts = np.empty(planes.shape[0], np.uint32)
+    _check(lib().cb_plane_score(ctx.h, cloud.h, _p(planes), C.c_size_t(planes.shape[0]), C.c_float(thresh), _p(counts)))
+    return counts
+
+
+def plane_residuals(ctx, cloud: Cloud, plane, thresh):
+    """cb_plane_residuals: (residuals[n], ascending inlier indices)."""
+    pl = np.ascontiguousarray(plane, np.float32).reshape(4)
+    res = np.empty(cloud.n, np.float32)
+    inl = np.empty(max(cloud.n, 1), np.uint64)
+    cnt = C.c_size_t()
+    _check(lib().cb_plane_residuals(ctx.h, cloud.h, _p(pl), C.c_float(thresh), _p(res), _p(inl), C.byref(cnt)))
+    return res, inl[:cnt.value].astype(np.int64)
+
+
+def ransac_plane(ctx, cloud: Cloud, seed, max_iter=100, thresh=0.1, inlier_count_thresh=None, re_estimate=True):
+    """cb_ransac_plane (PlaneRANSACEstimator3f::estimate with the seed injected). Defaults are the reference's
+    (ransac_hyperplane_estimator.hpp:18): target n/2 + n%2, 100 iterations, threshold 0.1, re-estimation on."""
+    n = cloud.n
+    if inlier_count_thresh is None:
+        inlier_count_thresh = n // 2 + n % 2
+    res = RansacPlaneResult()
+    inl = np.empty(max(n, 1), np.uint64)
+    resid = np.empty(max(n, 1), np.float32)
+    _check(lib().cb_ransac_plane(ctx.h, cloud.h, C.c_uint32(seed), C.c_size_t(inlier_count_thresh),
+                                 C.c_size_t(max_iter), C.c_float(thresh), C.c_int(int(re_estimate)), C.byref(res),
+                                 _p(inl), _p(resid)))
+    out = {k: int(getattr(res, k)) for k in ("iterations", "best_iteration", "num_inliers", "kernel_launches")}
+    out.update({k: float(getattr(res, k)) for k in ("gpu_ms_total", "gpu_ms_fit", "gpu_ms_score", "gpu_ms_reestimate",
+                                                    "gpu_ms_final")})
+    out["plane"] = np.array(list(res.plane), np.float32)
+    out["hyp_plane"] = np.array(list(res.hyp_plane), np.float32)
+    out["inliers"] = inl[:res.num_inliers].astype(np.int64)
+    out["residuals"] = resid[:n].copy()
+    return out
 
 
 def mean_cov(ctx, pts: Cloud):

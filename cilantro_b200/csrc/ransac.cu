@@ -17,10 +17,10 @@
 #include "nn_search.cuh"
 #include "reduce.cuh"
 #include "host_solve.hpp"
+#include "ransac_sampler.hpp"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <random>
 #include <vector>
 
 using namespace cb;
@@ -280,9 +280,7 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
   if (inlier_count_thresh > n) inlier_count_thresh = n;   // :68
   const float x_max = sqrt_threshold(thresh);
 
-  std::vector<size_t> perm(n);
-  for (size_t i = 0; i < n; i++) perm[i] = i;
-  std::mt19937 rng(seed);  // :73 with the seed injected
+  RansacSampler sampler(n, seed);  // :72-73 with the seed injected
 
   float best_T[12];
   t34_identity(best_T);
@@ -305,16 +303,7 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
   while (!done && it < max_iter && rc == CB_OK) {
     const size_t nb = std::min(B, max_iter - it);
     // sample (:83-91): partial Fisher-Yates on a permutation that persists across hypotheses
-    for (size_t b = 0; b < nb; b++) {
-      size_t prev_size = n;
-      for (size_t i = 0; i < sample_size; i++) {
-        std::uniform_int_distribution<size_t> dist(0, prev_size - 1);
-        const size_t r = dist(rng);
-        h_idx[b * 3 + i] = (uint32_t)perm[r];
-        prev_size--;
-        std::swap(perm[r], perm[prev_size]);
-      }
-    }
+    for (size_t b = 0; b < nb; b++) sampler.next(sample_size, &h_idx[b * 3]);
     // estimateModel(sample) (:94, ransac_transform_estimator.hpp:72-82): Kabsch on the sample
     if (sample_size > 0) {
       cudaMemcpyAsync(d_idx, h_idx.data(), nb * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream);

@@ -209,3 +209,36 @@ def mean_shift_scene(blobs, per_blob, sigma=1.0, seed=1):
     perm = rng.permutation(blobs * per_blob)
     return {"points": np.ascontiguousarray(pts.reshape(-1, 3)[perm], np.float32), "blob": blob[perm],
             "centres": centres, "sigma": float(sigma)}
+
+
+def plane_scene(n, seed=1, noise=0.002, extent=4.0):
+    """A room corner for plane RANSAC: a floor (~45 % of the points) and a wall (~25 %), each a square of side
+    `extent` with truncated-Gaussian noise (sigma = noise, cut at 2.5 sigma) along its normal, plus ~30 % clutter
+    uniform in the room's box. The scene is rotated by a random rigid transform. Returns dict(points (n,3) float32,
+    labels (n,) 0 floor / 1 wall / 2 clutter, planes (2,4) float64 true (n0, n1, n2, d) of floor and wall,
+    noise)."""
+    rng = np.random.default_rng(seed)
+    n_floor, n_wall = int(0.45 * n), int(0.25 * n)
+    n_clut = n - n_floor - n_wall
+
+    def slab(m):
+        z = rng.standard_normal(4 * m + 8)
+        return (z[np.abs(z) <= 2.5][:m]) * noise
+
+    floor = np.column_stack([rng.uniform(0, extent, n_floor), rng.uniform(0, extent, n_floor), slab(n_floor)])
+    wall = np.column_stack([rng.uniform(0, extent, n_wall), 0.5 * extent + slab(n_wall),
+                            rng.uniform(0.05 * extent, 0.75 * extent, n_wall)])
+    clutter = rng.uniform([0.0, 0.0, 0.05 * extent], [extent, extent, 0.75 * extent], (n_clut, 3))
+    pts = np.concatenate([floor, wall, clutter])
+    labels = np.concatenate([np.zeros(n_floor, np.int64), np.ones(n_wall, np.int64), np.full(n_clut, 2, np.int64)])
+    T = np.asarray(rigid_from_axis_angle(rng.standard_normal(3), rng.uniform(0.2, 1.0), rng.uniform(-2, 2, 3)),
+                   np.float64)
+    R, t = T[:, :3], T[:, 3]
+    pts = pts @ R.T + t
+    planes = []
+    for nrm, off in (((0.0, 0.0, 1.0), 0.0), ((0.0, 1.0, 0.0), -0.5 * extent)):
+        nn = R @ np.array(nrm)
+        planes.append(np.append(nn, off - nn @ t))
+    perm = rng.permutation(n)
+    return {"points": np.ascontiguousarray(pts[perm], np.float32), "labels": labels[perm], "planes": np.array(planes),
+            "noise": float(noise)}

@@ -15,8 +15,8 @@
 //   PrincipalComponentAnalysis3f                            core/principal_component_analysis.hpp:8-89
 //   NormalEstimation3f                                      core/normal_estimation.hpp:11-421
 //   Points[Normals][Colors]GridDownsampler3f                core/grid_downsampler.hpp:8-340
-//   PointCloud3f (points / normals / colors, size, hasNormals, transform, gridDownsample[d],
-//                 estimateNormals{KNN,Radius,KNNInRadius})  utilities/point_cloud.hpp:14-22,246-420,557
+//   PointCloud3f (points / normals / colors, size, hasNormals, transform, gridDownsample[d], index subsets, remove,
+//                 estimateNormals{KNN,Radius,KNNInRadius})  utilities/point_cloud.hpp:14-81,154-199,246-420,557
 //   Timer                                                   utilities/timer.hpp
 // Eigen3 is an external dependency of cilantro that is absent from the build image, so the containers
 // below are minimal Eigen-free stand-ins with the memory layout cilantro uses (column-major 3 x N,
@@ -36,6 +36,7 @@
 #include <limits>
 #include <memory>
 #include <random>
+#include <set>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -1138,6 +1139,59 @@ struct PointCloud3f {
   PointCloud3f() = default;
   // PLY passthrough (utilities/point_cloud.hpp:118-121, :502-543; b200_ply.hpp)
   explicit PointCloud3f(const std::string& file_name) { fromPLYFile(file_name); }
+  // the points listed in `indices` (negate: every other point), sorted and without duplicates, with their normals
+  // and colours (utilities/point_cloud.hpp:32-81). The reference leaves the points uninitialised when the cloud has
+  // neither normals nor colours; they are copied here in every case.
+  template <typename IndexT>
+  PointCloud3f(const PointCloud3f& cloud, const std::vector<IndexT>& indices, bool negate = false) {
+    std::set<IndexT> keep;
+    if (negate) {
+      const std::set<IndexT> drop(indices.begin(), indices.end());
+      for (size_t i = 0; i < cloud.size(); i++)
+        if (!drop.count(static_cast<IndexT>(i))) keep.insert(static_cast<IndexT>(i));
+    } else {
+      keep.insert(indices.begin(), indices.end());
+    }
+    const bool has_n = cloud.hasNormals(), has_c = cloud.hasColors();
+    points.resize(3, keep.size());
+    if (has_n) normals.resize(3, keep.size());
+    if (has_c) colors.resize(3, keep.size());
+    size_t k = 0;
+    for (IndexT i : keep) {
+      points.setCol(k, cloud.points.col((size_t)i));
+      if (has_n) normals.setCol(k, cloud.normals.col((size_t)i));
+      if (has_c) colors.setCol(k, cloud.colors.col((size_t)i));
+      k++;
+    }
+  }
+  // remove(indices) (utilities/point_cloud.hpp:154-199): each removed point takes the place of the last kept one, so
+  // the order of the survivors is the reference's, not the original order
+  template <typename IndexT>
+  PointCloud3f& remove(const std::vector<IndexT>& indices) {
+    if (indices.empty()) return *this;
+    const std::set<IndexT> drop(indices.begin(), indices.end());
+    if (drop.size() >= size()) return clear();
+    size_t valid = size() - 1;
+    while (drop.count(static_cast<IndexT>(valid))) valid--;
+    const bool has_n = hasNormals(), has_c = hasColors();
+    auto swap_cols = [](VectorSet3f& m, size_t a, size_t b) {
+      const Vector3f t = m.col(a);
+      m.setCol(a, m.col(b));
+      m.setCol(b, t);
+    };
+    for (auto it = drop.begin(); it != drop.end() && (size_t)*it < valid; ++it) {
+      swap_cols(points, (size_t)*it, valid);
+      if (has_n) swap_cols(normals, (size_t)*it, valid);
+      if (has_c) swap_cols(colors, (size_t)*it, valid);
+      valid--;
+      while ((size_t)*it < valid && drop.count(static_cast<IndexT>(valid))) valid--;
+    }
+    const size_t n0 = size(), n1 = valid + 1;
+    points.resize(3, n1);
+    if (normals.cols() == n0) normals.resize(3, n1);
+    if (colors.cols() == n0) colors.resize(3, n1);
+    return *this;
+  }
   PointCloud3f& fromPLYFile(const std::string& file_name, bool /*preload*/ = true) {
     std::vector<float> p, n, c;
     b200::ply::read(file_name, p, n, c);

@@ -411,6 +411,45 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
                     size_t inlier_count_thresh, size_t max_iter, float thresh, int re_estimate,
                     cb_ransac_result* res, uint64_t* inliers, float* residuals);
 
+/* ---- plane RANSAC -----------------------------------------------------------------------------
+ * Planes are float32[4] (n0, n1, n2, d): the coefficients of Eigen::Hyperplane<float, 3>. The residual of point p is
+ * HyperplaneRANSACEstimator::computeResiduals' absDistance (model_estimation/ransac_hyperplane_estimator.hpp:47-55),
+ * r = |((n0 x) + ((n1 y) + (n2 z))) + d| in fp32, and p is an inlier iff r <= thresh (ransac_base.hpp:96-101): NaN
+ * residuals never are, and a negative or NaN threshold admits nothing. Single GPU: a cloud with index_offset != 0
+ * gives CB_ERR_UNSUPPORTED.
+ * cb_plane_score: the inlier counts of H planes (planes4 = H x 4 floats) over the cloud, one pass per batch of
+ * planes; replaces computeResiduals + the scan for each hypothesis. */
+int cb_plane_score(cb_context* ctx, const cb_cloud* cloud, const float* planes4, size_t H, float thresh,
+                   uint32_t* counts);
+/* computeResiduals(plane) (:47-55) into residuals[n] and the inlier scan (ransac_base.hpp:96-101): inliers ascending,
+ * *num_inliers of them. residuals and inliers may be NULL. */
+int cb_plane_residuals(cb_context* ctx, const cb_cloud* cloud, const float* plane4, float thresh, float* residuals,
+                       uint64_t* inliers, size_t* num_inliers);
+typedef struct cb_ransac_plane_result {
+  float plane[4];            /* the model: re-estimated when re_estimate != 0, else the kept hypothesis */
+  float hyp_plane[4];        /* the kept hypothesis before re-estimation (NaN when none was kept) */
+  uint64_t iterations;       /* getNumberOfPerformedIterations() */
+  uint64_t best_iteration;   /* 0-based iteration of the kept hypothesis */
+  uint64_t num_inliers;
+  double gpu_ms_total;       /* device time of the call */
+  double gpu_ms_fit;         /* ... of which the hypothesis fits */
+  double gpu_ms_score;       /* ... the scoring of the hypotheses */
+  double gpu_ms_reestimate;  /* ... the masked moments of the re-estimation */
+  double gpu_ms_final;       /* ... the final residuals and the inlier compaction */
+  uint64_t kernel_launches;
+} cb_ransac_plane_result;
+/* RandomSampleConsensusBase::estimate() (ransac_base.hpp:64-131) with HyperplaneRANSACEstimator<float, 3>
+ * (PlaneRANSACEstimator3f), sample size 3, the seed injected in place of std::random_device (:73); DESIGN §4.12.
+ * Samples are drawn on the host in the reference's order, fitted on the device by the closed form of the 3-point
+ * plane, scored in batches of growing size, and scanned in order, so that the kept hypothesis, the early exit (:114)
+ * and the iteration count are those of the sequential loop. Re-estimation (:118-128): PCA of the kept hypothesis's
+ * inliers, moments summed in double on the device. No hypothesis with sample_size inliers: NaN plane, 0 inliers.
+ * inliers (n entries) and residuals (n) may be NULL. A context with a communicator of more than one rank:
+ * CB_ERR_UNSUPPORTED. */
+int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_t inlier_count_thresh,
+                    size_t max_iter, float thresh, int re_estimate, cb_ransac_plane_result* res, uint64_t* inliers,
+                    float* residuals);
+
 /* ---- covariance / PCA ------------------------------------------------------------------------
  * Replaces Covariance<float,3>::operator() (core/covariance.hpp:31-80) and
  * PrincipalComponentAnalysis<float,3> (core/principal_component_analysis.hpp:76-84).

@@ -76,6 +76,15 @@ def main():
     c_rd, c_rs = capi.Cloud(ctx, rd), capi.Cloud(ctx, rs)
     capi.ransac_rigid(ctx, c_rd, c_rs, seed=5, max_iter=64, thresh=0.01)
     capi.pca(ctx, capi.Cloud(ctx, pts))
+    # plane RANSAC: early exit with re-estimation, a full run of growing batches, tiny clouds, a NaN row
+    ps = synth.plane_scene(N, seed=3)["points"]
+    ps[7] = np.nan
+    pc = capi.Cloud(ctx, ps)
+    capi.ransac_plane(ctx, pc, 1, max_iter=250, thresh=0.01, inlier_count_thresh=N // 7)
+    capi.ransac_plane(ctx, pc, 2, max_iter=300, thresh=0.01, inlier_count_thresh=N + 1, re_estimate=False)
+    capi.plane_score(ctx, pc, np.tile([0.0, 0.0, 1.0, 0.0], (1100, 1)), 0.01)
+    for m in (0, 1, 2, 3):
+        capi.ransac_plane(ctx, capi.Cloud(ctx, ps[:m]), 4, max_iter=5)
     ctx.close()
     print("sanitize target: all checks passed")
 
