@@ -42,7 +42,7 @@ def _env():
 
 
 def build(force=False, verbose=False, defines=(), out=None):
-    """defines/out: build an experimental variant (e.g. defines=["CB_ICP_MIN_BLOCKS=3"], out="x.so")."""
+    """defines/out: build an experimental variant (e.g. defines=["CB_SEGMENT_COUNTERS=1"], out="libcilantro_b200_counters.so")."""
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     target = LIB if out is None else os.path.join(HERE, out)
     flags = NVCC_FLAGS + [f"-D{d}" for d in defines] + (["-Xptxas", "-v"] if verbose else [])

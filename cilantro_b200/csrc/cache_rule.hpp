@@ -1,5 +1,5 @@
 // The exclusion-cache rule of the device-resident ICP loop (icp_loop.cu), as ONE function that compiles for the device
-// (the two cached-pass kernels call it) and for the host (tests/cpp/test_cache_rule.cpp drives it against a brute-force
+// (the cached-pass kernel calls it) and for the host (tests/cpp/test_cache_rule.cpp drives it against a brute-force
 // search with the tightest exclusion radius there is: the computed distance of the second-nearest point).
 //
 // The claim it implements. A search under transform T_k returned for source point s the nearest reference point m and a

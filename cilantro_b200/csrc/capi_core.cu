@@ -687,9 +687,8 @@ static int icp_fill_args(cb_icp* icp, const cb_icp_params* prm, const float* T, 
   // The per-query result is only written when something will read it back (inner Gauss-Newton
   // iterations >= 2, cb_icp_accumulate); cb_icp_correspondences re-runs the search otherwise.
   // The match positions are always kept: they seed the next iteration's search (warm start, warp_search.cuh).
-  static const bool no_warm = getenv("CB_NO_WARM_START") != nullptr;  // A/B switch for measurements
-  a->warm_pos = (icp->warm_ok && !no_warm) ? icp->d_nn_pos : nullptr;
-  a->nn_pos = (store || !no_warm) ? icp->d_nn_pos : nullptr;
+  a->warm_pos = icp->warm_ok ? icp->d_nn_pos : nullptr;
+  a->nn_pos = icp->d_nn_pos;
   a->nn_d2 = store ? icp->d_nn_d2 : nullptr;
   std::memcpy(icp->T_search, T, sizeof(icp->T_search));
   icp->max_d2_search = prm->max_d2;
@@ -846,11 +845,10 @@ int cb_icp_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res) {
   int hand_over = 0;
   {
     // Default correspondence engine, one Gauss-Newton step per iteration (the reference's defaults): the
-    // device-resident loop (icp_loop.cu). CB_HOST_LOOP=1 keeps the host-driven loop below for A/B measurements;
-    // engine modes, inner Gauss-Newton iterations and multi-rank runs without the fused exchange always use it.
-    static const bool host_loop = getenv("CB_HOST_LOOP") != nullptr;
+    // device-resident loop (icp_loop.cu). prm->host_loop keeps the host-driven loop below; engine modes, inner
+    // Gauss-Newton iterations and multi-rank runs without the fused exchange always use it.
     const bool one_step = prm->metric == CB_ICP_POINT_TO_POINT || prm->max_opt_iter == 1;
-    if (!host_loop && !prm->host_loop && !engine_mode(prm) && one_step && (ctx->world == 1 || exchange_available(ctx))) {
+    if (!prm->host_loop && !engine_mode(prm) && one_step && (ctx->world == 1 || exchange_available(ctx))) {
       const int rc = icp_loop_estimate(icp, prm, res, &hand_over);
       if (rc != CB_OK || !hand_over) return rc;
       // the run is not converging: continue from the device loop's state with the host-driven loop below

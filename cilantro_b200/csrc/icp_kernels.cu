@@ -30,12 +30,10 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes) 
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
 
-#ifndef CB_ICP_MIN_BLOCKS
-#define CB_ICP_MIN_BLOCKS 5
-#endif
+constexpr int kIcpMinBlocks = 5;  // resident blocks per SM the pass kernel's register budget is set for
 
 template <int MODE, bool SEARCH>
-__global__ void __launch_bounds__(kBlock, CB_ICP_MIN_BLOCKS) icp_pass_kernel(const IcpArgs a, const bool has_pt, const bool has_pl) {
+__global__ void __launch_bounds__(kBlock, kIcpMinBlocks) icp_pass_kernel(const IcpArgs a, const bool has_pt, const bool has_pl) {
   constexpr int NV = (MODE == kModeP2P || MODE == kModeP2PCentered) ? kP2PValues : (MODE == kModeCombined ? kCombinedValues : 1);
   double acc[NV];
 #pragma unroll
@@ -200,14 +198,7 @@ int launch_icp_pass(cb_context* ctx, const IcpArgs& a, int mode, bool search, bo
   CB_TRY(get_reduce_scratch(ctx, blocks, kMaxValues, &args.rs));
   // reduction passes carry the fused NVLink all-reduce + host mailbox epilogue when the context has it
   ctx->pass_armed = (mode != kModeKnn) && arm_exchange(ctx, &args.rs.ex);
-  {
-    // ~2 waves of resident blocks; CB_PREFETCH_BLOCKS overrides it for experiments
-    static const int env_pf = [] {
-      const char* e = getenv("CB_PREFETCH_BLOCKS");
-      return e ? atoi(e) : -1;
-    }();
-    args.prefetch_blocks = env_pf >= 0 ? (uint32_t)env_pf : (uint32_t)(2 * ctx->sm_count * CB_ICP_MIN_BLOCKS);
-  }
+  args.prefetch_blocks = (uint32_t)(2 * ctx->sm_count * kIcpMinBlocks);  // ~2 waves of resident blocks
   if (mode == kModeKnn) {
     icp_pass_kernel<kModeKnn, true><<<blocks, kBlock, 0, ctx->stream>>>(args, false, false);
   } else if (mode == kModeP2P) {

@@ -48,14 +48,8 @@ constexpr int kBlock = kReduceBlock;
 // large ones (a tile without flagged queries still costs its block a few microseconds of latency, so fewer, larger
 // tiles). Either variant is correct for any number of flagged queries. Small tiles pay off in the first warm iteration
 // only (later ones search mostly empty tiles already); the two sizes are timing choices (bench.py, DESIGN §4.2).
-#ifndef CB_LOOP_QPT_DENSE
-#define CB_LOOP_QPT_DENSE 4
-#endif
-#ifndef CB_LOOP_QPT
-#define CB_LOOP_QPT 32
-#endif
-constexpr int kQptDense = CB_LOOP_QPT_DENSE;
-constexpr int kQptWarm = CB_LOOP_QPT;
+constexpr int kQptDense = 4;
+constexpr int kQptWarm = 32;
 constexpr int kDenseIters = 1;
 
 struct LoopArgs {
@@ -238,112 +232,19 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
   cx.wc_pl = a.wc_pl;
 }
 
-#ifndef CB_WARM_QPT
-#define CB_WARM_QPT 4
-#endif
-#ifndef CB_WARM_MIN_BLOCKS
-#define CB_WARM_MIN_BLOCKS 2
-#endif
-constexpr int kWarmQpt = CB_WARM_QPT;           // queries per thread and tile of the cached pass
-constexpr int kWarmTile = kWarmQpt * kBlock;    // queries per tile of the cached pass
-
 // ---- kernel 1 of a warm iteration: the cached pass ------------------------------------------------------------------
-// Elementwise over the source cloud, no search code, no shared-memory staging: per query 16 B (point) + 8 B (cache)
-// streamed and one 16 B gather of the cached match (+ 16 B normal for the plane term). Queries that pass the
-// exclusion test accumulate their pair here; the others are flagged in a bit mask (one word per 32 consecutive
-// queries) for the search kernel. PERSISTENT: the grid is a whole number of resident blocks per SM, a block walks
-// the tiles blockIdx.x, + gridDim.x, ... (static round-robin: every tile costs the same, and the assignment —
-// hence the summation order — is fixed), the next tile's streamed loads are in flight while the current tile is
-// evaluated, and the moments are reduced ONCE per block (a per-tile reduction cost as much as the tile itself).
-// The block rows go through the same deterministic grid reduction into rs.result + 32.
-template <int MODE>
-__global__ void __launch_bounds__(kBlock, CB_WARM_MIN_BLOCKS) icp_cached_kernel(const __grid_constant__ LoopArgs a) {
-  constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
-  __shared__ BlockCtx cx;
-  __shared__ AsyncReduceSmem<NV> rsm;
-  const unsigned int tid = threadIdx.x, lane = tid & 31u;
-  const uint32_t ntiles = (a.n_src + kWarmTile - 1) / kWarmTile;
-  // everything that does not depend on the loop state is requested before the state arrives
-  float4 s[kWarmQpt];
-  float r[kWarmQpt];
-  int seed[kWarmQpt];
-  auto stream_loads = [&](uint32_t tile) {
-#pragma unroll
-    for (int k = 0; k < kWarmQpt; k++) {
-      const uint32_t i = tile * kWarmTile + k * kBlock + tid;
-      const bool active = tile < ntiles && i < a.n_src;
-      s[k] = active ? __ldg(a.src_pts + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-      r[k] = active ? __ldcg(a.cache_r + i) : 0.f;
-      seed[k] = active ? __ldcg(a.cache_pos + i) : -1;
-    }
-  };
-  stream_loads(blockIdx.x);
-  if (tid == 0) {
-    rsm.arrived = 0u;
-    load_block_ctx(a, cx);
-  }
-  __syncthreads();
-  if (cx.done) return;
-  if (a.trace && blockIdx.x == 0 && tid == 0) {
-    const int slot = __ldcg(&a.st->iters) & 63;
-    a.st->trace[slot][0] = global_timer_ns();
-    a.st->trace[slot][4] = 0ull;
-  }
-  double acc[NV];
-#pragma unroll
-  for (int v = 0; v < NV; v++) acc[v] = 0.0;
-#pragma unroll 1
-  for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const uint32_t base = tile * kWarmTile;
-    float4 p[kWarmQpt], pn[kWarmQpt], sc[kWarmQpt];
-    float rc[kWarmQpt];
-    int sd[kWarmQpt];
-    const bool want_nrm = (MODE == kModeCombined) && a.has_pl != 0;
-#pragma unroll
-    for (int k = 0; k < kWarmQpt; k++) {
-      sc[k] = s[k];
-      rc[k] = r[k];
-      sd[k] = seed[k];
-      const bool g = sd[k] >= 0 && rc[k] > 0.f;
-      p[k] = g ? __ldg(a.dst.pts + sd[k]) : make_float4(0.f, 0.f, 0.f, 0.f);
-      // the plane term's normal rides along with the match (inside accumulate_pair it would be a second dependent
-      // round trip per pair)
-      pn[k] = (g && want_nrm) ? __ldg(a.dst.nrm + sd[k]) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    stream_loads(tile + gridDim.x);  // next tile of this block: in flight during the evaluation below
-#pragma unroll
-    for (int k = 0; k < kWarmQpt; k++) {
-      const uint32_t i = base + k * kBlock + tid;
-      const bool active = i < a.n_src;
-      bool miss = active;
-      if (active && rc[k] > 0.f) {
-        // the exclusion test (cache_rule.hpp): hit -> the cached match is this iteration's exact search result
-        rule::Verdict v;
-        float4 pm = p[k];
-        rule::cached_match_test(cx.T, cx.Tp, sc[k].x, sc[k].y, sc[k].z, rc[k], sd[k], a.max_d2, [&] { return p[k]; }, pm, v);
-        miss = v.miss;
-        if (!miss) a.cache_r[i] = v.r2;
-        if (v.pair) {
-          const float4 nk = pn[k];
-          accumulate_pair<MODE, true>(
-              acc, cx, a.has_pt != 0, a.has_pl != 0, pm, v.qx, v.qy, v.qz, a.src_nrm != nullptr, [&] { return nk; },
-              [&] { return __ldg(a.src_nrm + i); }, v.d2);
-        }
-      }
-      const unsigned int mm = __ballot_sync(0xffffffffu, miss);
-      if (lane == 0 && (base + k * kBlock + (tid & ~31u)) < a.n_src) a.miss_mask[(base + k * kBlock + tid) >> 5] = mm;
-    }
-  }
-  double tot = 0;
-  if (!grid_reduce_async_tail<NV>(acc, a.rs, rsm, tot)) return;
-  if (lane < NV) a.rs.result[32 + lane] = tot;
-}
-
-// ---- the cached pass, asynchronous-copy pipeline (the shipped version) ---------------------------------------------------
-// Same arithmetic, same tile walk, same flags and sums as icp_cached_kernel above; what changes is how the data gets
-// to the thread. The register version needs 128 registers -> 2 blocks/SM, few warp slots occupied, long-scoreboard
-// stalls on top - each thread can only keep the loads in flight that it has registers for. Here every thread runs a private three-deep pipeline of
-// cp.async copies into shared memory (LDGSTS: no destination register, no scoreboard slot):
+// Elementwise over the source cloud, no search code: per query 16 B (point) + 8 B (cache) streamed and one 16 B
+// gather of the cached match (+ 16 B normal for the plane term). Queries that pass the exclusion test accumulate
+// their pair here; the others are flagged in a bit mask (one word per 32 consecutive queries) for the search kernel.
+// PERSISTENT: the grid is a whole number of resident blocks per SM, a block walks the tiles blockIdx.x, + gridDim.x,
+// ... (static round-robin: every tile costs the same, and the assignment — hence the summation order — is fixed),
+// the next tiles' loads are in flight while the current tile is evaluated, and the moments are reduced ONCE per
+// block (a per-tile reduction cost as much as the tile itself). The block rows go through the same deterministic grid
+// reduction into rs.result + 32.
+// The loads are not staged in registers: a register-staged version needed 128 registers -> 2 blocks/SM, few warp
+// slots occupied, long-scoreboard stalls on top - each thread can only keep the loads in flight that it has registers
+// for. Here every thread runs a private three-deep pipeline of cp.async copies into shared memory (LDGSTS: no
+// destination register, no scoreboard slot):
 //   stage A (tile k+2)  the streamed arrays: its queries' point (16 B), exclusion radius (4 B), cached match (4 B)
 //   stage B (tile k+1)  the gathers, once A has landed: the matched destination point (+ normal for the plane term)
 //   stage C (tile k)    evaluation from shared memory
@@ -498,9 +399,7 @@ __global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_c
   if (lane < NV) a.rs.result[32 + lane] = tot;
 }
 
-#ifndef CB_LOOP_MIN_BLOCKS
-#define CB_LOOP_MIN_BLOCKS 4
-#endif
+constexpr int kSearchMinBlocks = 4;  // resident blocks per SM the search kernel's register budget is set for
 
 // ---- kernel 2 of an iteration (the only one of a cold iteration): search + finish ------------------------------------------
 // kCold: nothing is cached, every query of the tile is searched (one 256-query chunk per block). Otherwise the
@@ -508,7 +407,7 @@ __global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_c
 // ascending order, and dense warps search them. The searching thread accumulates its pair; the last warp of the
 // grid adds the cached pass's totals, all-reduces with the peers, solves, and writes the next transform.
 template <int MODE, int kQpt, bool kCold>
-__global__ void __launch_bounds__(kBlock, CB_LOOP_MIN_BLOCKS) icp_search_kernel(const __grid_constant__ LoopArgs a) {
+__global__ void __launch_bounds__(kBlock, kSearchMinBlocks) icp_search_kernel(const __grid_constant__ LoopArgs a) {
   static_assert(!kCold || kQpt == 1, "a cold iteration searches one chunk per block");
   constexpr int kTile = kQpt * kBlock;  // queries per block
   constexpr int kWords = kTile / 32;    // mask words per tile
@@ -668,10 +567,20 @@ __global__ void __launch_bounds__(32, 1) icp_finish_kernel(const __grid_constant
 
 }  // namespace
 
-// launch with programmatic stream serialization (see pdl_wait above); CB_NO_PDL=1 falls back to plain launches
+// widening of a search beyond the nearest distance, in cell edges of the destination grid: first iteration
+// (no motion known yet), floor and cap of 2 x (the query's last motion)
+constexpr float kSlackFirst = 0.20f, kSlackMin = 0.02f, kSlackMax = 0.30f;
+constexpr int kBatch = 16;  // iterations per batch after the first one (the host reads LoopState once per batch)
+// The first batch is short: by its end a converging run searches a fraction of a percent of its queries per
+// iteration; a run that still searches more than kGiveUpShare of them is handed over to the host-driven loop
+// (the exclusion cache costs more than it saves there).
+constexpr int kFirstBatch = 4;
+constexpr int kBridgeBatch = 2;  // enqueued behind the first batch: covers the host's look at the first batch's state
+constexpr double kGiveUpShare = 0.15;
+
+// launch with programmatic stream serialization (see pdl_wait above)
 template <class Kernel>
 static cudaError_t launch_pdl(Kernel k, int blocks, int threads, size_t smem, cudaStream_t stream, const LoopArgs& a) {
-  static const bool no_pdl = getenv("CB_NO_PDL") != nullptr;
   cudaLaunchConfig_t cfg;
   std::memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)blocks);
@@ -680,10 +589,32 @@ static cudaError_t launch_pdl(Kernel k, int blocks, int threads, size_t smem, cu
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = no_pdl ? 0 : 1;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, k, a);
+}
+
+// Enqueues the kernels of ICP iteration `it` of this call: the search kernel alone in the cold first iteration (nothing
+// cached yet), else the cached pass and the search kernel over its flagged queries; then the finish kernel.
+template <int MODE>
+static int enqueue_iteration(cb_context* ctx, const LoopArgs& a, int it, int blocks_cold, int blocks_cached,
+                             int blocks_dense, int blocks_search) {
+  const bool cold = (it == 0);
+  if (cold) {
+    CB_CUDA(launch_pdl(icp_search_kernel<MODE, 1, true>, blocks_cold, kBlock, 0, ctx->stream, a));
+  } else {
+    CB_CUDA(launch_pdl(icp_cached_pipe_kernel<MODE>, blocks_cached, kBlock, sizeof(PipeSmem<MODE == kModeCombined>),
+                       ctx->stream, a));
+    if (it <= kDenseIters)
+      CB_CUDA(launch_pdl(icp_search_kernel<MODE, kQptDense, false>, blocks_dense, kBlock, 0, ctx->stream, a));
+    else
+      CB_CUDA(launch_pdl(icp_search_kernel<MODE, kQptWarm, false>, blocks_search, kBlock, 0, ctx->stream, a));
+  }
+  CB_CUDA(launch_pdl(icp_finish_kernel<MODE>, 1, 32, 0, ctx->stream, a));
+  ctx->launches += cold ? 1 : 2;
+  ctx->launches += 1;
+  return CB_OK;
 }
 
 int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res, int* hand_over) {
@@ -726,45 +657,31 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   a.bail = (prm->w_pl > 0.f) && !dst_has_normals;
   a.cache_pos = icp->d_nn_pos;
   a.cache_r = icp->d_nn_d2;
-  {
-    // widening of a search beyond the nearest distance, in cell edges of the destination grid: first iteration
-    // (no motion known yet), floor and cap of 2 x (the query's last motion). CB_LOOP_SLACK="first,min,max".
-    float f[3] = {0.20f, 0.02f, 0.30f};
-    if (const char* e = getenv("CB_LOOP_SLACK")) sscanf(e, "%f,%f,%f", &f[0], &f[1], &f[2]);
-    const float h = 1.0f / a.dst.inv_h;
-    a.slack_first = f[0] * h;
-    a.slack_min = f[1] * h;
-    a.slack_max = f[2] * h;
-  }
+  const float h = 1.0f / a.dst.inv_h;  // cell edge of the destination grid
+  a.slack_first = kSlackFirst * h;
+  a.slack_min = kSlackMin * h;
+  a.slack_max = kSlackMax * h;
   a.st = icp->d_state;
   static const bool trace = getenv("CB_LOOP_TRACE") != nullptr;
   a.trace = trace ? 1 : 0;
   // cold iteration (first launch: nothing cached): search kernel alone, one 256-query chunk per block; warm
-  // iterations: cached pass (kWarmTile queries per block) + search kernel over the flagged queries
+  // iterations: cached pass (kPipeTile queries per tile) + search kernel over the flagged queries
   const int blocks_cold = std::max(1, (int)((ns + kBlock - 1) / kBlock));
   const int blocks_search = std::max(1, (int)((ns + (size_t)kQptWarm * kBlock - 1) / ((size_t)kQptWarm * kBlock)));
   const int blocks_dense = std::max(1, (int)((ns + (size_t)kQptDense * kBlock - 1) / ((size_t)kQptDense * kBlock)));
-  // persistent cached pass: a whole number of resident blocks per SM (never more blocks than tiles).
-  // CB_CACHED_REGS=1 selects the register-staged version (icp_cached_kernel) for A/B measurements.
-  static const bool cached_regs = getenv("CB_CACHED_REGS") != nullptr;
-  const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
-  const size_t pipe_smem = p2p ? sizeof(PipeSmem<false>) : sizeof(PipeSmem<true>);
-  int blocks_cached;
-  if (cached_regs) {
-    blocks_cached = std::max(1, std::min(ctx->sm_count * CB_WARM_MIN_BLOCKS, (int)((ns + kWarmTile - 1) / kWarmTile)));
-  } else {
-    // once per device (function attributes belong to the device the context is on, not to the process)
-    static bool attr_set_dev[64] = {};
-    bool& attr_set = attr_set_dev[ctx->device & 63];
-    if (!attr_set) {
-      CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeP2PCentered>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)sizeof(PipeSmem<false>)));
-      CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeCombined>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)sizeof(PipeSmem<true>)));
-      attr_set = true;
-    }
-    blocks_cached = std::max(1, std::min(ctx->sm_count * (p2p ? 4 : 3), (int)((ns + kPipeTile - 1) / kPipeTile)));
+  // once per device (function attributes belong to the device the context is on, not to the process)
+  static bool attr_set_dev[64] = {};
+  bool& attr_set = attr_set_dev[ctx->device & 63];
+  if (!attr_set) {
+    CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeP2PCentered>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)sizeof(PipeSmem<false>)));
+    CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeCombined>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)sizeof(PipeSmem<true>)));
+    attr_set = true;
   }
+  // persistent cached pass: a whole number of resident blocks per SM (never more blocks than tiles)
+  const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
+  const int blocks_cached = std::max(1, std::min(ctx->sm_count * (p2p ? 4 : 3), (int)((ns + kPipeTile - 1) / kPipeTile)));
   CB_TRY(get_reduce_scratch(ctx, blocks_cold, kMaxValues, &a.rs));
   if (!icp->d_miss_mask) CB_CUDA(cudaMalloc(&icp->d_miss_mask, (ns / 32 + 2) * sizeof(uint32_t)));
   a.miss_mask = icp->d_miss_mask;
@@ -788,17 +705,6 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   CB_CUDA(cudaMemcpyAsync(icp->d_state, hs, sizeof(*hs), cudaMemcpyHostToDevice, ctx->stream));
 
   int issued = 0;
-  static const int kBatch = [] {
-    const char* e = getenv("CB_LOOP_BATCH");
-    return e ? std::max(1, atoi(e)) : 16;
-  }();
-  // The first batch is short: by its end a converging run searches a fraction of a percent of its queries per
-  // iteration; a run that still searches more than kGiveUpShare of them is handed over to the host-driven loop
-  // (the exclusion cache costs more than it saves there). CB_LOOP_NO_HANDOVER=1 keeps the device loop regardless.
-  static const bool no_handover = getenv("CB_LOOP_NO_HANDOVER") != nullptr;
-  constexpr int kFirstBatch = 4;
-  constexpr int kBridgeBatch = 2;  // enqueued behind the first batch: covers the host's look at the first batch's state
-  constexpr double kGiveUpShare = 0.15;
   // Batches are enqueued ONE AHEAD of the batch whose state the host is looking at: the device never waits for the host
   // between batches (with several ranks such a gap shows up as a peer wait in the next iteration), and the
   // hand-over / convergence decisions lag by at most one batch. Two pinned copies of LoopState alternate.
@@ -811,40 +717,10 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
     for (int k = 0; k < n; ++k) {
       if (prm->flush_l2) CB_TRY(cb_context_flush_l2(ctx));
       if (timing) CB_CUDA(cudaEventRecord(icp->events[2 * (issued + k)], ctx->stream));
-      const bool cold = (issued + k == 0);
-      if (prm->metric == CB_ICP_POINT_TO_POINT) {
-        if (cold) {
-          CB_CUDA(launch_pdl(icp_search_kernel<kModeP2PCentered, 1, true>, blocks_cold, kBlock, 0, ctx->stream, a));
-        } else {
-          if (cached_regs)
-            icp_cached_kernel<kModeP2PCentered><<<blocks_cached, kBlock, 0, ctx->stream>>>(a);
-          else
-            CB_CUDA(launch_pdl(icp_cached_pipe_kernel<kModeP2PCentered>, blocks_cached, kBlock, pipe_smem, ctx->stream, a));
-          if (issued + k <= kDenseIters)
-            CB_CUDA(launch_pdl(icp_search_kernel<kModeP2PCentered, kQptDense, false>, blocks_dense, kBlock, 0, ctx->stream, a));
-          else
-            CB_CUDA(launch_pdl(icp_search_kernel<kModeP2PCentered, kQptWarm, false>, blocks_search, kBlock, 0, ctx->stream, a));
-        }
-      } else {
-        if (cold) {
-          CB_CUDA(launch_pdl(icp_search_kernel<kModeCombined, 1, true>, blocks_cold, kBlock, 0, ctx->stream, a));
-        } else {
-          if (cached_regs)
-            icp_cached_kernel<kModeCombined><<<blocks_cached, kBlock, 0, ctx->stream>>>(a);
-          else
-            CB_CUDA(launch_pdl(icp_cached_pipe_kernel<kModeCombined>, blocks_cached, kBlock, pipe_smem, ctx->stream, a));
-          if (issued + k <= kDenseIters)
-            CB_CUDA(launch_pdl(icp_search_kernel<kModeCombined, kQptDense, false>, blocks_dense, kBlock, 0, ctx->stream, a));
-          else
-            CB_CUDA(launch_pdl(icp_search_kernel<kModeCombined, kQptWarm, false>, blocks_search, kBlock, 0, ctx->stream, a));
-        }
-      }
-      if (prm->metric == CB_ICP_POINT_TO_POINT)
-        CB_CUDA(launch_pdl(icp_finish_kernel<kModeP2PCentered>, 1, 32, 0, ctx->stream, a));
+      if (p2p)
+        CB_TRY(enqueue_iteration<kModeP2PCentered>(ctx, a, issued + k, blocks_cold, blocks_cached, blocks_dense, blocks_search));
       else
-        CB_CUDA(launch_pdl(icp_finish_kernel<kModeCombined>, 1, 32, 0, ctx->stream, a));
-      ctx->launches += cold ? 1 : 2;
-      ctx->launches += 1;
+        CB_TRY(enqueue_iteration<kModeCombined>(ctx, a, issued + k, blocks_cold, blocks_cached, blocks_dense, blocks_search));
       if (timing) CB_CUDA(cudaEventRecord(icp->events[2 * (issued + k) + 1], ctx->stream));
     }
     CB_CUDA(cudaGetLastError());
@@ -866,7 +742,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
     ++checked;
     if (hs->done != 0 || issued >= max_iter) {
       stop = true;  // converged / failed (launches already enqueued return at once) or everything is enqueued
-    } else if (!no_handover && hs->iters >= kFirstBatch && hs->searched_all > kGiveUpShare * hs->queries_all) {
+    } else if (hs->iters >= kFirstBatch && hs->searched_all > kGiveUpShare * hs->queries_all) {
       stop = true;  // not converging: no further batch; the one already in flight (if any) still completes
       give_up = true;
     }

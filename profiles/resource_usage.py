@@ -6,7 +6,7 @@ import subprocess
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "cilantro_b200", "libcilantro_b200.so")
-HOT = ("icp_search_kernel", "icp_cached_pipe_kernel", "icp_cached_kernel", "icp_finish_kernel", "icp_pass_kernel",
+HOT = ("icp_search_kernel", "icp_cached_pipe_kernel", "icp_finish_kernel", "icp_pass_kernel",
        "pairs_pass_kernel", "kmeans_assign_kernel", "ransac_score_kernel", "inlier_moments_kernel", "moments_kernel",
        "normals_knn_kernel", "normals_radius_kernel", "knn_k_kernel", "radius_kernel", "residual_kernel",
        "segment_kernel", "shift_kernel", "round_kernel", "rep_kernel", "plane_score_kernel", "plane_fit_kernel",

@@ -1,5 +1,5 @@
 // Host-side property test of the exclusion-cache rule the device-resident ICP loop runs (cilantro_b200/csrc/cache_rule.hpp
-// is the SAME source the two cached-pass kernels compile; here it is compiled for the host, directed rounding through
+// is the SAME source the cached-pass kernel compiles; here it is compiled for the host, directed rounding through
 // <cfenv>). A brute-force search with the contract arithmetic plays the search kernel and hands the rule the TIGHTEST
 // valid exclusion radius (the computed distance of the second-nearest point); over a converging sequence of transforms
 // every verdict of the rule is compared with a fresh brute-force search:

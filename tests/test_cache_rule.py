@@ -1,5 +1,5 @@
 """The exclusion-cache rule of the device-resident ICP loop, on the host. cilantro_b200/csrc/cache_rule.hpp is the one
-source of the rule: the two cached-pass kernels of icp_loop.cu compile it for the device, tests/cpp/test_cache_rule.cpp
+source of the rule: the cached-pass kernel of icp_loop.cu compiles it for the device, tests/cpp/test_cache_rule.cpp
 compiles it for the host (directed rounding through <cfenv>) and checks every verdict against a brute-force search with
 the contract arithmetic — tightest valid exclusion radius, converging transform sequences, lattice inputs with exact ties,
 and an inflated radius that must be caught. No GPU involved; the device side of the same claim is
@@ -24,12 +24,14 @@ def test_cache_rule_against_brute_force_on_the_host(tmp_path):
     assert "all cache-rule checks passed" in out.stdout and "FAIL" not in out.stdout
 
 
-def test_the_kernels_compile_the_same_rule():
-    """Both cached-pass kernels call rule::cached_match_test, searches store rule::cache_radius, and icp_loop.cu keeps no
-    private copy of the bound arithmetic (the directed-rounding intrinsics of the test live in cache_rule.hpp only)."""
+def test_the_cached_pass_kernel_compiles_the_same_rule():
+    """The one cached-pass kernel calls rule::cached_match_test, searches store rule::cache_radius, and icp_loop.cu keeps
+    no private copy of the bound arithmetic (the directed-rounding intrinsics of the test live in cache_rule.hpp only)."""
     with open(os.path.join(CSRC, "icp_loop.cu")) as f:
         src = re.sub(r"//[^\n]*", "", f.read())
-    assert len(re.findall(r"rule::cached_match_test\(", src)) == 2
+    cached_kernels = re.findall(r"__global__\s+void\s+__launch_bounds__\(.*?\)\s*(\w*cached\w*)\(", src)
+    assert cached_kernels == ["icp_cached_pipe_kernel"]
+    assert len(re.findall(r"rule::cached_match_test\(", src)) == 1
     assert len(re.findall(r"rule::cache_radius\(", src)) >= 1
     assert "__fsub_rd" not in src and "__fmul_rd" not in src and "kDown17" not in src
     with open(os.path.join(CSRC, "cache_rule.hpp")) as f:
