@@ -31,43 +31,49 @@ struct BinGrid {
   float inv;                // 1 / bin_size (fp32, like bin_size_.cwiseInverse())
   long long mnx, mny, mnz;  // minimum bin coordinate per axis
   uint64_t ny, nz;
-  uint64_t mx, my, mz;  // last valid relative coordinate per axis (clamp for non-finite input)
+  uint64_t none;            // key of a point with a non-finite coordinate: one past the largest bin key
 };
 
 inline int blocks_for(const cb_context* ctx, size_t n) {
   return (int)std::max<size_t>(1, std::min<size_t>((n + kThreads - 1) / kThreads, (size_t)ctx->sm_count * 16));
 }
 
-__device__ __forceinline__ uint64_t rel_bin(float v, float inv, long long mn, uint64_t last) {
-  // (ptrdiff_t)std::floor(point[i] * bin_size_inv_[i]); NaN / Inf are undefined in the reference and are
-  // clamped into the grid here
-  const long long b = __float2ll_rd(__fmul_rn(v, inv));
-  if (b <= mn) return 0;
-  const uint64_t r = (uint64_t)(b - mn);
-  return r > last ? last : r;
+// (ptrdiff_t)std::floor(point[i] * bin_size_inv_[i]) relative to the cloud's minimum bin. The bounding box
+// covers every finite coordinate, so a finite point's bin lies inside the grid.
+__device__ __forceinline__ uint64_t rel_bin(float v, float inv, long long mn) {
+  return (uint64_t)(__float2ll_rd(__fmul_rn(v, inv)) - mn);
 }
 
+// A point with a NaN / Inf coordinate belongs to no bin (its bin is undefined in the reference): it gets the
+// key g.none, sorts after every finite point and is left out of the bins.
 __global__ void bin_key_kernel(const float* __restrict__ raw, size_t n, BinGrid g, uint64_t* __restrict__ keys,
                                uint32_t* __restrict__ vals) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const uint64_t ix = rel_bin(raw[3 * i], g.inv, g.mnx, g.mx);
-    const uint64_t iy = rel_bin(raw[3 * i + 1], g.inv, g.mny, g.my);
-    const uint64_t iz = rel_bin(raw[3 * i + 2], g.inv, g.mnz, g.mz);
-    keys[i] = (ix * g.ny + iy) * g.nz + iz;
+    const float x = raw[3 * i], y = raw[3 * i + 1], z = raw[3 * i + 2];
+    uint64_t key = g.none;
+    if (isfinite(x) && isfinite(y) && isfinite(z)) {
+      const uint64_t ix = rel_bin(x, g.inv, g.mnx), iy = rel_bin(y, g.inv, g.mny), iz = rel_bin(z, g.inv, g.mnz);
+      key = (ix * g.ny + iy) * g.nz + iz;
+    }
+    keys[i] = key;
     vals[i] = (uint32_t)i;
   }
 }
 
-__global__ void head_flag_kernel(const uint64_t* __restrict__ keys, size_t n, uint32_t* __restrict__ flags) {
+__global__ void head_flag_kernel(const uint64_t* __restrict__ keys, size_t n, uint64_t none,
+                                 uint32_t* __restrict__ flags) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i <= n; i += (size_t)gridDim.x * blockDim.x)
-    flags[i] = (i < n && (i == 0 || keys[i] != keys[i - 1])) ? 1u : 0u;
+    flags[i] = (i < n && keys[i] != none && (i == 0 || keys[i] != keys[i - 1])) ? 1u : 0u;
 }
 
-// after the exclusive scan, flags[i] = number of bin heads before i; heads write their position
-__global__ void bin_start_kernel(const uint64_t* __restrict__ keys, size_t n, const uint32_t* __restrict__ scanned,
-                                 uint32_t* __restrict__ bin_start) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+// after the exclusive scan, flags[i] = number of bin heads before i and flags[n] = nbins; heads write their
+// position, and bin_start[nbins] = the end of the finite points (the first non-finite one, or n)
+__global__ void bin_start_kernel(const uint64_t* __restrict__ keys, size_t n, uint64_t none,
+                                 const uint32_t* __restrict__ scanned, uint32_t* __restrict__ bin_start) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     if (i == 0 || keys[i] != keys[i - 1]) bin_start[scanned[i]] = (uint32_t)i;
+    if (i == n - 1 && keys[i] != none) bin_start[scanned[n]] = (uint32_t)n;
+  }
 }
 
 struct BinOut {
@@ -79,10 +85,10 @@ struct BinOut {
 };
 
 __global__ void bin_reduce_kernel(const float* __restrict__ raw, const float* __restrict__ raw_nrm,
-                                  const float* __restrict__ raw_col, const uint32_t* __restrict__ order, size_t n,
+                                  const float* __restrict__ raw_col, const uint32_t* __restrict__ order,
                                   const uint32_t* __restrict__ bin_start, uint32_t nbins, BinOut o) {
   for (uint32_t b = blockIdx.x * blockDim.x + threadIdx.x; b < nbins; b += gridDim.x * blockDim.x) {
-    const uint32_t s = bin_start[b], e = (b + 1 < nbins) ? bin_start[b + 1] : (uint32_t)n;
+    const uint32_t s = bin_start[b], e = bin_start[b + 1];
     uint32_t i = order[s];
     float px = raw[3 * (size_t)i], py = raw[3 * (size_t)i + 1], pz = raw[3 * (size_t)i + 2];  // buildAccumulator
     float nx = 0.f, ny = 0.f, nz = 0.f, cr = 0.f, cg = 0.f, cb_ = 0.f;
@@ -205,8 +211,8 @@ int downsample_device(cb_context* ctx, const float* d_raw, const float* d_nrm, c
   CB_CHECK(total < 9.0e18L, CB_ERR_UNSUPPORTED, "bin grid too large for a 64-bit key (bin_size too small for the extent)");
   g.mnx = lo[0]; g.mny = lo[1]; g.mnz = lo[2];
   g.ny = dim[1]; g.nz = dim[2];
-  g.mx = dim[0] - 1; g.my = dim[1] - 1; g.mz = dim[2] - 1;
-  const int key_bits = bits_for(dim[0] * dim[1] * dim[2]);
+  g.none = dim[0] * dim[1] * dim[2];
+  const int key_bits = bits_for(g.none + 1);
 
   DeviceBufs bufs(ctx);
   uint64_t *d_keys, *d_keys2;
@@ -220,15 +226,16 @@ int downsample_device(cb_context* ctx, const float* d_raw, const float* d_nrm, c
   bin_key_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_raw, n, g, d_keys, d_vals);
   ctx->launches += 1;
   CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_vals, d_keys2, d_vals2, n, key_bits));
-  head_flag_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_keys, n, d_flags);
+  head_flag_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_keys, n, g.none, d_flags);
   ctx->launches += 1;
   CB_TRY(exclusive_scan_u32(ctx, d_flags, n + 1, 0u));  // flags[n] = number of bins; flags[n + 1] = sentinel
   uint32_t nbins = 0;
   CB_CUDA(cudaMemcpyAsync(&nbins, d_flags + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
-  CB_CHECK(nbins >= 1 && nbins <= n, CB_ERR_CUDA, "internal: inconsistent bin count");
-  CB_TRY(bufs.alloc(&d_start, nbins));
-  bin_start_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_keys, n, d_flags, d_start);
+  CB_CHECK(nbins <= n, CB_ERR_CUDA, "internal: inconsistent bin count");
+  if (nbins == 0) return CB_OK;  // no point with three finite coordinates
+  CB_TRY(bufs.alloc(&d_start, (size_t)nbins + 1));
+  bin_start_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_keys, n, g.none, d_flags, d_start);
   BinOut o;
   o.nrm = nullptr;
   o.col = nullptr;
@@ -238,7 +245,7 @@ int downsample_device(cb_context* ctx, const float* d_raw, const float* d_nrm, c
   CB_TRY(bufs.alloc(&o.cnt, nbins));
   CB_TRY(bufs.alloc(&o.first, nbins));
   const int bb = blocks_for(ctx, nbins);
-  bin_reduce_kernel<<<bb, kThreads, 0, ctx->stream>>>(d_raw, d_nrm, d_col, d_vals, n, d_start, nbins, o);
+  bin_reduce_kernel<<<bb, kThreads, 0, ctx->stream>>>(d_raw, d_nrm, d_col, d_vals, d_start, nbins, o);
   ctx->launches += 2;
   CB_CUDA(cudaGetLastError());
   // output order

@@ -9,6 +9,9 @@
 // each thread keeps kPts points in registers so one LDS.128 feeds kPts distance evaluations.
 // Per-cluster sums are accumulated in double with shared-memory atomics (one block-private copy),
 // then flushed with global double atomics; counts likewise.
+// A point with a NaN / Inf coordinate never satisfies d < best, so it keeps label 0; it adds nothing
+// to any sum or count and the empty-cluster repair never picks it (the reference leaves its label
+// uninitialised and sums it, so one such point would turn centroid 0 into NaN for good).
 #include "cb_internal.hpp"
 #include "host_solve.hpp"
 #include <algorithm>
@@ -80,6 +83,7 @@ __global__ void __launch_bounds__(kBlock) kmeans_assign_kernel(const float* __re
       if (i < n) {
         if (labels[i] != (uint32_t)bi[u]) any_changed = 1;
         labels[i] = (uint32_t)bi[u];
+        if (!(isfinite(px[u]) && isfinite(py[u]) && isfinite(pz[u]))) continue;
         double* s = (kSmemSums ? s_sums : sums) + (size_t)bi[u] * 4;
         atomicAdd(s + 0, (double)px[u]);
         atomicAdd(s + 1, (double)py[u]);
@@ -100,13 +104,16 @@ __global__ void __launch_bounds__(kBlock) kmeans_assign_kernel(const float* __re
 
 // farthest member of cluster `target` from point c (kmeans.hpp:151-169): packs (dist bits, ~index)
 // so that atomicMax picks the largest distance and, on ties, the LOWEST index (the serial order).
+// Members with a non-finite coordinate are skipped (they are in no sum).
 __global__ void farthest_member_kernel(const float* __restrict__ raw, size_t n, const uint32_t* __restrict__ labels,
                                        uint32_t target, float cx, float cy, float cz,
                                        unsigned long long* __restrict__ out) {
   unsigned long long best = 0;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     if (labels[i] != target) continue;
-    const float dx = __fsub_rn(cx, raw[3 * i]), dy = __fsub_rn(cy, raw[3 * i + 1]), dz = __fsub_rn(cz, raw[3 * i + 2]);
+    const float x = raw[3 * i], y = raw[3 * i + 1], z = raw[3 * i + 2];
+    if (!(isfinite(x) && isfinite(y) && isfinite(z))) continue;
+    const float dx = __fsub_rn(cx, x), dy = __fsub_rn(cy, y), dz = __fsub_rn(cz, z);
     const float d = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
     const unsigned long long key =
         ((unsigned long long)__float_as_uint(d) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)i);
