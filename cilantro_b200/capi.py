@@ -132,6 +132,54 @@ class MeanShiftParams(C.Structure):
 FLT_EPSILON = float(np.finfo(np.float32).eps)
 
 
+class WarpParams(C.Structure):
+    _fields_ = [
+        ("w_pt", C.c_float),
+        ("w_pl", C.c_float),
+        ("stiffness", C.c_float),
+        ("huber", C.c_float),
+        ("gn_tol", C.c_float),
+        ("cg_tol", C.c_float),
+        ("tol", C.c_float),
+        ("max_d2", C.c_float),
+        ("reg_coeff", C.c_float),
+        ("max_iter", C.c_int32),
+        ("max_gn_iter", C.c_uint64),
+        ("max_cg_iter", C.c_uint64),
+        ("search_dir", C.c_int32),
+        ("require_reciprocal", C.c_int32),
+        ("one_to_one", C.c_int32),
+        ("reserved_", C.c_int32),
+        ("inlier_fraction", C.c_double),
+    ]
+
+
+class WarpResult(C.Structure):
+    _fields_ = [
+        ("iterations", C.c_int32),
+        ("converged", C.c_int32),
+        ("last_delta", C.c_float),
+        ("reserved_", C.c_int32),
+        ("num_corr", C.c_uint64),
+        ("gn_steps", C.c_uint64),
+        ("cg_iterations", C.c_uint64),
+        ("gpu_ms_search", C.c_double),
+        ("gpu_ms_solve", C.c_double),
+        ("kernel_launches", C.c_uint64),
+    ]
+
+
+class WarpSolveResult(C.Structure):
+    _fields_ = [
+        ("converged", C.c_int32),
+        ("cg_error", C.c_float),
+        ("gn_steps", C.c_uint64),
+        ("cg_iterations", C.c_uint64),
+        ("cg_iterations_last", C.c_uint64),
+        ("kernel_launches", C.c_uint64),
+    ]
+
+
 # every symbol include/cilantro_b200.h declares (tests/test_capi_host.py checks that the .so exports them and that this list matches the header)
 EXPORTED = [
     "cb_last_error", "cb_version",
@@ -149,6 +197,8 @@ EXPORTED = [
     "cb_kmeans_cluster", "cb_kmeans_assign", "cb_kmeans_seed_indices",
     "cb_ransac_score", "cb_ransac_residuals", "cb_ransac_rigid",
     "cb_plane_score", "cb_plane_residuals", "cb_ransac_plane",
+    "cb_warp_default_params", "cb_warp_icp_create", "cb_warp_icp_destroy", "cb_warp_icp_estimate", "cb_warp_icp_solve",
+    "cb_warp_icp_residuals", "cb_warp_icp_correspondences",
     "cb_mean_cov", "cb_pca", "cb_transform_points",
 ]
 
@@ -739,6 +789,110 @@ def ransac_plane(ctx, cloud: Cloud, seed, max_iter=100, thresh=0.1, inlier_count
     out["inliers"] = inl[:res.num_inliers].astype(np.int64)
     out["residuals"] = resid[:n].copy()
     return out
+
+
+def warp_params(w_pt=0.0, w_pl=1.0, stiffness=1.0, huber=1e-4, max_gn_iter=10, gn_tol=1e-5, max_cg_iter=1000,
+                cg_tol=1e-5, max_iter=15, tol=1e-5, max_d2=1e-4, reg_sigma=1.0, search_dir="second_to_first",
+                inlier_fraction=1.0, require_reciprocal=False, one_to_one=False):
+    """cb_warp_params; the defaults are CombinedMetricDenseWarpFieldICP's (max_d2 = 0.01^2)."""
+    p = WarpParams()
+    lib().cb_warp_default_params(C.byref(p))
+    p.w_pt, p.w_pl, p.stiffness, p.huber = w_pt, w_pl, stiffness, huber
+    p.max_gn_iter, p.gn_tol, p.max_cg_iter, p.cg_tol = int(max_gn_iter), gn_tol, int(max_cg_iter), cg_tol
+    p.max_iter, p.tol, p.max_d2 = int(max_iter), tol, max_d2
+    p.reg_coeff = rbf_coeff(reg_sigma)
+    p.search_dir = SEARCH_DIR[search_dir] if isinstance(search_dir, str) else int(search_dir)
+    p.inlier_fraction = float(inlier_fraction)
+    p.require_reciprocal = int(require_reciprocal)
+    p.one_to_one = int(one_to_one)
+    return p
+
+
+def neighborhood_csr(idx, d2, counts=None):
+    """Neighbourhood lists as the (offsets, index, value) CSR of cb_warp_icp_create, from the [n, k] tables of
+    knn_radius (entries < 0 or past counts[i] unused). radius_search already returns that CSR."""
+    idx = np.asarray(idx)
+    keep = idx >= 0
+    if counts is not None:
+        keep &= np.arange(idx.shape[1])[None, :] < np.asarray(counts)[:, None]
+    off = np.zeros(idx.shape[0] + 1, np.uint64)
+    off[1:] = np.cumsum(keep.sum(1))
+    return off, np.ascontiguousarray(idx[keep], np.int64), np.ascontiguousarray(np.asarray(d2)[keep], np.float32)
+
+
+def _t_set(T, n):
+    if T is None:
+        return None
+    T = np.ascontiguousarray(T, np.float32).reshape(n, 12)
+    return T
+
+
+class WarpIcp:
+    """cb_warp_icp_*: SimpleCombinedMetricDenseRigidWarpFieldICP3f. Transforms are (n_src, 3, 4) float32."""
+
+    def __init__(self, ctx, dst: Cloud, src: Cloud, reg_offsets, reg_index, reg_value):
+        self.ctx, self.dst, self.src = ctx, dst, src
+        off = np.ascontiguousarray(reg_offsets, np.uint64)
+        idx = np.ascontiguousarray(reg_index, np.int64)
+        val = np.ascontiguousarray(reg_value, np.float32)
+        h = C.c_void_p()
+        _check(lib().cb_warp_icp_create(ctx.h, dst.h, src.h, _p(off), _p(idx), _p(val),
+                                        C.c_size_t(max(off.shape[0] - 1, 0)), C.byref(h)))
+        self.h = h
+        ctx._adopt(self)
+
+    def close(self):
+        if self.h:
+            lib().cb_warp_icp_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def estimate(self, T_init=None, **kw):
+        prm = kw.pop("params", None) or warp_params(**kw)
+        n = self.src.n
+        T = np.empty((max(n, 1), 12), np.float32)
+        res = WarpResult()
+        _check(lib().cb_warp_icp_estimate(self.h, C.byref(prm), _p(_t_set(T_init, n)), _p(T), C.byref(res)))
+        return {"T": T[:n].reshape(n, 3, 4), "iterations": int(res.iterations), "converged": bool(res.converged),
+                "last_delta": float(res.last_delta), "num_corr": int(res.num_corr), "gn_steps": int(res.gn_steps),
+                "cg_iterations": int(res.cg_iterations), "gpu_ms_search": float(res.gpu_ms_search),
+                "gpu_ms_solve": float(res.gpu_ms_solve), "kernel_launches": int(res.kernel_launches)}
+
+    def solve(self, first, second, T_src=None, **kw):
+        prm = kw.pop("params", None) or warp_params(**kw)
+        n = self.src.n
+        f = np.ascontiguousarray(first, np.uint64)
+        s = np.ascontiguousarray(second, np.uint64)
+        T = np.empty((max(n, 1), 12), np.float32)
+        x = np.empty((max(n, 1), 6), np.float32)
+        res = WarpSolveResult()
+        _check(lib().cb_warp_icp_solve(self.h, C.byref(prm), _p(_t_set(T_src, n)), _p(f), _p(s), None,
+                                       C.c_size_t(f.shape[0]), _p(T), _p(x), C.byref(res)))
+        return {"T": T[:n].reshape(n, 3, 4), "x": x[:n], "converged": bool(res.converged), "gn_steps": int(res.gn_steps),
+                "cg_iterations": int(res.cg_iterations), "cg_iterations_last": int(res.cg_iterations_last),
+                "cg_error": float(res.cg_error), "kernel_launches": int(res.kernel_launches)}
+
+    def residuals(self, T, **kw):
+        prm = kw.pop("params", None) or warp_params(**kw)
+        n = self.src.n
+        out = np.empty(max(n, 1), np.float32)
+        _check(lib().cb_warp_icp_residuals(self.h, C.byref(prm), _p(_t_set(T, n)), _p(out)))
+        return out[:n]
+
+    def correspondences(self):
+        n = max(self.src.n, 1)
+        i1 = np.empty(n, np.uint64)
+        i2 = np.empty(n, np.uint64)
+        v = np.empty(n, np.float32)
+        cnt = C.c_size_t()
+        _check(lib().cb_warp_icp_correspondences(self.h, _p(i1), _p(i2), _p(v), C.byref(cnt)))
+        c = cnt.value
+        return i1[:c].astype(np.int64), i2[:c].astype(np.int64), v[:c]
 
 
 def mean_cov(ctx, pts: Cloud):

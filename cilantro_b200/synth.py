@@ -242,3 +242,32 @@ def plane_scene(n, seed=1, noise=0.002, extent=4.0):
     perm = rng.permutation(n)
     return {"points": np.ascontiguousarray(pts[perm], np.float32), "labels": labels[perm], "planes": np.array(planes),
             "noise": float(noise)}
+
+
+def warp_pair(n, seed=1, spacing=0.005, bend=0.01, noise=0.0005):
+    """A non-rigid registration pair. dst: n points uniform on a smooth height field z = h(x, y) over a square of side
+    L = spacing sqrt(n) (mean spacing `spacing`), with its analytic unit normals. src: every dst point moved by a
+    smooth bend of amplitude `bend` (one period across the square in each coordinate), then by a small rigid offset
+    (1 degree about a tilted axis, translation of 0.3 `bend` per axis), plus N(0, noise^2) noise per axis, in the same
+    order as dst. Returns dict(dst, dst_normals, src (n,3) float32, spacing, side L)."""
+    rng = np.random.default_rng(seed)
+    L = spacing * np.sqrt(n)
+    k = 2.0 * np.pi / L
+    xy = rng.uniform(0.0, L, (n, 2))
+    x, y = xy[:, 0], xy[:, 1]
+    amp = 0.08 * L
+    z = amp * np.sin(0.5 * k * x) * np.cos(0.5 * k * y)
+    hx = amp * 0.5 * k * np.cos(0.5 * k * x) * np.cos(0.5 * k * y)
+    hy = -amp * 0.5 * k * np.sin(0.5 * k * x) * np.sin(0.5 * k * y)
+    dst = np.stack([x, y, z], 1)
+    nrm = np.stack([-hx, -hy, np.ones(n)], 1)
+    nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
+    disp = bend * np.stack([np.sin(k * x), np.cos(k * y), np.sin(k * (x + y))], 1)
+    ax = np.array([0.3, -0.2, 1.0]) / np.linalg.norm([0.3, -0.2, 1.0])
+    th = np.deg2rad(1.0)
+    K = np.array([[0, -ax[2], ax[1]], [ax[2], 0, -ax[0]], [-ax[1], ax[0], 0]])
+    R = np.eye(3) + np.sin(th) * K + (1 - np.cos(th)) * K @ K
+    c = dst.mean(0)
+    src = (dst + disp - c) @ R.T + c + 0.3 * bend * np.array([1.0, -1.0, 0.5]) + rng.normal(0.0, noise, (n, 3))
+    return {"dst": np.ascontiguousarray(dst, np.float32), "dst_normals": np.ascontiguousarray(nrm, np.float32),
+            "src": np.ascontiguousarray(src, np.float32), "spacing": float(spacing), "side": float(L)}

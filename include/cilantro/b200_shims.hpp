@@ -10,6 +10,8 @@
 //   KDTree3f<>                                              core/kd_tree.hpp:144-397
 //   SimplePointToPointMetricRigidICP3f                      registration/icp_common_instances.hpp:250
 //   SimpleCombinedMetricRigidICP3f                          registration/icp_common_instances.hpp:261
+//   SimpleCombinedMetricDenseRigidWarpFieldICP3f            registration/icp_common_instances.hpp:99-144,284-285
+//   TransformSet<RigidTransform3f>, transformPoints         core/space_transformations.hpp:60-136,195-223
 //   KMeans3f<>                                              clustering/kmeans.hpp:9-59,205-207
 //   RigidTransformRANSACEstimator3f<>                       model_estimation/ransac_transform_estimator.hpp:9-122
 //   PrincipalComponentAnalysis3f                            core/principal_component_analysis.hpp:8-89
@@ -390,6 +392,11 @@ public:
   auto search(const QueryT& q, const KNNInRadiusNeighborhoodSpecification<float, CountT>& nh) const {
     return kNNInRadiusSearch(q, (size_t)nh.maxNumberOfNeighbors, nh.radius);
   }
+  // the form with an output argument (core/kd_tree.hpp:320-381), as the reference's examples call it
+  template <typename SpecT>
+  void search(const ConstVectorSetMatrixMap3f& queries, const SpecT& nh, NeighborhoodSetResult& result) const {
+    result = search(queries, nh);
+  }
   const ConstVectorSetMatrixMap3f& getPointsMatrixMap() const { return data_map_; }  // core/kd_tree.hpp:172-174
   cb_cloud* b200_cloud() const { return cloud_.h; }  // the device-resident cloud (reused by ConnectedComponentExtraction3f)
 
@@ -683,6 +690,214 @@ inline void transformPoints(const RigidTransform3f& tform, const ConstVectorSetM
   b200::check(cb_transform_points(b200::Context::get(), tform.data(), points.data(), points.cols(), result.data()),
               "cb_transform_points");
 }
+
+// ---- TransformSet<RigidTransform3f> (core/space_transformations.hpp:60-136) -----------------------------------
+// One transform per point: what the warp-field ICP estimates. Only the surface its callers use.
+template <class TransformT>
+class TransformSet : public std::vector<TransformT> {
+public:
+  using std::vector<TransformT>::vector;
+  TransformSet& setIdentity() {
+    for (auto& t : *this) t.setIdentity();
+    return *this;
+  }
+};
+using RigidTransformSet3f = TransformSet<RigidTransform3f>;
+
+// transformPoints(tforms, in, out) (core/space_transformations.hpp:195-223): point i by transform i, in the device's
+// float order ((R_r0 x + (R_r1 y + R_r2 z)) + t_r, RigidTransform3f::operator*)
+inline void transformPoints(const TransformSet<RigidTransform3f>& tforms, const ConstVectorSetMatrixMap3f& points,
+                            VectorSet3f& result) {
+  if (tforms.size() != points.cols()) throw std::runtime_error("transformPoints: one transform per point expected");
+  result.resize(3, points.cols());
+  for (size_t i = 0; i < points.cols(); i++) result.setCol(i, tforms[i] * points.col(i));
+}
+
+// ---- SimpleCombinedMetricDenseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:99-144, 284-285) ----------
+// CombinedMetricDenseWarpFieldICP<RigidTransform<float,3>> (icp_warp_field_combined_metric_dense.hpp) with the Simple
+// instance's evaluators (unity data-term weights, RBFKernelWeightEvaluator<float, float, true> regularisation weights)
+// on cb_warp_icp_* (DESIGN §4.13). The correspondence engine takes the default settings only; another search
+// direction, reciprocity, one-to-one or fraction makes estimate() throw (CB_ERR_UNSUPPORTED).
+class SimpleCombinedMetricDenseRigidWarpFieldICP3f {
+public:
+  using Transform = TransformSet<RigidTransform3f>;
+  using PointToPointCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
+  using PointToPlaneCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
+  using RegularizationWeightEvaluator = RBFKernelWeightEvaluator<float, float, true>;
+
+  // regularization_neighborhoods: one list per neighbourhood, N[0] the centre (what KDTree3f<>::search returns)
+  template <typename IndexT>
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f(const ConstVectorSetMatrixMap3f& dst_p,
+                                               const ConstVectorSetMatrixMap3f& dst_n,
+                                               const ConstVectorSetMatrixMap3f& src_p,
+                                               const std::vector<NeighborSet<float, IndexT>>& regularization_neighborhoods)
+      : n_src_(src_p.cols()) {
+    const float* dn = (dst_n.cols() == dst_p.cols() && dst_p.cols() > 0) ? dst_n.data() : nullptr;
+    b200::check(cb_cloud_create_pair(b200::Context::get(), dst_p.data(), dn, dst_p.cols(), 0, src_p.data(), nullptr,
+                                     src_p.cols(), 0, &dst_.h, &src_.h),
+                "cb_cloud_create_pair");
+    std::vector<uint64_t> off(regularization_neighborhoods.size() + 1, 0);
+    std::vector<int64_t> idx;
+    std::vector<float> val;
+    for (size_t j = 0; j < regularization_neighborhoods.size(); j++) {
+      for (const auto& nb : regularization_neighborhoods[j]) {
+        idx.push_back(static_cast<int64_t>(nb.index));
+        val.push_back(nb.value);
+      }
+      off[j + 1] = idx.size();
+    }
+    b200::check(cb_warp_icp_create(b200::Context::get(), dst_.h, src_.h, off.data(), idx.data(), val.data(),
+                                   regularization_neighborhoods.size(), &icp_),
+                "cb_warp_icp_create");
+    cb_warp_default_params(&prm_);
+    std::memset(&res_, 0, sizeof(res_));
+    res_.last_delta = std::numeric_limits<float>::infinity();
+    transform_init_.assign(n_src_, RigidTransform3f());
+    transform_.assign(n_src_, RigidTransform3f());
+  }
+  ~SimpleCombinedMetricDenseRigidWarpFieldICP3f() {
+    if (icp_) cb_warp_icp_destroy(icp_);
+  }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f(const SimpleCombinedMetricDenseRigidWarpFieldICP3f&) = delete;
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& operator=(const SimpleCombinedMetricDenseRigidWarpFieldICP3f&) = delete;
+
+  CorrespondenceSearchEngineB200& correspondenceSearchEngine() { return engine_; }
+  PointToPointCorrespondenceWeightEvaluator& pointToPointCorrespondenceWeightEvaluator() { return pt_eval_; }
+  PointToPlaneCorrespondenceWeightEvaluator& pointToPlaneCorrespondenceWeightEvaluator() { return pl_eval_; }
+  RegularizationWeightEvaluator& regularizationWeightEvaluator() { return reg_eval_; }
+
+  // IterativeClosestPointBase surface (registration/icp_base.hpp:40-106)
+  size_t getMaxNumberOfIterations() const { return (size_t)prm_.max_iter; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setMaxNumberOfIterations(size_t n) {
+    prm_.max_iter = (int32_t)n;
+    return *this;
+  }
+  float getConvergenceTolerance() const { return prm_.tol; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setConvergenceTolerance(float tol) {
+    prm_.tol = tol;
+    return *this;
+  }
+  const Transform& getInitialTransform() const { return transform_init_; }
+  Transform& initialTransform() { return transform_init_; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setInitialTransform(const Transform& T) {
+    transform_init_ = T;
+    return *this;
+  }
+  size_t getNumberOfPerformedIterations() const { return (size_t)res_.iterations; }
+  float getLastUpdateNorm() const { return res_.last_delta; }
+  bool hasConverged() const { return res_.last_delta < prm_.tol; }  // icp_base.hpp:106
+  const Transform& getTransform() const { return transform_; }
+
+  // CombinedMetricDenseWarpFieldICP surface
+  float getPointToPointMetricWeight() const { return prm_.w_pt; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setPointToPointMetricWeight(float w) {
+    prm_.w_pt = w;
+    return *this;
+  }
+  float getPointToPlaneMetricWeight() const { return prm_.w_pl; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setPointToPlaneMetricWeight(float w) {
+    prm_.w_pl = w;
+    return *this;
+  }
+  float getStiffnessRegularizationWeight() const { return prm_.stiffness; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setStiffnessRegularizationWeight(float w) {
+    prm_.stiffness = w;
+    return *this;
+  }
+  size_t getMaxNumberOfGaussNewtonIterations() const { return (size_t)prm_.max_gn_iter; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setMaxNumberOfGaussNewtonIterations(size_t n) {
+    prm_.max_gn_iter = n;
+    return *this;
+  }
+  float getGaussNewtonConvergenceTolerance() const { return prm_.gn_tol; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setGaussNewtonConvergenceTolerance(float tol) {
+    prm_.gn_tol = tol;
+    return *this;
+  }
+  size_t getMaxNumberOfConjugateGradientIterations() const { return (size_t)prm_.max_cg_iter; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setMaxNumberOfConjugateGradientIterations(size_t n) {
+    prm_.max_cg_iter = n;
+    return *this;
+  }
+  float getConjugateGradientConvergenceTolerance() const { return prm_.cg_tol; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setConjugateGradientConvergenceTolerance(float tol) {
+    prm_.cg_tol = tol;
+    return *this;
+  }
+  float getHuberLossBoundary() const { return prm_.huber; }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setHuberLossBoundary(float huber_boundary) {
+    prm_.huber = huber_boundary;
+    return *this;
+  }
+
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& estimate() {
+    if (transform_init_.size() != n_src_) throw std::runtime_error("initial transform: one transform per source point expected");
+    fill();
+    std::vector<float> T_in(12 * n_src_), T_out(12 * n_src_);
+    for (size_t i = 0; i < n_src_; i++) std::memcpy(&T_in[12 * i], transform_init_[i].data(), 12 * sizeof(float));
+    b200::check(cb_warp_icp_estimate(icp_, &prm_, T_in.data(), T_out.data(), &res_), "cb_warp_icp_estimate");
+    transform_.resize(n_src_);
+    for (size_t i = 0; i < n_src_; i++) transform_[i] = RigidTransform3f(&T_out[12 * i]);
+    corr_fresh_ = false;
+    return *this;
+  }
+  SimpleCombinedMetricDenseRigidWarpFieldICP3f& estimate(size_t max_iter, float conv_tol) {
+    prm_.max_iter = (int32_t)max_iter;
+    prm_.tol = conv_tol;
+    return estimate();
+  }
+
+  // getResiduals() -> computeResiduals() (icp_warp_field_combined_metric_dense.hpp:216-236): 1 x N_src
+  std::vector<float> getResiduals() {
+    fill();
+    std::vector<float> T(12 * n_src_), r(n_src_);
+    for (size_t i = 0; i < n_src_ && i < transform_.size(); i++) std::memcpy(&T[12 * i], transform_[i].data(), 12 * sizeof(float));
+    b200::check(cb_warp_icp_residuals(icp_, &prm_, T.data(), r.data()), "cb_warp_icp_residuals");
+    return r;
+  }
+
+  // correspondenceSearchEngine().getCorrespondences() after estimate(): the last iteration's list
+  const CorrespondenceSet<float, size_t>& getCorrespondences() {
+    if (!corr_fresh_) {
+      std::vector<uint64_t> a(n_src_), b(n_src_);
+      std::vector<float> v(n_src_);
+      size_t cnt = 0;
+      b200::check(cb_warp_icp_correspondences(icp_, a.data(), b.data(), v.data(), &cnt), "cb_warp_icp_correspondences");
+      corr_.resize(cnt);
+      for (size_t i = 0; i < cnt; i++) corr_[i] = {(size_t)a[i], (size_t)b[i], v[i]};
+      corr_fresh_ = true;
+    }
+    return corr_;
+  }
+
+  uint64_t getNumberOfConjugateGradientIterations() const { return res_.cg_iterations; }  // over the last estimate()
+  double getLastEstimateDeviceMilliseconds() const { return res_.gpu_ms_search + res_.gpu_ms_solve; }
+
+private:
+  void fill() {
+    cb_icp_params e;
+    cb_icp_default_params(&e);
+    engine_.fill(e);
+    prm_.max_d2 = e.max_d2;
+    prm_.search_dir = e.search_dir;
+    prm_.inlier_fraction = e.inlier_fraction;
+    prm_.require_reciprocal = e.require_reciprocal;
+    prm_.one_to_one = e.one_to_one;
+    prm_.reg_coeff = reg_eval_.b200_coeff();
+  }
+  size_t n_src_;
+  b200::CloudHandle dst_, src_;
+  cb_warp_icp* icp_ = nullptr;
+  cb_warp_params prm_;
+  cb_warp_result res_;
+  Transform transform_init_, transform_;
+  CorrespondenceSearchEngineB200 engine_;
+  PointToPointCorrespondenceWeightEvaluator pt_eval_;
+  PointToPlaneCorrespondenceWeightEvaluator pl_eval_;
+  RegularizationWeightEvaluator reg_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
+  CorrespondenceSet<float, size_t> corr_;
+  bool corr_fresh_ = false;
+};
 
 // ---- KMeans3f<> -------------------------------------------------------------------------------------
 template <typename PointIndexT = size_t, typename ClusterIndexT = size_t>
@@ -1289,6 +1504,24 @@ struct PointCloud3f {
   bool hasNormals() const { return size() > 0 && normals.cols() == size(); }
   bool hasColors() const { return size() > 0 && colors.cols() == size(); }
   bool isEmpty() const { return size() == 0; }
+  // per-point transforms (a warp field): points by transformPoints(tforms, ...), normals by the linear parts
+  PointCloud3f& transform(const TransformSet<RigidTransform3f>& tforms) {
+    VectorSet3f out;
+    transformPoints(tforms, points, out);
+    points = out;
+    if (hasNormals()) {
+      TransformSet<RigidTransform3f> R = tforms;
+      for (auto& t : R)
+        for (int r = 0; r < 3; r++) t.translation(r) = 0.f;
+      transformPoints(R, normals, out);
+      normals = out;
+    }
+    return *this;
+  }
+  PointCloud3f transformed(const TransformSet<RigidTransform3f>& tforms) const {
+    PointCloud3f res = *this;
+    return res.transform(tforms);
+  }
   PointCloud3f& transform(const RigidTransform3f& T) {  // utilities/point_cloud.hpp (rigid overload)
     VectorSet3f out;
     transformPoints(T, points, out);

@@ -450,6 +450,96 @@ int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_
                     size_t max_iter, float thresh, int re_estimate, cb_ransac_plane_result* res, uint64_t* inliers,
                     float* residuals);
 
+/* ---- non-rigid ICP: dense rigid warp field ------------------------------------------------------
+ * cb_warp_icp_* replaces SimpleCombinedMetricDenseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:99-144,
+ * 284-285) = CombinedMetricDenseWarpFieldICP (registration/icp_warp_field_combined_metric_dense.hpp) on the loop of
+ * IterativeClosestPointBase::estimate (icp_base.hpp:68-87); DESIGN §4.13. Every source point i carries its own rigid
+ * transform T_i (float32[12] per point, row-major [R | t]). One ICP iteration: the 1-NN of T_i s_i in the destination
+ * within max_d2 (the grid search of cb_find_correspondences), then estimateDenseWarpFieldCombinedMetric
+ * (warp_field_estimation.hpp:368-715): per point 6 unknowns (Euler a, b, c and a translation) linearised about zero,
+ * point-to-point (3 rows, weight sqrt(w_pt)) and point-to-plane (1 row, sqrt(w_pl)) data terms, and per regularisation
+ * arc 6 Huber-loss rows of weight sqrt(stiffness) sqrt(exp(reg_coeff d2)); Gauss-Newton steps solved by a Jacobi-
+ * preconditioned conjugate gradient with zero initial guess; then T_i <- rotation(dT_i T_i) (TransformSet::preApply)
+ * and last_delta = sqrt(max_i |dR_i - I|_F^2 + |dt_i|^2). The loop stops when last_delta < tol or at max_iter.
+ * Regularisation neighbourhoods: a host CSR in the layout cb_radius_search returns (n_reg lists; list j is entries
+ * offsets[j] .. offsets[j+1]-1 of index / value). Each list N gives the arcs (N[0], N[j]) for j >= 1 with value
+ * N[j].value; an empty list gives none (the reference's size() - 1 underflows there), and a self-arc (N[0] == N[j])
+ * gives none (its two Jacobian entries cancel). Rejected: a neighbour index outside [0, n_src) (CB_ERR_INVALID),
+ * w_pl > 0 on a destination without normals (CB_ERR_INVALID; the reference returns identities and later reads the
+ * missing normals), any non-default correspondence-engine option, a cloud with index_offset != 0, a context with
+ * more than one rank, and clouds of 2^31 - 1 points or more (CB_ERR_UNSUPPORTED; point indices travel as signed
+ * 32-bit values through the search). A non-finite source point gets no
+ * correspondence. With no data term (both weights <= 0, or no correspondence) every T_i of the iteration is the
+ * identity and the estimator reports false (:398-408). */
+typedef struct cb_warp_params {
+  float w_pt;            /* point_to_point_weight_, default 0 */
+  float w_pl;            /* point_to_plane_weight_, default 1 */
+  float stiffness;       /* stiffness_weight_, default 1 */
+  float huber;           /* huber_boundary_, default 1e-4 */
+  float gn_tol;          /* gauss_newton_convergence_tol_, default 1e-5 */
+  float cg_tol;          /* conjugate_gradient_convergence_tol_, default 1e-5 */
+  float tol;             /* icp_base.hpp:25, default 1e-5 */
+  float max_d2;          /* SQUARED; correspondence_search_kd_tree.hpp:49, default 0.01*0.01 */
+  float reg_coeff;       /* RBFKernelWeightEvaluator<float, float, true>: -0.5f / (sigma * sigma); default sigma 1 */
+  int32_t max_iter;      /* icp_base.hpp:24, default 15 */
+  uint64_t max_gn_iter;  /* default 10 */
+  uint64_t max_cg_iter;  /* default 1000 */
+  /* correspondence-engine options as in cb_icp_params; only the defaults are supported here */
+  int32_t search_dir;
+  int32_t require_reciprocal;
+  int32_t one_to_one;
+  int32_t reserved_;
+  double inlier_fraction;
+} cb_warp_params;
+
+typedef struct cb_warp_result {
+  int32_t iterations;       /* getNumberOfPerformedIterations() */
+  int32_t converged;        /* hasConverged(): last_delta < tol */
+  float last_delta;
+  int32_t reserved_;
+  uint64_t num_corr;        /* correspondences of the last iteration */
+  uint64_t gn_steps;        /* Gauss-Newton steps over all iterations */
+  uint64_t cg_iterations;   /* conjugate-gradient iterations over all steps */
+  double gpu_ms_search;     /* CUDA-event time of the correspondence searches */
+  double gpu_ms_solve;      /* ... of the assembly, CG and compose kernels */
+  uint64_t kernel_launches;
+} cb_warp_result;
+
+typedef struct cb_warp_solve_result {
+  int32_t converged;        /* the estimator's return value */
+  float cg_error;           /* sqrt(|r|^2 / |b|^2) after the last step's CG (0 when |b| = 0) */
+  uint64_t gn_steps;
+  uint64_t cg_iterations;   /* over all steps */
+  uint64_t cg_iterations_last;
+  uint64_t kernel_launches;
+} cb_warp_solve_result;
+
+typedef struct cb_warp_icp cb_warp_icp;
+
+void cb_warp_default_params(cb_warp_params* p);
+/* dst (with normals for w_pl > 0) and src must outlive the object. The neighbourhoods are validated, uploaded once and
+ * turned into a per-point arc incidence on the device (stable radix sort by point). */
+int cb_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const uint64_t* reg_offsets,
+                       const int64_t* reg_index, const float* reg_value, size_t n_reg, cb_warp_icp** out);
+void cb_warp_icp_destroy(cb_warp_icp* icp);
+/* estimate() followed by getTransform(): T_init (n_src x 12, NULL = identities) -> T_out (n_src x 12). */
+int cb_warp_icp_estimate(cb_warp_icp* icp, const cb_warp_params* prm, const float* T_init, float* T_out,
+                         cb_warp_result* res);
+/* estimateDenseWarpFieldCombinedMetric on the source transformed by T_src (n_src x 12, NULL = identities) with the
+ * caller's correspondences (dst index corr_first[c], src index corr_second[c]; corr_value may be NULL: the Simple
+ * instance weighs data terms with UnityWeightEvaluator). T_out (n_src x 12) = the estimated per-point transforms;
+ * x_out (n_src x 6, may be NULL) = the estimator's unknowns (a, b, c, tx, ty, tz) per point, from which T_out is
+ * built (with one Gauss-Newton step: the CG solution of the normal equations). An index out of range: CB_ERR_INVALID. */
+int cb_warp_icp_solve(cb_warp_icp* icp, const cb_warp_params* prm, const float* T_src, const uint64_t* corr_first,
+                      const uint64_t* corr_second, const float* corr_value, size_t n_corr, float* T_out, float* x_out,
+                      cb_warp_solve_result* res);
+/* computeResiduals() (icp_warp_field_combined_metric_dense.hpp:216-236) for the per-point transforms T (n_src x 12):
+ * unbounded 1-NN of T_i s_i, out[i] = w_pt |d - p|^2 + w_pl (n_d . (d - p))^2; NaN when dst is empty. */
+int cb_warp_icp_residuals(cb_warp_icp* icp, const cb_warp_params* prm, const float* T, float* out);
+/* getCorrespondences() after the last iteration of the last estimate(), ascending source index; arrays hold n_src. */
+int cb_warp_icp_correspondences(cb_warp_icp* icp, uint64_t* index_first, uint64_t* index_second, float* value,
+                                size_t* count);
+
 /* ---- covariance / PCA ------------------------------------------------------------------------
  * Replaces Covariance<float,3>::operator() (core/covariance.hpp:31-80) and
  * PrincipalComponentAnalysis<float,3> (core/principal_component_analysis.hpp:76-84).

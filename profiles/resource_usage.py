@@ -10,7 +10,7 @@ HOT = ("icp_search_kernel", "icp_cached_pipe_kernel", "icp_finish_kernel", "icp_
        "pairs_pass_kernel", "kmeans_assign_kernel", "ransac_score_kernel", "inlier_moments_kernel", "moments_kernel",
        "normals_knn_kernel", "normals_radius_kernel", "knn_k_kernel", "radius_kernel", "residual_kernel",
        "segment_kernel", "shift_kernel", "round_kernel", "rep_kernel", "plane_score_kernel", "plane_fit_kernel",
-       "plane_moments_kernel", "inlier_scatter_kernel")
+       "plane_moments_kernel", "inlier_scatter_kernel", "warp_assemble_kernel", "warp_cg_kernel", "warp_compose_kernel")
 
 
 def main():

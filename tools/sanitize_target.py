@@ -85,6 +85,19 @@ def main():
     capi.plane_score(ctx, pc, np.tile([0.0, 0.0, 1.0, 0.0], (1100, 1)), 0.01)
     for m in (0, 1, 2, 3):
         capi.ransac_plane(ctx, capi.Cloud(ctx, ps[:m]), 4, max_iter=5)
+    # dense warp-field ICP: assembly, the cooperative CG and compose over a few iterations, a solve with a fixed list,
+    # residuals, and a NaN source point
+    wp = synth.warp_pair(2000, seed=4)
+    wp["src"][11] = np.nan
+    wsrc = capi.Cloud(ctx, wp["src"])
+    widx, wd2, wcnt = capi.knn_radius(ctx, wsrc, wsrc, 12)
+    wicp = capi.WarpIcp(ctx, capi.Cloud(ctx, wp["dst"], wp["dst_normals"]), wsrc,
+                        *capi.neighborhood_csr(widx, wd2, wcnt))
+    got = wicp.estimate(w_pt=0.1, stiffness=200.0, huber=1e-2, reg_sigma=0.015, max_iter=3, max_d2=0.04 ** 2,
+                        max_gn_iter=2, max_cg_iter=50)
+    f, s, _ = wicp.correspondences()
+    wicp.solve(f, s, w_pt=0.1, max_gn_iter=1, max_cg_iter=20)
+    wicp.residuals(got["T"], w_pt=0.1)
     ctx.close()
     print("sanitize target: all checks passed")
 
