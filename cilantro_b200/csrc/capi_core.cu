@@ -31,17 +31,17 @@ int get_reduce_scratch(cb_context* ctx, int blocks, int nv, ReduceScratch* out) 
   const size_t need = ((size_t)blocks + groups) * (size_t)nv;
   if (ctx->partials_cap < need) {
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (ctx->d_partials) CB_CUDA(cudaFree(ctx->d_partials));
+    CB_TRY(ctx->mem.free(ctx->d_partials));
     const size_t cap = std::max<size_t>(need, (size_t)8192 * 32);
-    CB_CUDA(cudaMalloc(&ctx->d_partials, cap * sizeof(double)));
+    CB_TRY(ctx->mem.alloc(&ctx->d_partials, cap));
     ctx->partials_cap = cap;
   }
   if (ctx->counter_cap < groups + 1) {
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (ctx->d_counter) CB_CUDA(cudaFree(ctx->d_counter));
+    CB_TRY(ctx->mem.free(ctx->d_counter));
     const size_t cap = std::max<size_t>(groups + 1, 4096);
-    CB_CUDA(cudaMalloc(&ctx->d_counter, cap * sizeof(unsigned int)));
-    CB_CUDA(cudaMemset(ctx->d_counter, 0, cap * sizeof(unsigned int)));
+    CB_TRY(ctx->mem.alloc(&ctx->d_counter, cap));
+    CB_CUDA(cudaMemsetAsync(ctx->d_counter, 0, cap * sizeof(unsigned int), ctx->stream));
     ctx->counter_cap = cap;
   }
   out->partials = ctx->d_partials;
@@ -67,17 +67,18 @@ static int upload_peer_tables(cb_context* ctx) {
     hv[p] = xchg_vals(base);
     hf[p] = xchg_flags(base);
   }
-  CB_CUDA(cudaMemcpy(ctx->d_peer_vals, hv, sizeof(hv), cudaMemcpyHostToDevice));
-  CB_CUDA(cudaMemcpy(ctx->d_peer_flags, hf, sizeof(hf), cudaMemcpyHostToDevice));
+  CB_CUDA(cudaMemcpyAsync(ctx->d_peer_vals, hv, sizeof(hv), cudaMemcpyHostToDevice, ctx->stream));
+  CB_CUDA(cudaMemcpyAsync(ctx->d_peer_flags, hf, sizeof(hf), cudaMemcpyHostToDevice, ctx->stream));
+  CB_CUDA(cudaStreamSynchronize(ctx->stream));
   return CB_OK;
 }
 
 static int setup_exchange(cb_context* ctx) {
-  CB_CUDA(cudaMalloc(&ctx->d_xchg, kXchgBytes));
+  CB_CUDA(cudaMalloc(&ctx->d_xchg, kXchgBytes));  // not from ctx->mem: CUDA IPC cannot export pool memory
   CB_CUDA(cudaMemset(ctx->d_xchg, 0, kXchgBytes));
-  CB_CUDA(cudaMalloc(&ctx->d_peer_vals, kMaxRanks * sizeof(double*)));
-  CB_CUDA(cudaMalloc(&ctx->d_peer_flags, kMaxRanks * sizeof(unsigned long long*)));
-  CB_CUDA(cudaHostAlloc(&ctx->h_sync, (64 + 4 * 64) * sizeof(unsigned long long), cudaHostAllocMapped));
+  CB_TRY(ctx->mem.alloc(&ctx->d_peer_vals, kMaxRanks));
+  CB_TRY(ctx->mem.alloc(&ctx->d_peer_flags, kMaxRanks));
+  CB_TRY(ctx->mem.alloc_host(&ctx->h_sync, 64 + 4 * 64, cudaHostAllocMapped));
   std::memset(ctx->h_sync, 0, (64 + 4 * 64) * sizeof(unsigned long long));
   ctx->peer_xchg[0] = ctx->d_xchg;
   CB_TRY(upload_peer_tables(ctx));
@@ -166,6 +167,29 @@ const char* cb_last_error(void) { return cb::g_err.c_str(); }
 const char* cb_version(void) { return "cilantro_b200 0.1 (sm_90a)"; }
 
 // ---- context ------------------------------------------------------------------------------------
+static int context_init(cb_context* ctx) {
+  cudaDeviceProp prop;
+  CB_CUDA(cudaGetDeviceProperties(&prop, ctx->device));
+  ctx->sm_count = prop.multiProcessorCount;
+  ctx->l2_bytes = (size_t)prop.l2CacheSize;
+  ctx->hbm_bytes = prop.totalGlobalMem;
+  snprintf(ctx->name, sizeof(ctx->name), "%s", prop.name);
+  CB_CUDA(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
+  {
+    // All cloud / index / scratch buffers come from the stream-ordered pool. Keep freed memory in the
+    // pool (default: returned to the OS at every synchronise, which made repeated cloud creation pay
+    // page allocation again each time: large outliers in the end-to-end call).
+    cudaMemPool_t pool;
+    CB_CUDA(cudaDeviceGetDefaultMemPool(&pool, ctx->device));
+    uint64_t keep = UINT64_MAX;
+    CB_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep));
+  }
+  CB_TRY(ctx->mem.alloc(&ctx->d_result, 64));
+  CB_CUDA(cudaMemsetAsync(ctx->d_result, 0, 64 * sizeof(double), ctx->stream));
+  CB_TRY(ctx->mem.alloc_host(&ctx->h_result, 64));
+  return setup_exchange(ctx);
+}
+
 int cb_context_create(int device, cb_context** out) {
   CB_CHECK(out, CB_ERR_INVALID, "out is null");
   *out = nullptr;
@@ -180,29 +204,11 @@ int cb_context_create(int device, cb_context** out) {
   CB_CUDA(cudaSetDevice(device));
   cb_context* ctx = new cb_context;
   ctx->device = device;
-  cudaDeviceProp prop;
-  CB_CUDA(cudaGetDeviceProperties(&prop, device));
-  ctx->sm_count = prop.multiProcessorCount;
-  ctx->l2_bytes = (size_t)prop.l2CacheSize;
-  ctx->hbm_bytes = prop.totalGlobalMem;
-  snprintf(ctx->name, sizeof(ctx->name), "%s", prop.name);
-  CB_CUDA(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
-  {
-    // All cloud / index / scratch buffers come from the stream-ordered pool. Keep freed memory in the
-    // pool (default: returned to the OS at every synchronise, which made repeated cloud creation pay
-    // page allocation again each time: large outliers in the end-to-end call).
-    cudaMemPool_t pool;
-    CB_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
-    uint64_t keep = UINT64_MAX;
-    CB_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep));
+  const int rc = context_init(ctx);
+  if (rc != CB_OK) {
+    cb_context_destroy(ctx);  // also destroys the stream and the exchange region
+    return rc;
   }
-  CB_CUDA(cudaMalloc(&ctx->d_result, 64 * sizeof(double)));
-  CB_CUDA(cudaMemset(ctx->d_result, 0, 64 * sizeof(double)));
-  CB_CUDA(cudaMallocHost(&ctx->h_result, 64 * sizeof(double)));
-  CB_CUDA(cudaEventCreate(&ctx->ev0));
-  CB_CUDA(cudaEventCreate(&ctx->ev1));
-  CB_CUDA(cudaEventCreate(&ctx->ev2));
-  CB_TRY(setup_exchange(ctx));
   *out = ctx;
   return CB_OK;
 }
@@ -212,23 +218,14 @@ void cb_context_destroy(cb_context* ctx) {
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
   nccl_destroy(ctx);
-  if (ctx->d_partials) cudaFree(ctx->d_partials);
-  if (ctx->d_counter) cudaFree(ctx->d_counter);
-  if (ctx->d_result) cudaFree(ctx->d_result);
-  if (ctx->h_result) cudaFreeHost(ctx->h_result);
-  if (ctx->d_flush) cudaFree(ctx->d_flush);
   for (int p = 0; p < kMaxRanks; ++p)
     if (ctx->peer_xchg[p] && ctx->peer_xchg[p] != ctx->d_xchg) cudaIpcCloseMemHandle(ctx->peer_xchg[p]);
   if (ctx->d_xchg) cudaFree(ctx->d_xchg);
-  if (ctx->d_peer_vals) cudaFree(ctx->d_peer_vals);
-  if (ctx->d_peer_flags) cudaFree(ctx->d_peer_flags);
-  if (ctx->h_sync) cudaFreeHost(ctx->h_sync);
-  if (ctx->ev0) cudaEventDestroy(ctx->ev0);
-  if (ctx->ev1) cudaEventDestroy(ctx->ev1);
-  if (ctx->ev2) cudaEventDestroy(ctx->ev2);
-  if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-  if (ctx->stream) cudaStreamDestroy(ctx->stream);
-  delete ctx;
+  if (ctx->d_flush) cudaFree(ctx->d_flush);
+  const cudaStream_t stream = ctx->stream, copy_stream = ctx->copy_stream;
+  delete ctx;  // ctx->mem frees its buffers on the stream, so the streams go after it
+  if (copy_stream) cudaStreamDestroy(copy_stream);
+  if (stream) cudaStreamDestroy(stream);
 }
 
 int cb_context_synchronize(cb_context* ctx) {
@@ -252,6 +249,8 @@ int cb_context_flush_l2(cb_context* ctx) {
   CB_CUDA(cudaSetDevice(ctx->device));
   if (!ctx->d_flush) {
     ctx->flush_bytes = std::max<size_t>((size_t)256 << 20, 2 * ctx->l2_bytes);
+    // not from ctx->mem: taken from the pool, this buffer would claim memory that the calls timed after a flush
+    // then have to map again
     CB_CUDA(cudaMalloc(&ctx->d_flush, ctx->flush_bytes));
   }
   CB_CUDA(cudaMemsetAsync(ctx->d_flush, 0x5a, ctx->flush_bytes, ctx->stream));
@@ -331,27 +330,62 @@ int cb_context_comm_info(cb_context* ctx, int* rank, int* world) {
 }
 
 // ---- clouds -------------------------------------------------------------------------------------
+// d_raw (and d_raw_nrm) of a new cloud, from its scope
+static int alloc_raw(cb_cloud* c, bool normals) {
+  if (c->n == 0) return CB_OK;
+  CB_TRY(c->mem.alloc(&c->d_raw, 3 * c->n));
+  if (normals) CB_TRY(c->mem.alloc(&c->d_raw_nrm, 3 * c->n));
+  return CB_OK;
+}
+
+static int upload_raw(cb_cloud* c, const float* xyz, const float* nrm, cudaMemcpyKind kind, cudaStream_t s) {
+  if (c->n == 0) return CB_OK;
+  CB_CUDA(cudaMemcpyAsync(c->d_raw, xyz, 3 * c->n * sizeof(float), kind, s));
+  if (nrm) CB_CUDA(cudaMemcpyAsync(c->d_raw_nrm, nrm, 3 * c->n * sizeof(float), kind, s));
+  return CB_OK;
+}
+
+static int cloud_fill(cb_cloud* c, const float* xyz, const float* normals, cudaMemcpyKind kind) {
+  CB_TRY(alloc_raw(c, normals));
+  CB_TRY(upload_raw(c, xyz, normals, kind, c->ctx->stream));
+  // the caller's buffers may be released as soon as this returns
+  if (c->n > 0) CB_CUDA(cudaStreamSynchronize(c->ctx->stream));
+  return CB_OK;
+}
+
 static int cloud_create_common(cb_context* ctx, const float* xyz, const float* normals, size_t n, uint64_t off,
                                cudaMemcpyKind kind, cb_cloud** out) {
   CB_CHECK(ctx && out, CB_ERR_INVALID, "null argument");
   CB_CHECK(n == 0 || xyz, CB_ERR_INVALID, "xyz is null");
   CB_CHECK(n < (1ull << 31), CB_ERR_INVALID, "point sets of >= 2^31 points are not supported");
   CB_CUDA(cudaSetDevice(ctx->device));
-  cb_cloud* c = new cb_cloud;
-  c->ctx = ctx;
-  c->n = n;
-  c->index_offset = off;
-  if (n > 0) {
-    CB_CUDA(cudaMallocAsync(&c->d_raw, 3 * n * sizeof(float), ctx->stream));
-    CB_CUDA(cudaMemcpyAsync(c->d_raw, xyz, 3 * n * sizeof(float), kind, ctx->stream));
-    if (normals) {
-      CB_CUDA(cudaMallocAsync(&c->d_raw_nrm, 3 * n * sizeof(float), ctx->stream));
-      CB_CUDA(cudaMemcpyAsync(c->d_raw_nrm, normals, 3 * n * sizeof(float), kind, ctx->stream));
-    }
-    // the caller's buffers may be released as soon as this returns
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
+  cb_cloud* c = new cb_cloud(ctx, n, off);
+  const int rc = cloud_fill(c, xyz, normals, kind);
+  if (rc != CB_OK) {
+    delete c;
+    return rc;
   }
   *out = c;
+  return CB_OK;
+}
+
+static int pair_fill(cb_cloud* a, const float* xyz_a, const float* normals_a, cb_cloud* b, const float* xyz_b,
+                     const float* normals_b) {
+  cb_context* ctx = a->ctx;
+  ScopedEvents ev;
+  CB_TRY(ev.create());
+  // allocations are stream-ordered on the main stream; the copy stream starts after them
+  CB_TRY(alloc_raw(a, normals_a));
+  CB_TRY(alloc_raw(b, normals_b));
+  CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
+  CB_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ev.e0, 0));
+  CB_TRY(upload_raw(a, xyz_a, normals_a, cudaMemcpyHostToDevice, ctx->stream));
+  CB_TRY(upload_raw(b, xyz_b, normals_b, cudaMemcpyHostToDevice, ctx->copy_stream));
+  CB_CUDA(cudaEventRecord(ev.e1, ctx->copy_stream));
+  CB_TRY(ensure_index(a));  // host-blocking in places; the second upload proceeds meanwhile
+  CB_CUDA(cudaStreamWaitEvent(ctx->stream, ev.e1, 0));
+  CB_TRY(ensure_index(b));
+  CB_CUDA(cudaStreamSynchronize(ctx->stream));
   return CB_OK;
 }
 
@@ -368,59 +402,46 @@ int cb_cloud_create_pair(cb_context* ctx, const float* xyz_a, const float* norma
   CB_CUDA(cudaSetDevice(ctx->device));
   *out_a = *out_b = nullptr;
   if (!ctx->copy_stream) CB_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-  ScopedEvents ev;
-  CB_TRY(ev.create());
-  cb_cloud* a = new cb_cloud;
-  cb_cloud* b = new cb_cloud;
-  a->ctx = b->ctx = ctx;
-  a->n = n_a;
-  b->n = n_b;
-  a->index_offset = offset_a;
-  b->index_offset = offset_b;
-  auto fail = [&](int rc) {
-    cb_cloud_destroy(a);
-    cb_cloud_destroy(b);
-    return rc;
-  };
-  auto upload = [&](cb_cloud* c, const float* xyz, const float* nrm, cudaStream_t s) -> int {
-    if (c->n == 0) return CB_OK;
-    CB_CUDA(cudaMemcpyAsync(c->d_raw, xyz, 3 * c->n * sizeof(float), cudaMemcpyHostToDevice, s));
-    if (nrm) CB_CUDA(cudaMemcpyAsync(c->d_raw_nrm, nrm, 3 * c->n * sizeof(float), cudaMemcpyHostToDevice, s));
-    return CB_OK;
-  };
-  // allocations are stream-ordered on the main stream; the copy stream starts after them
-  if (n_a) {
-    if (cudaMallocAsync(&a->d_raw, 3 * n_a * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-    if (normals_a && cudaMallocAsync(&a->d_raw_nrm, 3 * n_a * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-  }
-  if (n_b) {
-    if (cudaMallocAsync(&b->d_raw, 3 * n_b * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-    if (normals_b && cudaMallocAsync(&b->d_raw_nrm, 3 * n_b * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-  }
-  if (cudaEventRecord(ev.e0, ctx->stream) != cudaSuccess || cudaStreamWaitEvent(ctx->copy_stream, ev.e0, 0) != cudaSuccess)
-    return fail(CB_ERR_CUDA);
-  int rc = upload(a, xyz_a, normals_a, ctx->stream);
-  if (rc == CB_OK) rc = upload(b, xyz_b, normals_b, ctx->copy_stream);
-  if (rc == CB_OK && cudaEventRecord(ev.e1, ctx->copy_stream) != cudaSuccess) rc = CB_ERR_CUDA;
-  if (rc == CB_OK) rc = ensure_index(a);  // host-blocking in places; the second upload proceeds meanwhile
-  if (rc == CB_OK && cudaStreamWaitEvent(ctx->stream, ev.e1, 0) != cudaSuccess) rc = CB_ERR_CUDA;
-  if (rc == CB_OK) rc = ensure_index(b);
-  if (rc == CB_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = CB_ERR_CUDA;
+  cb_cloud* a = new cb_cloud(ctx, n_a, offset_a);
+  cb_cloud* b = new cb_cloud(ctx, n_b, offset_b);
+  const int rc = pair_fill(a, xyz_a, normals_a, b, xyz_b, normals_b);
   if (rc != CB_OK) {  // the failing call has set the message
-    cudaStreamSynchronize(ctx->copy_stream);
-    return fail(rc);
+    cudaStreamSynchronize(ctx->copy_stream);  // b's upload may still be writing into its buffers
+    delete a;
+    delete b;
+    return rc;
   }
   *out_a = a;
   *out_b = b;
   return CB_OK;
 }
 
+// Fills a new cloud from one rank's block of points [first, first + n_block) (host or device memory, `kind`): each
+// rank copies only its block into the zero-initialised arrays, and with several ranks one integer-sum all-reduce of
+// them is an exact all-gather of bit patterns. Collective when ctx->world > 1.
+static int fill_replicated(cb_cloud* c, const float* xyz_block, const float* normals_block, size_t n_block,
+                           uint64_t first, cudaMemcpyKind kind) {
+  cb_context* ctx = c->ctx;
+  const size_t words = 3 * c->n;
+  if (words == 0) return CB_OK;
+  for (int pass = 0; pass < (normals_block ? 2 : 1); ++pass) {
+    float** d = pass == 0 ? &c->d_raw : &c->d_raw_nrm;
+    CB_TRY(c->mem.alloc(d, words));
+    if (ctx->world > 1) CB_CUDA(cudaMemsetAsync(*d, 0, words * sizeof(float), ctx->stream));
+    if (n_block)
+      CB_CUDA(cudaMemcpyAsync(*d + 3 * first, pass == 0 ? xyz_block : normals_block, 3 * n_block * sizeof(float), kind,
+                              ctx->stream));
+    if (ctx->world > 1) CB_TRY(nccl_allreduce_sum_u32(ctx, reinterpret_cast<uint32_t*>(*d), words));
+  }
+  CB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return CB_OK;
+}
+
 // A cloud every rank needs in full (the destination cloud of a sharded ICP), created from its contiguous blocks: each
-// rank uploads ONLY its block over its own PCIe link, the blocks are exchanged over NVLink (one integer-sum
-// all-reduce of the zero-initialised arrays = an exact all-gather of bit patterns). Replaces N uploads of the whole
-// cloud (N x the PCIe time for the same bytes) when the caller's data is already partitioned - or cheaply sliceable,
-// as in bench.py's end-to-end leg. Collective: every rank of the communicator calls it with the same n_total and
-// the same presence of normals.
+// rank uploads ONLY its block over its own PCIe link, the blocks are exchanged over NVLink (fill_replicated). Replaces
+// N uploads of the whole cloud (N x the PCIe time for the same bytes) when the caller's data is already partitioned - or
+// cheaply sliceable, as in bench.py's end-to-end leg. Collective: every rank of the communicator calls it with the same
+// n_total and the same presence of normals (a rank with an empty block passes any non-null pointer).
 int cb_cloud_create_replicated(cb_context* ctx, const float* xyz_block, const float* normals_block, size_t n_block,
                                uint64_t first_index, size_t n_total, cb_cloud** out) {
   CB_CHECK(ctx && out, CB_ERR_INVALID, "null argument");
@@ -428,38 +449,12 @@ int cb_cloud_create_replicated(cb_context* ctx, const float* xyz_block, const fl
   CB_CHECK(first_index + n_block <= n_total, CB_ERR_INVALID, "block outside the cloud");
   CB_CHECK(n_total < (1ull << 31), CB_ERR_INVALID, "point sets of >= 2^31 points are not supported");
   CB_CUDA(cudaSetDevice(ctx->device));
-  cb_cloud* c = new cb_cloud;
-  c->ctx = ctx;
-  c->n = n_total;
-  c->index_offset = 0;
   *out = nullptr;
-  auto fail = [&](int rc) {
-    cb_cloud_destroy(c);
+  cb_cloud* c = new cb_cloud(ctx, n_total, 0);
+  const int rc = fill_replicated(c, xyz_block, normals_block, n_block, first_index, cudaMemcpyHostToDevice);
+  if (rc != CB_OK) {
+    delete c;
     return rc;
-  };
-  if (n_total > 0) {
-    const size_t words = 3 * n_total;
-    if (cudaMallocAsync(&c->d_raw, words * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-    if (normals_block || ctx->world > 1) {
-      // (with several ranks the presence of normals must be the same everywhere; a rank with an empty block passes
-      // any non-null pointer)
-      if (normals_block && cudaMallocAsync(&c->d_raw_nrm, words * sizeof(float), ctx->stream) != cudaSuccess)
-        return fail(CB_ERR_CUDA);
-    }
-    for (int pass = 0; pass < 2; ++pass) {
-      float* d = pass == 0 ? c->d_raw : c->d_raw_nrm;
-      const float* h = pass == 0 ? xyz_block : normals_block;
-      if (!d) continue;
-      if (ctx->world > 1 && cudaMemsetAsync(d, 0, words * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-      if (n_block && cudaMemcpyAsync(d + 3 * first_index, h, 3 * n_block * sizeof(float), cudaMemcpyHostToDevice,
-                                     ctx->stream) != cudaSuccess)
-        return fail(CB_ERR_CUDA);
-      if (ctx->world > 1) {
-        const int rc = nccl_allreduce_sum_u32(ctx, reinterpret_cast<uint32_t*>(d), words);
-        if (rc != CB_OK) return fail(rc);
-      }
-    }
-    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
   }
   *out = c;
   return CB_OK;
@@ -479,12 +474,6 @@ void cb_cloud_destroy(cb_cloud* c) {
   if (!c) return;
   cudaSetDevice(c->ctx->device);
   cudaStreamSynchronize(c->ctx->stream);
-  if (c->d_raw) cudaFreeAsync(c->d_raw, c->ctx->stream);
-  if (c->d_raw_nrm) cudaFreeAsync(c->d_raw_nrm, c->ctx->stream);
-  if (c->d_pts) cudaFreeAsync(c->d_pts, c->ctx->stream);
-  if (c->d_nrm) cudaFreeAsync(c->d_nrm, c->ctx->stream);
-  if (c->d_cell_start) cudaFreeAsync(c->d_cell_start, c->ctx->stream);
-  if (c->d_blocks) cudaFreeAsync(c->d_blocks, c->ctx->stream);
   delete c;
 }
 
@@ -505,7 +494,7 @@ int cb_cloud_grid_info(const cb_cloud* c, float* cell_edge, int* dims3, double* 
 
 // ---- nearest neighbour ----------------------------------------------------------------------------
 static int knn1_device(cb_context* ctx, const cb_cloud* ref, const cb_cloud* qry, const float* T12, float max_d2,
-                       int** d_idx_out, float** d_d2_out) {
+                       DeviceScope& scope, int** d_idx_out, float** d_d2_out) {
   CB_CHECK(ctx && ref && qry, CB_ERR_INVALID, "null argument");
   CB_CHECK(ref->ctx == ctx && qry->ctx == ctx, CB_ERR_INVALID, "cloud belongs to another context");
   CB_CUDA(cudaSetDevice(ctx->device));
@@ -513,9 +502,8 @@ static int knn1_device(cb_context* ctx, const cb_cloud* ref, const cb_cloud* qry
   CB_TRY(ensure_index(const_cast<cb_cloud*>(qry)));
   int* d_idx = nullptr;
   float* d_d2 = nullptr;
-  const size_t nq = std::max<size_t>(qry->n, 1);
-  CB_CUDA(cudaMallocAsync(&d_idx, nq * sizeof(int), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_d2, nq * sizeof(float), ctx->stream));
+  CB_TRY(scope.alloc(&d_idx, qry->n));
+  CB_TRY(scope.alloc(&d_d2, qry->n));
   IcpArgs a{};
   a.dst = grid_view(ref);
   a.src_pts = qry->d_pts;
@@ -534,17 +522,16 @@ static int knn1_device(cb_context* ctx, const cb_cloud* ref, const cb_cloud* qry
 
 int cb_knn1_radius(cb_context* ctx, const cb_cloud* ref, const cb_cloud* qry, const float* T12, float max_d2,
                    int64_t* idx, float* d2) {
+  DeviceScope scope(ctx);
   int* d_idx = nullptr;
   float* d_d2 = nullptr;
-  CB_TRY(knn1_device(ctx, ref, qry, T12, max_d2, &d_idx, &d_d2));
+  CB_TRY(knn1_device(ctx, ref, qry, T12, max_d2, scope, &d_idx, &d_d2));
   const size_t nq = qry->n;
   std::vector<int> h_idx(nq);
   if (nq) {
     CB_CUDA(cudaMemcpyAsync(h_idx.data(), d_idx, nq * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     if (d2) CB_CUDA(cudaMemcpyAsync(d2, d_d2, nq * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   }
-  CB_CUDA(cudaFreeAsync(d_idx, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_d2, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (idx)
     for (size_t i = 0; i < nq; i++) idx[i] = h_idx[i] < 0 ? -1 : (int64_t)h_idx[i] + (int64_t)ref->index_offset;
@@ -557,9 +544,10 @@ int cb_find_correspondences(cb_context* ctx, const cb_cloud* ref, const cb_cloud
   CB_CHECK(count, CB_ERR_INVALID, "count is null");
   *count = 0;
   if (ref && ref->n == 0) return CB_OK;  // correspondence_search_kd_tree_utilities.hpp:16-19
+  DeviceScope scope(ctx);
   int* d_idx = nullptr;
   float* d_d2 = nullptr;
-  CB_TRY(knn1_device(ctx, ref, qry, T12, max_d2, &d_idx, &d_d2));
+  CB_TRY(knn1_device(ctx, ref, qry, T12, max_d2, scope, &d_idx, &d_d2));
   const size_t nq = qry->n;
   std::vector<int> h_idx(nq);
   std::vector<float> h_d2(nq);
@@ -567,8 +555,6 @@ int cb_find_correspondences(cb_context* ctx, const cb_cloud* ref, const cb_cloud
     CB_CUDA(cudaMemcpyAsync(h_idx.data(), d_idx, nq * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaMemcpyAsync(h_d2.data(), d_d2, nq * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   }
-  CB_CUDA(cudaFreeAsync(d_idx, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_d2, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   size_t k = 0;  // compaction in query order (:45-50)
   for (size_t i = 0; i < nq; i++) {
@@ -586,14 +572,13 @@ int cb_transform_points(cb_context* ctx, const float* T12, const float* xyz, siz
   CB_CHECK(ctx && T12 && (n == 0 || (xyz && out)), CB_ERR_INVALID, "null argument");
   if (n == 0) return CB_OK;
   CB_CUDA(cudaSetDevice(ctx->device));
+  DeviceScope scope(ctx);
   float *d_in = nullptr, *d_out = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_in, 3 * n * sizeof(float), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_out, 3 * n * sizeof(float), ctx->stream));
+  CB_TRY(scope.alloc(&d_in, 3 * n));
+  CB_TRY(scope.alloc(&d_out, 3 * n));
   CB_CUDA(cudaMemcpyAsync(d_in, xyz, 3 * n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   CB_TRY(launch_transform_points(ctx, to_rigid(T12), d_in, n, d_out));
   CB_CUDA(cudaMemcpyAsync(out, d_out, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_in, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_out, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   return CB_OK;
 }
@@ -627,21 +612,27 @@ static int global_mean(cb_context* ctx, const cb_cloud* c, bool allreduce, float
   return CB_OK;
 }
 
+static int icp_init(cb_icp* icp) {
+  // dst is replicated on every rank, src is sharded: only the src mean needs the all-reduce
+  CB_TRY(global_mean(icp->ctx, icp->dst, false, icp->dst_mean));
+  CB_TRY(global_mean(icp->ctx, icp->src, true, icp->src_mean));
+  CB_TRY(icp->mem.alloc(&icp->d_nn_pos, icp->src->n));
+  CB_TRY(icp->mem.alloc(&icp->d_nn_d2, icp->src->n));
+  return CB_OK;
+}
+
 int cb_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, cb_icp** out) {
   CB_CHECK(ctx && dst && src && out, CB_ERR_INVALID, "null argument");
   CB_CHECK(dst->ctx == ctx && src->ctx == ctx, CB_ERR_INVALID, "cloud belongs to another context");
   CB_CUDA(cudaSetDevice(ctx->device));
   CB_TRY(ensure_index(const_cast<cb_cloud*>(dst)));
   CB_TRY(ensure_index(const_cast<cb_cloud*>(src)));
-  cb_icp* icp = new cb_icp;
-  icp->ctx = ctx;
-  icp->dst = dst;
-  icp->src = src;
-  // dst is replicated on every rank, src is sharded: only the src mean needs the all-reduce
-  CB_TRY(global_mean(ctx, dst, false, icp->dst_mean));
-  CB_TRY(global_mean(ctx, src, true, icp->src_mean));
-  CB_CUDA(cudaMallocAsync(&icp->d_nn_pos, std::max<size_t>(src->n, 1) * sizeof(int), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&icp->d_nn_d2, std::max<size_t>(src->n, 1) * sizeof(float), ctx->stream));
+  cb_icp* icp = new cb_icp(ctx, dst, src);
+  const int rc = icp_init(icp);
+  if (rc != CB_OK) {
+    delete icp;
+    return rc;
+  }
   *out = icp;
   return CB_OK;
 }
@@ -650,14 +641,7 @@ void cb_icp_destroy(cb_icp* icp) {
   if (!icp) return;
   cudaSetDevice(icp->ctx->device);
   cudaStreamSynchronize(icp->ctx->stream);
-  if (icp->d_nn_pos) cudaFreeAsync(icp->d_nn_pos, icp->ctx->stream);
-  if (icp->d_nn_d2) cudaFreeAsync(icp->d_nn_d2, icp->ctx->stream);
-  engine_release_pairs(icp->ctx, &icp->pairs);
-  if (icp->d_state) cudaFree(icp->d_state);
-  if (icp->d_miss_mask) cudaFree(icp->d_miss_mask);
-  if (icp->src_full) cb_cloud_destroy(icp->src_full);
-  if (icp->h_state) cudaFreeHost(icp->h_state);
-  if (icp->h_state2) cudaFreeHost(icp->h_state2);
+  delete icp->src_full;
   for (cudaEvent_t e : icp->batch_ev)
     if (e) cudaEventDestroy(e);
   for (cudaEvent_t e : icp->events) cudaEventDestroy(e);
@@ -723,28 +707,14 @@ static int ensure_src_full(cb_icp* icp) {
            "engine modes across ranks: the source shards need index_offset = their first global index");
   const bool nrm = tot[1] > 0.5;
   CB_CHECK(!nrm || (int)(tot[1] + 0.5) == ctx->world, CB_ERR_INVALID, "source normals on some ranks only");
-  cb_cloud* c = new cb_cloud;
-  c->ctx = ctx;
-  c->n = n_total;
-  c->index_offset = 0;
-  const size_t words = 3 * n_total;
-  auto fail = [&](int rc) {
-    cb_cloud_destroy(c);
+  // (nrm: every rank has normals; otherwise none has)
+  cb_cloud* c = new cb_cloud(ctx, n_total, 0);
+  int rc = fill_replicated(c, src->d_raw, src->d_raw_nrm, src->n, src->index_offset, cudaMemcpyDeviceToDevice);
+  if (rc == CB_OK) rc = ensure_index(c);
+  if (rc != CB_OK) {
+    delete c;
     return rc;
-  };
-  for (int pass = 0; pass < (nrm ? 2 : 1); ++pass) {
-    float** d = pass == 0 ? &c->d_raw : &c->d_raw_nrm;
-    const float* mine = pass == 0 ? src->d_raw : src->d_raw_nrm;
-    if (cudaMallocAsync(d, std::max<size_t>(words, 1) * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-    if (cudaMemsetAsync(*d, 0, words * sizeof(float), ctx->stream) != cudaSuccess) return fail(CB_ERR_CUDA);
-    if (src->n && cudaMemcpyAsync(*d + 3 * src->index_offset, mine, 3 * src->n * sizeof(float), cudaMemcpyDeviceToDevice,
-                                  ctx->stream) != cudaSuccess)
-      return fail(CB_ERR_CUDA);
-    const int rc = nccl_allreduce_sum_u32(ctx, reinterpret_cast<uint32_t*>(*d), words);
-    if (rc != CB_OK) return fail(rc);
   }
-  const int rc = ensure_index(c);
-  if (rc != CB_OK) return fail(rc);
   icp->src_full = c;
   return CB_OK;
 }
@@ -766,7 +736,7 @@ static int icp_update(cb_icp* icp, const cb_icp_params* prm, const float* T, flo
     // updateCorrespondences(): the explicit list (icp_engine.cu); the passes below accumulate over it
     if (k0) CB_CUDA(cudaEventRecord(k0, ctx->stream));
     CB_TRY(ensure_src_full(icp));
-    CB_TRY(engine_find_pairs(ctx, icp->dst, esrc(icp), prm, T, &icp->pairs));
+    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, esrc(icp), prm, T, &icp->pairs));
     if (k1) CB_CUDA(cudaEventRecord(k1, ctx->stream));
   }
   if (prm->metric == CB_ICP_POINT_TO_POINT) {
@@ -1069,13 +1039,13 @@ int cb_icp_residuals(cb_icp* icp, const cb_icp_params* prm, const float* T12, fl
   if (ns == 0) return CB_OK;
   CB_CHECK(prm->metric == CB_ICP_POINT_TO_POINT || icp->dst->d_nrm || icp->dst->n == 0, CB_ERR_INVALID,
            "dst has no normals");
+  DeviceScope scope(ctx);
   float* d_out = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_out, ns * sizeof(float), ctx->stream));
+  CB_TRY(scope.alloc(&d_out, ns));
   CB_TRY(launch_residuals(ctx, grid_view(icp->dst), icp->src->d_pts,
                           prm->metric == CB_ICP_COMBINED ? icp->src->d_nrm : nullptr, (uint32_t)ns, to_rigid(T12),
                           prm->metric, prm->w_pt, prm->w_pl, d_out));
   CB_CUDA(cudaMemcpyAsync(out, d_out, ns * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_out, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   return CB_OK;
 }

@@ -90,6 +90,29 @@ struct GridView {
 
 constexpr int kBlockCells = 8;  // coarse block edge in cells
 
+// Owner of device and pinned host memory: everything alloc()ed is cudaFreeAsync()ed on the context's stream, and
+// everything alloc_host()ed is cudaFreeHost()ed, when the scope goes out of scope. Objects (context, clouds, ICP
+// objects) hold one for their buffers; functions hold one for their per-call scratch. The only device memory outside
+// a scope is the context's IPC-exported exchange region and its L2 flush buffer (cb_context::d_xchg, d_flush).
+struct DeviceScope {
+  cb_context* ctx;
+  std::vector<void*> ptrs;
+  std::vector<void*> host;
+  explicit DeviceScope(cb_context* c) : ctx(c) {}
+  DeviceScope(const DeviceScope&) = delete;
+  DeviceScope& operator=(const DeviceScope&) = delete;
+  template <class T>
+  int alloc(T** p, size_t count);
+  // pinned host memory (flags of cudaHostAlloc, e.g. cudaHostAllocMapped)
+  template <class T>
+  int alloc_host(T** p, size_t count, unsigned flags = cudaHostAllocDefault);
+  // hands p over to `owner` (typically an object's scope: a result built among per-call scratch)
+  void move_to(DeviceScope& owner, void* p);
+  // stream-ordered free of one buffer of this scope before the scope ends (buffers that regrow)
+  int free(void* p);
+  ~DeviceScope();
+};
+
 }  // namespace cb
 
 struct cb_context {
@@ -107,15 +130,15 @@ struct cb_context {
   size_t counter_cap = 0;
   double* d_result = nullptr;  // 64 doubles
   double* h_result = nullptr;  // pinned, 64 doubles
-  void* d_flush = nullptr;
+  void* d_flush = nullptr;  // L2 flush buffer (cb_context_flush_l2); cudaMalloc'ed, outside the pool
   size_t flush_bytes = 0;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
   cudaStream_t copy_stream = nullptr;  // second stream: uploads overlapped with index builds (cb_cloud_create_pair)
   // NCCL (loaded lazily with dlopen; see nccl_dyn.cpp)
   void* nccl_comm = nullptr;
   int rank = 0, world = 1;
   // fused exchange (struct Exchange): one cudaMalloc'ed region [flags 2 x kMaxRanks u64 | values
-  // 2 x kMaxRanks x 32 f64] exported to the peers with CUDA IPC, and a mapped pinned host mailbox
+  // 2 x kMaxRanks x 32 f64] exported to the peers with CUDA IPC, and a mapped pinned host mailbox.
+  // d_xchg is the one buffer outside `mem`: CUDA IPC cannot export memory of the stream-ordered pool.
   void* d_xchg = nullptr;                 // this rank's region
   void* peer_xchg[cb::kMaxRanks] = {nullptr};  // every rank's region as seen from this device (self included)
   double** d_peer_vals = nullptr;         // device copies of the two pointer tables
@@ -125,15 +148,19 @@ struct cb_context {
   bool ex_ready = false;                  // tables valid for the current (rank, world)
   bool ex_attached = false;               // cb_comm_ipc_attach has mapped the peers' tables (once per context)
   bool pass_armed = false;                // the last reduction pass carried the fused exchange
+  // every other buffer above, freed on `stream` (cb_context_destroy deletes the context before the stream)
+  cb::DeviceScope mem{this};
 };
 
 constexpr size_t kXchgFlagBytes = 2 * cb::kMaxRanks * sizeof(unsigned long long);
 constexpr size_t kXchgBytes = kXchgFlagBytes + 2 * cb::kMaxRanks * cb::kExchangeVals * sizeof(double);
 
 struct cb_cloud {
+  cb_cloud(cb_context* c, size_t n_, uint64_t off) : ctx(c), n(n_), index_offset(off), mem(c) {}
   cb_context* ctx = nullptr;
   size_t n = 0;
   uint64_t index_offset = 0;
+  cb::DeviceScope mem;  // every buffer below
   float* d_raw = nullptr;      // 3n packed xyz, original order
   float* d_raw_nrm = nullptr;  // 3n packed normals or nullptr
   // grid index (built lazily by cb::ensure_index)
@@ -149,6 +176,42 @@ struct cb_cloud {
 };
 
 namespace cb {
+
+template <class T>
+int DeviceScope::alloc(T** p, size_t count) {
+  *p = nullptr;
+  CB_CUDA(cudaMallocAsync((void**)p, (count ? count : 1) * sizeof(T), ctx->stream));
+  ptrs.push_back(*p);
+  return CB_OK;
+}
+template <class T>
+int DeviceScope::alloc_host(T** p, size_t count, unsigned flags) {
+  *p = nullptr;
+  CB_CUDA(cudaHostAlloc((void**)p, (count ? count : 1) * sizeof(T), flags));
+  host.push_back(*p);
+  return CB_OK;
+}
+inline void DeviceScope::move_to(DeviceScope& owner, void* p) {
+  for (size_t i = 0; i < ptrs.size(); i++)
+    if (ptrs[i] == p) {
+      ptrs.erase(ptrs.begin() + (long)i);
+      owner.ptrs.push_back(p);
+      return;
+    }
+}
+inline int DeviceScope::free(void* p) {
+  for (size_t i = 0; i < ptrs.size(); i++)
+    if (ptrs[i] == p) {
+      ptrs.erase(ptrs.begin() + (long)i);
+      CB_CUDA(cudaFreeAsync(p, ctx->stream));
+      return CB_OK;
+    }
+  return CB_OK;
+}
+inline DeviceScope::~DeviceScope() {
+  for (void* p : ptrs) cudaFreeAsync(p, ctx->stream);
+  for (void* p : host) cudaFreeHost(p);
+}
 
 int ensure_index(cb_cloud* c);
 // Finite-coordinate bounding box of n packed xyz points in device memory (synchronises the stream).
@@ -167,33 +230,6 @@ int get_reduce_scratch(cb_context* ctx, int blocks, int nv, ReduceScratch* out);
 bool arm_exchange(cb_context* ctx, Exchange* ex);
 bool exchange_available(const cb_context* ctx);  // fused exchange usable (tables mapped, not switched off)
 int wait_exchange(cb_context* ctx, int count, double* out);
-
-// Scoped stream-ordered scratch: everything alloc()ed is cudaFreeAsync()ed on the context's stream when the
-// object goes out of scope, unless release()d to the caller.
-struct DeviceScope {
-  cb_context* ctx;
-  std::vector<void*> ptrs;
-  explicit DeviceScope(cb_context* c) : ctx(c) {}
-  DeviceScope(const DeviceScope&) = delete;
-  DeviceScope& operator=(const DeviceScope&) = delete;
-  template <class T>
-  int alloc(T** p, size_t count) {
-    *p = nullptr;
-    CB_CUDA(cudaMallocAsync((void**)p, (count ? count : 1) * sizeof(T), ctx->stream));
-    ptrs.push_back(*p);
-    return CB_OK;
-  }
-  void release(void* p) {
-    for (size_t i = 0; i < ptrs.size(); i++)
-      if (ptrs[i] == p) {
-        ptrs.erase(ptrs.begin() + (long)i);
-        return;
-      }
-  }
-  ~DeviceScope() {
-    for (void* p : ptrs) cudaFreeAsync(p, ctx->stream);
-  }
-};
 
 // A pair of CUDA events that is destroyed on every exit path.
 struct ScopedEvents {
@@ -225,10 +261,10 @@ inline bool engine_mode(const cb_icp_params* p) {
          (p->inlier_fraction > 0.0 && p->inlier_fraction < 1.0);
 }
 // findCorrespondences(tform) of CorrespondenceSearchKDTree (correspondence_search_kd_tree.hpp:107-229) for
-// the current estimate T: searches, union / intersection, fraction and one-to-one filters. Replaces *pairs.
-int engine_find_pairs(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const cb_icp_params* prm,
-                      const float* T12, EnginePairs* pairs);
-void engine_release_pairs(cb_context* ctx, EnginePairs* pairs);
+// the current estimate T: searches, union / intersection, fraction and one-to-one filters. Replaces *pairs, whose
+// buffers belong to `owner`.
+int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const cb_cloud* src,
+                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs);
 
 // nccl_dyn.cpp
 int nccl_unique_id(void* out128);

@@ -182,10 +182,10 @@ int bits_for(uint64_t count) {  // bits needed to represent values 0 .. count-1
 
 using DeviceBufs = DeviceScope;  // scoped stream-ordered allocations (cb_internal.hpp)
 
-// Device-side core: inputs are packed xyz arrays in device memory; outputs are freshly allocated device
-// arrays of *out_n entries (caller frees with cudaFreeAsync on ctx->stream; nullptr when *out_n == 0).
-int downsample_device(cb_context* ctx, const float* d_raw, const float* d_nrm, const float* d_col, size_t n,
-                      float bin_size, size_t min_points, int order, float** out_pts, float** out_nrm,
+// Device-side core: inputs are packed xyz arrays in device memory; outputs are device arrays of *out_n entries
+// allocated from the caller's scope `out` (nullptr when *out_n == 0).
+int downsample_device(cb_context* ctx, DeviceScope& out, const float* d_raw, const float* d_nrm, const float* d_col,
+                      size_t n, float bin_size, size_t min_points, int order, float** out_pts, float** out_nrm,
                       float** out_col, size_t* out_n) {
   *out_pts = nullptr;
   if (out_nrm) *out_nrm = nullptr;
@@ -270,16 +270,15 @@ int downsample_device(cb_context* ctx, const float* d_raw, const float* d_nrm, c
   *out_n = m;
   if (m == 0) return CB_OK;
   float *r_pts = nullptr, *r_nrm = nullptr, *r_col = nullptr;
-  CB_TRY(bufs.alloc(&r_pts, 3 * m));
-  if (d_nrm && out_nrm) CB_TRY(bufs.alloc(&r_nrm, 3 * m));
-  if (d_col && out_col) CB_TRY(bufs.alloc(&r_col, 3 * m));
+  CB_TRY(out.alloc(&r_pts, 3 * m));
+  if (d_nrm && out_nrm) CB_TRY(out.alloc(&r_nrm, 3 * m));
+  if (d_col && out_col) CB_TRY(out.alloc(&r_col, 3 * m));
   emit_kernel<<<bb, kThreads, 0, ctx->stream>>>(d_rank_bin, d_flags, o, nbins, minp, r_pts, r_nrm, r_col);
   ctx->launches += 1;
   CB_CUDA(cudaGetLastError());
-  bufs.release(r_pts);
   *out_pts = r_pts;
-  if (r_nrm) { bufs.release(r_nrm); *out_nrm = r_nrm; }
-  if (r_col) { bufs.release(r_col); *out_col = r_col; }
+  if (r_nrm) *out_nrm = r_nrm;
+  if (r_col) *out_col = r_col;
   return CB_OK;
 }
 
@@ -309,15 +308,13 @@ extern "C" int cb_grid_downsample(cb_context* ctx, const float* xyz, const float
   }
   float *o_pts = nullptr, *o_nrm = nullptr, *o_col = nullptr;
   size_t m = 0;
-  CB_TRY(downsample_device(ctx, d_raw, d_nrm, d_col, n, bin_size, min_points_in_bin, order, &o_pts, &o_nrm, &o_col, &m));
+  CB_TRY(downsample_device(ctx, in, d_raw, d_nrm, d_col, n, bin_size, min_points_in_bin, order, &o_pts, &o_nrm, &o_col,
+                           &m));
   if (m > 0) {
     CB_CUDA(cudaMemcpyAsync(out_xyz, o_pts, 3 * m * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
     if (o_nrm) CB_CUDA(cudaMemcpyAsync(out_normals, o_nrm, 3 * m * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
     if (o_col) CB_CUDA(cudaMemcpyAsync(out_colors, o_col, 3 * m * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   }
-  if (o_pts) cudaFreeAsync(o_pts, ctx->stream);
-  if (o_nrm) cudaFreeAsync(o_nrm, ctx->stream);
-  if (o_col) cudaFreeAsync(o_col, ctx->stream);
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   *out_n = m;
   return CB_OK;
@@ -336,19 +333,18 @@ extern "C" int cb_cloud_grid_downsample(cb_context* ctx, const cb_cloud* cloud, 
     CB_TRY(ev.create());
     CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
   }
+  DeviceBufs bufs(ctx);
   float *o_pts = nullptr, *o_nrm = nullptr;
   size_t m = 0;
-  CB_TRY(downsample_device(ctx, cloud->d_raw, cloud->d_raw_nrm, nullptr, cloud->n, bin_size, min_points_in_bin, order,
+  CB_TRY(downsample_device(ctx, bufs, cloud->d_raw, cloud->d_raw_nrm, nullptr, cloud->n, bin_size, min_points_in_bin, order,
                            &o_pts, &o_nrm, nullptr, &m));
   if (gpu_ms) CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
-  const int rc = cb_cloud_create_from_device(ctx, o_pts, o_nrm, m, cloud->index_offset, out);
-  if (o_pts) cudaFreeAsync(o_pts, ctx->stream);
-  if (o_nrm) cudaFreeAsync(o_nrm, ctx->stream);
+  CB_TRY(cb_cloud_create_from_device(ctx, o_pts, o_nrm, m, cloud->index_offset, out));
   if (gpu_ms) {
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
     CB_CUDA(cudaEventElapsedTime(gpu_ms, ev.e0, ev.e1));
   }
-  return rc;
+  return CB_OK;
 }
 
 extern "C" int cb_cloud_download(cb_context* ctx, const cb_cloud* cloud, float* xyz, float* normals) {

@@ -334,27 +334,27 @@ inline int grid_blocks(const cb_context* ctx, size_t n, int per_sm = 8) {
 int exclusive_scan_u32(cb_context* ctx, uint32_t* d_data, size_t n, uint32_t total) {
   // d_data has n + 1 entries; on return d_data[i] = sum_{j<i} in[j], d_data[n] = total
   const size_t nblocks = (n + kScanBlock - 1) / kScanBlock;
+  DeviceScope scope(ctx);
   uint32_t* d_sums = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_sums, std::max<size_t>(1, nblocks) * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_sums, nblocks));
   scan_block_kernel<<<(unsigned)nblocks, kThreads, 0, ctx->stream>>>(d_data, n, d_sums);
   scan_sums_kernel<<<1, 1024, 0, ctx->stream>>>(d_sums, nblocks);
   scan_add_kernel<<<(unsigned)nblocks, kThreads, 0, ctx->stream>>>(d_data, n, d_sums, total);
   ctx->launches += 3;
   CB_CUDA(cudaGetLastError());
-  CB_CUDA(cudaFreeAsync(d_sums, ctx->stream));
   return CB_OK;
 }
 
 int points_bbox(cb_context* ctx, const float* d_raw, size_t n, float mn[3], float mx[3]) {
+  DeviceScope scope(ctx);
   int* d_bb = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_bb, 6 * sizeof(int), ctx->stream));
+  CB_TRY(scope.alloc(&d_bb, 6));
   bbox_init_kernel<<<1, 32, 0, ctx->stream>>>(d_bb);
   bbox_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_raw, n, d_bb);
   ctx->launches += 2;
   int h_bb[6];
   CB_CUDA(cudaMemcpyAsync(h_bb, d_bb, sizeof(h_bb), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_bb, ctx->stream));
   for (int a = 0; a < 3; a++) {
     mn[a] = ordered_to_float(h_bb[a]);
     mx[a] = ordered_to_float(h_bb[3 + a]);
@@ -372,7 +372,7 @@ int ensure_index(cb_cloud* c) {
   if (n == 0) {
     c->nx = c->ny = c->nz = 1;
     c->h = c->inv_h = 1.f;
-    CB_CUDA(cudaMallocAsync(&c->d_cell_start, 2 * sizeof(uint32_t), ctx->stream));
+    CB_TRY(c->mem.alloc(&c->d_cell_start, 2));
     CB_CUDA(cudaMemsetAsync(c->d_cell_start, 0, 2 * sizeof(uint32_t), ctx->stream));
     c->indexed = true;
     return CB_OK;
@@ -390,11 +390,14 @@ int ensure_index(cb_cloud* c) {
   m0 = std::min<double>(std::max(m0, 1.0), kMaxDim);
   double h = max_ext / m0;
 
+  // Scratch in `scope`; the index arrays in c->mem, so a failure leaves the cloud as it was (not indexed,
+  // nothing allocated: every buffer of a failed attempt is freed with its scope or the cloud).
+  DeviceScope scope(ctx);
   uint32_t* d_cell_id = nullptr;
-  uint32_t* d_hist = nullptr;
+  uint32_t* d_hist = nullptr;  // becomes the cell_start of the index
   unsigned long long* d_stats = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_cell_id, n * sizeof(uint32_t), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_stats, 2 * sizeof(unsigned long long), ctx->stream));
+  CB_TRY(scope.alloc(&d_cell_id, n));
+  CB_TRY(scope.alloc(&d_stats, 2));
   GridParams gp;
   size_t ncells = 0;
   double mean_occ = 0;
@@ -423,8 +426,8 @@ int ensure_index(cb_cloud* c) {
     gp.ny = dims[1];
     gp.nz = dims[2];
     ncells = (size_t)dims[0] * dims[1] * dims[2];
-    if (d_hist) CB_CUDA(cudaFreeAsync(d_hist, ctx->stream));
-    CB_CUDA(cudaMallocAsync(&d_hist, (ncells + 1) * sizeof(uint32_t), ctx->stream));
+    CB_TRY(scope.free(d_hist));
+    CB_TRY(scope.alloc(&d_hist, ncells + 1));
     CB_CUDA(cudaMemsetAsync(d_hist, 0, (ncells + 1) * sizeof(uint32_t), ctx->stream));
     CB_CUDA(cudaMemsetAsync(d_stats, 0, 2 * sizeof(unsigned long long), ctx->stream));
     hist_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(c->d_raw, n, gp, d_cell_id, d_hist);
@@ -462,52 +465,51 @@ int ensure_index(cb_cloud* c) {
   uint32_t* d_perm = nullptr;
   uint32_t* d_big = nullptr;
   uint32_t* d_tmp = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_cursor, ncells * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_cursor, ncells));
   CB_CUDA(cudaMemsetAsync(d_cursor, 0, ncells * sizeof(uint32_t), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_perm, n * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_perm, n));
   const size_t big_cap = n / kBigCell + 2;
-  CB_CUDA(cudaMallocAsync(&d_big, (big_cap + 1) * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_big, big_cap + 1));
   CB_CUDA(cudaMemsetAsync(d_big, 0, sizeof(uint32_t), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_tmp, n * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_tmp, n));
   scatter_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_cell_id, n, d_hist, d_cursor, d_perm);
   sort_small_cells_kernel<<<grid_blocks(ctx, ncells), kThreads, 0, ctx->stream>>>(d_hist, ncells, d_perm, d_big + 1,
                                                                                  d_big);
   sort_big_cells_kernel<<<ctx->sm_count * 2, kThreads, 0, ctx->stream>>>(d_hist, d_big + 1, d_big, d_perm, d_tmp);
   // 5. gather
-  CB_CUDA(cudaMallocAsync(&c->d_pts, n * sizeof(float4), ctx->stream));
-  if (c->d_raw_nrm) CB_CUDA(cudaMallocAsync(&c->d_nrm, n * sizeof(float4), ctx->stream));
-  gather_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(c->d_raw, c->d_raw_nrm, d_perm, n, c->d_pts,
-                                                                   c->d_nrm);
+  float4 *d_pts = nullptr, *d_nrm = nullptr;
+  CB_TRY(scope.alloc(&d_pts, n));
+  if (c->d_raw_nrm) CB_TRY(scope.alloc(&d_nrm, n));
+  gather_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(c->d_raw, c->d_raw_nrm, d_perm, n, d_pts, d_nrm);
   ctx->launches += 4;
   CB_CUDA(cudaGetLastError());
-  c->d_cell_start = d_hist;  // keeps (ncells + 1) entries; freed with cudaFree in cb_cloud_destroy
   // 6. coarse occupancy: the list of non-empty 8x8x8-cell blocks for the far-query path
+  uint4* d_blocks = nullptr;
   {
     const int bx = (gp.nx + kBlockCells - 1) / kBlockCells, by = (gp.ny + kBlockCells - 1) / kBlockCells,
               bz = (gp.nz + kBlockCells - 1) / kBlockCells;
     const size_t nb = (size_t)bx * by * bz;
     uint32_t* d_cnt = nullptr;
-    CB_CUDA(cudaMallocAsync(&d_cnt, (2 * nb + 2) * sizeof(uint32_t), ctx->stream));
+    CB_TRY(scope.alloc(&d_cnt, 2 * nb + 2));
     uint32_t* d_flag = d_cnt + nb;  // nb + 2 entries
     block_count_kernel<<<grid_blocks(ctx, (nb + 1) * 32), kThreads, 0, ctx->stream>>>(d_hist, gp.nx, gp.ny, gp.nz, bx, by, bz,
                                                                          d_cnt, d_flag);
     CB_TRY(exclusive_scan_u32(ctx, d_flag, nb + 1, 0u));
     // at most min(nb, n) blocks are non-empty: sized without waiting for the count, which is read back at
     // the final synchronise below
-    CB_CUDA(cudaMallocAsync(&c->d_blocks, std::max<size_t>(std::min(nb, n), 1) * sizeof(uint4), ctx->stream));
-    block_emit_kernel<<<grid_blocks(ctx, nb), kThreads, 0, ctx->stream>>>(d_cnt, d_flag, bx, by, bz, c->d_blocks);
+    CB_TRY(scope.alloc(&d_blocks, std::min(nb, n)));
+    block_emit_kernel<<<grid_blocks(ctx, nb), kThreads, 0, ctx->stream>>>(d_cnt, d_flag, bx, by, bz, d_blocks);
     ctx->launches += 2;
     CB_CUDA(cudaGetLastError());
     CB_CUDA(cudaMemcpyAsync(&c->nblocks, d_flag + nb, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaFreeAsync(d_cnt, ctx->stream));
   }
-  CB_CUDA(cudaFreeAsync(d_cell_id, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_stats, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_cursor, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_perm, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_big, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_tmp, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
+  // the index arrays go to the cloud (its scope frees them in cb_cloud_destroy)
+  for (void* p : {(void*)d_hist, (void*)d_pts, (void*)d_nrm, (void*)d_blocks}) scope.move_to(c->mem, p);
+  c->d_cell_start = d_hist;  // (ncells + 1) entries
+  c->d_pts = d_pts;
+  c->d_nrm = d_nrm;
+  c->d_blocks = d_blocks;
   c->indexed = true;
   return CB_OK;
 }

@@ -241,18 +241,14 @@ int launch_pairs_pass(cb_context* ctx, const IcpArgs& a, const EnginePairs& pair
   return CB_OK;
 }
 
-void engine_release_pairs(cb_context* ctx, EnginePairs* pairs) {
-  if (pairs->first) cudaFreeAsync(pairs->first, ctx->stream);
-  if (pairs->second) cudaFreeAsync(pairs->second, ctx->stream);
-  if (pairs->d2) cudaFreeAsync(pairs->d2, ctx->stream);
-  *pairs = EnginePairs();
-}
-
-int engine_find_pairs(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const cb_icp_params* prm,
-                      const float* T12, EnginePairs* pairs) {
+int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const cb_cloud* src,
+                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs) {
   // (with several ranks the caller passes the whole source cloud, replicated: capi_core.cu, ensure_src_full)
   CB_CHECK(prm->search_dir >= CB_SECOND_TO_FIRST && prm->search_dir <= CB_BOTH, CB_ERR_INVALID, "bad search_dir");
-  engine_release_pairs(ctx, pairs);
+  CB_TRY(owner.free(pairs->first));
+  CB_TRY(owner.free(pairs->second));
+  CB_TRY(owner.free(pairs->d2));
+  *pairs = EnginePairs();
   const uint32_t n_src = (uint32_t)src->n, n_dst = (uint32_t)dst->n;
   const bool want_s2f = prm->search_dir != CB_FIRST_TO_SECOND, want_f2s = prm->search_dir != CB_SECOND_TO_FIRST;
   if (n_src == 0 || n_dst == 0) return CB_OK;  // empty trees: no correspondences
@@ -276,33 +272,24 @@ int engine_find_pairs(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src,
     a.out_d2 = s2f_d2;
     CB_TRY(launch_icp_pass(ctx, a, kModeKnn, true, false, false));
   }
-  cb_cloud moved;  // {T src_j}: the reference's src_trans_tree_ (:201-203), rebuilt for this estimate
   if (want_f2s) {
     CB_TRY(dev.alloc(&f2s_idx, n_dst));
     CB_TRY(dev.alloc(&f2s_d2, n_dst));
-    moved.ctx = ctx;
-    moved.n = n_src;
-    CB_CUDA(cudaMallocAsync(&moved.d_raw, 3 * (size_t)n_src * sizeof(float), ctx->stream));
-    int rc = launch_transform_points(ctx, rigid_of(T12), src->d_raw, n_src, moved.d_raw);
-    if (rc == CB_OK) rc = ensure_index(&moved);
-    if (rc == CB_OK) {
-      IcpArgs a;
-      std::memset(&a, 0, sizeof(a));
-      a.dst = grid_view(&moved);
-      a.src_pts = dst->d_pts;
-      a.n_src = n_dst;
-      a.T = rigid_of(nullptr);
-      a.Tin = rigid_of(nullptr);
-      a.max_d2 = prm->max_d2;
-      a.out_idx = f2s_idx;
-      a.out_d2 = f2s_d2;
-      rc = launch_icp_pass(ctx, a, kModeKnn, true, false, false);
-    }
-    if (moved.d_raw) cudaFreeAsync(moved.d_raw, ctx->stream);
-    if (moved.d_pts) cudaFreeAsync(moved.d_pts, ctx->stream);
-    if (moved.d_cell_start) cudaFreeAsync(moved.d_cell_start, ctx->stream);
-    if (moved.d_blocks) cudaFreeAsync(moved.d_blocks, ctx->stream);
-    CB_TRY(rc);
+    cb_cloud moved(ctx, n_src, 0);  // {T src_j}: the reference's src_trans_tree_ (:201-203), rebuilt for this estimate
+    CB_TRY(moved.mem.alloc(&moved.d_raw, 3 * (size_t)n_src));
+    CB_TRY(launch_transform_points(ctx, rigid_of(T12), src->d_raw, n_src, moved.d_raw));
+    CB_TRY(ensure_index(&moved));
+    IcpArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.dst = grid_view(&moved);
+    a.src_pts = dst->d_pts;
+    a.n_src = n_dst;
+    a.T = rigid_of(nullptr);
+    a.Tin = rigid_of(nullptr);
+    a.max_d2 = prm->max_d2;
+    a.out_idx = f2s_idx;
+    a.out_d2 = f2s_d2;
+    CB_TRY(launch_icp_pass(ctx, a, kModeKnn, true, false, false));
   }
   // pre-filter list
   Candidates c;
@@ -364,9 +351,7 @@ int engine_find_pairs(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src,
   pairs->second = b.s[b.cur];
   pairs->d2 = b.d[b.cur];
   pairs->count = m;
-  dev.release(pairs->first);
-  dev.release(pairs->second);
-  dev.release(pairs->d2);
+  for (void* p : {(void*)pairs->first, (void*)pairs->second, (void*)pairs->d2}) dev.move_to(owner, p);
   return CB_OK;
 }
 

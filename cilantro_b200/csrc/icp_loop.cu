@@ -623,10 +623,8 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   const uint64_t launches0 = ctx->launches;
   const int max_iter = std::max(prm->max_iter, 0);
   const int timing = prm->timing;
-  if (!icp->d_state) {
-    CB_CUDA(cudaMalloc(&icp->d_state, sizeof(LoopState)));
-    CB_CUDA(cudaMallocHost(&icp->h_state, sizeof(LoopState)));
-  }
+  if (!icp->d_state) CB_TRY(icp->mem.alloc(&icp->d_state, 1));
+  if (!icp->h_state) CB_TRY(icp->mem.alloc_host(&icp->h_state, 1));
   while (timing != 0 && (int)icp->events.size() < 2 * max_iter) {
     cudaEvent_t e;
     CB_CUDA(cudaEventCreate(&e));
@@ -683,7 +681,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
   const int blocks_cached = std::max(1, std::min(ctx->sm_count * (p2p ? 4 : 3), (int)((ns + kPipeTile - 1) / kPipeTile)));
   CB_TRY(get_reduce_scratch(ctx, blocks_cold, kMaxValues, &a.rs));
-  if (!icp->d_miss_mask) CB_CUDA(cudaMalloc(&icp->d_miss_mask, (ns / 32 + 2) * sizeof(uint32_t)));
+  if (!icp->d_miss_mask) CB_TRY(icp->mem.alloc(&icp->d_miss_mask, ns / 32 + 2));
   a.miss_mask = icp->d_miss_mask;
   Exchange ex;
   std::memset(&ex, 0, sizeof(ex));
@@ -708,7 +706,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   // Batches are enqueued ONE AHEAD of the batch whose state the host is looking at: the device never waits for the host
   // between batches (with several ranks such a gap shows up as a peer wait in the next iteration), and the
   // hand-over / convergence decisions lag by at most one batch. Two pinned copies of LoopState alternate.
-  if (!icp->h_state2) CB_CUDA(cudaMallocHost(&icp->h_state2, sizeof(LoopState)));
+  if (!icp->h_state2) CB_TRY(icp->mem.alloc_host(&icp->h_state2, 1));
   for (int e = 0; e < 2; ++e)
     if (!icp->batch_ev[e]) CB_CUDA(cudaEventCreateWithFlags(&icp->batch_ev[e], cudaEventDisableTiming));
   LoopState* hbuf[2] = {icp->h_state, icp->h_state2};

@@ -35,9 +35,11 @@ struct LoopState {
 }  // namespace cb
 
 struct cb_icp {
+  cb_icp(cb_context* c, const cb_cloud* d, const cb_cloud* s) : ctx(c), dst(d), src(s), mem(c) {}
   cb_context* ctx = nullptr;
   const cb_cloud* dst = nullptr;
   const cb_cloud* src = nullptr;
+  cb::DeviceScope mem;  // every buffer below (device and pinned host)
   float dst_mean[3] = {0, 0, 0};
   float src_mean[3] = {0, 0, 0};
   int* d_nn_pos = nullptr;  // per sorted src point: sorted dst position of its match, -1 none

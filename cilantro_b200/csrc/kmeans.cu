@@ -183,22 +183,14 @@ int kmeans_step(cb_context* ctx, const cb_cloud* pts, const KMeansBuffers& b, co
   return CB_OK;
 }
 
-int alloc_buffers(cb_context* ctx, size_t n, size_t K, KMeansBuffers* b) {
-  CB_CUDA(cudaMalloc(&b->d_cent, std::max<size_t>(K, 1) * sizeof(float4)));
-  CB_CUDA(cudaMalloc(&b->d_labels, std::max<size_t>(n, 1) * sizeof(uint32_t)));
+int alloc_buffers(cb_context* ctx, DeviceScope& scope, size_t n, size_t K, KMeansBuffers* b) {
+  CB_TRY(scope.alloc(&b->d_cent, K));
+  CB_TRY(scope.alloc(&b->d_labels, n));
   CB_CUDA(cudaMemsetAsync(b->d_labels, 0, std::max<size_t>(n, 1) * sizeof(uint32_t), ctx->stream));  // kmeans.hpp:82
-  CB_CUDA(cudaMalloc(&b->d_sums, std::max<size_t>(K, 1) * 4 * sizeof(double)));
-  CB_CUDA(cudaMalloc(&b->d_changed, sizeof(unsigned int)));
-  CB_CUDA(cudaMalloc(&b->d_far, sizeof(unsigned long long)));
+  CB_TRY(scope.alloc(&b->d_sums, std::max<size_t>(K, 1) * 4));
+  CB_TRY(scope.alloc(&b->d_changed, 1));
+  CB_TRY(scope.alloc(&b->d_far, 1));
   return CB_OK;
-}
-
-void free_buffers(KMeansBuffers* b) {
-  if (b->d_cent) cudaFree(b->d_cent);
-  if (b->d_labels) cudaFree(b->d_labels);
-  if (b->d_sums) cudaFree(b->d_sums);
-  if (b->d_changed) cudaFree(b->d_changed);
-  if (b->d_far) cudaFree(b->d_far);
 }
 
 int download_labels(cb_context* ctx, const KMeansBuffers& b, size_t n, uint64_t* labels) {
@@ -235,14 +227,13 @@ int cb_kmeans_assign(cb_context* ctx, const cb_cloud* pts, const float* centroid
                      double* sums, uint64_t* counts) {
   CB_CHECK(ctx && pts && centroids && k > 0, CB_ERR_INVALID, "bad arguments");
   CB_CUDA(cudaSetDevice(ctx->device));
+  DeviceScope scope(ctx);
   KMeansBuffers b;
-  int rc = alloc_buffers(ctx, pts->n, k, &b);
+  CB_TRY(alloc_buffers(ctx, scope, pts->n, k, &b));
   std::vector<double> h_sums;
   bool changed = false;
-  if (rc == CB_OK) rc = kmeans_step(ctx, pts, b, centroids, k, h_sums, &changed);
-  if (rc == CB_OK) rc = download_labels(ctx, b, pts->n, labels);
-  free_buffers(&b);
-  CB_TRY(rc);
+  CB_TRY(kmeans_step(ctx, pts, b, centroids, k, h_sums, &changed));
+  CB_TRY(download_labels(ctx, b, pts->n, labels));
   for (size_t j = 0; j < k; j++) {
     if (sums)
       for (int r = 0; r < 3; r++) sums[3 * j + r] = h_sums[4 * j + r];
@@ -254,31 +245,28 @@ int cb_kmeans_assign(cb_context* ctx, const cb_cloud* pts, const float* centroid
 int cb_kmeans_cluster(cb_context* ctx, const cb_cloud* pts, float* centroids, size_t k, size_t max_iter, float tol,
                       uint64_t* labels, cb_kmeans_result* res) {
   CB_CHECK(ctx && pts && centroids && k > 0, CB_ERR_INVALID, "bad arguments");
-  CB_CHECK(ctx->world == 1 || true, CB_ERR_INVALID, "");
   CB_CUDA(cudaSetDevice(ctx->device));
   const uint64_t launches0 = ctx->launches;
+  DeviceScope scope(ctx);
   KMeansBuffers b;
-  int rc = alloc_buffers(ctx, pts->n, k, &b);
-  if (rc != CB_OK) {
-    free_buffers(&b);
-    return rc;
-  }
+  CB_TRY(alloc_buffers(ctx, scope, pts->n, k, &b));
+  ScopedEvents ev;
+  CB_TRY(ev.create());
   const float tol_sq = tol * tol;
   std::vector<float> old;
   std::vector<double> s;
   size_t it = 0;
-  CB_CUDA(cudaEventRecord(ctx->ev0, ctx->stream));
+  CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
   while (it < max_iter) {
     bool changed = false;
-    rc = kmeans_step(ctx, pts, b, centroids, k, s, &changed);
-    if (rc != CB_OK) break;
+    CB_TRY(kmeans_step(ctx, pts, b, centroids, k, s, &changed));
     if (!changed && it > 0) break;                              // kmeans.hpp:122
     if (tol > 0.f) old.assign(centroids, centroids + 3 * k);   // :123
     // :134-176 empty-cluster repair, on the reduced sums. The farthest-member search is a device
     // reduction; in the sharded case every rank proposes its best and the global best is taken.
     std::vector<double> cnt(k);
     for (size_t j = 0; j < k; j++) cnt[j] = s[4 * j + 3];
-    for (size_t i = 0; i < k && rc == CB_OK; i++) {
+    for (size_t i = 0; i < k; i++) {
       if (cnt[i] != 0.0) continue;
       size_t max_ind = 0;
       for (size_t j = 1; j < k; j++)
@@ -288,34 +276,29 @@ int cb_kmeans_cluster(cb_context* ctx, const cb_cloud* pts, float* centroids, si
       const float oc[3] = {(float)s[4 * max_ind] * inv, (float)s[4 * max_ind + 1] * inv, (float)s[4 * max_ind + 2] * inv};
       if (ctx->world > 1) {
         set_error("empty-cluster repair is not implemented for sharded k-means");
-        rc = CB_ERR_UNSUPPORTED;
-        break;
+        return CB_ERR_UNSUPPORTED;
       }
-      cudaMemsetAsync(b.d_far, 0, sizeof(unsigned long long), ctx->stream);
+      CB_CUDA(cudaMemsetAsync(b.d_far, 0, sizeof(unsigned long long), ctx->stream));
       const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (pts->n + 255) / 256));
       farthest_member_kernel<<<blocks, 256, 0, ctx->stream>>>(pts->d_raw, pts->n, b.d_labels, (uint32_t)max_ind, oc[0],
                                                               oc[1], oc[2], b.d_far);
       ctx->launches += 1;
+      CB_CUDA(cudaGetLastError());
       unsigned long long key = 0;
-      cudaMemcpyAsync(&key, b.d_far, sizeof(key), cudaMemcpyDeviceToHost, ctx->stream);
-      if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-        set_error("farthest_member_kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-        rc = CB_ERR_CUDA;
-        break;
-      }
+      CB_CUDA(cudaMemcpyAsync(&key, b.d_far, sizeof(key), cudaMemcpyDeviceToHost, ctx->stream));
+      CB_CUDA(cudaStreamSynchronize(ctx->stream));
       if (!key) continue;  // cannot happen: the largest cluster has members
       const uint32_t far_idx = 0xffffffffu - (uint32_t)(key & 0xffffffffull);
       // move the point to cluster i (:172-175); note the reference does NOT add it to cluster i's sum
       const uint32_t new_label = (uint32_t)i;
-      cudaMemcpyAsync(b.d_labels + far_idx, &new_label, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream);
+      CB_CUDA(cudaMemcpyAsync(b.d_labels + far_idx, &new_label, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
       float p[3];
-      cudaMemcpyAsync(p, pts->d_raw + 3 * (size_t)far_idx, sizeof(p), cudaMemcpyDeviceToHost, ctx->stream);
-      cudaStreamSynchronize(ctx->stream);
+      CB_CUDA(cudaMemcpyAsync(p, pts->d_raw + 3 * (size_t)far_idx, sizeof(p), cudaMemcpyDeviceToHost, ctx->stream));
+      CB_CUDA(cudaStreamSynchronize(ctx->stream));
       for (int r = 0; r < 3; r++) s[4 * max_ind + r] -= (double)p[r];
       cnt[max_ind] -= 1.0;
       cnt[i] += 1.0;
     }
-    if (rc != CB_OK) break;
     for (size_t j = 0; j < k; j++) {  // :179-181  centroid = sum * (1 / count)
       const float inv = 1.0f / (float)cnt[j];
       for (int r = 0; r < 3; r++) centroids[3 * j + r] = (float)s[4 * j + r] * inv;
@@ -331,20 +314,17 @@ int cb_kmeans_cluster(cb_context* ctx, const cb_cloud* pts, float* centroids, si
       if (mx < tol_sq) break;
     }
   }
-  if (rc == CB_OK) {
-    cudaEventRecord(ctx->ev1, ctx->stream);
-    rc = download_labels(ctx, b, pts->n, labels);
-    cudaStreamSynchronize(ctx->stream);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-    if (res) {
-      res->iterations = it;
-      res->gpu_ms_total = ms;
-      res->kernel_launches = ctx->launches - launches0;
-    }
+  CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
+  CB_TRY(download_labels(ctx, b, pts->n, labels));
+  CB_CUDA(cudaStreamSynchronize(ctx->stream));
+  float ms = 0.f;
+  CB_CUDA(cudaEventElapsedTime(&ms, ev.e0, ev.e1));
+  if (res) {
+    res->iterations = it;
+    res->gpu_ms_total = ms;
+    res->kernel_launches = ctx->launches - launches0;
   }
-  free_buffers(&b);
-  return rc;
+  return CB_OK;
 }
 
 }  // extern "C"

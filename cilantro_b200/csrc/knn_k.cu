@@ -64,12 +64,13 @@ extern "C" int cb_knn_radius(cb_context* ctx, const cb_cloud* ref, const cb_clou
   const size_t nq = qry->n;
   if (nq == 0) return CB_OK;
   const Rigid T = rigid_from_t12(T12);
+  DeviceScope scope(ctx);
   int* d_idx = nullptr;
   float* d_d2 = nullptr;
   uint32_t* d_cnt = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_idx, nq * k * sizeof(int), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_d2, nq * k * sizeof(float), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_cnt, nq * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_idx, nq * k));
+  CB_TRY(scope.alloc(&d_d2, nq * k));
+  CB_TRY(scope.alloc(&d_cnt, nq));
   const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (nq + kBlock - 1) / kBlock));
   const GridView g = grid_view(ref);
   if (k <= 4)
@@ -90,9 +91,6 @@ extern "C" int cb_knn_radius(cb_context* ctx, const cb_cloud* ref, const cb_clou
   CB_CUDA(cudaMemcpyAsync(h_idx.data(), d_idx, nq * k * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaMemcpyAsync(d2, d_d2, nq * k * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   if (counts) CB_CUDA(cudaMemcpyAsync(counts, d_cnt, nq * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_idx, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_d2, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_cnt, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   for (size_t i = 0; i < nq * k; i++) idx[i] = h_idx[i] < 0 ? -1 : (int64_t)h_idx[i] + (int64_t)ref->index_offset;
   return CB_OK;
@@ -113,8 +111,9 @@ extern "C" int cb_radius_search(cb_context* ctx, const cb_cloud* ref, const cb_c
   offsets[0] = 0;
   if (nq == 0) return CB_OK;
   const Rigid T = rigid_from_t12(T12);
+  DeviceScope scope(ctx);
   uint32_t* d_off = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_off, (nq + 2) * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_off, nq + 2));
   CB_CUDA(cudaMemsetAsync(d_off, 0, (nq + 2) * sizeof(uint32_t), ctx->stream));
   const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (nq + kBlock - 1) / kBlock));
   const GridView g = grid_view(ref);
@@ -132,19 +131,14 @@ extern "C" int cb_radius_search(cb_context* ctx, const cb_cloud* ref, const cb_c
   }
   offsets[nq] = sum;
   *total = (size_t)sum;
-  if (sum == 0 || !idx || !d2 || capacity < sum) {
-    CB_CUDA(cudaFreeAsync(d_off, ctx->stream));
+  if (sum == 0 || !idx || !d2 || capacity < sum)
     return CB_OK;  // sizing call, or the caller's buffers are too small: *total says what is needed
-  }
-  if (sum >= (1ull << 32)) {
-    cudaFreeAsync(d_off, ctx->stream);
-    CB_CHECK(false, CB_ERR_UNSUPPORTED, "radius search: more than 2^32 - 1 neighbour pairs in one call");
-  }
+  CB_CHECK(sum < (1ull << 32), CB_ERR_UNSUPPORTED, "radius search: more than 2^32 - 1 neighbour pairs in one call");
   CB_TRY(exclusive_scan_u32(ctx, d_off, nq + 1, 0u));
   int* d_idx = nullptr;
   float* d_d2 = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_idx, sum * sizeof(int), ctx->stream));
-  CB_CUDA(cudaMallocAsync(&d_d2, sum * sizeof(float), ctx->stream));
+  CB_TRY(scope.alloc(&d_idx, sum));
+  CB_TRY(scope.alloc(&d_d2, sum));
   radius_kernel<true><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, radius2, nullptr, d_off, d_idx,
                                                          d_d2);
   segment_heapsort_kernel<<<blocks, kBlock, 0, ctx->stream>>>(d_off, (uint32_t)nq, d_idx, d_d2);
@@ -153,9 +147,6 @@ extern "C" int cb_radius_search(cb_context* ctx, const cb_cloud* ref, const cb_c
   std::vector<int> h_idx(sum);
   CB_CUDA(cudaMemcpyAsync(h_idx.data(), d_idx, sum * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaMemcpyAsync(d2, d_d2, sum * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_idx, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_d2, ctx->stream));
-  CB_CUDA(cudaFreeAsync(d_off, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   for (size_t i = 0; i < sum; i++) idx[i] = (int64_t)h_idx[i] + (int64_t)ref->index_offset;
   return CB_OK;

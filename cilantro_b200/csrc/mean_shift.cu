@@ -386,12 +386,8 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
       while (b1 < n_act && pairs + h_cnt[b1] <= budget) pairs += h_cnt[b1++];
       const uint32_t nb = b1 - b0;
       if (pairs > pair_cap) {
-        if (d_idx) {
-          scope.release(d_idx);
-          scope.release(d_d2);
-          CB_CUDA(cudaFreeAsync(d_idx, ctx->stream));
-          CB_CUDA(cudaFreeAsync(d_d2, ctx->stream));
-        }
+        CB_TRY(scope.free(d_idx));
+        CB_TRY(scope.free(d_d2));
         pair_cap = std::max<uint64_t>(pairs, std::min<uint64_t>(budget, 2 * pair_cap));
         CB_TRY(scope.alloc(&d_idx, pair_cap));
         CB_TRY(scope.alloc(&d_d2, pair_cap));

@@ -230,12 +230,13 @@ extern "C" int cb_cloud_estimate_normals(cb_context* ctx, cb_cloud* cloud, int k
   if (n == 0) return CB_OK;
   CB_TRY(ensure_index(cloud));
   const bool use_ref = use_current_as_ref && cloud->d_nrm;  // like PointCloud: only when normals exist
-  if (!cloud->d_raw_nrm) CB_CUDA(cudaMallocAsync(&cloud->d_raw_nrm, 3 * n * sizeof(float), ctx->stream));
-  if (!cloud->d_nrm) CB_CUDA(cudaMallocAsync(&cloud->d_nrm, n * sizeof(float4), ctx->stream));
+  if (!cloud->d_raw_nrm) CB_TRY(cloud->mem.alloc(&cloud->d_raw_nrm, 3 * n));
+  if (!cloud->d_nrm) CB_TRY(cloud->mem.alloc(&cloud->d_nrm, n));
+  DeviceScope scope(ctx);
   float* d_curv = nullptr;
   float* d_cov = nullptr;
-  if (curvature) CB_CUDA(cudaMallocAsync(&d_curv, n * sizeof(float), ctx->stream));
-  if (cov6) CB_CUDA(cudaMallocAsync(&d_cov, 6 * n * sizeof(float), ctx->stream));
+  if (curvature) CB_TRY(scope.alloc(&d_curv, n));
+  if (cov6) CB_TRY(scope.alloc(&d_cov, 6 * n));
   NormalOut o;
   o.raw_nrm = cloud->d_raw_nrm;
   o.nrm = cloud->d_nrm;
@@ -279,8 +280,6 @@ extern "C" int cb_cloud_estimate_normals(cb_context* ctx, cb_cloud* cloud, int k
   if (curvature)
     CB_CUDA(cudaMemcpyAsync(curvature, d_curv, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   if (cov6) CB_CUDA(cudaMemcpyAsync(cov6, d_cov, 6 * n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-  if (d_curv) CB_CUDA(cudaFreeAsync(d_curv, ctx->stream));
-  if (d_cov) CB_CUDA(cudaFreeAsync(d_cov, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (gpu_ms) CB_CUDA(cudaEventElapsedTime(gpu_ms, ev.e0, ev.e1));
   return CB_OK;

@@ -95,8 +95,9 @@ int radix_sort_pairs_u64(cb_context* ctx, uint64_t* d_keys, uint32_t* d_vals, ui
   CB_CHECK(n < (1ull << 32), CB_ERR_INVALID, "radix sort: more than 2^32 - 1 elements");
   const uint32_t ntiles = (uint32_t)((n + kTile - 1) / kTile);
   const size_t hn = (size_t)kDigits * ntiles;
+  DeviceScope scope(ctx);
   uint32_t* d_hist = nullptr;
-  CB_CUDA(cudaMallocAsync(&d_hist, (hn + 1) * sizeof(uint32_t), ctx->stream));
+  CB_TRY(scope.alloc(&d_hist, hn + 1));
   uint64_t* kin = d_keys;
   uint32_t* vin = d_vals;
   uint64_t* kout = d_keys_tmp;
@@ -117,7 +118,6 @@ int radix_sort_pairs_u64(cb_context* ctx, uint64_t* d_keys, uint32_t* d_vals, ui
     CB_CUDA(cudaMemcpyAsync(d_keys, kin, n * sizeof(uint64_t), cudaMemcpyDeviceToDevice, ctx->stream));
     CB_CUDA(cudaMemcpyAsync(d_vals, vin, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
   }
-  CB_CUDA(cudaFreeAsync(d_hist, ctx->stream));
   return CB_OK;
 }
 

@@ -181,13 +181,13 @@ int score_batch(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const
   ctx->launches += 1;
   CB_CUDA(cudaGetLastError());
   if (ctx->world > 1) {
+    DeviceScope scope(ctx);
     double* d_tmp = nullptr;
-    CB_CUDA(cudaMallocAsync(&d_tmp, (size_t)H * sizeof(double), ctx->stream));
+    CB_TRY(scope.alloc(&d_tmp, (size_t)H));
     u32_to_f64_kernel<<<(H + 255) / 256, 256, 0, ctx->stream>>>(d_counts, d_tmp, H);
     CB_TRY(nccl_allreduce_sum_f64(ctx, d_tmp, (size_t)H));
     f64_to_u32_kernel<<<(H + 255) / 256, 256, 0, ctx->stream>>>(d_tmp, d_counts, H);
     ctx->launches += 2;
-    CB_CUDA(cudaFreeAsync(d_tmp, ctx->stream));
   }
   return CB_OK;
 }
@@ -219,26 +219,20 @@ int cb_ransac_score(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, c
   CB_TRY(check_pair(ctx, dst, src));
   CB_CHECK(H == 0 || (T_h && counts), CB_ERR_INVALID, "null argument");
   const float x_max = sqrt_threshold(thresh);
+  DeviceScope scope(ctx);
   float* d_T = nullptr;
   uint32_t* d_counts = nullptr;
-  const size_t cap = std::min<size_t>(std::max<size_t>(H, 1), kMaxBatch);
-  CB_CUDA(cudaMalloc(&d_T, cap * 12 * sizeof(float)));
-  CB_CUDA(cudaMalloc(&d_counts, cap * sizeof(uint32_t)));
-  int rc = CB_OK;
-  for (size_t h0 = 0; h0 < H && rc == CB_OK; h0 += kMaxBatch) {
+  const size_t cap = std::min<size_t>(H, kMaxBatch);
+  CB_TRY(scope.alloc(&d_T, cap * 12));
+  CB_TRY(scope.alloc(&d_counts, cap));
+  for (size_t h0 = 0; h0 < H; h0 += kMaxBatch) {
     const int hn = (int)std::min<size_t>(kMaxBatch, H - h0);
-    cudaMemcpyAsync(d_T, T_h + 12 * h0, (size_t)hn * 12 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
-    rc = score_batch(ctx, dst, src, d_T, hn, x_max, d_counts);
-    if (rc != CB_OK) break;
-    cudaMemcpyAsync(counts + h0, d_counts, (size_t)hn * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
-    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-      set_error("ransac_score_kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-      rc = CB_ERR_CUDA;
-    }
+    CB_CUDA(cudaMemcpyAsync(d_T, T_h + 12 * h0, (size_t)hn * 12 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CB_TRY(score_batch(ctx, dst, src, d_T, hn, x_max, d_counts));
+    CB_CUDA(cudaMemcpyAsync(counts + h0, d_counts, (size_t)hn * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
   }
-  cudaFree(d_T);
-  cudaFree(d_counts);
-  return rc;
+  return CB_OK;
 }
 
 int cb_ransac_residuals(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const float* T12, float thresh,
@@ -248,11 +242,11 @@ int cb_ransac_residuals(cb_context* ctx, const cb_cloud* dst, const cb_cloud* sr
   const size_t n = dst->n;
   std::vector<float> h(n);
   if (n) {
+    DeviceScope scope(ctx);
     float* d_out = nullptr;
-    CB_CUDA(cudaMallocAsync(&d_out, n * sizeof(float), ctx->stream));
+    CB_TRY(scope.alloc(&d_out, n));
     CB_TRY(residuals_device(ctx, dst, src, T12, d_out));
     CB_CUDA(cudaMemcpyAsync(h.data(), d_out, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaFreeAsync(d_out, ctx->stream));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
   }
   size_t k = 0;
@@ -288,34 +282,32 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
   bool have_best = false, done = false;
 
   const size_t B = 1024;  // hypotheses generated and scored per round trip
+  DeviceScope scope(ctx);
   float* d_T = nullptr;
   uint32_t* d_counts = nullptr;
   uint32_t* d_idx = nullptr;
   float* d_pairs = nullptr;
-  CB_CUDA(cudaMalloc(&d_T, B * 12 * sizeof(float)));
-  CB_CUDA(cudaMalloc(&d_counts, B * sizeof(uint32_t)));
-  CB_CUDA(cudaMalloc(&d_idx, B * 3 * sizeof(uint32_t)));
-  CB_CUDA(cudaMalloc(&d_pairs, B * 3 * 6 * sizeof(float)));
+  CB_TRY(scope.alloc(&d_T, B * 12));
+  CB_TRY(scope.alloc(&d_counts, B));
+  CB_TRY(scope.alloc(&d_idx, B * 3));
+  CB_TRY(scope.alloc(&d_pairs, B * 3 * 6));
   std::vector<uint32_t> h_idx(B * 3), h_counts(B);
   std::vector<float> h_pairs(B * 18), h_T(B * 12);
-  int rc = CB_OK;
-  cudaEventRecord(ctx->ev0, ctx->stream);
-  while (!done && it < max_iter && rc == CB_OK) {
+  ScopedEvents ev;
+  CB_TRY(ev.create());
+  CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
+  while (!done && it < max_iter) {
     const size_t nb = std::min(B, max_iter - it);
     // sample (:83-91): partial Fisher-Yates on a permutation that persists across hypotheses
     for (size_t b = 0; b < nb; b++) sampler.next(sample_size, &h_idx[b * 3]);
     // estimateModel(sample) (:94, ransac_transform_estimator.hpp:72-82): Kabsch on the sample
     if (sample_size > 0) {
-      cudaMemcpyAsync(d_idx, h_idx.data(), nb * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream);
+      CB_CUDA(cudaMemcpyAsync(d_idx, h_idx.data(), nb * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
       gather_pairs_kernel<<<(int)((nb * 3 + 255) / 256), 256, 0, ctx->stream>>>(dst->d_raw, src->d_raw, d_idx, nb * 3,
                                                                               d_pairs);
       ctx->launches += 1;
-      cudaMemcpyAsync(h_pairs.data(), d_pairs, nb * 18 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream);
-      if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-        set_error("gather_pairs_kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-        rc = CB_ERR_CUDA;
-        break;
-      }
+      CB_CUDA(cudaMemcpyAsync(h_pairs.data(), d_pairs, nb * 18 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+      CB_CUDA(cudaStreamSynchronize(ctx->stream));
     }
     for (size_t b = 0; b < nb; b++) {
       double m[16] = {0};
@@ -330,15 +322,10 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
       }
       kabsch_from_moments(m, &h_T[b * 12]);
     }
-    cudaMemcpyAsync(d_T, h_T.data(), nb * 12 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
-    rc = score_batch(ctx, dst, src, d_T, (int)nb, x_max, d_counts);
-    if (rc != CB_OK) break;
-    cudaMemcpyAsync(h_counts.data(), d_counts, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream);
-    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-      set_error("ransac_score_kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-      rc = CB_ERR_CUDA;
-      break;
-    }
+    CB_CUDA(cudaMemcpyAsync(d_T, h_T.data(), nb * 12 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CB_TRY(score_batch(ctx, dst, src, d_T, (int)nb, x_max, d_counts));
+    CB_CUDA(cudaMemcpyAsync(h_counts.data(), d_counts, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
     // sequential semantics over the batch (:103-114)
     for (size_t b = 0; b < nb; b++) {
       it++;
@@ -358,42 +345,31 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
   }
   // no hypothesis ever reached sample_size inliers: model_inliers_ is empty, so the re-estimation
   // is a Kabsch over zero pairs = identity (transform_estimation.hpp:20-23)
-  if (rc == CB_OK && re_estimate && have_best) {  // :118-128
+  if (re_estimate && have_best) {  // :118-128
     const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 4, (n + kReduceBlock - 1) / kReduceBlock));
     ReduceScratch rs;
     CB_TRY(get_reduce_scratch(ctx, blocks, 16, &rs));
     inlier_moments_kernel<<<blocks, kReduceBlock, 0, ctx->stream>>>(dst->d_raw, src->d_raw, n, rigid_of(best_T), x_max, rs);
     ctx->launches += 1;
     double m[16];
-    cudaMemcpyAsync(ctx->h_result, ctx->d_result, sizeof(m), cudaMemcpyDeviceToHost, ctx->stream);
-    if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-      set_error("inlier_moments_kernel failed: %s", cudaGetErrorString(cudaGetLastError()));
-      rc = CB_ERR_CUDA;
-    } else {
-      std::memcpy(m, ctx->h_result, sizeof(m));
-      kabsch_from_moments(m, best_T);
-    }
+    CB_CUDA(cudaMemcpyAsync(ctx->h_result, ctx->d_result, sizeof(m), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    std::memcpy(m, ctx->h_result, sizeof(m));
+    kabsch_from_moments(m, best_T);
   }
   size_t n_inl = best_count;
-  if (rc == CB_OK) {
-    cudaEventRecord(ctx->ev1, ctx->stream);
-    rc = cb_ransac_residuals(ctx, dst, src, best_T, thresh, residuals, inliers, &n_inl);
-  }
-  if (rc == CB_OK) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
-    std::memcpy(res->T, best_T, sizeof(best_T));
-    res->iterations = it;
-    res->num_inliers = n_inl;
-    res->best_iteration = best_it;
-    res->gpu_ms_total = ms;
-    res->kernel_launches = ctx->launches - launches0;
-  }
-  cudaFree(d_T);
-  cudaFree(d_counts);
-  cudaFree(d_idx);
-  cudaFree(d_pairs);
-  return rc;
+  CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
+  CB_TRY(cb_ransac_residuals(ctx, dst, src, best_T, thresh, residuals, inliers, &n_inl));
+  CB_CUDA(cudaEventSynchronize(ev.e1));  // (cb_ransac_residuals does not synchronise an empty cloud)
+  float ms = 0.f;
+  CB_CUDA(cudaEventElapsedTime(&ms, ev.e0, ev.e1));
+  std::memcpy(res->T, best_T, sizeof(best_T));
+  res->iterations = it;
+  res->num_inliers = n_inl;
+  res->best_iteration = best_it;
+  res->gpu_ms_total = ms;
+  res->kernel_launches = ctx->launches - launches0;
+  return CB_OK;
 }
 
 }  // extern "C"

@@ -349,6 +349,8 @@ int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_
 
   Events ev;
   CB_TRY(ev.create());
+  ScopedEvents total;
+  CB_TRY(total.create());
   DeviceScope scope(ctx);
   uint32_t* d_idx = nullptr;
   float4* d_planes = nullptr;
@@ -358,7 +360,7 @@ int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_
   CB_TRY(scope.alloc(&d_counts, kMaxBatch));
   std::vector<uint32_t> h_idx(3 * (size_t)kMaxBatch, 0u), h_counts(kMaxBatch);
   std::vector<float> h_planes(4 * (size_t)kMaxBatch);
-  CB_CUDA(cudaEventRecord(ctx->ev0, ctx->stream));
+  CB_CUDA(cudaEventRecord(total.e0, ctx->stream));
   size_t batch = kFirstBatch;
   // Batches grow geometrically: an early exit wastes at most as many hypotheses as already ran, and a run without
   // an early exit soon scores full batches.
@@ -410,11 +412,11 @@ int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_
   CB_CUDA(cudaEventRecord(ev.e[3], ctx->stream));
   CB_TRY(residuals_and_inliers(ctx, cloud, plane, thresh, residuals, inliers, &n_inl));
   CB_CUDA(cudaEventRecord(ev.e[4], ctx->stream));
-  CB_CUDA(cudaEventRecord(ctx->ev1, ctx->stream));
-  CB_CUDA(cudaEventSynchronize(ctx->ev1));
+  CB_CUDA(cudaEventRecord(total.e1, ctx->stream));
+  CB_CUDA(cudaEventSynchronize(total.e1));
   ms_final = ev.ms(3, 4);
   float ms = 0.f;
-  cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
+  CB_CUDA(cudaEventElapsedTime(&ms, total.e0, total.e1));
   std::memcpy(res->plane, plane, sizeof(plane));
   std::memcpy(res->hyp_plane, best, sizeof(best));
   res->iterations = it;

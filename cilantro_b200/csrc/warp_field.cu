@@ -35,8 +35,14 @@
 using namespace cb;
 namespace cg = cooperative_groups;
 
+namespace {
+struct WarpStats;
+}
+
 struct cb_warp_icp {
+  explicit cb_warp_icp(cb_context* c) : ctx(c), mem(c) {}
   cb_context* ctx = nullptr;
+  cb::DeviceScope mem;  // every buffer below (device and pinned host)
   const cb_cloud* dst = nullptr;
   const cb_cloud* src = nullptr;
   uint32_t n = 0;        // source points
@@ -60,8 +66,8 @@ struct cb_warp_icp {
   int* d_nn = nullptr;        // [n] last search: dst index or -1
   float* d_nn_d2 = nullptr;
   double* d_part = nullptr;   // CG reduction partials [5][grid]
-  void* d_stats = nullptr;
-  void* h_stats = nullptr;    // pinned
+  WarpStats* d_stats = nullptr;
+  WarpStats* h_stats = nullptr;  // pinned
   int cg_grid = 0;
   bool have_corr = false;
 };
@@ -754,6 +760,67 @@ void cb_warp_default_params(cb_warp_params* p) {
   p->inlier_fraction = 1.0;
 }
 
+// Device buffers of a new warp-field ICP object: arcs (lo, hi, d2) uploaded and their incidence sorted by point.
+static int warp_init(cb_warp_icp* w, const std::vector<uint32_t>& lo, const std::vector<uint32_t>& hi,
+                     const std::vector<float>& d2) {
+  cb_context* ctx = w->ctx;
+  const uint32_t n = w->n;
+  const size_t nn = std::max<size_t>(n, 1), m = std::max<size_t>(w->n_arcs, 1);
+  cudaStream_t s = ctx->stream;
+  CB_TRY(w->mem.alloc(&w->d_arc_lo, m));
+  CB_TRY(w->mem.alloc(&w->d_arc_hi, m));
+  CB_TRY(w->mem.alloc(&w->d_arc_d2, m));
+  CB_TRY(w->mem.alloc(&w->d_arc_c, 6 * m));
+  CB_TRY(w->mem.alloc(&w->d_inc_off, nn + 1));
+  CB_TRY(w->mem.alloc(&w->d_inc_arc, 2 * m));
+  CB_TRY(w->mem.alloc(&w->d_inc_other, 2 * m));
+  CB_TRY(w->mem.alloc(&w->d_T, 12 * nn));
+  CB_TRY(w->mem.alloc(&w->d_warped, nn));
+  CB_TRY(w->mem.alloc(&w->d_xs, 6 * nn));
+  CB_TRY(w->mem.alloc(&w->d_B, 21 * nn));
+  CB_TRY(w->mem.alloc(&w->d_b, 6 * nn));
+  CB_TRY(w->mem.alloc(&w->d_inv, 6 * nn));
+  CB_TRY(w->mem.alloc(&w->d_vec, 30 * nn));
+  CB_TRY(w->mem.alloc(&w->d_nn, nn));
+  CB_TRY(w->mem.alloc(&w->d_nn_d2, nn));
+  CB_TRY(w->mem.alloc(&w->d_stats, 1));
+  CB_TRY(w->mem.alloc_host(&w->h_stats, 1));
+  // cooperative grid: every block resident (occupancy API), no more blocks than points need
+  int per_sm = 0;
+  CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, warp_cg_kernel, kBlock, 0));
+  CB_CHECK(per_sm >= 1, CB_ERR_CUDA, "the CG kernel cannot be resident");
+  w->cg_grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (nn + kBlock - 1) / kBlock));
+  CB_TRY(w->mem.alloc(&w->d_part, 5 * (size_t)w->cg_grid));
+  const uint32_t m32 = w->n_arcs, total = 2 * m32;
+  if (m32) {
+    CB_CUDA(cudaMemcpyAsync(w->d_arc_lo, lo.data(), m32 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CB_CUDA(cudaMemcpyAsync(w->d_arc_hi, hi.data(), m32 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CB_CUDA(cudaMemcpyAsync(w->d_arc_d2, d2.data(), m32 * sizeof(float), cudaMemcpyHostToDevice, s));
+  }
+  DeviceScope scope(ctx);
+  uint64_t *keys = nullptr, *keys_tmp = nullptr;
+  uint32_t *vals = nullptr, *vals_tmp = nullptr;
+  CB_TRY(scope.alloc(&keys, total));
+  CB_TRY(scope.alloc(&keys_tmp, total));
+  CB_TRY(scope.alloc(&vals, total));
+  CB_TRY(scope.alloc(&vals_tmp, total));
+  if (m32) {
+    incidence_keys_kernel<<<grid_for(ctx, m32), kBlock, 0, s>>>(w->d_arc_lo, w->d_arc_hi, m32, keys, vals);
+    ctx->launches += 1;
+    CB_CUDA(cudaGetLastError());
+    int bits = 1;
+    while (bits < 32 && (1ull << bits) < (uint64_t)nn) bits++;
+    CB_TRY(radix_sort_pairs_u64(ctx, keys, vals, keys_tmp, vals_tmp, total, bits));
+  }
+  incidence_fill_kernel<<<grid_for(ctx, (size_t)total + 1), kBlock, 0, s>>>(keys, vals, total, n, w->d_arc_lo,
+                                                                           w->d_arc_hi, w->d_inc_arc, w->d_inc_other,
+                                                                           w->d_inc_off);
+  ctx->launches += 1;
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaStreamSynchronize(s));
+  return CB_OK;
+}
+
 int cb_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const uint64_t* reg_offsets,
                        const int64_t* reg_index, const float* reg_value, size_t n_reg, cb_warp_icp** out) {
   CB_CHECK(ctx && dst && src && out, CB_ERR_INVALID, "null argument");
@@ -794,70 +861,14 @@ int cb_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src
   CB_CHECK(lo.size() < 0x7fffffffull, CB_ERR_UNSUPPORTED, "too many regularisation arcs (2^31 - 1 at most)");
   CB_CUDA(cudaSetDevice(ctx->device));
   CB_TRY(ensure_index(const_cast<cb_cloud*>(dst)));
-  cb_warp_icp* w = new cb_warp_icp;
-  w->ctx = ctx;
+  cb_warp_icp* w = new cb_warp_icp(ctx);
   w->dst = dst;
   w->src = src;
   w->n = n;
   w->n_arcs = (uint32_t)lo.size();
-  int rc = [&]() -> int {
-    const size_t nn = std::max<size_t>(n, 1), m = std::max<size_t>(w->n_arcs, 1);
-    cudaStream_t s = ctx->stream;
-    CB_CUDA(cudaMallocAsync(&w->d_arc_lo, m * sizeof(uint32_t), s));
-    CB_CUDA(cudaMallocAsync(&w->d_arc_hi, m * sizeof(uint32_t), s));
-    CB_CUDA(cudaMallocAsync(&w->d_arc_d2, m * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_arc_c, 6 * m * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_inc_off, (nn + 1) * sizeof(uint32_t), s));
-    CB_CUDA(cudaMallocAsync(&w->d_inc_arc, 2 * m * sizeof(uint32_t), s));
-    CB_CUDA(cudaMallocAsync(&w->d_inc_other, 2 * m * sizeof(uint32_t), s));
-    CB_CUDA(cudaMallocAsync(&w->d_T, 12 * nn * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_warped, nn * sizeof(float4), s));
-    CB_CUDA(cudaMallocAsync(&w->d_xs, 6 * nn * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_B, 21 * nn * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_b, 6 * nn * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_inv, 6 * nn * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_vec, 30 * nn * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_nn, nn * sizeof(int), s));
-    CB_CUDA(cudaMallocAsync(&w->d_nn_d2, nn * sizeof(float), s));
-    CB_CUDA(cudaMallocAsync(&w->d_stats, sizeof(WarpStats), s));
-    CB_CUDA(cudaMallocHost(&w->h_stats, sizeof(WarpStats)));
-    // cooperative grid: every block resident (occupancy API), no more blocks than points need
-    int per_sm = 0;
-    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, warp_cg_kernel, kBlock, 0));
-    CB_CHECK(per_sm >= 1, CB_ERR_CUDA, "the CG kernel cannot be resident");
-    w->cg_grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (nn + kBlock - 1) / kBlock));
-    CB_CUDA(cudaMallocAsync(&w->d_part, 5 * (size_t)w->cg_grid * sizeof(double), s));
-    const uint32_t m32 = w->n_arcs, total = 2 * m32;
-    if (m32) {
-      CB_CUDA(cudaMemcpyAsync(w->d_arc_lo, lo.data(), m32 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-      CB_CUDA(cudaMemcpyAsync(w->d_arc_hi, hi.data(), m32 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-      CB_CUDA(cudaMemcpyAsync(w->d_arc_d2, d2.data(), m32 * sizeof(float), cudaMemcpyHostToDevice, s));
-    }
-    DeviceScope scope(ctx);
-    uint64_t *keys = nullptr, *keys_tmp = nullptr;
-    uint32_t *vals = nullptr, *vals_tmp = nullptr;
-    CB_TRY(scope.alloc(&keys, total));
-    CB_TRY(scope.alloc(&keys_tmp, total));
-    CB_TRY(scope.alloc(&vals, total));
-    CB_TRY(scope.alloc(&vals_tmp, total));
-    if (m32) {
-      incidence_keys_kernel<<<grid_for(ctx, m32), kBlock, 0, s>>>(w->d_arc_lo, w->d_arc_hi, m32, keys, vals);
-      ctx->launches += 1;
-      CB_CUDA(cudaGetLastError());
-      int bits = 1;
-      while (bits < 32 && (1ull << bits) < (uint64_t)nn) bits++;
-      CB_TRY(radix_sort_pairs_u64(ctx, keys, vals, keys_tmp, vals_tmp, total, bits));
-    }
-    incidence_fill_kernel<<<grid_for(ctx, (size_t)total + 1), kBlock, 0, s>>>(keys, vals, total, n, w->d_arc_lo,
-                                                                             w->d_arc_hi, w->d_inc_arc, w->d_inc_other,
-                                                                             w->d_inc_off);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
-    CB_CUDA(cudaStreamSynchronize(s));
-    return CB_OK;
-  }();
+  const int rc = warp_init(w, lo, hi, d2);
   if (rc != CB_OK) {
-    cb_warp_icp_destroy(w);
+    delete w;
     return rc;
   }
   *out = w;
@@ -867,13 +878,6 @@ int cb_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src
 void cb_warp_icp_destroy(cb_warp_icp* w) {
   if (!w) return;
   cudaSetDevice(w->ctx->device);
-  cudaStreamSynchronize(w->ctx->stream);
-  void* ptrs[] = {w->d_arc_lo, w->d_arc_hi, w->d_arc_d2, w->d_arc_c, w->d_inc_off, w->d_inc_arc, w->d_inc_other,
-                  w->d_T, w->d_warped, w->d_xs, w->d_B, w->d_b, w->d_inv, w->d_vec, w->d_nn, w->d_nn_d2, w->d_part,
-                  w->d_stats};
-  for (void* p : ptrs)
-    if (p) cudaFreeAsync(p, w->ctx->stream);
-  if (w->h_stats) cudaFreeHost(w->h_stats);
   cudaStreamSynchronize(w->ctx->stream);
   delete w;
 }
