@@ -79,6 +79,7 @@ struct GridView {
   float ox, oy, oz;            // grid origin (bbox min)
   float inv_h;                 // 1 / cell edge
   float h_safe;                // cell edge * (1 - 2^-10): conservative edge for lower bounds
+  float hs2;                   // h_safe^2 clamped to a finite, conservative value (grid_view)
   int nx, ny, nz;
   uint32_t n;
   // Non-empty coarse blocks (kBlockCells^3 cells each): x = X, y = Y, z = Z block coordinates, w = number

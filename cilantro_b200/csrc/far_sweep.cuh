@@ -10,7 +10,7 @@
 //   2. walk: blocks with lower bound > R or >= bound() are skipped, the others are scanned row by row with
 //      the same row pruning and the same scan() as the shell sweeps.
 // Exactness: a skipped block cannot hold a point that belongs to the result (distance bounds use the same
-// 2^-10-cell margin and h_safe as nn_search.cuh; upper bounds are inflated the same way), and the candidate
+// 2^-10-cell margin and hs2 as nn_search.cuh; upper bounds are inflated the same way), and the candidate
 // handling (strict d2 < bound, ties on the original index) is the caller's scan(), unchanged. The walk visits
 // every candidate at most once, so callers reset their result before calling far_sweep.
 //
@@ -76,22 +76,22 @@ __device__ __forceinline__ void far_sweep(const GridView& g, float qx, float qy,
   const float fx = cell_coord(qx, g.ox, g.inv_h), fy = cell_coord(qy, g.oy, g.inv_h),
               fz = cell_coord(qz, g.oz, g.inv_h);
   const int cy = (int)floorf(fy), cz = (int)floorf(fz);
-  const float hs2 = g.h_safe * g.h_safe;
+  const float hs2 = g.hs2;
   const float h_up = g.h_safe * 1.00390625f;  // >= h (1 + 2^-10): h_safe = h (1 - 2^-10)
   const float r2 = far_radius_bound(g, fx, fy, fz, k_needed, h_up * h_up);
   for (uint32_t i = 0; i < g.nblocks; ++i) {
     const uint4 b = __ldg(g.blocks + i);
     const float lo = block_bounds(b, fx, fy, fz, g.nx, g.ny, g.nz).lo2 * hs2;
-    if (lo > r2 || lo >= bound()) continue;
+    if (lo > r2 || lo > bound()) continue;
     const int x0 = (int)b.x * kBlockCells, x1 = min(x0 + kBlockCells, g.nx);
     const int ye = min((int)(b.y + 1) * kBlockCells, g.ny), ze = min((int)(b.z + 1) * kBlockCells, g.nz);
     for (int rz = (int)b.z * kBlockCells; rz < ze; ++rz) {
       const float gz = slab_gap(fz, cz, rz);
       const float gz2 = gz * gz;
-      if (gz2 * hs2 >= bound()) continue;
+      if (gz2 * hs2 > bound()) continue;
       for (int ry = (int)b.y * kBlockCells; ry < ye; ++ry) {
         const float gy = slab_gap(fy, cy, ry);
-        if ((gy * gy + gz2) * hs2 >= bound()) continue;
+        if ((gy * gy + gz2) * hs2 > bound()) continue;
         const uint32_t base = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx;
         const uint32_t s = __ldg(g.cell_start + base + x0), e = __ldg(g.cell_start + base + x1);
         if (s < e) scan(s, e);

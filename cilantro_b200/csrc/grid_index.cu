@@ -5,10 +5,12 @@
 // Pipeline (all on the context stream):
 //   bbox reduce -> [host: pick cell edge] -> cell id + histogram -> occupancy stats
 //   (-> shrink the cell edge and redo while non-empty cells hold too many points)
-//   -> exclusive scan -> atomic scatter of point indices -> per-cell index sort (deterministic
-//   layout) -> gather into the cell-sorted float4 arrays.
+//   -> exclusive scan -> atomic scatter of point indices -> per-cell index sort (or, when some cell
+//   holds more than kHugeCell points, one stable radix sort of (cell, index)) -> gather into the
+//   cell-sorted float4 arrays. Either way every cell lists its points in ascending original index.
 #include "cb_internal.hpp"
 #include "nn_search.cuh"
+#include <cfloat>
 #include <cmath>
 #include <algorithm>
 
@@ -223,9 +225,10 @@ __global__ void scatter_kernel(const uint32_t* __restrict__ cell_id, size_t n, c
 
 // Make the layout independent of atomic arrival order: sort each cell's indices ascending.
 // Small cells: one thread per cell, insertion sort. Cells above kBigCell are left to
-// sort_big_cells_kernel (rank sort by one block per cell); above kHugeCell they keep arrival
-// order (degenerate inputs such as millions of coincident points; results are unaffected because
-// ties are broken on the original index, only the summation order of a query cloud may vary).
+// sort_big_cells_kernel (rank sort by one block per cell, O(m^2) for m points). A grid with a cell
+// above kHugeCell (degenerate inputs: millions of coincident points, a scan collapsed into a few cells
+// by a far outlier) skips all three kernels and is laid out by a stable radix sort instead
+// (ensure_index).
 constexpr uint32_t kBigCell = 32;
 constexpr uint32_t kHugeCell = 1u << 16;
 
@@ -237,10 +240,8 @@ __global__ void sort_small_cells_kernel(const uint32_t* __restrict__ cell_start,
     const uint32_t m = e - b;
     if (m < 2) continue;
     if (m > kBigCell) {
-      if (m <= kHugeCell) {
-        uint32_t slot = atomicAdd(big_count, 1u);
-        big_list[slot] = (uint32_t)c;
-      }
+      uint32_t slot = atomicAdd(big_count, 1u);
+      big_list[slot] = (uint32_t)c;
       continue;
     }
     for (uint32_t i = b + 1; i < e; ++i) {
@@ -270,6 +271,15 @@ __global__ void sort_big_cells_kernel(const uint32_t* __restrict__ cell_start, c
       perm[b + rank] = v;
     }
     __syncthreads();
+  }
+}
+
+// keys of the stable (cell, index) sort: the radix sort keeps equal cells in input (= index) order
+__global__ void cell_keys_kernel(const uint32_t* __restrict__ cell_id, size_t n, uint64_t* __restrict__ keys,
+                                 uint32_t* __restrict__ perm) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    keys[i] = cell_id[i];
+    perm[i] = (uint32_t)i;
   }
 }
 
@@ -401,6 +411,7 @@ int ensure_index(cb_cloud* c) {
   GridParams gp;
   size_t ncells = 0;
   double mean_occ = 0;
+  unsigned long long max_occ = 0;  // largest cell of the grid in gp
   for (int attempt = 0; attempt < 6; ++attempt) {
     // dims from the edge; keep every axis <= kMaxDim and the table <= cell_cap
     int dims[3];
@@ -437,6 +448,7 @@ int ensure_index(cb_cloud* c) {
     CB_CUDA(cudaMemcpyAsync(h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
     mean_occ = (double)n / (double)std::max<unsigned long long>(1, h_stats[0]);
+    max_occ = h_stats[1];
     const int maxdim = std::max({dims[0], dims[1], dims[2]});
     if (mean_occ <= 2.0 * kTargetOcc || maxdim >= kMaxDim || ncells * 4 > cell_cap) break;
     // shrink: occupancy of a surface scales ~h^2, of a volume ~h^3; use the square-root (stronger) step
@@ -460,28 +472,45 @@ int ensure_index(cb_cloud* c) {
 
   // 3. cell_start = exclusive scan of the histogram (in place; d_hist becomes cell_start)
   CB_TRY(exclusive_scan_u32(ctx, d_hist, ncells, (uint32_t)n));
-  // 4. scatter indices, deterministic order inside cells
-  uint32_t* d_cursor = nullptr;
+  // 4. point indices in cell order, ascending inside every cell (sums over a cloud in cell order are then the
+  //    same on every build)
   uint32_t* d_perm = nullptr;
-  uint32_t* d_big = nullptr;
-  uint32_t* d_tmp = nullptr;
-  CB_TRY(scope.alloc(&d_cursor, ncells));
-  CB_CUDA(cudaMemsetAsync(d_cursor, 0, ncells * sizeof(uint32_t), ctx->stream));
   CB_TRY(scope.alloc(&d_perm, n));
-  const size_t big_cap = n / kBigCell + 2;
-  CB_TRY(scope.alloc(&d_big, big_cap + 1));
-  CB_CUDA(cudaMemsetAsync(d_big, 0, sizeof(uint32_t), ctx->stream));
-  CB_TRY(scope.alloc(&d_tmp, n));
-  scatter_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_cell_id, n, d_hist, d_cursor, d_perm);
-  sort_small_cells_kernel<<<grid_blocks(ctx, ncells), kThreads, 0, ctx->stream>>>(d_hist, ncells, d_perm, d_big + 1,
-                                                                                 d_big);
-  sort_big_cells_kernel<<<ctx->sm_count * 2, kThreads, 0, ctx->stream>>>(d_hist, d_big + 1, d_big, d_perm, d_tmp);
+  if (max_occ <= kHugeCell) {
+    uint32_t* d_cursor = nullptr;
+    uint32_t* d_big = nullptr;
+    uint32_t* d_tmp = nullptr;
+    CB_TRY(scope.alloc(&d_cursor, ncells));
+    CB_CUDA(cudaMemsetAsync(d_cursor, 0, ncells * sizeof(uint32_t), ctx->stream));
+    const size_t big_cap = n / kBigCell + 2;
+    CB_TRY(scope.alloc(&d_big, big_cap + 1));
+    CB_CUDA(cudaMemsetAsync(d_big, 0, sizeof(uint32_t), ctx->stream));
+    CB_TRY(scope.alloc(&d_tmp, n));
+    scatter_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_cell_id, n, d_hist, d_cursor, d_perm);
+    sort_small_cells_kernel<<<grid_blocks(ctx, ncells), kThreads, 0, ctx->stream>>>(d_hist, ncells, d_perm,
+                                                                                   d_big + 1, d_big);
+    sort_big_cells_kernel<<<ctx->sm_count * 2, kThreads, 0, ctx->stream>>>(d_hist, d_big + 1, d_big, d_perm, d_tmp);
+    ctx->launches += 3;
+  } else {
+    // a rank sort of a cell this large would cost O(m^2): sort (cell, index) pairs of the whole cloud instead
+    uint64_t* d_keys = nullptr;
+    uint64_t* d_keys_tmp = nullptr;
+    uint32_t* d_vals_tmp = nullptr;
+    CB_TRY(scope.alloc(&d_keys, n));
+    CB_TRY(scope.alloc(&d_keys_tmp, n));
+    CB_TRY(scope.alloc(&d_vals_tmp, n));
+    cell_keys_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_cell_id, n, d_keys, d_perm);
+    ctx->launches += 1;
+    int bits = 1;
+    while (bits < 32 && ((ncells - 1) >> bits) != 0) ++bits;
+    CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_perm, d_keys_tmp, d_vals_tmp, n, bits));
+  }
   // 5. gather
   float4 *d_pts = nullptr, *d_nrm = nullptr;
   CB_TRY(scope.alloc(&d_pts, n));
   if (c->d_raw_nrm) CB_TRY(scope.alloc(&d_nrm, n));
   gather_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(c->d_raw, c->d_raw_nrm, d_perm, n, d_pts, d_nrm);
-  ctx->launches += 4;
+  ctx->launches += 1;
   CB_CUDA(cudaGetLastError());
   // 6. coarse occupancy: the list of non-empty 8x8x8-cell blocks for the far-query path
   uint4* d_blocks = nullptr;
@@ -524,6 +553,16 @@ GridView grid_view(const cb_cloud* c) {
   g.oz = c->oz;
   g.inv_h = c->inv_h;
   g.h_safe = (1.0f / c->inv_h) * (1.0f - 0.0009765625f);
+  // The one scale factor of every pruning bound (gap^2 * hs2, gap in cells). A point beyond a gap g lies at
+  // least (g + 2^-11) h away, so a bound only has to stay at or below its fp32 d2:
+  //  * h_safe^2 above FLT_MAX would be +inf (h > ~1.84e19): inf bounds prune rows holding finite d2, and 0 * inf
+  //    is NaN. FLT_MAX < h_safe^2 keeps every bound below the unclamped one, and a bound that still overflows
+  //    to inf only covers points whose fp32 d2 is inf as well;
+  //  * h_safe^2 below 2^-100 (h < ~8.9e-16): the d2 of a point beyond a face may then be subnormal, where fp32
+  //    loses the relative precision the margins rely on. Such grids prune nothing (the searches stay exact and
+  //    scan everything they reach).
+  const float hs = g.h_safe * g.h_safe;
+  g.hs2 = hs < 0x1p-100f ? 0.f : fminf(hs, FLT_MAX);
   g.nx = c->nx;
   g.ny = c->ny;
   g.nz = c->nz;

@@ -4,12 +4,12 @@
 // (core/kd_tree.hpp:284-291 -> 3rd_party/nanoflann/nanoflann.hpp:1709-1732,1886-1961) with a
 // bounded sweep over grid cells. Exactness argument (DESIGN.md "Grid search is exact"):
 //   * candidates are visited row by row (a row = all cells sharing (y, z)); a row, a cell or a
-//     whole shell is skipped only when a conservative lower bound of the distance from the query to
-//     every point in it is >= the best squared distance found so far;
+//     whole shell is skipped only when a lower bound of the fp32 d2 of every point in it is strictly
+//     greater than the best squared distance found so far (a bit-equal d2 may still win on its index);
 //   * the lower bounds are computed in cell units from the SAME float expression that assigned
-//     reference points to cells (cell_coord below), shrunk by 2^-10 cell and by h_safe = h(1-2^-10),
-//     which dominates the <= 2^-11-cell rounding uncertainty of that expression for grids of
-//     <= 1024 cells per axis;
+//     reference points to cells (cell_coord below), shrunk by 2^-10 cell and scaled by GridView::hs2
+//     (h_safe^2, h_safe = h(1-2^-10), clamped finite: grid_view), which dominates the <= 2^-11-cell
+//     rounding uncertainty of that expression for grids of <= 1024 cells per axis;
 //   * the search ends when the scanned block's nearest face is farther than the best distance.
 //
 // Arithmetic contract (must match oracle/cilantro_oracle.cpp bit for bit; fp32, RN, no FMA):
@@ -162,7 +162,7 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
   const float fy = cell_coord(qy, g.oy, g.inv_h);
   const float fz = cell_coord(qz, g.oz, g.inv_h);
   const int cx = (int)floorf(fx), cy = (int)floorf(fy), cz = (int)floorf(fz);
-  const float hs2 = g.h_safe * g.h_safe;
+  const float hs2 = g.hs2;
 
   // first shell that can contain grid cells at all
   int k0 = 0;
@@ -195,8 +195,8 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
     scan_range<kExact>(g.pts, s1, s2, qx, qy, qz, best);
     {
       const float gl = slab_gap(fx, cx, cx - 1), gr = slab_gap(fx, cx, cx + 1);
-      if (gl * gl * hs2 < best.d2) scan_range<kExact>(g.pts, s0, s1, qx, qy, qz, best);
-      if (gr * gr * hs2 < best.d2) scan_range<kExact>(g.pts, s2, s3, qx, qy, qz, best);
+      if (gl * gl * hs2 <= best.d2) scan_range<kExact>(g.pts, s0, s1, qx, qy, qz, best);
+      if (gr * gr * hs2 <= best.d2) scan_range<kExact>(g.pts, s2, s3, qx, qy, qz, best);
     }
     {
       const float gym = slab_gap(fy, cy, cy - 1), gyp = slab_gap(fy, cy, cy + 1);
@@ -206,7 +206,7 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
 #pragma unroll
       for (int t = 0; t < 8; ++t) {
         const float lb = (gy2[kDy[t] + 1] + gz2[kDz[t] + 1]) * hs2;
-        if (lb < best.d2 && rb[t] < re[t]) scan_range<kExact>(g.pts, rb[t], re[t], qx, qy, qz, best);
+        if (lb <= best.d2 && rb[t] < re[t]) scan_range<kExact>(g.pts, rb[t], re[t], qx, qy, qz, best);
       }
     }
     k = 2;
@@ -221,7 +221,7 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
         const int ry = cy + kRowDy[t], rz = cz + kRowDz[t];
         if (ry < 0 || ry >= g.ny || rz < 0 || rz >= g.nz) continue;
         const float gy = slab_gap(fy, cy, ry), gz = slab_gap(fz, cz, rz);
-        if ((gy * gy + gz * gz) * hs2 >= best.d2) continue;
+        if ((gy * gy + gz * gz) * hs2 > best.d2) continue;
         const uint32_t base = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx;
         const uint32_t b = __ldg(g.cell_start + base + x0), e = __ldg(g.cell_start + base + x1 + 1);
         scan_range<kExact>(g.pts, b, e, qx, qy, qz, best);
@@ -249,7 +249,7 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
         if (cz + kk < g.nz - 1) { cover = fminf(cover, (float)(cz + kk + 1) - fz); any = true; }
         if (!any) break;  // the whole grid has been scanned
         cover -= kCellMargin;
-        if (cover > 0.f && cover * cover * hs2 >= best.d2) break;
+        if (cover > 0.f && cover * cover * hs2 > best.d2) break;
       }
     }
     // Shell k: rows with max(|dy|,|dz|) == k take the full x-extent, inner rows only the two end cells.
@@ -272,12 +272,12 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
     for (int rz = z0; rz <= z1; ++rz) {
       const float gz = slab_gap(fz, cz, rz);
       const float gz2 = gz * gz;
-      if (gz2 * hs2 >= best.d2) continue;
+      if (gz2 * hs2 > best.d2) continue;
       const bool zshell = (rz - cz == k) || (cz - rz == k);
       for (int ry = y0; ry <= y1; ++ry) {
         const float gy = slab_gap(fy, cy, ry);
         const float gyz2 = gy * gy + gz2;
-        if (gyz2 * hs2 >= best.d2) continue;
+        if (gyz2 * hs2 > best.d2) continue;
         const uint32_t base = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx;
         if (zshell || (ry - cy == k) || (cy - ry == k)) {
           if (x0 <= x1) {
@@ -287,14 +287,14 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
         } else {
           if (xl >= 0 && xl < g.nx) {
             const float gx = slab_gap(fx, cx, xl);
-            if ((gx * gx + gyz2) * hs2 < best.d2) {
+            if ((gx * gx + gyz2) * hs2 <= best.d2) {
               const uint32_t b = __ldg(g.cell_start + base + xl), e = __ldg(g.cell_start + base + xl + 1);
               scan_range<kExact>(g.pts, b, e, qx, qy, qz, best);
             }
           }
           if (xr >= 0 && xr < g.nx) {
             const float gx = slab_gap(fx, cx, xr);
-            if ((gx * gx + gyz2) * hs2 < best.d2) {
+            if ((gx * gx + gyz2) * hs2 <= best.d2) {
               const uint32_t b = __ldg(g.cell_start + base + xr), e = __ldg(g.cell_start + base + xr + 1);
               scan_range<kExact>(g.pts, b, e, qx, qy, qz, best);
             }

@@ -53,7 +53,7 @@ __device__ __forceinline__ Best warp_grid_nearest(const GridView& g, WarpSearchS
 
   const float fx = cell_coord(qx, g.ox, g.inv_h), fy = cell_coord(qy, g.oy, g.inv_h), fz = cell_coord(qz, g.oz, g.inv_h);
   const int cx = (int)floorf(fx), cy = (int)floorf(fy), cz = (int)floorf(fz);
-  const float hs2 = g.h_safe * g.h_safe;
+  const float hs2 = g.hs2;
   const bool inside = active && g.n > 0 && cx >= 0 && cx < g.nx && cy >= 0 && cy < g.ny && cz >= 0 && cz < g.nz;
   bool slow = active && g.n > 0 && !inside;  // outside the grid: per-lane exact search at the end
 
@@ -98,17 +98,17 @@ __device__ __forceinline__ Best warp_grid_nearest(const GridView& g, WarpSearchS
       uint32_t first;
       uint32_t ncells;
       if (t == 0) {  // left x-neighbour
-        need = inside && cx > 0 && (gxl * gxl * hs2 < best.d2);
+        need = inside && cx > 0 && (gxl * gxl * hs2 <= best.d2);
         first = cbase + (uint32_t)(cx - 1);
         ncells = 1;
       } else if (t == 1) {  // right x-neighbour
-        need = inside && cx < g.nx - 1 && (gxr * gxr * hs2 < best.d2);
+        need = inside && cx < g.nx - 1 && (gxr * gxr * hs2 <= best.d2);
         first = cbase + (uint32_t)(cx + 1);
         ncells = 1;
       } else {
         const int ry = cy + kDy[t - 2], rz = cz + kDz[t - 2];
         const bool valid = inside && ry >= 0 && ry < g.ny && rz >= 0 && rz < g.nz;
-        need = valid && ((gy2[kDy[t - 2] + 1] + gz2[kDz[t - 2] + 1]) * hs2 < best.d2);
+        need = valid && ((gy2[kDy[t - 2] + 1] + gz2[kDz[t - 2] + 1]) * hs2 <= best.d2);
         first = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx + (uint32_t)xm;
         ncells = (uint32_t)(xp - xm + 1);
       }
@@ -161,7 +161,7 @@ __device__ __forceinline__ Best warp_grid_nearest(const GridView& g, WarpSearchS
     if (cz - 1 > 0) { cover = fminf(cover, fz - (float)(cz - 1)); any = true; }
     if (cz + 1 < g.nz - 1) { cover = fminf(cover, (float)(cz + 2) - fz); any = true; }
     cover -= kCellMargin;
-    const bool done = !any || (cover > 0.f && cover * cover * hs2 >= best.d2);
+    const bool done = !any || (cover > 0.f && cover * cover * hs2 > best.d2);
     if (!done || best.tie) slow = true;
   }
   if (slow) {

@@ -83,7 +83,7 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
 
   const float fx = cell_coord(qx, g.ox, g.inv_h), fy = cell_coord(qy, g.oy, g.inv_h), fz = cell_coord(qz, g.oz, g.inv_h);
   const int cx = (int)floorf(fx), cy = (int)floorf(fy), cz = (int)floorf(fz);
-  const float hs2 = g.h_safe * g.h_safe;
+  const float hs2 = g.hs2;
   const bool inside = active && g.n > 0 && cx >= 0 && cx < g.nx && cy >= 0 && cy < g.ny && cz >= 0 && cz < g.nz;
   bool slow = active && g.n > 0 && !inside;  // outside the grid: per-lane exact search at the end
 
@@ -103,7 +103,7 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
 
   // ---- phase A: own cell + work items --------------------------------------------------------------
   unsigned int count = 0;  // warp-uniform number of queued items
-  float wide2 = 0.f;       // regions with a lower bound >= wide2 are not scanned
+  float wide2 = 0.f;       // regions with a lower bound > wide2 are not scanned
   {
     const uint32_t cbase = inside ? ((uint32_t)cz * (uint32_t)g.ny + (uint32_t)cy) * (uint32_t)g.nx : 0u;
     uint32_t s1 = 0, s2 = 0;
@@ -134,17 +134,17 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
       uint32_t first;
       uint32_t ncells;
       if (t == 0) {  // left x-neighbour
-        need = inside && cx > 0 && (gxl * gxl * hs2 < wide2);
+        need = inside && cx > 0 && (gxl * gxl * hs2 <= wide2);
         first = cbase + (uint32_t)(cx - 1);
         ncells = 1;
       } else if (t == 1) {  // right x-neighbour
-        need = inside && cx < g.nx - 1 && (gxr * gxr * hs2 < wide2);
+        need = inside && cx < g.nx - 1 && (gxr * gxr * hs2 <= wide2);
         first = cbase + (uint32_t)(cx + 1);
         ncells = 1;
       } else {
         const int ry = cy + kDy[t - 2], rz = cz + kDz[t - 2];
         const bool valid = inside && ry >= 0 && ry < g.ny && rz >= 0 && rz < g.nz;
-        need = valid && ((gy2[kDy[t - 2] + 1] + gz2[kDz[t - 2] + 1]) * hs2 < wide2);
+        need = valid && ((gy2[kDy[t - 2] + 1] + gz2[kDz[t - 2] + 1]) * hs2 <= wide2);
         first = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx + (uint32_t)xm;
         ncells = (uint32_t)(xp - xm + 1);
       }
@@ -206,7 +206,7 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
     if (cz + 1 < g.nz - 1) { cover = fminf(cover, (float)(cz + 2) - fz); any = true; }
     cover -= kCellMargin;
     const float cover2 = (!any) ? kInf : (cover > 0.f ? cover * cover * hs2 : 0.f);
-    const bool done = cover2 >= out.d2;
+    const bool done = cover2 > out.d2;
     const bool tie = out.pos >= 0 && sec == out.d2;  // a second point at a bit-equal distance: index rule
     if (!done || tie) slow = true;
     out.D2 = fminf(fminf(sec, wide2), cover2);
