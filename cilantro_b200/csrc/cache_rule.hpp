@@ -65,7 +65,8 @@ inline float sqrt_ru(float a) { volatile float x = a; return directed(FE_UPWARD,
 inline float sqrt_rd(float a) { volatile float x = a; return directed(FE_DOWNWARD, [&] { return std::sqrt((float)x); }); }
 #endif
 
-// q = R s + t with the contract arithmetic: q_r = (R_r0 x + (R_r1 y + R_r2 z)) + t_r  (nn_search.cuh, apply_rigid)
+// q = R s + t with the contract arithmetic: q_r = (R_r0 x + (R_r1 y + R_r2 z)) + t_r: the transform every search kernel
+// applies to its queries
 template <class RigidT>
 CB_RULE_HD void transform_point(const RigidT& T, float x, float y, float z, float& qx, float& qy, float& qz) {
   qx = add_rn(add_rn(mul_rn(T.r[0], x), add_rn(mul_rn(T.r[1], y), mul_rn(T.r[2], z))), T.t[0]);

@@ -50,7 +50,7 @@ __device__ __forceinline__ void accumulate_pair(double* acc, const Args& a, bool
       s1 = __fsub_rn(qy, a.sm[1]);
       s2 = __fsub_rn(qz, a.sm[2]);
     } else {
-      apply_rigid(a.Tin, __fsub_rn(qx, a.sm[0]), __fsub_rn(qy, a.sm[1]), __fsub_rn(qz, a.sm[2]), s0, s1, s2);
+      rule::transform_point(a.Tin, __fsub_rn(qx, a.sm[0]), __fsub_rn(qy, a.sm[1]), __fsub_rn(qz, a.sm[2]), s0, s1, s2);
     }
     const float v0 = __fadd_rn(d0, s0), v1 = __fadd_rn(d1, s1), v2 = __fadd_rn(d2, s2);
     const float e0 = __fsub_rn(d0, s0), e1 = __fsub_rn(d1, s1), e2 = __fsub_rn(d2, s2);

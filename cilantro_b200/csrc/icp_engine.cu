@@ -205,7 +205,7 @@ __global__ void __launch_bounds__(kReduceBlock) pairs_pass_kernel(const IcpArgs 
     const size_t i = first[p], j = second[p];
     const float4 dp = make_float4(dst_raw[3 * i], dst_raw[3 * i + 1], dst_raw[3 * i + 2], 0.f);
     float qx, qy, qz;
-    apply_rigid(a.T, src_raw[3 * j], src_raw[3 * j + 1], src_raw[3 * j + 2], qx, qy, qz);
+    rule::transform_point(a.T, src_raw[3 * j], src_raw[3 * j + 1], src_raw[3 * j + 2], qx, qy, qz);
     accumulate_pair<MODE>(
         acc, a, has_pt, has_pl, dp, qx, qy, qz, src_nrm != nullptr,
         [&] { return make_float4(dst_nrm[3 * i], dst_nrm[3 * i + 1], dst_nrm[3 * i + 2], 0.f); },

@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(kBlock, kIcpMinBlocks) icp_pass_kernel(const I
   const bool active = i < a.n_src;
   const float4 s = active ? __ldg(a.src_pts + i) : make_float4(0.f, 0.f, 0.f, 0.f);
   float qx, qy, qz;
-  apply_rigid(a.T, s.x, s.y, s.z, qx, qy, qz);
+  rule::transform_point(a.T, s.x, s.y, s.z, qx, qy, qz);
   int pos = -1;
   float cd2 = 0.f;  // the correspondence's value (squared distance): input of the RBF weight evaluators
   if (SEARCH) {
@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(kBlock) residual_kernel(const GridView dst, co
     const float4 s = __ldg(src_pts + i);
     const int oi = __float_as_int(s.w);
     float qx, qy, qz;
-    apply_rigid(T, s.x, s.y, s.z, qx, qy, qz);
+    rule::transform_point(T, s.x, s.y, s.z, qx, qy, qz);
     const Best best = grid_nearest(dst, qx, qy, qz, 3.402823466e+38f);
     float res = __int_as_float(0x7fc00000);  // NaN when dst is empty (icp_*_metric.hpp:221-224)
     if (best.idx >= 0) {
@@ -146,7 +146,7 @@ __global__ void __launch_bounds__(kBlock) residual_kernel(const GridView dst, co
 __global__ void transform_points_kernel(const Rigid T, const float* __restrict__ in, size_t n, float* __restrict__ out) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     float qx, qy, qz;
-    apply_rigid(T, in[3 * i], in[3 * i + 1], in[3 * i + 2], qx, qy, qz);
+    rule::transform_point(T, in[3 * i], in[3 * i + 1], in[3 * i + 2], qx, qy, qz);
     out[3 * i] = qx;
     out[3 * i + 1] = qy;
     out[3 * i + 2] = qz;

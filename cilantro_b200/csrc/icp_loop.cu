@@ -175,10 +175,10 @@ __device__ __forceinline__ ChunkPair search_chunk_body(const LoopArgs& a, const 
   int sd = -1;
   if (act) {
     const float4 s = __ldg(a.src_pts + cp.i);
-    apply_rigid(cx.T, s.x, s.y, s.z, cp.qx, cp.qy, cp.qz);
+    rule::transform_point(cx.T, s.x, s.y, s.z, cp.qx, cp.qy, cp.qz);
     if (!kCold) {
       float ox, oy, oz;
-      apply_rigid(cx.Tp, s.x, s.y, s.z, ox, oy, oz);
+      rule::transform_point(cx.Tp, s.x, s.y, s.z, ox, oy, oz);
       const float ex = __fsub_rn(cp.qx, ox), ey = __fsub_rn(cp.qy, oy), ez = __fsub_rn(cp.qz, oz);
       const float dl = __fsqrt_ru(__fmaf_ru(ez, ez, __fmaf_ru(ey, ey, __fmul_ru(ex, ex))));
       // the next step is expected to be about half of this one, and a hit needs r - (motion) > d: widen by 2 x
@@ -221,7 +221,7 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
   cx.T = rigid_from_t12_dev(a.st->T);
   cx.Tp = rigid_from_t12_dev(a.st->T_prev);
   float smx, smy, smz;
-  apply_rigid(cx.T, a.src_mean[0], a.src_mean[1], a.src_mean[2], smx, smy, smz);  // transform_ * src_mean_
+  rule::transform_point(cx.T, a.src_mean[0], a.src_mean[1], a.src_mean[2], smx, smy, smz);  // transform_ * src_mean_
   cx.sm[0] = smx; cx.sm[1] = smy; cx.sm[2] = smz;
   cx.dm[0] = a.dm[0]; cx.dm[1] = a.dm[1]; cx.dm[2] = a.dm[2];
   cx.w_pt = a.w_pt;

@@ -26,7 +26,7 @@ __global__ void __launch_bounds__(kBlock) knn_k_kernel(const GridView g, const f
     const float4 s = __ldg(qry + qi);
     const int oi = __float_as_int(s.w);
     float qx, qy, qz;
-    apply_rigid(T, s.x, s.y, s.z, qx, qy, qz);
+    rule::transform_point(T, s.x, s.y, s.z, qx, qy, qz);
     float bd[K];
     int bi[K];
     int count = 0;
@@ -35,10 +35,7 @@ __global__ void __launch_bounds__(kBlock) knn_k_kernel(const GridView g, const f
     auto scan = [&](uint32_t b, uint32_t e) {
       for (uint32_t j = b; j < e; ++j) {
         const float4 p = __ldg(g.pts + j);
-        const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-        float r = __fmul_rn(dx, dx);
-        r = __fadd_rn(r, __fmul_rn(dy, dy));
-        r = __fadd_rn(r, __fmul_rn(dz, dz));
+        const float r = rule::contract_d2(qx, qy, qz, p.x, p.y, p.z);
         if (r < max_d2) kbest_insert<K>(bd, bi, k, count, r, __float_as_int(p.w));
       }
     };

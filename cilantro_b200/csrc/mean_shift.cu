@@ -35,13 +35,6 @@ constexpr int kSweepBlocksPerSm = 8;
 
 __device__ __forceinline__ bool finite3(float x, float y, float z) { return fabsf(x) + fabsf(y) + fabsf(z) < 3.0e38f; }
 
-__device__ __forceinline__ float dist2(float qx, float qy, float qz, const float4& p) {
-  const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-  float r = __fmul_rn(dx, dx);
-  r = __fadd_rn(r, __fmul_rn(dy, dy));
-  return __fadd_rn(r, __fmul_rn(dz, dz));
-}
-
 // packed xyz -> float4 seeds; active ids 0..n-1
 __global__ void init_seeds_kernel(const float* __restrict__ xyz, uint32_t n, float4* __restrict__ seeds,
                                   uint32_t* __restrict__ active) {
@@ -80,10 +73,7 @@ __global__ void shift_kernel(const float* __restrict__ raw, const uint32_t* __re
     const float inv = __fdiv_rn(1.0f, w_sum);
     const float mx = __fmul_rn(ax, inv), my = __fmul_rn(ay, inv), mz = __fmul_rn(az, inv);
     const float4 s = seeds[id];
-    const float dx = __fsub_rn(s.x, mx), dy = __fsub_rn(s.y, my), dz = __fsub_rn(s.z, mz);
-    float r = __fmul_rn(dx, dx);
-    r = __fadd_rn(r, __fmul_rn(dy, dy));
-    r = __fadd_rn(r, __fmul_rn(dz, dz));
+    const float r = rule::contract_d2(s.x, s.y, s.z, mx, my, mz);
     seeds[id] = make_float4(mx, my, mz, 0.f);
     if (!(r < tol2)) next[atomicAdd(next_count, 1u)] = id;
   }
@@ -183,7 +173,7 @@ __global__ void __launch_bounds__(kBlock, kSweepBlocksPerSm) round_kernel(const 
           for (uint32_t j = b; j < e; ++j) {
             const float4 p = __ldg(g.pts + j);
             const uint32_t o = (uint32_t)__float_as_int(p.w);
-            if (__ldg(head + o) >= i || !(dist2(sx, sy, sz, p) < tol2)) continue;
+            if (__ldg(head + o) >= i || !(rule::contract_d2(sx, sy, sz, p.x, p.y, p.z) < tol2)) continue;
             const uint32_t v = st[o];
             rep_below |= v == kRep;
             pending |= v == kUndecided;
@@ -220,7 +210,7 @@ __global__ void __launch_bounds__(kBlock, kSweepBlocksPerSm) rep_kernel(const Gr
             const float4 p = __ldg(g.pts + j);
             const uint32_t o = (uint32_t)__float_as_int(p.w);
             const uint32_t h = head[o];
-            if (h < best && state[o] == kRep && dist2(sx, sy, sz, p) < tol2) best = h;
+            if (h < best && state[o] == kRep && rule::contract_d2(sx, sy, sz, p.x, p.y, p.z) < tol2) best = h;
           }
         },
         [&]() { best = i; }, 0u);

@@ -12,10 +12,15 @@
 //     rounding uncertainty of that expression for grids of <= 1024 cells per axis;
 //   * the search ends when the scanned block's nearest face is farther than the best distance.
 //
-// Arithmetic contract (must match oracle/cilantro_oracle.cpp bit for bit; fp32, RN, no FMA):
-//   q_r = (R_r0*x + (R_r1*y + R_r2*z)) + t_r        d2 = ((dx*dx) + dy*dy) + dz*dz, d = q - ref
-//   accept iff d2 < max_d2; exact ties -> lowest original reference index.
+// Every sweep (this file's 1-NN, grid_sweep.cuh, far_sweep.cuh, warp_search.cuh, warp_search_wide.cuh) takes its
+// pieces of that argument from here: the query cell (query_cell), the first shell that holds cells (first_shell),
+// the row / cell gaps (slab_gap) and the termination test (open_face_gap).
+//
+// Arithmetic contract (must match oracle/cilantro_oracle.cpp bit for bit; fp32, RN, no FMA): the query is
+// rule::transform_point and every candidate's distance rule::contract_d2 (cache_rule.hpp, also compiled for the host
+// test); accept iff d2 < max_d2; exact ties -> lowest original reference index.
 #pragma once
+#include "cache_rule.hpp"
 #include "cb_internal.hpp"
 
 namespace cb {
@@ -37,13 +42,6 @@ inline Rigid rigid_from_t12(const float* T12) {
 
 __device__ __forceinline__ float sum3(float a0, float a1, float a2) { return __fadd_rn(a0, __fadd_rn(a1, a2)); }
 
-__device__ __forceinline__ void apply_rigid(const Rigid& T, float x, float y, float z, float& qx, float& qy,
-                                            float& qz) {
-  qx = __fadd_rn(sum3(__fmul_rn(T.r[0], x), __fmul_rn(T.r[1], y), __fmul_rn(T.r[2], z)), T.t[0]);
-  qy = __fadd_rn(sum3(__fmul_rn(T.r[3], x), __fmul_rn(T.r[4], y), __fmul_rn(T.r[5], z)), T.t[1]);
-  qz = __fadd_rn(sum3(__fmul_rn(T.r[6], x), __fmul_rn(T.r[7], y), __fmul_rn(T.r[8], z)), T.t[2]);
-}
-
 __device__ __forceinline__ void rotate_rigid(const Rigid& T, float x, float y, float z, float& qx, float& qy,
                                              float& qz) {
   qx = sum3(__fmul_rn(T.r[0], x), __fmul_rn(T.r[1], y), __fmul_rn(T.r[2], z));
@@ -64,6 +62,32 @@ __host__ __device__ __forceinline__ float cell_coord(float x, float o, float inv
   return (f == f) ? f : -16777216.f;  // NaN coordinates land far outside
 }
 
+// A query in cell units: continuous coordinate f and cell c = floor(f) per axis.
+struct QueryCell {
+  float fx, fy, fz;
+  int cx, cy, cz;
+};
+
+__device__ __forceinline__ QueryCell query_cell(const GridView& g, float qx, float qy, float qz) {
+  QueryCell c;
+  c.fx = cell_coord(qx, g.ox, g.inv_h);
+  c.fy = cell_coord(qy, g.oy, g.inv_h);
+  c.fz = cell_coord(qz, g.oz, g.inv_h);
+  c.cx = (int)floorf(c.fx);
+  c.cy = (int)floorf(c.fy);
+  c.cz = (int)floorf(c.fz);
+  return c;
+}
+
+// first Chebyshev shell around the query cell that can contain grid cells at all (0 = the cell is inside the grid)
+__device__ __forceinline__ int first_shell(const GridView& g, const QueryCell& c) {
+  int k0 = 0;
+  k0 = max(k0, c.cx < 0 ? -c.cx : (c.cx > g.nx - 1 ? c.cx - (g.nx - 1) : 0));
+  k0 = max(k0, c.cy < 0 ? -c.cy : (c.cy > g.ny - 1 ? c.cy - (g.ny - 1) : 0));
+  k0 = max(k0, c.cz < 0 ? -c.cz : (c.cz > g.nz - 1 ? c.cz - (g.nz - 1) : 0));
+  return k0;
+}
+
 struct Best {
   float d2;
   int idx;   // original reference index, -1 = none
@@ -71,10 +95,33 @@ struct Best {
   bool tie;  // fast pass only: some candidate had d2 bit-equal to the running best
 };
 
+__device__ __forceinline__ Best no_best(float max_d2) { return Best{max_d2, -1, -1, false}; }
+
 constexpr float kCellMargin = 0.0009765625f;  // 2^-10 cell
 
 __constant__ signed char kRowDy[9] = {0, -1, 1, 0, 0, -1, 1, -1, 1};
 __constant__ signed char kRowDz[9] = {0, 0, 0, -1, 1, -1, -1, 1, 1};
+
+// The candidate loop of the pooled searches: eval(d2, j) for every cell-sorted point j of [b, e).
+// The scan is a chain of load -> use steps, and the warps mostly wait on those loads (long scoreboard). Batches of
+// kW candidates put kW loads in flight per wait; slots past the end of the range are predicated off (no padded
+// arithmetic — a padded variant doubled the instruction count and was slower).
+template <class Eval>
+__device__ __forceinline__ void scan_batched(const float4* __restrict__ pts, uint32_t b, uint32_t e, float qx, float qy,
+                                             float qz, Eval&& eval) {
+  constexpr int kW = 4;
+  for (uint32_t j = b; j < e; j += kW) {
+    float4 p[kW];
+    p[0] = __ldg(pts + j);
+#pragma unroll
+    for (int u = 1; u < kW; u++)
+      if (j + u < e) p[u] = __ldg(pts + j + u);
+    eval(rule::contract_d2(qx, qy, qz, p[0].x, p[0].y, p[0].z), j);
+#pragma unroll
+    for (int u = 1; u < kW; u++)
+      if (j + u < e) eval(rule::contract_d2(qx, qy, qz, p[u].x, p[u].y, p[u].z), j + u);
+  }
+}
 
 // kExact = true resolves exact ties on the original index inside the loop. kExact = false (the fast
 // pass) keeps the first strictly smaller candidate and only RECORDS that a bit-equal distance was
@@ -88,10 +135,7 @@ __device__ __forceinline__ void scan_range(const float4* __restrict__ pts, uint3
 #pragma unroll 2
     for (uint32_t j = b; j < e; ++j) {
       const float4 p = __ldg(pts + j);
-      const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-      float r = __fmul_rn(dx, dx);
-      r = __fadd_rn(r, __fmul_rn(dy, dy));
-      r = __fadd_rn(r, __fmul_rn(dz, dz));
+      const float r = rule::contract_d2(qx, qy, qz, p.x, p.y, p.z);
       const int pi = __float_as_int(p.w);
       if (r < best.d2 || (r == best.d2 && pi < best.idx)) {
         best.d2 = r;
@@ -100,33 +144,14 @@ __device__ __forceinline__ void scan_range(const float4* __restrict__ pts, uint3
       }
     }
   } else {
-    // The scan is a chain of load -> use steps, and the warps mostly wait on those loads (long
-    // scoreboard). Batches of kW candidates put kW loads in flight per wait; slots past the end of the range are predicated off (no padded arithmetic —
-    // a padded variant doubled the instruction count and was slower).
-    constexpr int kW = 4;
-    auto eval = [&](const float4& p, uint32_t j) {
-      const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-      float r = __fmul_rn(dx, dx);
-      r = __fadd_rn(r, __fmul_rn(dy, dy));
-      r = __fadd_rn(r, __fmul_rn(dz, dz));
+    scan_batched(pts, b, e, qx, qy, qz, [&](float r, uint32_t j) {
       if (r < best.d2) {
         best.d2 = r;
         best.pos = (int)j;
       } else if (r == best.d2 && (int)j != skip_pos) {
         best.tie = true;
       }
-    };
-    for (uint32_t j = b; j < e; j += kW) {
-      float4 p[kW];
-      p[0] = __ldg(pts + j);
-#pragma unroll
-      for (int u = 1; u < kW; u++)
-        if (j + u < e) p[u] = __ldg(pts + j + u);
-      eval(p[0], j);
-#pragma unroll
-      for (int u = 1; u < kW; u++)
-        if (j + u < e) eval(p[u], j + u);
-    }
+    });
   }
 }
 
@@ -140,6 +165,23 @@ __device__ __forceinline__ float slab_gap(float f, int c, int r) {
   return g > 0.f ? g : 0.f;
 }
 
+// The termination test of every shell sweep. Returns false when the scanned block [c-kk, c+kk] already covers the
+// whole grid; otherwise gap receives the distance (cells, shrunk by the margin, may be <= 0) from the query to the
+// block's nearest face that still has grid cells beyond it. Every point not yet scanned lies beyond such a face, so
+// once gap > 0 and gap^2 hs2 > bound, none of them can pass d2 < bound or tie with it.
+__device__ __forceinline__ bool open_face_gap(const GridView& g, const QueryCell& c, int kk, float& gap) {
+  float cover = 3.0e38f;
+  bool any = false;
+  if (c.cx - kk > 0) { cover = fminf(cover, c.fx - (float)(c.cx - kk)); any = true; }
+  if (c.cx + kk < g.nx - 1) { cover = fminf(cover, (float)(c.cx + kk + 1) - c.fx); any = true; }
+  if (c.cy - kk > 0) { cover = fminf(cover, c.fy - (float)(c.cy - kk)); any = true; }
+  if (c.cy + kk < g.ny - 1) { cover = fminf(cover, (float)(c.cy + kk + 1) - c.fy); any = true; }
+  if (c.cz - kk > 0) { cover = fminf(cover, c.fz - (float)(c.cz - kk)); any = true; }
+  if (c.cz + kk < g.nz - 1) { cover = fminf(cover, (float)(c.cz + kk + 1) - c.fz); any = true; }
+  gap = cover - kCellMargin;
+  return any;
+}
+
 }  // namespace cb
 
 #include "far_sweep.cuh"
@@ -149,27 +191,15 @@ namespace cb {
 // Exact nearest neighbour of (qx,qy,qz) among the grid's points with d2 < max_d2.
 template <bool kExact>
 __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, float qy, float qz, float max_d2) {
-  Best best;
-  best.d2 = max_d2;
-  best.idx = -1;
-  best.pos = -1;
-  best.tie = false;
+  Best best = no_best(max_d2);
   if (g.n == 0) return best;
   // a NaN / Inf query is at no finite distance from anything: no candidate can pass d2 < best
   if (!(fabsf(qx) + fabsf(qy) + fabsf(qz) < 3.0e38f)) return best;
 
-  const float fx = cell_coord(qx, g.ox, g.inv_h);
-  const float fy = cell_coord(qy, g.oy, g.inv_h);
-  const float fz = cell_coord(qz, g.oz, g.inv_h);
-  const int cx = (int)floorf(fx), cy = (int)floorf(fy), cz = (int)floorf(fz);
+  const QueryCell c = query_cell(g, qx, qy, qz);
+  const int cx = c.cx, cy = c.cy, cz = c.cz;
   const float hs2 = g.hs2;
-
-  // first shell that can contain grid cells at all
-  int k0 = 0;
-  k0 = max(k0, cx < 0 ? -cx : (cx > g.nx - 1 ? cx - (g.nx - 1) : 0));
-  k0 = max(k0, cy < 0 ? -cy : (cy > g.ny - 1 ? cy - (g.ny - 1) : 0));
-  k0 = max(k0, cz < 0 ? -cz : (cz > g.nz - 1 ? cz - (g.nz - 1) : 0));
-
+  const int k0 = first_shell(g, c);
   int k = k0;
   if (k0 == 0) {
     // Query cell inside the grid (the common case). Shells 0 and 1: all 20 cell-table entries are
@@ -194,13 +224,13 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
     }
     scan_range<kExact>(g.pts, s1, s2, qx, qy, qz, best);
     {
-      const float gl = slab_gap(fx, cx, cx - 1), gr = slab_gap(fx, cx, cx + 1);
+      const float gl = slab_gap(c.fx, cx, cx - 1), gr = slab_gap(c.fx, cx, cx + 1);
       if (gl * gl * hs2 <= best.d2) scan_range<kExact>(g.pts, s0, s1, qx, qy, qz, best);
       if (gr * gr * hs2 <= best.d2) scan_range<kExact>(g.pts, s2, s3, qx, qy, qz, best);
     }
     {
-      const float gym = slab_gap(fy, cy, cy - 1), gyp = slab_gap(fy, cy, cy + 1);
-      const float gzm = slab_gap(fz, cz, cz - 1), gzp = slab_gap(fz, cz, cz + 1);
+      const float gym = slab_gap(c.fy, cy, cy - 1), gyp = slab_gap(c.fy, cy, cy + 1);
+      const float gzm = slab_gap(c.fz, cz, cz - 1), gzp = slab_gap(c.fz, cz, cz + 1);
       const float gy2[3] = {gym * gym, 0.f, gyp * gyp};
       const float gz2[3] = {gzm * gzm, 0.f, gzp * gzp};
 #pragma unroll
@@ -220,7 +250,7 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
         // visiting order: (0,0), then the 4 face rows, then the 4 corner rows
         const int ry = cy + kRowDy[t], rz = cz + kRowDz[t];
         if (ry < 0 || ry >= g.ny || rz < 0 || rz >= g.nz) continue;
-        const float gy = slab_gap(fy, cy, ry), gz = slab_gap(fz, cz, rz);
+        const float gy = slab_gap(c.fy, cy, ry), gz = slab_gap(c.fz, cz, rz);
         if ((gy * gy + gz * gz) * hs2 > best.d2) continue;
         const uint32_t base = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx;
         const uint32_t b = __ldg(g.cell_start + base + x0), e = __ldg(g.cell_start + base + x1 + 1);
@@ -228,29 +258,17 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
       }
     }
     k = 2;
-    // fall through to the termination test with k-1 = 1 completed shells
   }
 
+  // Shells < k are done. Same walk as grid_sweep (grid_sweep.cuh), plus an x-gap prune of the two end cells of
+  // inner rows.
   int row_budget = kFarRowBudget;
 #pragma unroll 1
   for (;; ++k) {
-    // Shells < k are done. Distance (cells) from the query to the nearest face of the scanned
-    // block [c-(k-1), c+(k-1)] that still has grid cells beyond it.
     {
-      const int kk = k - 1;
-      float cover = 3.0e38f;
-      bool any = false;
-      {
-        if (cx - kk > 0) { cover = fminf(cover, fx - (float)(cx - kk)); any = true; }
-        if (cx + kk < g.nx - 1) { cover = fminf(cover, (float)(cx + kk + 1) - fx); any = true; }
-        if (cy - kk > 0) { cover = fminf(cover, fy - (float)(cy - kk)); any = true; }
-        if (cy + kk < g.ny - 1) { cover = fminf(cover, (float)(cy + kk + 1) - fy); any = true; }
-        if (cz - kk > 0) { cover = fminf(cover, fz - (float)(cz - kk)); any = true; }
-        if (cz + kk < g.nz - 1) { cover = fminf(cover, (float)(cz + kk + 1) - fz); any = true; }
-        if (!any) break;  // the whole grid has been scanned
-        cover -= kCellMargin;
-        if (cover > 0.f && cover * cover * hs2 > best.d2) break;
-      }
+      float cover;
+      if (!open_face_gap(g, c, k - 1, cover)) break;  // the whole grid has been scanned
+      if (cover > 0.f && cover * cover * hs2 > best.d2) break;
     }
     // Shell k: rows with max(|dy|,|dz|) == k take the full x-extent, inner rows only the two end cells.
     const int z0 = max(cz - k, 0), z1 = min(cz + k, g.nz - 1);
@@ -258,10 +276,7 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
     row_budget -= (z1 - z0 + 1) * (y1 - y0 + 1);
     if (row_budget < 0) {
       // too much (mostly empty) space crossed shell by shell: restart on the list of non-empty blocks
-      best.d2 = max_d2;
-      best.idx = -1;
-      best.pos = -1;
-      best.tie = false;
+      best = no_best(max_d2);
       far_sweep(
           g, qx, qy, qz, 1u, [&]() { return best.d2; },
           [&](uint32_t b, uint32_t e) { scan_range<kExact>(g.pts, b, e, qx, qy, qz, best); });
@@ -270,12 +285,12 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
     const int xl = cx - k, xr = cx + k;
     const int x0 = max(xl, 0), x1 = min(xr, g.nx - 1);
     for (int rz = z0; rz <= z1; ++rz) {
-      const float gz = slab_gap(fz, cz, rz);
+      const float gz = slab_gap(c.fz, cz, rz);
       const float gz2 = gz * gz;
       if (gz2 * hs2 > best.d2) continue;
       const bool zshell = (rz - cz == k) || (cz - rz == k);
       for (int ry = y0; ry <= y1; ++ry) {
-        const float gy = slab_gap(fy, cy, ry);
+        const float gy = slab_gap(c.fy, cy, ry);
         const float gyz2 = gy * gy + gz2;
         if (gyz2 * hs2 > best.d2) continue;
         const uint32_t base = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx;
@@ -286,14 +301,14 @@ __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, f
           }
         } else {
           if (xl >= 0 && xl < g.nx) {
-            const float gx = slab_gap(fx, cx, xl);
+            const float gx = slab_gap(c.fx, cx, xl);
             if ((gx * gx + gyz2) * hs2 <= best.d2) {
               const uint32_t b = __ldg(g.cell_start + base + xl), e = __ldg(g.cell_start + base + xl + 1);
               scan_range<kExact>(g.pts, b, e, qx, qy, qz, best);
             }
           }
           if (xr >= 0 && xr < g.nx) {
-            const float gx = slab_gap(fx, cx, xr);
+            const float gx = slab_gap(c.fx, cx, xr);
             if ((gx * gx + gyz2) * hs2 <= best.d2) {
               const uint32_t b = __ldg(g.cell_start + base + xr), e = __ldg(g.cell_start + base + xr + 1);
               scan_range<kExact>(g.pts, b, e, qx, qy, qz, best);

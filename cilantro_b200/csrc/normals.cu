@@ -89,10 +89,7 @@ __global__ void __launch_bounds__(kBlock) normals_knn_kernel(const GridView g, i
     auto scan = [&](uint32_t b, uint32_t e) {
       for (uint32_t j = b; j < e; ++j) {
         const float4 p = __ldg(g.pts + j);
-        const float dx = __fsub_rn(s.x, p.x), dy = __fsub_rn(s.y, p.y), dz = __fsub_rn(s.z, p.z);
-        float r = __fmul_rn(dx, dx);
-        r = __fadd_rn(r, __fmul_rn(dy, dy));
-        r = __fadd_rn(r, __fmul_rn(dz, dz));
+        const float r = rule::contract_d2(s.x, s.y, s.z, p.x, p.y, p.z);
         if (!(r < max_d2)) continue;
         const int pi = __float_as_int(p.w);
         if (count == k) {
@@ -161,12 +158,7 @@ __global__ void __launch_bounds__(kBlock) normals_radius_kernel(const GridView g
     const float4 s = __ldg(g.pts + qi);
     const int oi = __float_as_int(s.w);
     auto bound = [&]() { return r2; };
-    auto dist2 = [&](const float4& p) {
-      const float dx = __fsub_rn(s.x, p.x), dy = __fsub_rn(s.y, p.y), dz = __fsub_rn(s.z, p.z);
-      float r = __fmul_rn(dx, dx);
-      r = __fadd_rn(r, __fmul_rn(dy, dy));
-      return __fadd_rn(r, __fmul_rn(dz, dz));
-    };
+    auto dist2 = [&](const float4& p) { return rule::contract_d2(s.x, s.y, s.z, p.x, p.y, p.z); };
     int count = 0;
     float mx = 0.f, my = 0.f, mz = 0.f;
     grid_sweep(g, s.x, s.y, s.z, bound, [&](uint32_t b, uint32_t e) {

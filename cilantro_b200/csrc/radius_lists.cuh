@@ -25,7 +25,7 @@ __global__ void __launch_bounds__(kRadiusBlock) radius_kernel(const cb::GridView
     const float4 s = __ldg(qry + qi);
     const int oi = __float_as_int(s.w);
     float qx, qy, qz;
-    cb::apply_rigid(T, s.x, s.y, s.z, qx, qy, qz);
+    cb::rule::transform_point(T, s.x, s.y, s.z, qx, qy, qz);
     uint32_t n = 0;
     const uint32_t base = kFill ? offsets[oi] : 0u;
     cb::grid_sweep(
@@ -33,10 +33,7 @@ __global__ void __launch_bounds__(kRadiusBlock) radius_kernel(const cb::GridView
         [&](uint32_t b, uint32_t e) {
           for (uint32_t j = b; j < e; ++j) {
             const float4 p = __ldg(g.pts + j);
-            const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-            float r = __fmul_rn(dx, dx);
-            r = __fadd_rn(r, __fmul_rn(dy, dy));
-            r = __fadd_rn(r, __fmul_rn(dz, dz));
+            const float r = cb::rule::contract_d2(qx, qy, qz, p.x, p.y, p.z);
             if (r < r2) {
               if (kFill) {
                 out_idx[base + n] = __float_as_int(p.w);

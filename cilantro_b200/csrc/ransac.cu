@@ -89,7 +89,7 @@ __global__ void ransac_residual_kernel(const float* __restrict__ dst, const floa
                                        const Rigid T, float* __restrict__ out) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     float qx, qy, qz;
-    apply_rigid(T, src[3 * i], src[3 * i + 1], src[3 * i + 2], qx, qy, qz);
+    rule::transform_point(T, src[3 * i], src[3 * i + 1], src[3 * i + 2], qx, qy, qz);
     const float e0 = __fsub_rn(qx, dst[3 * i]), e1 = __fsub_rn(qy, dst[3 * i + 1]), e2 = __fsub_rn(qz, dst[3 * i + 2]);
     out[i] = __fsqrt_rn(sum3(__fmul_rn(e0, e0), __fmul_rn(e1, e1), __fmul_rn(e2, e2)));
   }
@@ -107,7 +107,7 @@ __global__ void __launch_bounds__(kReduceBlock) inlier_moments_kernel(const floa
     const float s0 = src[3 * i], s1 = src[3 * i + 1], s2 = src[3 * i + 2];
     const float d0 = dst[3 * i], d1 = dst[3 * i + 1], d2 = dst[3 * i + 2];
     float qx, qy, qz;
-    apply_rigid(T, s0, s1, s2, qx, qy, qz);
+    rule::transform_point(T, s0, s1, s2, qx, qy, qz);
     const float e0 = __fsub_rn(qx, d0), e1 = __fsub_rn(qy, d1), e2 = __fsub_rn(qz, d2);
     const float x = sum3(__fmul_rn(e0, e0), __fmul_rn(e1, e1), __fmul_rn(e2, e2));
     if (!(x <= x_max)) continue;

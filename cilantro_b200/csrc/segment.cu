@@ -80,13 +80,6 @@ struct SegArgs {
   uint32_t* next_count;
 };
 
-__device__ __forceinline__ float dist2(float qx, float qy, float qz, const float4& p) {
-  const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-  float r = __fmul_rn(dx, dx);
-  r = __fadd_rn(r, __fmul_rn(dy, dy));
-  return __fadd_rn(r, __fmul_rn(dz, dz));
-}
-
 #ifdef CB_SEGMENT_COUNTERS
 __device__ unsigned long long g_uf_counts[5];  // unions, find steps, CAS, failed CAS, far-path resets
 #endif
@@ -138,7 +131,7 @@ __global__ void __launch_bounds__(kBlock, kBlocksPerSm) segment_kernel(const Seg
               const float4 p = __ldg(g.pts + j);
               const uint32_t oi = (uint32_t)__float_as_int(p.w);
               if (oi <= po) continue;
-              const float r = dist2(s.x, s.y, s.z, p);
+              const float r = rule::contract_d2(s.x, s.y, s.z, p.x, p.y, p.z);
               if (r < r2) emit(j, r, oi);
             }
           },
@@ -156,7 +149,7 @@ __global__ void __launch_bounds__(kBlock, kBlocksPerSm) segment_kernel(const Seg
           [&](uint32_t b, uint32_t e) {
             for (uint32_t j = b; j < e; ++j) {
               const float4 p = __ldg(g.pts + j);
-              const float r = dist2(s.x, s.y, s.z, p);
+              const float r = rule::contract_d2(s.x, s.y, s.z, p.x, p.y, p.z);
               if (!(r < r2)) continue;
               const uint32_t oi = (uint32_t)__float_as_int(p.w);
               if (!held) {
@@ -190,7 +183,7 @@ __global__ void __launch_bounds__(kBlock, kBlocksPerSm) segment_kernel(const Seg
           [&](uint32_t b, uint32_t e) {
             for (uint32_t j = b; j < e; ++j) {
               const float4 p = __ldg(g.pts + j);
-              const float r = dist2(s.x, s.y, s.z, p);
+              const float r = rule::contract_d2(s.x, s.y, s.z, p.x, p.y, p.z);
               if (r < max_d2) kbest_insert<K>(bd, bi, k, count, r, __float_as_int(p.w));
             }
           },

@@ -13,16 +13,16 @@
 // cell, a region is scanned iff its lower bound is below (sqrt(best) + slack)^2 instead of best, the two
 // smallest distances are tracked instead of one, and D2 = min(second smallest scanned, the widened bound,
 // the squared distance to the boundary of the scanned 3x3x3 block).
+// The shared-memory arrays and item decode (warp_search.cuh), the 4-wide candidate loop and the termination test
+// (nn_search.cuh) are the narrow search's. Phase A keeps its own copy of the region enumeration (compared against
+// wide2 instead of the best distance): calling queue_regions() here costs the <3,*> search kernels 4-12 B of spills.
 #pragma once
 #include "warp_search.cuh"
 
 namespace cb {
 
-struct WideSearchSmem {
-  float4 q[32];                // query position
-  unsigned long long key[32];  // merged best: d2 bits << 32 | sorted position (0xffffffff = none)
-  unsigned int sec[32];        // merged second-smallest d2 (float bits; non-negative floats order like uints)
-  uint2 item[kWarpItemsMax];   // .x = first cell index, .y = (#cells << 8) | lane
+struct WideSearchSmem : WarpQueue {
+  unsigned int sec[32];  // merged second-smallest d2 (float bits; non-negative floats order like uints)
 };
 
 struct WideBest {
@@ -46,25 +46,9 @@ __device__ __forceinline__ void two_smallest(float r, int j, float& b1, int& p1,
 // scans [b, e) tracking the two smallest distances; position `skip` (already accounted for) is ignored
 __device__ __forceinline__ void scan_range_two(const float4* __restrict__ pts, uint32_t b, uint32_t e, float qx, float qy,
                                                float qz, float& b1, int& p1, float& b2, int skip) {
-  constexpr int kW = 4;
-  auto eval = [&](const float4& p, uint32_t j) {
-    const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-    float r = __fmul_rn(dx, dx);
-    r = __fadd_rn(r, __fmul_rn(dy, dy));
-    r = __fadd_rn(r, __fmul_rn(dz, dz));
+  scan_batched(pts, b, e, qx, qy, qz, [&](float r, uint32_t j) {
     if ((int)j != skip) two_smallest(r, (int)j, b1, p1, b2);
-  };
-  for (uint32_t j = b; j < e; j += kW) {
-    float4 p[kW];
-    p[0] = __ldg(pts + j);
-#pragma unroll
-    for (int u = 1; u < kW; u++)
-      if (j + u < e) p[u] = __ldg(pts + j + u);
-    eval(p[0], j);
-#pragma unroll
-    for (int u = 1; u < kW; u++)
-      if (j + u < e) eval(p[u], j + u);
-  }
+  });
 }
 
 // All 32 lanes of the warp must call this (inactive lanes pass active = false).
@@ -81,21 +65,15 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
   out.pos = -1;
   out.D2 = 0.f;
 
-  const float fx = cell_coord(qx, g.ox, g.inv_h), fy = cell_coord(qy, g.oy, g.inv_h), fz = cell_coord(qz, g.oz, g.inv_h);
-  const int cx = (int)floorf(fx), cy = (int)floorf(fy), cz = (int)floorf(fz);
-  const float hs2 = g.hs2;
-  const bool inside = active && g.n > 0 && cx >= 0 && cx < g.nx && cy >= 0 && cy < g.ny && cz >= 0 && cz < g.nz;
+  const QueryCell c = query_cell(g, qx, qy, qz);
+  const bool inside = active && g.n > 0 && c.cx >= 0 && c.cx < g.nx && c.cy >= 0 && c.cy < g.ny && c.cz >= 0 && c.cz < g.nz;
   bool slow = active && g.n > 0 && !inside;  // outside the grid: per-lane exact search at the end
 
   float b1 = kInf, b2 = kInf;  // two smallest distances over ALL scanned candidates (regardless of max_d2)
   int p1 = -1;
   if (inside && warm_pos >= 0) {
     const float4 p = __ldg(g.pts + warm_pos);
-    const float dx = __fsub_rn(qx, p.x), dy = __fsub_rn(qy, p.y), dz = __fsub_rn(qz, p.z);
-    float r = __fmul_rn(dx, dx);
-    r = __fadd_rn(r, __fmul_rn(dy, dy));
-    r = __fadd_rn(r, __fmul_rn(dz, dz));
-    b1 = r;
+    b1 = rule::contract_d2(qx, qy, qz, p.x, p.y, p.z);
     p1 = warm_pos;
   }
   sm.q[lane] = make_float4(qx, qy, qz, 0.f);
@@ -105,11 +83,11 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
   unsigned int count = 0;  // warp-uniform number of queued items
   float wide2 = 0.f;       // regions with a lower bound > wide2 are not scanned
   {
-    const uint32_t cbase = inside ? ((uint32_t)cz * (uint32_t)g.ny + (uint32_t)cy) * (uint32_t)g.nx : 0u;
+    const uint32_t cbase = inside ? ((uint32_t)c.cz * (uint32_t)g.ny + (uint32_t)c.cy) * (uint32_t)g.nx : 0u;
     uint32_t s1 = 0, s2 = 0;
     if (inside) {
-      s1 = __ldg(g.cell_start + cbase + cx);
-      s2 = __ldg(g.cell_start + cbase + cx + 1);
+      s1 = __ldg(g.cell_start + cbase + c.cx);
+      s2 = __ldg(g.cell_start + cbase + c.cx + 1);
       scan_range_two(g.pts, s1, s2, qx, qy, qz, b1, p1, b2, warm_pos);
     }
     {
@@ -117,12 +95,12 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
       const float w = __fadd_ru(__fsqrt_ru(fminf(b1, max_d2)), slack);
       wide2 = __fmul_ru(w, w);
     }
-    const float gxl = slab_gap(fx, cx, cx - 1), gxr = slab_gap(fx, cx, cx + 1);
-    const float gym = slab_gap(fy, cy, cy - 1), gyp = slab_gap(fy, cy, cy + 1);
-    const float gzm = slab_gap(fz, cz, cz - 1), gzp = slab_gap(fz, cz, cz + 1);
+    const float gxl = slab_gap(c.fx, c.cx, c.cx - 1), gxr = slab_gap(c.fx, c.cx, c.cx + 1);
+    const float gym = slab_gap(c.fy, c.cy, c.cy - 1), gyp = slab_gap(c.fy, c.cy, c.cy + 1);
+    const float gzm = slab_gap(c.fz, c.cz, c.cz - 1), gzp = slab_gap(c.fz, c.cz, c.cz + 1);
     const float gy2[3] = {gym * gym, 0.f, gyp * gyp};
     const float gz2[3] = {gzm * gzm, 0.f, gzp * gzp};
-    const int xm = max(cx - 1, 0), xp = min(cx + 1, g.nx - 1);
+    const int xm = max(c.cx - 1, 0), xp = min(c.cx + 1, g.nx - 1);
     constexpr int kDy[8] = {-1, 1, 0, 0, -1, 1, -1, 1};
     constexpr int kDz[8] = {0, 0, -1, 1, -1, -1, 1, 1};
     // (Tried: a 10-bit need mask per lane, ONE warp scan and lane-major item order instead of a ballot per region -
@@ -134,17 +112,17 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
       uint32_t first;
       uint32_t ncells;
       if (t == 0) {  // left x-neighbour
-        need = inside && cx > 0 && (gxl * gxl * hs2 <= wide2);
-        first = cbase + (uint32_t)(cx - 1);
+        need = inside && c.cx > 0 && (gxl * gxl * g.hs2 <= wide2);
+        first = cbase + (uint32_t)(c.cx - 1);
         ncells = 1;
       } else if (t == 1) {  // right x-neighbour
-        need = inside && cx < g.nx - 1 && (gxr * gxr * hs2 <= wide2);
-        first = cbase + (uint32_t)(cx + 1);
+        need = inside && c.cx < g.nx - 1 && (gxr * gxr * g.hs2 <= wide2);
+        first = cbase + (uint32_t)(c.cx + 1);
         ncells = 1;
       } else {
-        const int ry = cy + kDy[t - 2], rz = cz + kDz[t - 2];
+        const int ry = c.cy + kDy[t - 2], rz = c.cz + kDz[t - 2];
         const bool valid = inside && ry >= 0 && ry < g.ny && rz >= 0 && rz < g.nz;
-        need = valid && ((gy2[kDy[t - 2] + 1] + gz2[kDz[t - 2] + 1]) * hs2 <= wide2);
+        need = valid && ((gy2[kDy[t - 2] + 1] + gz2[kDz[t - 2] + 1]) * g.hs2 <= wide2);
         first = ((uint32_t)rz * (uint32_t)g.ny + (uint32_t)ry) * (uint32_t)g.nx + (uint32_t)xm;
         ncells = (uint32_t)(xp - xm + 1);
       }
@@ -165,27 +143,24 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
 
   // ---- phase B: pooled scan of the queued regions ----------------------------------------------------
   for (unsigned int k = lane; k < count; k += 32) {
-    const uint2 it = sm.item[k];
-    const unsigned int ql = it.y & 31u, nc = it.y >> 8;
-    const float4 q = sm.q[ql];
-    const uint32_t b = __ldg(g.cell_start + it.x), e = __ldg(g.cell_start + it.x + nc);
-    if (b >= e) continue;
-    const unsigned long long cur = sm.key[ql];
+    const QueueItem it = queue_item(g, sm, k);
+    if (it.b >= it.e) continue;
+    const unsigned long long cur = sm.key[it.lane];
     float l1 = kInf, l2 = kInf;
     int lp = -1;
     // the only point that can be met twice is the warm seed, and only while it is the running best
-    scan_range_two(g.pts, b, e, q.x, q.y, q.z, l1, lp, l2, (int)(unsigned int)(cur & 0xffffffffull));
+    scan_range_two(g.pts, it.b, it.e, it.q.x, it.q.y, it.q.z, l1, lp, l2, (int)(unsigned int)(cur & 0xffffffffull));
     if (lp < 0) continue;
     float loser = l1;  // what this region contributes to "second smallest" besides l2
     if (l1 < max_d2) {
       const unsigned long long key = pack_key(l1, (unsigned int)lp);
-      const unsigned long long old = atomicMin(&sm.key[ql], key);
+      const unsigned long long old = atomicMin(&sm.key[it.lane], key);
       const float od2 = __uint_as_float((unsigned int)(old >> 32));
       // the loser of (previous best, this region's best) is a second-best candidate; the initial "none"
       // sentinel is not a point
       loser = ((unsigned int)(old & 0xffffffffull) == 0xffffffffu) ? kInf : fmaxf(od2, l1);
     }
-    atomicMin(&sm.sec[ql], __float_as_uint(fminf(l2, loser)));
+    atomicMin(&sm.sec[it.lane], __float_as_uint(fminf(l2, loser)));
   }
   __syncwarp();
 
@@ -196,16 +171,10 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
     out.d2 = __uint_as_float((unsigned int)(key >> 32));
     out.pos = (pos == 0xffffffffu) ? -1 : (int)pos;
     const float sec = __uint_as_float(sm.sec[lane]);
-    float cover = kInf;
-    bool any = false;
-    if (cx - 1 > 0) { cover = fminf(cover, fx - (float)(cx - 1)); any = true; }
-    if (cx + 1 < g.nx - 1) { cover = fminf(cover, (float)(cx + 2) - fx); any = true; }
-    if (cy - 1 > 0) { cover = fminf(cover, fy - (float)(cy - 1)); any = true; }
-    if (cy + 1 < g.ny - 1) { cover = fminf(cover, (float)(cy + 2) - fy); any = true; }
-    if (cz - 1 > 0) { cover = fminf(cover, fz - (float)(cz - 1)); any = true; }
-    if (cz + 1 < g.nz - 1) { cover = fminf(cover, (float)(cz + 2) - fz); any = true; }
-    cover -= kCellMargin;
-    const float cover2 = (!any) ? kInf : (cover > 0.f ? cover * cover * hs2 : 0.f);
+    // shells 0-1 are complete: squared distance to the nearest face with grid cells beyond it (kInf: none)
+    float cover;
+    const bool any = open_face_gap(g, c, 1, cover);
+    const float cover2 = (!any) ? kInf : (cover > 0.f ? cover * cover * g.hs2 : 0.f);
     const bool done = cover2 > out.d2;
     const bool tie = out.pos >= 0 && sec == out.d2;  // a second point at a bit-equal distance: index rule
     if (!done || tie) slow = true;

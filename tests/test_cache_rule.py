@@ -38,3 +38,8 @@ def test_the_cached_pass_kernel_compiles_the_same_rule():
         rule = f.read()
     for intrinsic in ("__fsub_rd", "__fmul_rd", "__fmul_ru", "__fmaf_ru", "__fsqrt_ru", "__fsqrt_rd"):
         assert intrinsic in rule
+    # the searches compute the contract distance through rule::contract_d2, never a private copy of it
+    for name in ("nn_search.cuh", "warp_search.cuh", "warp_search_wide.cuh", "radius_lists.cuh", "knn_k.cu",
+                 "segment.cu", "mean_shift.cu"):
+        with open(os.path.join(CSRC, name)) as f:
+            assert "__fmul_rn(dx, dx)" not in f.read(), name
