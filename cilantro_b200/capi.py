@@ -169,6 +169,27 @@ class WarpResult(C.Structure):
     ]
 
 
+class SparseWarpParams(C.Structure):
+    _fields_ = [("base", WarpParams), ("ctrl_coeff", C.c_float), ("reserved_", C.c_int32)]
+
+
+class SparseWarpResult(C.Structure):
+    _fields_ = [
+        ("iterations", C.c_int32),
+        ("converged", C.c_int32),
+        ("last_delta", C.c_float),
+        ("reserved_", C.c_int32),
+        ("num_corr", C.c_uint64),
+        ("gn_steps", C.c_uint64),
+        ("cg_iterations", C.c_uint64),
+        ("gpu_ms_search", C.c_double),
+        ("gpu_ms_resample", C.c_double),
+        ("gpu_ms_assemble", C.c_double),
+        ("gpu_ms_cg", C.c_double),
+        ("kernel_launches", C.c_uint64),
+    ]
+
+
 class WarpSolveResult(C.Structure):
     _fields_ = [
         ("converged", C.c_int32),
@@ -199,6 +220,9 @@ EXPORTED = [
     "cb_plane_score", "cb_plane_residuals", "cb_ransac_plane",
     "cb_warp_default_params", "cb_warp_icp_create", "cb_warp_icp_destroy", "cb_warp_icp_estimate", "cb_warp_icp_solve",
     "cb_warp_icp_residuals", "cb_warp_icp_correspondences",
+    "cb_sparse_warp_default_params", "cb_sparse_warp_icp_create", "cb_sparse_warp_icp_destroy",
+    "cb_sparse_warp_icp_estimate", "cb_sparse_warp_icp_solve", "cb_sparse_warp_icp_resample",
+    "cb_sparse_warp_icp_residuals", "cb_sparse_warp_icp_correspondences",
     "cb_mean_cov", "cb_pca", "cb_transform_points",
 ]
 
@@ -891,6 +915,101 @@ class WarpIcp:
         v = np.empty(n, np.float32)
         cnt = C.c_size_t()
         _check(lib().cb_warp_icp_correspondences(self.h, _p(i1), _p(i2), _p(v), C.byref(cnt)))
+        c = cnt.value
+        return i1[:c].astype(np.int64), i2[:c].astype(np.int64), v[:c]
+
+
+def sparse_warp_params(ctrl_sigma=1.0, **kw):
+    """cb_sparse_warp_params: warp_params(**kw) plus the control weights' sigma (default 1)."""
+    p = SparseWarpParams()
+    lib().cb_sparse_warp_default_params(C.byref(p))
+    p.base = warp_params(**kw)
+    p.ctrl_coeff = rbf_coeff(ctrl_sigma)
+    return p
+
+
+class SparseWarpIcp:
+    """cb_sparse_warp_icp_*: SimpleCombinedMetricSparseRigidWarpFieldICP3f. ctrl = (offsets, index, value), one list
+    of (node, squared distance) per source point; reg = the node neighbourhoods' CSR. Node transforms are (n_ctrl, 3, 4)
+    and dense transforms (n_src, 3, 4) float32."""
+
+    def __init__(self, ctx, dst: Cloud, src: Cloud, ctrl, n_ctrl, reg):
+        self.ctx, self.dst, self.src, self.n_ctrl = ctx, dst, src, int(n_ctrl)
+        coff = np.ascontiguousarray(ctrl[0], np.uint64)
+        cidx = np.ascontiguousarray(ctrl[1], np.int64)
+        cval = np.ascontiguousarray(ctrl[2], np.float32)
+        roff = np.ascontiguousarray(reg[0], np.uint64)
+        ridx = np.ascontiguousarray(reg[1], np.int64)
+        rval = np.ascontiguousarray(reg[2], np.float32)
+        h = C.c_void_p()
+        _check(lib().cb_sparse_warp_icp_create(ctx.h, dst.h, src.h, _p(coff), _p(cidx), _p(cval),
+                                               C.c_size_t(max(coff.shape[0] - 1, 0)), C.c_size_t(self.n_ctrl),
+                                               _p(roff), _p(ridx), _p(rval), C.c_size_t(max(roff.shape[0] - 1, 0)),
+                                               C.byref(h)))
+        self.h = h
+        ctx._adopt(self)
+
+    def close(self):
+        if self.h:
+            lib().cb_sparse_warp_icp_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def estimate(self, T_init=None, **kw):
+        prm = kw.pop("params", None) or sparse_warp_params(**kw)
+        n, m = self.src.n, self.n_ctrl
+        T = np.empty((max(m, 1), 12), np.float32)
+        Td = np.empty((max(n, 1), 12), np.float32)
+        res = SparseWarpResult()
+        _check(lib().cb_sparse_warp_icp_estimate(self.h, C.byref(prm), _p(_t_set(T_init, m)), _p(T), _p(Td),
+                                                 C.byref(res)))
+        out = {"T": T[:m].reshape(m, 3, 4), "T_dense": Td[:n].reshape(n, 3, 4), "iterations": int(res.iterations),
+               "converged": bool(res.converged), "last_delta": float(res.last_delta)}
+        out.update({k: int(getattr(res, k)) for k in ("num_corr", "gn_steps", "cg_iterations", "kernel_launches")})
+        out.update({k: float(getattr(res, k)) for k in ("gpu_ms_search", "gpu_ms_resample", "gpu_ms_assemble",
+                                                        "gpu_ms_cg")})
+        return out
+
+    def solve(self, first, second, T_dense_src=None, **kw):
+        prm = kw.pop("params", None) or sparse_warp_params(**kw)
+        n, m = self.src.n, self.n_ctrl
+        f = np.ascontiguousarray(first, np.uint64)
+        s = np.ascontiguousarray(second, np.uint64)
+        T = np.empty((max(m, 1), 12), np.float32)
+        x = np.empty((max(m, 1), 6), np.float32)
+        res = WarpSolveResult()
+        _check(lib().cb_sparse_warp_icp_solve(self.h, C.byref(prm), _p(_t_set(T_dense_src, n)), _p(f), _p(s), None,
+                                              C.c_size_t(f.shape[0]), _p(T), _p(x), C.byref(res)))
+        return {"T": T[:m].reshape(m, 3, 4), "x": x[:m], "converged": bool(res.converged), "gn_steps": int(res.gn_steps),
+                "cg_iterations": int(res.cg_iterations), "cg_iterations_last": int(res.cg_iterations_last),
+                "cg_error": float(res.cg_error), "kernel_launches": int(res.kernel_launches)}
+
+    def resample(self, T_ctrl, **kw):
+        prm = kw.pop("params", None) or sparse_warp_params(**kw)
+        n, m = self.src.n, self.n_ctrl
+        Td = np.empty((max(n, 1), 12), np.float32)
+        _check(lib().cb_sparse_warp_icp_resample(self.h, C.byref(prm), _p(_t_set(T_ctrl, m)), _p(Td)))
+        return Td[:n].reshape(n, 3, 4)
+
+    def residuals(self, T_dense, **kw):
+        prm = kw.pop("params", None) or sparse_warp_params(**kw)
+        n = self.src.n
+        out = np.empty(max(n, 1), np.float32)
+        _check(lib().cb_sparse_warp_icp_residuals(self.h, C.byref(prm), _p(_t_set(T_dense, n)), _p(out)))
+        return out[:n]
+
+    def correspondences(self):
+        n = max(self.src.n, 1)
+        i1 = np.empty(n, np.uint64)
+        i2 = np.empty(n, np.uint64)
+        v = np.empty(n, np.float32)
+        cnt = C.c_size_t()
+        _check(lib().cb_sparse_warp_icp_correspondences(self.h, _p(i1), _p(i2), _p(v), C.byref(cnt)))
         c = cnt.value
         return i1[:c].astype(np.int64), i2[:c].astype(np.int64), v[:c]
 

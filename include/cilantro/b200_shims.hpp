@@ -12,6 +12,8 @@
 //   SimpleCombinedMetricRigidICP3f                          registration/icp_common_instances.hpp:261
 //   SimpleCombinedMetricDenseRigidWarpFieldICP3f            registration/icp_common_instances.hpp:99-144,284-285
 //   TransformSet<RigidTransform3f>, transformPoints         core/space_transformations.hpp:60-136,195-223
+//   SimpleCombinedMetricSparseRigidWarpFieldICP3f           registration/icp_common_instances.hpp:146-199,313-314
+//   VectorSet<float,3>, KDTree<float,3>, NeighborhoodSet    core/data_containers.hpp, kd_tree.hpp, nearest_neighbors.hpp
 //   KMeans3f<>                                              clustering/kmeans.hpp:9-59,205-207
 //   RigidTransformRANSACEstimator3f<>                       model_estimation/ransac_transform_estimator.hpp:9-122
 //   PrincipalComponentAnalysis3f                            core/principal_component_analysis.hpp:8-89
@@ -205,6 +207,8 @@ template <typename ScalarT = float, typename IndexT = size_t>
 using NeighborSet = std::vector<Neighbor<ScalarT, IndexT>>;
 template <typename ScalarT = float, typename IndexT = size_t>
 using Neighborhood = NeighborSet<ScalarT, IndexT>;
+template <typename ScalarT = float, typename IndexT = size_t>
+using NeighborhoodSet = std::vector<NeighborSet<ScalarT, IndexT>>;  // core/nearest_neighbors.hpp
 
 // neighbourhood specifications (core/nearest_neighbors.hpp:58-87); radii are squared distances
 template <typename CountT = size_t>
@@ -405,6 +409,24 @@ private:
   ConstVectorSetMatrixMap3f data_map_;
   b200::CloudHandle cloud_;
 };
+
+// VectorSet<float, 3> and KDTree<float, 3> (core/data_containers.hpp, core/kd_tree.hpp): the 3-D float instances are
+// the only ones; any other scalar or dimension is a compile-time error.
+namespace b200 {
+template <class ScalarT, long EigenDim>
+struct Instance3f {
+  static_assert(sizeof(ScalarT) == 0, "cilantro_b200 provides the <float, 3> instances only");
+};
+template <>
+struct Instance3f<float, 3> {
+  using VectorSet = VectorSet3f;
+  using KDTree = KDTree3f<>;
+};
+}  // namespace b200
+template <class ScalarT, long EigenDim>
+using VectorSet = typename b200::Instance3f<ScalarT, EigenDim>::VectorSet;
+template <class ScalarT, long EigenDim, class... DistanceAdaptorT>
+using KDTree = typename b200::Instance3f<ScalarT, EigenDim>::KDTree;
 
 // ---- ICP ---------------------------------------------------------------------------------------------
 enum struct CorrespondenceSearchDirection { FIRST_TO_SECOND, SECOND_TO_FIRST, BOTH };
@@ -895,6 +917,213 @@ private:
   PointToPointCorrespondenceWeightEvaluator pt_eval_;
   PointToPlaneCorrespondenceWeightEvaluator pl_eval_;
   RegularizationWeightEvaluator reg_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
+  CorrespondenceSet<float, size_t> corr_;
+  bool corr_fresh_ = false;
+};
+
+// ---- SimpleCombinedMetricSparseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:146-199, 313-314) ---------
+// CombinedMetricSparseWarpFieldICP<RigidTransform<float,3>> (icp_warp_field_combined_metric_sparse.hpp) with the Simple
+// instance's evaluators (unity data-term weights, RBFKernelWeightEvaluator<float, float, true> control and
+// regularisation weights) on cb_sparse_warp_icp_* (DESIGN §4.14). getTransform() holds one transform per control
+// node, getDenseWarpField() one per source point. The correspondence engine takes the default settings only.
+class SimpleCombinedMetricSparseRigidWarpFieldICP3f {
+public:
+  using Transform = TransformSet<RigidTransform3f>;
+  using PointToPointCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
+  using PointToPlaneCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
+  using ControlWeightEvaluator = RBFKernelWeightEvaluator<float, float, true>;
+  using RegularizationWeightEvaluator = RBFKernelWeightEvaluator<float, float, true>;
+
+  // src_to_control_nn: one list of (node, squared distance) per source point; regularization_nn: one list per node
+  // neighbourhood, N[0] the centre (what KDTree<float, 3>::search over the nodes returns)
+  template <typename IndexT, typename RegIndexT>
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f(const ConstVectorSetMatrixMap3f& dst_p,
+                                                const ConstVectorSetMatrixMap3f& dst_n,
+                                                const ConstVectorSetMatrixMap3f& src_p,
+                                                const std::vector<NeighborSet<float, IndexT>>& src_to_control_nn,
+                                                size_t num_control_nodes,
+                                                const std::vector<NeighborSet<float, RegIndexT>>& regularization_nn)
+      : n_src_(src_p.cols()), n_ctrl_(num_control_nodes) {
+    const float* dn = (dst_n.cols() == dst_p.cols() && dst_p.cols() > 0) ? dst_n.data() : nullptr;
+    b200::check(cb_cloud_create_pair(b200::Context::get(), dst_p.data(), dn, dst_p.cols(), 0, src_p.data(), nullptr,
+                                     src_p.cols(), 0, &dst_.h, &src_.h),
+                "cb_cloud_create_pair");
+    std::vector<uint64_t> coff, roff;
+    std::vector<int64_t> cidx, ridx;
+    std::vector<float> cval, rval;
+    csr(src_to_control_nn, coff, cidx, cval);
+    csr(regularization_nn, roff, ridx, rval);
+    b200::check(cb_sparse_warp_icp_create(b200::Context::get(), dst_.h, src_.h, coff.data(), cidx.data(), cval.data(),
+                                          src_to_control_nn.size(), n_ctrl_, roff.data(), ridx.data(), rval.data(),
+                                          regularization_nn.size(), &icp_),
+                "cb_sparse_warp_icp_create");
+    cb_sparse_warp_default_params(&prm_);
+    std::memset(&res_, 0, sizeof(res_));
+    res_.last_delta = std::numeric_limits<float>::infinity();
+    transform_init_.assign(n_ctrl_, RigidTransform3f());
+    transform_.assign(n_ctrl_, RigidTransform3f());
+    transform_dense_.assign(n_src_, RigidTransform3f());
+  }
+  ~SimpleCombinedMetricSparseRigidWarpFieldICP3f() {
+    if (icp_) cb_sparse_warp_icp_destroy(icp_);
+  }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f(const SimpleCombinedMetricSparseRigidWarpFieldICP3f&) = delete;
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& operator=(const SimpleCombinedMetricSparseRigidWarpFieldICP3f&) = delete;
+
+  CorrespondenceSearchEngineB200& correspondenceSearchEngine() { return engine_; }
+  PointToPointCorrespondenceWeightEvaluator& pointToPointCorrespondenceWeightEvaluator() { return pt_eval_; }
+  PointToPlaneCorrespondenceWeightEvaluator& pointToPlaneCorrespondenceWeightEvaluator() { return pl_eval_; }
+  ControlWeightEvaluator& controlWeightEvaluator() { return ctrl_eval_; }
+  RegularizationWeightEvaluator& regularizationWeightEvaluator() { return reg_eval_; }
+
+  // IterativeClosestPointBase surface (registration/icp_base.hpp:40-106)
+  size_t getMaxNumberOfIterations() const { return (size_t)prm_.base.max_iter; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setMaxNumberOfIterations(size_t n) {
+    prm_.base.max_iter = (int32_t)n;
+    return *this;
+  }
+  float getConvergenceTolerance() const { return prm_.base.tol; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setConvergenceTolerance(float tol) {
+    prm_.base.tol = tol;
+    return *this;
+  }
+  const Transform& getInitialTransform() const { return transform_init_; }
+  Transform& initialTransform() { return transform_init_; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setInitialTransform(const Transform& T) {
+    transform_init_ = T;
+    return *this;
+  }
+  size_t getNumberOfPerformedIterations() const { return (size_t)res_.iterations; }
+  float getLastUpdateNorm() const { return res_.last_delta; }
+  bool hasConverged() const { return res_.last_delta < prm_.base.tol; }  // icp_base.hpp:106
+  const Transform& getTransform() const { return transform_; }
+  const Transform& getDenseWarpField() const { return transform_dense_; }
+
+  // CombinedMetricSparseWarpFieldICP surface
+  float getPointToPointMetricWeight() const { return prm_.base.w_pt; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setPointToPointMetricWeight(float w) {
+    prm_.base.w_pt = w;
+    return *this;
+  }
+  float getPointToPlaneMetricWeight() const { return prm_.base.w_pl; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setPointToPlaneMetricWeight(float w) {
+    prm_.base.w_pl = w;
+    return *this;
+  }
+  float getStiffnessRegularizationWeight() const { return prm_.base.stiffness; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setStiffnessRegularizationWeight(float w) {
+    prm_.base.stiffness = w;
+    return *this;
+  }
+  size_t getMaxNumberOfGaussNewtonIterations() const { return (size_t)prm_.base.max_gn_iter; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setMaxNumberOfGaussNewtonIterations(size_t n) {
+    prm_.base.max_gn_iter = n;
+    return *this;
+  }
+  float getGaussNewtonConvergenceTolerance() const { return prm_.base.gn_tol; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setGaussNewtonConvergenceTolerance(float tol) {
+    prm_.base.gn_tol = tol;
+    return *this;
+  }
+  size_t getMaxNumberOfConjugateGradientIterations() const { return (size_t)prm_.base.max_cg_iter; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setMaxNumberOfConjugateGradientIterations(size_t n) {
+    prm_.base.max_cg_iter = n;
+    return *this;
+  }
+  float getConjugateGradientConvergenceTolerance() const { return prm_.base.cg_tol; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setConjugateGradientConvergenceTolerance(float tol) {
+    prm_.base.cg_tol = tol;
+    return *this;
+  }
+  float getHuberLossBoundary() const { return prm_.base.huber; }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setHuberLossBoundary(float huber_boundary) {
+    prm_.base.huber = huber_boundary;
+    return *this;
+  }
+
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& estimate() {
+    if (transform_init_.size() != n_ctrl_) throw std::runtime_error("initial transform: one transform per control node expected");
+    fill();
+    std::vector<float> T_in(12 * n_ctrl_), T_out(12 * n_ctrl_), T_dense(12 * n_src_);
+    for (size_t j = 0; j < n_ctrl_; j++) std::memcpy(&T_in[12 * j], transform_init_[j].data(), 12 * sizeof(float));
+    b200::check(cb_sparse_warp_icp_estimate(icp_, &prm_, T_in.data(), T_out.data(), T_dense.data(), &res_),
+                "cb_sparse_warp_icp_estimate");
+    for (size_t j = 0; j < n_ctrl_; j++) transform_[j] = RigidTransform3f(&T_out[12 * j]);
+    for (size_t i = 0; i < n_src_; i++) transform_dense_[i] = RigidTransform3f(&T_dense[12 * i]);
+    corr_fresh_ = false;
+    return *this;
+  }
+  SimpleCombinedMetricSparseRigidWarpFieldICP3f& estimate(size_t max_iter, float conv_tol) {
+    prm_.base.max_iter = (int32_t)max_iter;
+    prm_.base.tol = conv_tol;
+    return estimate();
+  }
+
+  // getResiduals() -> computeResiduals() (icp_warp_field_combined_metric_sparse.hpp:243-263) on the dense field
+  std::vector<float> getResiduals() {
+    fill();
+    std::vector<float> T(12 * n_src_), r(n_src_);
+    for (size_t i = 0; i < n_src_; i++) std::memcpy(&T[12 * i], transform_dense_[i].data(), 12 * sizeof(float));
+    b200::check(cb_sparse_warp_icp_residuals(icp_, &prm_, T.data(), r.data()), "cb_sparse_warp_icp_residuals");
+    return r;
+  }
+
+  // correspondenceSearchEngine().getCorrespondences() after estimate(): the last iteration's list
+  const CorrespondenceSet<float, size_t>& getCorrespondences() {
+    if (!corr_fresh_) {
+      std::vector<uint64_t> a(n_src_), b(n_src_);
+      std::vector<float> v(n_src_);
+      size_t cnt = 0;
+      b200::check(cb_sparse_warp_icp_correspondences(icp_, a.data(), b.data(), v.data(), &cnt),
+                  "cb_sparse_warp_icp_correspondences");
+      corr_.resize(cnt);
+      for (size_t i = 0; i < cnt; i++) corr_[i] = {(size_t)a[i], (size_t)b[i], v[i]};
+      corr_fresh_ = true;
+    }
+    return corr_;
+  }
+
+  uint64_t getNumberOfConjugateGradientIterations() const { return res_.cg_iterations; }  // over the last estimate()
+  double getLastEstimateDeviceMilliseconds() const {
+    return res_.gpu_ms_search + res_.gpu_ms_resample + res_.gpu_ms_assemble + res_.gpu_ms_cg;
+  }
+
+private:
+  template <typename IndexT>
+  static void csr(const std::vector<NeighborSet<float, IndexT>>& lists, std::vector<uint64_t>& off,
+                  std::vector<int64_t>& idx, std::vector<float>& val) {
+    off.assign(lists.size() + 1, 0);
+    for (size_t j = 0; j < lists.size(); j++) {
+      for (const auto& nb : lists[j]) {
+        idx.push_back(static_cast<int64_t>(nb.index));
+        val.push_back(nb.value);
+      }
+      off[j + 1] = idx.size();
+    }
+  }
+  void fill() {
+    cb_icp_params e;
+    cb_icp_default_params(&e);
+    engine_.fill(e);
+    prm_.base.max_d2 = e.max_d2;
+    prm_.base.search_dir = e.search_dir;
+    prm_.base.inlier_fraction = e.inlier_fraction;
+    prm_.base.require_reciprocal = e.require_reciprocal;
+    prm_.base.one_to_one = e.one_to_one;
+    prm_.base.reg_coeff = reg_eval_.b200_coeff();
+    prm_.ctrl_coeff = ctrl_eval_.b200_coeff();
+  }
+  size_t n_src_, n_ctrl_;
+  b200::CloudHandle dst_, src_;
+  cb_sparse_warp_icp* icp_ = nullptr;
+  cb_sparse_warp_params prm_;
+  cb_sparse_warp_result res_;
+  Transform transform_init_, transform_, transform_dense_;
+  CorrespondenceSearchEngineB200 engine_;
+  PointToPointCorrespondenceWeightEvaluator pt_eval_;
+  PointToPlaneCorrespondenceWeightEvaluator pl_eval_;
+  ControlWeightEvaluator ctrl_eval_;        // sigma 1 (common_pair_evaluators.hpp:51)
+  RegularizationWeightEvaluator reg_eval_;  // sigma 1
   CorrespondenceSet<float, size_t> corr_;
   bool corr_fresh_ = false;
 };

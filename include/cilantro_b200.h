@@ -540,6 +540,80 @@ int cb_warp_icp_residuals(cb_warp_icp* icp, const cb_warp_params* prm, const flo
 int cb_warp_icp_correspondences(cb_warp_icp* icp, uint64_t* index_first, uint64_t* index_second, float* value,
                                 size_t* count);
 
+/* ---- non-rigid ICP: sparse rigid warp field on control nodes ------------------------------------
+ * cb_sparse_warp_icp_* replaces SimpleCombinedMetricSparseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:
+ * 146-199, 313-314) = CombinedMetricSparseWarpFieldICP (registration/icp_warp_field_combined_metric_sparse.hpp) on the
+ * loop of IterativeClosestPointBase::estimate (icp_base.hpp:68-87); DESIGN §4.14. n_ctrl control nodes carry one rigid
+ * transform each (float32[12], row-major [R | t]); source point i carries a control list (the nodes n_ik that move it,
+ * with squared distances d2_ik) and its dense transform is resampleTransforms (warp_field_utilities.hpp:14-48):
+ * w_ik = exp(ctrl_coeff d2_ik) over the list in the given order, T_i = (rotation(sum w R / W), sum w t / W),
+ * W = sum w, the identity when W = 0. One ICP iteration: the 1-NN of T_i s_i within max_d2 (as cb_warp_icp), then
+ * estimateSparseWarpFieldCombinedMetric (warp_field_estimation.hpp:1388-1846): 6 unknowns per node starting at zero,
+ * point i linearised at the weighted mean (sum_k w_ik x_{n_ik}) / W_i of its list sorted by node, the dense
+ * estimator's data rows with the entry of node n_ik scaled by sqrt(w) w_ik / W_i and the residual by sqrt(w) (rows
+ * of zero when W_i = 0), and the Huber arcs (N[0], N[j]) of the node neighbourhoods as in cb_warp_icp; then the node
+ * transforms are composed as TransformSet::preApply, resampled onto the points, and
+ * last_delta = sqrt(max_j |dR_j - I|_F^2 + |dt_j|^2) over the nodes.
+ * Defined here where the reference is undefined or silent: a control-list count other than n_src, a control index
+ * >= n_ctrl and a regularisation index >= n_ctrl are CB_ERR_INVALID; an empty control list gives the identity and
+ * no data rows; a node no point and no arc touches keeps the identity; duplicate nodes in one list are summed (the
+ * sort is stable). Everything else (empty neighbourhoods, self-arcs, non-finite points, w_pl > 0 without normals,
+ * engine options, ranks, the 2^31 - 1 point limit) follows cb_warp_icp. */
+typedef struct cb_sparse_warp_params {
+  cb_warp_params base;   /* the dense parameters; base.reg_coeff weighs the regularisation arcs */
+  float ctrl_coeff;      /* control weights, RBFKernelWeightEvaluator<float, float, true>: -0.5f / sigma^2, sigma 1 */
+  int32_t reserved_;
+} cb_sparse_warp_params;
+
+typedef struct cb_sparse_warp_result {
+  int32_t iterations;       /* getNumberOfPerformedIterations() */
+  int32_t converged;        /* hasConverged(): last_delta < tol */
+  float last_delta;
+  int32_t reserved_;
+  uint64_t num_corr;        /* correspondences of the last iteration */
+  uint64_t gn_steps;        /* Gauss-Newton steps over all iterations */
+  uint64_t cg_iterations;   /* conjugate-gradient iterations over all steps */
+  double gpu_ms_search;     /* CUDA-event time of the correspondence searches */
+  double gpu_ms_resample;   /* ... of resampling node transforms onto the points (after each compose) */
+  double gpu_ms_assemble;   /* ... of the per-point and per-node assembly */
+  double gpu_ms_cg;         /* ... of the CG launches */
+  uint64_t kernel_launches;
+} cb_sparse_warp_result;
+
+typedef struct cb_sparse_warp_icp cb_sparse_warp_icp;
+
+void cb_sparse_warp_default_params(cb_sparse_warp_params* p);
+/* dst (with normals for w_pl > 0) and src must outlive the object. Control lists: a host CSR of n_ctrl_lists lists
+ * (= n_src) of (node index, squared distance), e.g. the kNN of each source point among the nodes; regularisation
+ * neighbourhoods: a CSR over the nodes as in cb_warp_icp_create. Both are validated and uploaded once; the
+ * node -> (point, entry) and arc incidences are built on the device by the stable radix sort. */
+int cb_sparse_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const uint64_t* ctrl_offsets,
+                              const int64_t* ctrl_index, const float* ctrl_value, size_t n_ctrl_lists, size_t n_ctrl,
+                              const uint64_t* reg_offsets, const int64_t* reg_index, const float* reg_value,
+                              size_t n_reg, cb_sparse_warp_icp** out);
+void cb_sparse_warp_icp_destroy(cb_sparse_warp_icp* icp);
+/* estimate() followed by getTransform() and getDenseWarpField(): T_init (n_ctrl x 12, NULL = identities) -> T_out
+ * (n_ctrl x 12); T_dense_out (n_src x 12, may be NULL) = the resampled per-point transforms. */
+int cb_sparse_warp_icp_estimate(cb_sparse_warp_icp* icp, const cb_sparse_warp_params* prm, const float* T_init,
+                                float* T_out, float* T_dense_out, cb_sparse_warp_result* res);
+/* estimateSparseWarpFieldCombinedMetric on the source transformed by T_dense_src (n_src x 12, NULL = identities) with
+ * the caller's correspondences (as cb_warp_icp_solve). T_out (n_ctrl x 12) = the estimated node transforms; x_out
+ * (n_ctrl x 6, may be NULL) = the unknowns (a, b, c, tx, ty, tz) per node. An index out of range: CB_ERR_INVALID. */
+int cb_sparse_warp_icp_solve(cb_sparse_warp_icp* icp, const cb_sparse_warp_params* prm, const float* T_dense_src,
+                             const uint64_t* corr_first, const uint64_t* corr_second, const float* corr_value,
+                             size_t n_corr, float* T_out, float* x_out, cb_warp_solve_result* res);
+/* resampleTransforms (warp_field_utilities.hpp:14-48) with the control weights of prm: node transforms T_ctrl
+ * (n_ctrl x 12) -> T_dense_out (n_src x 12). */
+int cb_sparse_warp_icp_resample(cb_sparse_warp_icp* icp, const cb_sparse_warp_params* prm, const float* T_ctrl,
+                                float* T_dense_out);
+/* computeResiduals() (icp_warp_field_combined_metric_sparse.hpp:243-263) for the dense field T_dense (n_src x 12), as
+ * cb_warp_icp_residuals. */
+int cb_sparse_warp_icp_residuals(cb_sparse_warp_icp* icp, const cb_sparse_warp_params* prm, const float* T_dense,
+                                 float* out);
+/* getCorrespondences() after the last iteration of the last estimate(), ascending source index; arrays hold n_src. */
+int cb_sparse_warp_icp_correspondences(cb_sparse_warp_icp* icp, uint64_t* index_first, uint64_t* index_second,
+                                       float* value, size_t* count);
+
 /* ---- covariance / PCA ------------------------------------------------------------------------
  * Replaces Covariance<float,3>::operator() (core/covariance.hpp:31-80) and
  * PrincipalComponentAnalysis<float,3> (core/principal_component_analysis.hpp:76-84).

@@ -98,6 +98,25 @@ def main():
     f, s, _ = wicp.correspondences()
     wicp.solve(f, s, w_pt=0.1, max_gn_iter=1, max_cg_iter=20)
     wicp.residuals(got["T"], w_pt=0.1)
+    # sparse warp-field ICP: weights, resampling, assembly at points and nodes, the cooperative CG with its extra grid
+    # sync and compose over the nodes; a duplicate node in one list, an empty list and a node nothing touches
+    nodes = wsrc.grid_downsample(0.025)
+    off, idx, val = capi.neighborhood_csr(*capi.knn_radius(ctx, nodes, wsrc, 4))
+    cl = [list(idx[off[i]:off[i + 1]]) for i in range(len(off) - 1)]
+    cv = [list(val[off[i]:off[i + 1]]) for i in range(len(off) - 1)]
+    cl[3], cv[3] = cl[3] + cl[3][:1], cv[3] + cv[3][:1]
+    cl[5], cv[5] = [], []
+    coff = np.zeros(len(cl) + 1, np.uint64)
+    coff[1:] = np.cumsum([len(a) for a in cl])
+    ctrl = (coff, np.concatenate([np.asarray(a, np.int64) for a in cl]), np.concatenate([np.asarray(a, np.float32) for a in cv]))
+    sicp = capi.SparseWarpIcp(ctx, capi.Cloud(ctx, wp["dst"], wp["dst_normals"]), wsrc, ctrl, nodes.n + 1,
+                              capi.neighborhood_csr(*capi.knn_radius(ctx, nodes, nodes, 8)))
+    got = sicp.estimate(stiffness=200.0, huber=1e-2, reg_sigma=0.075, ctrl_sigma=0.0125, max_iter=3,
+                        max_d2=0.02 ** 2, max_gn_iter=2, max_cg_iter=50)
+    f, s, _ = sicp.correspondences()
+    sicp.solve(f, s, T_dense_src=got["T_dense"], max_gn_iter=1, max_cg_iter=20, ctrl_sigma=0.0125)
+    sicp.resample(got["T"], ctrl_sigma=0.0125)
+    sicp.residuals(got["T_dense"])
     ctx.close()
     print("sanitize target: all checks passed")
 
