@@ -18,8 +18,8 @@
 // (triangle inequality); if the cached match's distance under T_{k+1} — evaluated with the contract arithmetic,
 // i.e. the very number the search would compute for it — is below that, the match is provably still the unique
 // nearest neighbour and its (index, d2) is what the full search would return, bit for bit. Only the queries
-// that fail the test are searched again; they are compacted over the block first, so the search runs on dense
-// warps. All bounds are rounded conservatively (directed rounding + 2^-18 relative margins, far above the
+// that fail the test are searched again, inside the same pass: each warp queues the ones it flagged, so the search
+// runs on dense warps. All bounds are rounded conservatively (directed rounding + 2^-18 relative margins, far above the
 // 6-ulp error of the fp32 distance evaluation); an exact tie can never pass the strict test.
 // As ICP converges the per-iteration motion shrinks geometrically and almost every query takes the cached path:
 // the iteration becomes one streaming pass (16 B query + 8 B cache + one 16 B gather per source point).
@@ -41,16 +41,6 @@ namespace cb {
 namespace {
 
 constexpr int kBlock = kReduceBlock;
-// 256-query chunks per block (tile size / 256) of the search kernel of a warm iteration. The host cannot know how many
-// queries an iteration will have to search again, but the sequence is predictable for a converging run (10^6, 19 %, 7 %,
-// 0.07 %, then a few dozen queries at 1 M): the first kDenseIters warm iteration(s) use small tiles (a tile's first 256
-// flagged queries are searched by the inline body, only the rest by the slower out-of-line copy), later iterations
-// large ones (a tile without flagged queries still costs its block a few microseconds of latency, so fewer, larger
-// tiles). Either variant is correct for any number of flagged queries. Small tiles pay off in the first warm iteration
-// only (later ones search mostly empty tiles already); the two sizes are timing choices (bench.py, DESIGN §4.2).
-constexpr int kQptDense = 4;
-constexpr int kQptWarm = 32;
-constexpr int kDenseIters = 1;
 
 struct LoopArgs {
   GridView dst;
@@ -64,7 +54,6 @@ struct LoopArgs {
   float src_mean[3];  // src_mean_ (the kernel applies the current transform)
   int has_pt, has_pl;  // combined metric: which terms are on
   int bail;            // plane terms wanted but dst has no normals -> identity update (transform_estimation.hpp:269-272)
-  uint32_t* miss_mask; // one word per 32 consecutive sorted queries: bit set = the cached pass could not decide it
   int* cache_pos;      // per sorted query: sorted dst position of its match (-1 none)
   float* cache_r;      // per sorted query: every OTHER dst point is at least this far away (<= 0: unknown)
   float slack_first, slack_min, slack_max;  // widening of the search beyond the nearest distance (warp_search_wide.cuh)
@@ -146,12 +135,15 @@ __device__ __forceinline__ void loop_solve(const LoopArgs* ap, const BlockCtx* c
   st->searched_last = st->searched_cur;
   st->searched_cur = 0ull;
   if (delta < a.tol) st->done = 1;  // icp_base.hpp:83
-  if (a.trace) st->trace[(st->iters - 1) & 63][3] = global_timer_ns();
+  if (a.trace) {
+    st->trace[(st->iters - 1) & 63][3] = global_timer_ns();
+    st->trace[st->iters & 63][5] = 0ull;  // the next iteration's kernels take the maximum over their warps
+  }
   __threadfence();
 }
 
-// One chunk of <= 256 queued queries of the tile: lane-dense wide search and cache update. Returns the searching
-// thread's pair: query index i, transformed query q, match position pos (-1 none / inactive lane).
+// One lane-dense warp search (query i on every lane with act set) and cache update. Returns the searching lane's
+// pair: query index i, transformed query q, match position pos (-1 none / inactive lane).
 struct ChunkPair {
   uint32_t i;
   int pos;
@@ -159,15 +151,13 @@ struct ChunkPair {
   float d2;  // the match's squared distance (correspondence value)
 };
 
+// kCold: nothing cached yet (no warm seed, first-iteration slack). Otherwise the query failed the exclusion test:
+// its cached match seeds the search and its last motion sets the slack.
 template <bool kCold>
 __device__ __forceinline__ ChunkPair search_chunk_body(const LoopArgs& a, const BlockCtx& cx, WideSearchSmem* wsm,
-                                                       const unsigned short* queue, unsigned int c, unsigned int total,
-                                                       uint32_t base) {
-  const unsigned int tid = threadIdx.x;
-  const bool act = c + tid < total;
-  const unsigned int slot = act ? (kCold ? c + tid : (unsigned int)queue[c + tid]) : 0u;
+                                                       bool act, uint32_t i) {
   ChunkPair cp;
-  cp.i = base + slot;
+  cp.i = i;
   cp.pos = -1;
   cp.qx = cp.qy = cp.qz = 0.f;
   cp.d2 = 0.f;
@@ -196,20 +186,19 @@ __device__ __forceinline__ ChunkPair search_chunk_body(const LoopArgs& a, const 
   return cp;
 }
 
-// Out-of-line copy for the chunks beyond the first of a tile (more than 256 of its queries need a search: rare once
-// the cache is warm). Behind a pointer the grid parameters are no longer constant-bank operands and ptxas spills
-// kilobytes per thread at this register budget, and so it did with the inline body inside a loop (loop-invariant
-// parameter loads hoisted into registers); the first chunk therefore stays inline and loop-free in the kernel.
-__device__ __noinline__ void search_chunk_far(const LoopArgs* ap, const BlockCtx* cxp, WideSearchSmem* wsm,
-                                              const unsigned short* queue, unsigned int c, unsigned int total,
-                                              uint32_t base, ChunkPair* out) {
-  *out = search_chunk_body<false>(*ap, *cxp, wsm, queue, c, total, base);
+// Out-of-line search of the cached pass: called from inside its tile loop, where the streaming registers and the
+// moment accumulators are live. Inlined there, the search's loop-invariant parameter loads were hoisted into
+// registers and the streaming loop spilled; behind the call only the call site saves and restores registers, once per
+// warp search.
+__device__ __noinline__ void search_chunk_far(const LoopArgs* ap, const BlockCtx* cxp, WideSearchSmem* wsm, bool act,
+                                              uint32_t i, ChunkPair* out) {
+  *out = search_chunk_body<false>(*ap, *cxp, wsm, act, i);
 }
 
 // Programmatic dependent launch (sm_90+): a kernel launched with the programmatic-stream-serialization attribute may
 // be scheduled while its predecessor in the stream is still running; it must execute pdl_wait() before it touches
 // anything the predecessor (or, transitively, earlier kernels: the predecessor passed its own pdl_wait first) wrote.
-// The predecessor allows that early scheduling with pdl_launch_dependents(). Used between the three kernels of an
+// The predecessor allows that early scheduling with pdl_launch_dependents(). Used between the two kernels of an
 // iteration so that the launch latency of the next kernel overlaps the tail of the previous one.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -232,15 +221,19 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
   cx.wc_pl = a.wc_pl;
 }
 
-// ---- kernel 1 of a warm iteration: the cached pass ------------------------------------------------------------------
-// Elementwise over the source cloud, no search code: per query 16 B (point) + 8 B (cache) streamed and one 16 B
-// gather of the cached match (+ 16 B normal for the plane term). Queries that pass the exclusion test accumulate
-// their pair here; the others are flagged in a bit mask (one word per 32 consecutive queries) for the search kernel.
+// ---- kernel 1 of a warm iteration: the cached pass and the search of what it could not decide ---------------------
+// Elementwise over the source cloud: per query 16 B (point) + 8 B (cache) streamed and one 16 B gather of the cached
+// match (+ 16 B normal for the plane term). Queries that pass the exclusion test accumulate their pair at once. The
+// others are searched by the warp that flagged them: after each 32-query slot the warp's ballot appends the flagged
+// query indices, in ascending order, to a warp-private queue; as soon as 32 are queued the warp searches them
+// lane-dense (search_chunk_far: same slack rule, warm seed and cache update as the cold search), and at the end of its
+// tiles it searches what is left. Only __syncwarp is involved, so a searching warp holds up no other warp of its
+// block, and the searching lane adds its pair to the same accumulators.
 // PERSISTENT: the grid is a whole number of resident blocks per SM, a block walks the tiles blockIdx.x, + gridDim.x,
-// ... (static round-robin: every tile costs the same, and the assignment — hence the summation order — is fixed),
-// the next tiles' loads are in flight while the current tile is evaluated, and the moments are reduced ONCE per
-// block (a per-tile reduction cost as much as the tile itself). The block rows go through the same deterministic grid
-// reduction into rs.result + 32.
+// ... (static round-robin: every tile costs the same, and the assignment — hence, with the fixed queue order, the
+// summation order — is fixed), the next tiles' loads are in flight while the current tile is evaluated, and the
+// moments are reduced ONCE per block (a per-tile reduction cost as much as the tile itself). The block rows go through
+// one deterministic grid reduction per iteration into rs.result, read by the finish kernel.
 // The loads are not staged in registers: a register-staged version needed 128 registers -> 2 blocks/SM, few warp
 // slots occupied, long-scoreboard stalls on top - each thread can only keep the loads in flight that it has registers
 // for. Here every thread runs a private three-deep pipeline of cp.async copies into shared memory (LDGSTS: no
@@ -249,10 +242,17 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
 //   stage B (tile k+1)  the gathers, once A has landed: the matched destination point (+ normal for the plane term)
 //   stage C (tile k)    evaluation from shared memory
 // Each thread only ever reads what it copied itself, so cp.async.wait_group is all the synchronisation there is -
-// no block barrier inside the tile loop. Tiles are kPipeQpt x 256 queries (2 per thread): three A buffers and two B
-// buffers are 52 KB (p2p) / 68 KB (combined) per block, 4 / 3 blocks per SM.
-constexpr int kPipeQpt = 2;
-constexpr int kPipeTile = kPipeQpt * kBlock;
+// no block barrier inside the tile loop.
+// Shared memory per block: the pipeline (three A buffers, two B buffers) and one WideSearchSmem per warp (27.6 KB,
+// the queue included), 1 KB of reduction slots and state.
+//   p2p: 256-query tiles (one query per thread): 26 KB of pipeline, 56 KB per block -> 4 blocks per SM in the 228 KB
+//        of an H100 SM, 64 registers. (512-query tiles would need 82 KB per block: 2 blocks per SM.)
+//   combined: 512-query tiles: 68 KB of pipeline, 98 KB per block -> 2 blocks per SM, 128 registers. At 3 blocks
+//        (80 registers, 256-query tiles) the exclusion test and the 28 accumulators spilled on every query, and with
+//        3 x 65 KB of shared memory the L1 left for those spills was too small: the 10 M pass ran 3x slower.
+// Both keep 1024 queries per SM in flight in the pipeline.
+__host__ __device__ constexpr int pipe_qpt(bool normals) { return normals ? 2 : 1; }
+__host__ __device__ constexpr int pipe_min_blocks(bool normals) { return normals ? 2 : 4; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void cp_async_16_cg(void* dst_smem, const void* src) {
@@ -272,31 +272,38 @@ __device__ __forceinline__ void cp_async_wait() {
 
 template <bool kNormals>
 struct PipeSmem {
-  float4 src[3][kPipeTile];
-  float r[3][kPipeTile];
-  int seed[3][kPipeTile];
-  float4 pt[2][kPipeTile];
-  float4 nr[kNormals ? 2 : 1][kNormals ? kPipeTile : 1];
+  static constexpr int kT = pipe_qpt(kNormals) * kBlock;  // queries per tile
+  float4 src[3][kT];
+  float r[3][kT];
+  int seed[3][kT];
+  float4 pt[2][kT];
+  float4 nr[kNormals ? 2 : 1][kNormals ? kT : 1];
 };
 
 template <int MODE>
-__global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_cached_pipe_kernel(const __grid_constant__ LoopArgs a) {
+__global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)) icp_cached_pipe_kernel(const __grid_constant__ LoopArgs a) {
   constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
   constexpr bool kNormals = (MODE == kModeCombined);
+  constexpr int kQpt = pipe_qpt(kNormals), kTile = kQpt * kBlock;
   extern __shared__ __align__(16) unsigned char pipe_raw[];
   PipeSmem<kNormals>& ps = *reinterpret_cast<PipeSmem<kNormals>*>(pipe_raw);
   __shared__ BlockCtx cx;
   __shared__ AsyncReduceSmem<NV> rsm;
-  const unsigned int tid = threadIdx.x, lane = tid & 31u;
-  const uint32_t ntiles = (a.n_src + kPipeTile - 1) / kPipeTile;
+  __shared__ WideSearchSmem wsm[kBlock / 32];
+  const unsigned int tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  // per warp: flagged query indices waiting for a search, ascending. The queue lives in the warp's search buffer: it
+  // is only filled between searches, and each lane reads its entry before the search overwrites the buffer. (A queue
+  // of its own, 1 KB per block, would leave the p2p pass 176 B short of 4 blocks per SM.)
+  uint32_t* wq = wsm[warp].sec;
+  const uint32_t ntiles = (a.n_src + kTile - 1) / kTile;
   const bool want_nrm = kNormals && a.has_pl != 0;
 
   // stage A of tile `tile` into buffer `buf`: nothing here depends on the loop state
   auto stage_a = [&](uint32_t tile, int buf) {
     if (tile < ntiles) {
 #pragma unroll
-      for (int k = 0; k < kPipeQpt; k++) {
-        const uint32_t slot = k * kBlock + tid, i = tile * kPipeTile + slot;
+      for (int k = 0; k < kQpt; k++) {
+        const uint32_t slot = k * kBlock + tid, i = tile * kTile + slot;
         if (i < a.n_src) {
           cp_async_16_cg(&ps.src[buf][slot], a.src_pts + i);
           cp_async_4(&ps.r[buf][slot], a.cache_r + i);
@@ -310,8 +317,8 @@ __global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_c
   auto stage_b = [&](uint32_t tile, int abuf, int bbuf) {
     if (tile < ntiles) {
 #pragma unroll
-      for (int k = 0; k < kPipeQpt; k++) {
-        const uint32_t slot = k * kBlock + tid, i = tile * kPipeTile + slot;
+      for (int k = 0; k < kQpt; k++) {
+        const uint32_t slot = k * kBlock + tid, i = tile * kTile + slot;
         if (i < a.n_src) {
           const int sd = ps.seed[abuf][slot];
           if (sd >= 0 && ps.r[abuf][slot] > 0.f) {
@@ -325,13 +332,12 @@ __global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_c
   };
 
   const uint32_t t0 = blockIdx.x, stride = gridDim.x;
-  // (No pdl_launch_dependents() here: released early, the search kernel's blocks were handed to whichever SMs finished
-  // their share of this pass first - a few SMs ended up with all of its tiles, and iterations that still search many
-  // queries ran 25 % slower.)
   // The dependency wait comes BEFORE the first copies: the cache arrays are rewritten every iteration, their 4-byte
   // copies go through L1 (cp.async.ca), and only accesses after griddepcontrol.wait are guaranteed to see the previous
-  // kernels' writes. What programmatic launch still buys here: the blocks are resident when the finish kernel ends.
+  // kernels' writes. What programmatic launch buys here: the blocks are resident when the finish kernel ends, and the
+  // one-warp finish kernel of this iteration, released at once, is resident and waiting when this grid drains.
   pdl_wait();
+  pdl_launch_dependents();
   stage_a(t0, 0);           // group: A(0)
   stage_a(t0 + stride, 1);  // group: A(1)
   if (tid == 0) {
@@ -353,6 +359,30 @@ __global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_c
   double acc[NV];
 #pragma unroll
   for (int v = 0; v < NV; v++) acc[v] = 0.0;
+  // the warp's row of the block reduction: what the warp folded before each search (and, at the end, the rest)
+  if (lane < NV) rsm.slot[warp][lane] = 0.0;
+  __syncwarp();  // (lane 0 adds to the whole row)
+  // The warp searches the queries queued in wq[0, n) on lanes < n; the searching lane accumulates its pair. The
+  // accumulators are folded into the warp's row first and restart from zero, so that no register of the streaming
+  // loop is live across the search call (held there, all of acc[] was kept in local memory for the whole loop).
+  unsigned int queued = 0, searched = 0;  // warp-uniform
+  auto search_queued = [&](unsigned int n) {
+    __syncwarp();
+    warp_sum_to_slot<NV, true>(acc, rsm);
+#pragma unroll
+    for (int v = 0; v < NV; v++) acc[v] = 0.0;
+    const bool act = lane < n;
+    ChunkPair cp;
+    search_chunk_far(&a, &cx, &wsm[warp], act, act ? wq[lane] : 0u, &cp);
+    if (cp.pos >= 0) {
+      const float4 dp = __ldg(a.dst.pts + cp.pos);
+      accumulate_pair<MODE, true>(
+          acc, cx, a.has_pt != 0, a.has_pl != 0, dp, cp.qx, cp.qy, cp.qz, a.src_nrm != nullptr,
+          [&] { return __ldg(a.dst.nrm + cp.pos); }, [&] { return __ldg(a.src_nrm + cp.i); }, cp.d2);
+    }
+    searched += n;
+    __syncwarp();  // every lane has read its entry before the queue is refilled
+  };
   // iteration n evaluates tile t0 + n*stride; on entry the committed groups are ... A(n+1), B(n)
   int abuf = 0, bbuf = 0;
 #pragma unroll 1
@@ -362,9 +392,9 @@ __global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_c
     cp_async_wait<2>();                            // pending at most {B(n), A(n+2)}: A(n+1) has landed
     stage_b(tile + stride, abuf1, bbuf ^ 1);       // group: B(n+1)
     cp_async_wait<2>();                            // pending at most {A(n+2), B(n+1)}: B(n) has landed
-    const uint32_t base = tile * kPipeTile;
+    const uint32_t base = tile * kTile;
 #pragma unroll
-    for (int k = 0; k < kPipeQpt; k++) {
+    for (int k = 0; k < kQpt; k++) {
       const uint32_t slot = k * kBlock + tid, i = base + slot;
       const bool active = i < a.n_src;
       bool miss = active;
@@ -387,134 +417,83 @@ __global__ void __launch_bounds__(kBlock, (MODE == kModeCombined) ? 3 : 4) icp_c
           }
         }
       }
+      // flagged queries -> the warp's queue; the ones that do not fit wait in their lane's register (i) until the
+      // 32 queued ones have been searched
       const unsigned int mm = __ballot_sync(0xffffffffu, miss);
-      if (lane == 0 && (base + k * kBlock + (tid & ~31u)) < a.n_src) a.miss_mask[(base + k * kBlock + tid) >> 5] = mm;
+      const unsigned int at = queued + __popc(mm & ((1u << lane) - 1u));
+      if (miss && at < 32u) wq[at] = i;
+      queued += __popc(mm);
+      if (queued >= 32u) {
+        search_queued(32u);
+        queued -= 32u;
+        if (miss && at >= 32u) wq[at - 32u] = i;
+      }
     }
     abuf = abuf1;
     bbuf ^= 1;
   }
   cp_async_wait<0>();
+  if (queued > 0u) search_queued(queued);
+  if (lane == 0 && searched > 0u) {
+    atomicAdd(&a.st->searched_cur, (unsigned long long)searched);
+    if (a.trace) atomicAdd(&a.st->trace[__ldcg(&a.st->iters) & 63][4], (unsigned long long)searched);
+  }
+  if (a.trace && lane == 0) atomicMax(&a.st->trace[__ldcg(&a.st->iters) & 63][5], global_timer_ns());
+  warp_sum_to_slot<NV, true>(acc, rsm);
   double tot = 0;
-  if (!grid_reduce_async_tail<NV>(acc, a.rs, rsm, tot)) return;
-  if (lane < NV) a.rs.result[32 + lane] = tot;
+  if (!grid_reduce_slots_tail<NV>(a.rs, rsm, tot)) return;
+  // the last warp of the grid hands this GPU's totals to icp_finish_kernel
+  if (lane < NV) a.rs.result[lane] = tot;
+  if (a.trace && lane == 0) a.st->trace[__ldcg(&a.st->iters) & 63][1] = global_timer_ns();
 }
 
 constexpr int kSearchMinBlocks = 4;  // resident blocks per SM the search kernel's register budget is set for
 
-// ---- kernel 2 of an iteration (the only one of a cold iteration): search + finish ------------------------------------------
-// kCold: nothing is cached, every query of the tile is searched (one 256-query chunk per block). Otherwise the
-// block compacts the flagged queries of its tile (kQpt x 256 queries) from the bit masks of the cached pass, in
-// ascending order, and dense warps search them. The searching thread accumulates its pair; the last warp of the
-// grid adds the cached pass's totals, all-reduces with the peers, solves, and writes the next transform.
-template <int MODE, int kQpt, bool kCold>
+// ---- the cold iteration (the first of a call: nothing cached yet): search, then the finish kernel -----------------
+// Every query is searched, one 256-query chunk per block, lane-dense; the searching thread accumulates its pair and
+// the last warp of the grid hands this GPU's totals to icp_finish_kernel.
+template <int MODE>
 __global__ void __launch_bounds__(kBlock, kSearchMinBlocks) icp_search_kernel(const __grid_constant__ LoopArgs a) {
-  static_assert(!kCold || kQpt == 1, "a cold iteration searches one chunk per block");
-  constexpr int kTile = kQpt * kBlock;  // queries per block
-  constexpr int kWords = kTile / 32;    // mask words per tile
   constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
   __shared__ BlockCtx cx;
   __shared__ WideSearchSmem wsm[kBlock / 32];
   __shared__ AsyncReduceSmem<NV> rsm;
-  __shared__ unsigned short queue[kCold ? 1 : kTile];  // slots of the tile that need a search, ascending
-  __shared__ unsigned int smask[kWords], spre[kWords + 1];
 
   const unsigned int tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-  const uint32_t base = blockIdx.x * kTile;
-  unsigned int total = 0;
-  pdl_wait();               // masks, cached totals and cache updates of the cached pass (state of the previous finish)
+  const uint32_t base = blockIdx.x * kBlock;
+  pdl_wait();               // the state of the previous finish kernel
   pdl_launch_dependents();  // the one-warp finish kernel may be scheduled now and wait for this grid to drain
   if (tid == 0) {
     rsm.arrived = 0u;
     load_block_ctx(a, cx);
   }
-  if (!kCold) {
-    if (warp == 1) {  // (warp 0's first lane is busy with the state): mask words of the tile -> exclusive prefix of their populations
-      unsigned int carry = 0;
-#pragma unroll
-      for (int w0 = 0; w0 < kWords; w0 += 32) {
-        const uint32_t w = (base >> 5) + w0 + lane;
-        const unsigned int m = (w0 + (int)lane < kWords && w * 32u < a.n_src) ? __ldcg(a.miss_mask + w) : 0u;
-        unsigned int inc = __popc(m);
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const unsigned int t = __shfl_up_sync(0xffffffffu, inc, o);
-          if ((int)lane >= o) inc += t;
-        }
-        if (w0 + (int)lane < kWords) {
-          smask[w0 + lane] = m;
-          spre[w0 + lane + 1] = carry + inc;
-        }
-        carry += __shfl_sync(0xffffffffu, inc, 31);
-      }
-      if (lane == 0) spre[0] = 0u;
-    }
-  }
   __syncthreads();
   if (cx.done) return;  // converged (or failed) in an earlier launch of this batch
   const int trace_slot = a.trace ? (__ldcg(&a.st->iters) & 63) : 0;
   if (a.trace && blockIdx.x == 0 && tid == 0) {
-    a.st->trace[trace_slot][5] = global_timer_ns();
-    if (kCold) {
-      a.st->trace[trace_slot][0] = a.st->trace[trace_slot][5];
-      a.st->trace[trace_slot][4] = 0ull;
-    }
+    a.st->trace[trace_slot][0] = global_timer_ns();
+    a.st->trace[trace_slot][4] = 0ull;
   }
-  if (kCold) {
-    total = (base < a.n_src) ? min((uint32_t)kTile, a.n_src - base) : 0u;
-  } else {
-    total = spre[kWords];
-    if (total > 0) {  // block-uniform
-#pragma unroll
-      for (int k = 0; k < kQpt; k++) {
-        const unsigned int j = k * (kBlock / 32) + warp;  // mask word of slots k*256 + warp*32 .. +31
-        const unsigned int m = smask[j];
-        if ((m >> lane) & 1u) queue[spre[j] + __popc(m & ((1u << lane) - 1u))] = (unsigned short)(k * kBlock + tid);
-      }
-      __syncthreads();
-    }
-  }
+  const unsigned int total = (base < a.n_src) ? min((uint32_t)kBlock, a.n_src - base) : 0u;
   if (tid == 0 && total > 0) {
     atomicAdd(&a.st->searched_cur, (unsigned long long)total);
     if (a.trace) atomicAdd(&a.st->trace[trace_slot][4], (unsigned long long)total);
   }
-  double tot = 0;
-  if (total == 0) {
-    // nothing to search in this tile (the usual case once the cache is warm): warp 0 contributes a zero row
-    if (warp != 0) return;
-    if (!grid_reduce_rows_tail<NV>(0.0, a.rs, (int)lane, tot)) return;
-  } else {
-    // ---- dense warps search the queued queries; the searching thread accumulates its pair ------------------------
-    double acc[NV];
+  double acc[NV];
 #pragma unroll
-    for (int v = 0; v < NV; v++) acc[v] = 0.0;
-    if ((tid & ~31u) < total) {
-      const ChunkPair cp = search_chunk_body<kCold>(a, cx, &wsm[warp], queue, 0u, total, base);
-      if (cp.pos >= 0) {
-        const float4 dp = __ldg(a.dst.pts + cp.pos);
-        accumulate_pair<MODE, true>(
-            acc, cx, a.has_pt != 0, a.has_pl != 0, dp, cp.qx, cp.qy, cp.qz, a.src_nrm != nullptr,
-            [&] { return __ldg(a.dst.nrm + cp.pos); }, [&] { return __ldg(a.src_nrm + cp.i); }, cp.d2);
-      }
+  for (int v = 0; v < NV; v++) acc[v] = 0.0;
+  if ((tid & ~31u) < total) {
+    const ChunkPair cp = search_chunk_body<true>(a, cx, &wsm[warp], tid < total, base + tid);
+    if (cp.pos >= 0) {
+      const float4 dp = __ldg(a.dst.pts + cp.pos);
+      accumulate_pair<MODE, true>(
+          acc, cx, a.has_pt != 0, a.has_pl != 0, dp, cp.qx, cp.qy, cp.qz, a.src_nrm != nullptr,
+          [&] { return __ldg(a.dst.nrm + cp.pos); }, [&] { return __ldg(a.src_nrm + cp.i); }, cp.d2);
     }
-    if constexpr (kQpt > 1) {
-#pragma unroll 1
-      for (unsigned int c = kBlock; c < total; c += kBlock) {
-        if (c + (tid & ~31u) >= total) break;  // warp-uniform; later chunks are empty for this warp too
-        ChunkPair cp;
-        search_chunk_far(&a, &cx, &wsm[warp], queue, c, total, base, &cp);
-        if (cp.pos >= 0) {
-          const float4 dp = __ldg(a.dst.pts + cp.pos);
-          accumulate_pair<MODE, true>(
-              acc, cx, a.has_pt != 0, a.has_pl != 0, dp, cp.qx, cp.qy, cp.qz, a.src_nrm != nullptr,
-              [&] { return __ldg(a.dst.nrm + cp.pos); }, [&] { return __ldg(a.src_nrm + cp.i); }, cp.d2);
-        }
-      }
-    }
-    // ---- reduction ----------------------------------------------------------------------------------------------------
-    if (!grid_reduce_async_tail<NV>(acc, a.rs, rsm, tot)) return;
   }
-  // the last warp of the grid adds the cached pass's totals and hands this GPU's sums to icp_finish_kernel
-  if (!kCold && lane < NV) tot += __ldcg(a.rs.result + 32 + lane);  // fixed order: search + cached
+  if (a.trace && lane == 0) atomicMax(&a.st->trace[trace_slot][5], global_timer_ns());
+  double tot = 0;
+  if (!grid_reduce_async_tail<NV>(acc, a.rs, rsm, tot)) return;
   if (lane < NV) a.rs.result[lane] = tot;
   if (a.trace && lane == 0) a.st->trace[trace_slot][1] = global_timer_ns();
 }
@@ -530,7 +509,7 @@ __global__ void __launch_bounds__(32, 1) icp_finish_kernel(const __grid_constant
   __shared__ double sbuf[kCombinedValues + 8];
   static_assert(NV + 2 <= kExchangeVals, "row of the fused exchange");
   const unsigned int lane = threadIdx.x;
-  pdl_wait();               // this GPU's totals (search kernel), the state of the previous iteration
+  pdl_wait();               // this GPU's totals (cached pass or cold search kernel), the state of the previous iteration
   pdl_launch_dependents();  // the next iteration's cached pass may start streaming
   if (lane == 0) load_block_ctx(a, cx);
   __syncwarp();
@@ -595,25 +574,17 @@ static cudaError_t launch_pdl(Kernel k, int blocks, int threads, size_t smem, cu
   return cudaLaunchKernelEx(&cfg, k, a);
 }
 
-// Enqueues the kernels of ICP iteration `it` of this call: the search kernel alone in the cold first iteration (nothing
-// cached yet), else the cached pass and the search kernel over its flagged queries; then the finish kernel.
+// Enqueues the kernels of ICP iteration `it` of this call: the search kernel in the cold first iteration (nothing
+// cached yet), else the cached pass with its search of the flagged queries; then the finish kernel.
 template <int MODE>
-static int enqueue_iteration(cb_context* ctx, const LoopArgs& a, int it, int blocks_cold, int blocks_cached,
-                             int blocks_dense, int blocks_search) {
-  const bool cold = (it == 0);
-  if (cold) {
-    CB_CUDA(launch_pdl(icp_search_kernel<MODE, 1, true>, blocks_cold, kBlock, 0, ctx->stream, a));
-  } else {
+static int enqueue_iteration(cb_context* ctx, const LoopArgs& a, int it, int blocks_cold, int blocks_cached) {
+  if (it == 0)
+    CB_CUDA(launch_pdl(icp_search_kernel<MODE>, blocks_cold, kBlock, 0, ctx->stream, a));
+  else
     CB_CUDA(launch_pdl(icp_cached_pipe_kernel<MODE>, blocks_cached, kBlock, sizeof(PipeSmem<MODE == kModeCombined>),
                        ctx->stream, a));
-    if (it <= kDenseIters)
-      CB_CUDA(launch_pdl(icp_search_kernel<MODE, kQptDense, false>, blocks_dense, kBlock, 0, ctx->stream, a));
-    else
-      CB_CUDA(launch_pdl(icp_search_kernel<MODE, kQptWarm, false>, blocks_search, kBlock, 0, ctx->stream, a));
-  }
   CB_CUDA(launch_pdl(icp_finish_kernel<MODE>, 1, 32, 0, ctx->stream, a));
-  ctx->launches += cold ? 1 : 2;
-  ctx->launches += 1;
+  ctx->launches += 2;
   return CB_OK;
 }
 
@@ -662,27 +633,37 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   a.st = icp->d_state;
   static const bool trace = getenv("CB_LOOP_TRACE") != nullptr;
   a.trace = trace ? 1 : 0;
-  // cold iteration (first launch: nothing cached): search kernel alone, one 256-query chunk per block; warm
-  // iterations: cached pass (kPipeTile queries per tile) + search kernel over the flagged queries
+  // cold iteration (first launch: nothing cached): search kernel, one 256-query chunk per block; warm iterations:
+  // the persistent cached pass (PipeSmem::kT queries per tile), which also searches the queries it flags
   const int blocks_cold = std::max(1, (int)((ns + kBlock - 1) / kBlock));
-  const int blocks_search = std::max(1, (int)((ns + (size_t)kQptWarm * kBlock - 1) / ((size_t)kQptWarm * kBlock)));
-  const int blocks_dense = std::max(1, (int)((ns + (size_t)kQptDense * kBlock - 1) / ((size_t)kQptDense * kBlock)));
-  // once per device (function attributes belong to the device the context is on, not to the process)
+  // once per device (function attributes belong to the device the context is on, not to the process): the pipeline's
+  // dynamic shared memory, the whole shared-memory carveout (4 / 2 blocks of 56 / 98 KB per SM), and how many blocks
+  // of the cached pass are resident per SM
   static bool attr_set_dev[64] = {};
+  static int resident_dev[64][2] = {};
   bool& attr_set = attr_set_dev[ctx->device & 63];
+  int* resident = resident_dev[ctx->device & 63];
   if (!attr_set) {
     CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeP2PCentered>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)sizeof(PipeSmem<false>)));
     CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeCombined>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)sizeof(PipeSmem<true>)));
+    CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeP2PCentered>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 (int)cudaSharedmemCarveoutMaxShared));
+    CB_CUDA(cudaFuncSetAttribute(icp_cached_pipe_kernel<kModeCombined>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 (int)cudaSharedmemCarveoutMaxShared));
+    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident[0], icp_cached_pipe_kernel<kModeP2PCentered>, kBlock,
+                                                          sizeof(PipeSmem<false>)));
+    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident[1], icp_cached_pipe_kernel<kModeCombined>, kBlock,
+                                                          sizeof(PipeSmem<true>)));
     attr_set = true;
   }
   // persistent cached pass: a whole number of resident blocks per SM (never more blocks than tiles)
   const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
-  const int blocks_cached = std::max(1, std::min(ctx->sm_count * (p2p ? 4 : 3), (int)((ns + kPipeTile - 1) / kPipeTile)));
+  const int per_sm = std::max(1, resident[p2p ? 0 : 1]);
+  const size_t tile = (size_t)pipe_qpt(!p2p) * kBlock;
+  const int blocks_cached = std::max(1, std::min(ctx->sm_count * per_sm, (int)((ns + tile - 1) / tile)));
   CB_TRY(get_reduce_scratch(ctx, blocks_cold, kMaxValues, &a.rs));
-  if (!icp->d_miss_mask) CB_TRY(icp->mem.alloc(&icp->d_miss_mask, ns / 32 + 2));
-  a.miss_mask = icp->d_miss_mask;
   Exchange ex;
   std::memset(&ex, 0, sizeof(ex));
   const bool fused = ctx->world > 1 && arm_exchange(ctx, &ex);  // tables + timeout; the pass number lives in LoopState
@@ -716,9 +697,9 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
       if (prm->flush_l2) CB_TRY(cb_context_flush_l2(ctx));
       if (timing) CB_CUDA(cudaEventRecord(icp->events[2 * (issued + k)], ctx->stream));
       if (p2p)
-        CB_TRY(enqueue_iteration<kModeP2PCentered>(ctx, a, issued + k, blocks_cold, blocks_cached, blocks_dense, blocks_search));
+        CB_TRY(enqueue_iteration<kModeP2PCentered>(ctx, a, issued + k, blocks_cold, blocks_cached));
       else
-        CB_TRY(enqueue_iteration<kModeCombined>(ctx, a, issued + k, blocks_cold, blocks_cached, blocks_dense, blocks_search));
+        CB_TRY(enqueue_iteration<kModeCombined>(ctx, a, issued + k, blocks_cold, blocks_cached));
       if (timing) CB_CUDA(cudaEventRecord(icp->events[2 * (issued + k) + 1], ctx->stream));
     }
     CB_CUDA(cudaGetLastError());
@@ -759,7 +740,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
     unsigned long long prev = 0;
     for (int k = std::max(0, iters - 64); k < iters; ++k) {
       const unsigned long long* t = hs->trace[k & 63];
-      fprintf(stderr, "[rank %d iteration %d] searched %llu of %zu queries; start->search kernel %.1f us, ->reduced %.1f us, ->peers %.1f us, ->solved %.1f us; period %.1f us\n",
+      fprintf(stderr, "[rank %d iteration %d] searched %llu of %zu queries; start->last warp at the reduction %.1f us, ->reduced %.1f us, ->peers %.1f us, ->solved %.1f us; period %.1f us\n",
               ctx->rank, k, t[4], ns, (t[5] - t[0]) * 1e-3, (t[1] - t[5]) * 1e-3, (t[2] - t[1]) * 1e-3, (t[3] - t[2]) * 1e-3,
               prev ? (t[0] - prev) * 1e-3 : 0.0);
       prev = t[0];

@@ -27,8 +27,8 @@ struct LoopState {
   double queries_all;                // source points of all ranks
   double sums[32];    // its reduced moments / normal equations (all ranks)
   // CB_LOOP_TRACE=1: per executed iteration (mod 64): %globaltimer at kernel start / local reduction done /
-  // peers' rows summed / state written, the number of queries that needed a search, %globaltimer at the start of
-  // the search kernel
+  // peers' rows summed / state written, the number of queries that needed a search, %globaltimer when the last warp
+  // of the grid reached the reduction (its tiles and searches done)
   unsigned long long trace[64][6];
 };
 
@@ -59,7 +59,6 @@ struct cb_icp {
   cb::LoopState* h_state = nullptr;  // pinned
   cb::LoopState* h_state2 = nullptr; // pinned: the batches' states alternate between the two
   cudaEvent_t batch_ev[2] = {nullptr, nullptr};  // end of a batch + its state copy
-  uint32_t* d_miss_mask = nullptr;   // cached pass -> search kernel: one bit per sorted query
   cb_cloud* src_full = nullptr;      // world > 1, engine modes: the whole source cloud replicated on this rank (owned)
   bool loop_last = false;            // the last estimate() ran on the device loop
   uint64_t searched_last = 0;        // queries its last iteration searched again (CB_LOOP_TRACE / cb_icp_loop_cache)

@@ -263,16 +263,16 @@ __device__ __forceinline__ bool grid_reduce_rows_tail(double row, const ReduceSc
   return true;
 }
 
-// Returns true on exactly ONE warp of the grid - the last to arrive - with `tot` = this GPU's total of value
-// `lane` (lane < NV); every other warp returns false as soon as its part is done. The caller continues alone on
-// that warp (exchange, publication, the device-resident solve of icp_loop.cu).
-template <int NV>
-__device__ __forceinline__ bool grid_reduce_async_tail(double (&acc)[NV], const ReduceScratch& rs, AsyncReduceSmem<NV>& sm,
-                                                       double& tot) {
+// The warp's sums of acc[] -> its slot of the block row: stored (kAdd = false) or added to what the warp parked there
+// before (kAdd = true; the slot must then have been zeroed by the warp). Fixed order.
+// kAdd is for callers that fold acc[] inside a loop and go on accumulating: it reduces value by value, because ptxas
+// turns the transposing butterfly's selects into indexed local-memory loads, and inside a loop that kept a local copy
+// of acc[] written on every accumulation.
+template <int NV, bool kAdd>
+__device__ __forceinline__ void warp_sum_to_slot(double (&acc)[NV], AsyncReduceSmem<NV>& sm) {
   static_assert(NV <= 32, "one lane per value");
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  constexpr int kWarps = kReduceBlock / 32;
-  if constexpr (NV == 16) {
+  if constexpr (NV == 16 && !kAdd) {
     const double t16 = warp_transpose_reduce<16>(acc, lane);
     if ((lane & 1) == 0) sm.slot[warp][lane >> 1] = t16;
   } else {
@@ -281,10 +281,18 @@ __device__ __forceinline__ bool grid_reduce_async_tail(double (&acc)[NV], const 
       double v = acc[i];
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-      if (lane == 0) sm.slot[warp][i] = v;
+      if (lane == 0) sm.slot[warp][i] = kAdd ? sm.slot[warp][i] + v : v;
     }
   }
   __syncwarp();
+}
+
+// Block and grid levels once every warp of the block has filled its slot (warp_sum_to_slot): same return value as
+// grid_reduce_async_tail.
+template <int NV>
+__device__ __forceinline__ bool grid_reduce_slots_tail(const ReduceScratch& rs, AsyncReduceSmem<NV>& sm, double& tot) {
+  const int lane = threadIdx.x & 31;
+  constexpr int kWarps = kReduceBlock / 32;
   unsigned int t = 0;
   if (lane == 0) {
     __threadfence_block();
@@ -300,6 +308,16 @@ __device__ __forceinline__ bool grid_reduce_async_tail(double (&acc)[NV], const 
     for (int w = 0; w < kWarps; w++) row += ((volatile double*)sm.slot[w])[lane];
   }
   return grid_reduce_rows_tail<NV>(row, rs, lane, tot);
+}
+
+// Returns true on exactly ONE warp of the grid - the last to arrive - with `tot` = this GPU's total of value
+// `lane` (lane < NV); every other warp returns false as soon as its part is done. The caller continues alone on
+// that warp (exchange, publication, the device-resident solve of icp_loop.cu).
+template <int NV>
+__device__ __forceinline__ bool grid_reduce_async_tail(double (&acc)[NV], const ReduceScratch& rs, AsyncReduceSmem<NV>& sm,
+                                                       double& tot) {
+  warp_sum_to_slot<NV, false>(acc, sm);
+  return grid_reduce_slots_tail<NV>(rs, sm, tot);
 }
 
 // ... -> (optional) fused all-reduce over NVLink peer memory -> device result + mapped host mailbox

@@ -32,9 +32,10 @@ def main():
             fn = None
     rows = sorted(set(rows))  # kernels of a shared header (radius_lists.cuh) appear once per translation unit
     out = ["# Kernel resources (`cuobjdump --dump-resource-usage`, sm_90a)", "",
-           "STACK is per-thread local memory the kernel reserves: call frames of the out-of-line far-chunk search",
-           "(`search_chunk_far`, DESIGN §4.2), the k-best arrays of the general-k search, and spills. The loop's cached pass",
-           "(`icp_cached_pipe_kernel`) and the k-means / RANSAC kernels stay (almost) in registers.",
+           "STACK is per-thread local memory the kernel reserves: call frames of the out-of-line search of the loop's",
+           "cached pass (`search_chunk_far`, DESIGN §4.2), the k-best arrays of the general-k search, and spills. The cached",
+           "pass (`icp_cached_pipe_kernel`, static shared memory without its dynamic pipeline buffers) keeps its per-query",
+           "path in registers; the k-means / RANSAC kernels stay (almost) in registers.",
            "`MODE` template values: 0 correspondences only, 1 p2p raw moments, 2 combined, 3 p2p pivoted moments.", "",
            "| kernel | registers | stack B | static smem B |", "|---|---:|---:|---:|"]
     for name, reg, stack, smem, _local in rows:

@@ -139,32 +139,24 @@ def main():
     # (report, summary file, title, note, traffic key = (workload, regime part))
     jobs = [
         (f"{rnd}_icp_cold_p2p_1m.ncu-rep", f"{rnd}_icp_search_kernel_cold_p2p_1m.md",
-         "icp_search_kernel<p2p, 1, cold> - first iteration of an estimate() call, 1 M -> 1 M",
+         "icp_search_kernel<p2p> - first iteration of an estimate() call, 1 M -> 1 M",
          "Every query is searched (nothing cached): transform + warp-pooled WIDE grid 1-NN (exclusion bound for the cache) + "
          "pivoted Kabsch moments + block/grid reduction. " + flush, ("icp_p2p_1m", "first_iteration", "search")),
         (f"{rnd}_icp_cached_p2p_1m.ncu-rep", f"{rnd}_icp_cached_pipe_kernel_p2p_1m.md",
-         "icp_cached_pipe_kernel<p2p> - cached pass of a converged iteration, 1 M -> 1 M",
+         "icp_cached_pipe_kernel<p2p> - cached pass (with its searches) of a converged iteration, 1 M -> 1 M",
          "Per query: point + cache streamed, cached match gathered (cp.async pipeline through shared memory), exclusion test, "
-         "moments of the pairs that pass; the rest flagged for the search kernel. " + flush, ("icp_p2p_1m", "converged_iteration", "cached")),
-        (f"{rnd}_icp_warm_search_p2p_1m.ncu-rep", f"{rnd}_icp_search_kernel_warm_p2p_1m.md",
-         "icp_search_kernel<p2p, 32, warm> - search kernel of a converged iteration, 1 M -> 1 M",
-         "Tiles of 8192 queries; a handful of flagged queries in the whole cloud: almost every block only contributes a zero row. "
-         + flush, ("icp_p2p_1m", "converged_iteration", "search")),
+         "moments of the pairs that pass; the rest searched by the warp that flagged them. " + flush, ("icp_p2p_1m", "converged_iteration", "cached")),
         (f"{rnd}_icp_finish_p2p_1m.ncu-rep", f"{rnd}_icp_finish_kernel_p2p_1m.md",
          "icp_finish_kernel<p2p> - exchange + solve, one warp", "Totals -> (peer all-reduce when world > 1) -> Kabsch, rotation(), "
          "compose, convergence test -> LoopState.", ("icp_p2p_1m", "converged_iteration", "finish")),
         (f"{rnd}_icp_cold_combined_10m.ncu-rep", f"{rnd}_icp_search_kernel_cold_combined_10m.md",
-         "icp_search_kernel<combined, 1, cold> - first iteration, 10 M -> 10 M (BASELINE config 3 on one GPU)",
+         "icp_search_kernel<combined> - first iteration, 10 M -> 10 M (BASELINE config 3 on one GPU)",
          "As above with the 28-value Gauss-Newton normal equations (point + plane terms). " + flush,
          ("icp_combined_10m", "first_iteration", "search")),
         (f"{rnd}_icp_cached_combined_10m.ncu-rep", f"{rnd}_icp_cached_pipe_kernel_combined_10m.md",
          "icp_cached_pipe_kernel<combined> - cached pass of a converged iteration, 10 M -> 10 M",
          "560 MB algorithmic (16 B point + 8 B cache + 16 B match + 16 B normal per query). " + flush,
          ("icp_combined_10m", "converged_iteration", "cached")),
-        (f"{rnd}_icp_warm_search_combined_10m.ncu-rep", f"{rnd}_icp_search_kernel_warm_combined_10m.md",
-         "icp_search_kernel<combined, 16, warm> - search kernel of a converged iteration, 10 M -> 10 M",
-         "2442 tiles of 4096 queries (captured before the tile size of converged iterations went to 8192 and before the "
-         "launches became programmatic-dependent; the 10 M captures were not repeated), a few hundred flagged queries. " + flush, ("icp_combined_10m", "converged_iteration", "search")),
         (f"{rnd}_kmeans_50m.ncu-rep", f"{rnd}_kmeans_assign_kernel.md", "kmeans_assign_kernel - bench.py kmeans_50m (BASELINE config 4)",
          "50 M points x 1024 centroids, the shipped kernel with its occupancy-sized persistent grid: fused assignment + "
          "per-cluster double sums (shared-memory atomics).", None),

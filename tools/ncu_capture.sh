@@ -6,17 +6,15 @@ cd "$(dirname "$0")/.."
 mkdir -p captures
 NCU="ncu --set full --clock-control none --import-source on"
 if [ -z "${SKIP_1M:-}" ]; then
-# device-resident ICP loop, 1 M p2p: 2 estimate() calls x (1 cold + 14 x (cached + search)) launches
-FLUSH=1 $NCU -k regex:icp_search_kernel -s 15 -c 1 -o captures/r02_icp_cold_p2p_1m python tools/loop_run.py 1000000 p2p 15 > /dev/null 2>&1
+# device-resident ICP loop, 1 M p2p: 2 estimate() calls x (1 cold search + 14 cached passes, each + 1 finish) launches
+FLUSH=1 $NCU -k regex:icp_search_kernel -s 1 -c 1 -o captures/r02_icp_cold_p2p_1m python tools/loop_run.py 1000000 p2p 15 > /dev/null 2>&1
 FLUSH=1 $NCU -k regex:icp_cached_pipe_kernel -s 10 -c 1 -o captures/r02_icp_cached_p2p_1m python tools/loop_run.py 1000000 p2p 15 > /dev/null 2>&1
 FLUSH=1 $NCU -k regex:icp_finish_kernel -s 12 -c 1 -o captures/r02_icp_finish_p2p_1m python tools/loop_run.py 1000000 p2p 15 > /dev/null 2>&1
-FLUSH=1 $NCU -k regex:icp_search_kernel -s 11 -c 1 -o captures/r02_icp_warm_search_p2p_1m python tools/loop_run.py 1000000 p2p 15 > /dev/null 2>&1
 fi
 if [ -z "${SKIP_10M:-}" ]; then
 # 10 M combined
-FLUSH=1 $NCU -k regex:icp_search_kernel -s 10 -c 1 -o captures/r02_icp_cold_combined_10m python tools/loop_run.py 10000000 combined 10 > /dev/null 2>&1
+FLUSH=1 $NCU -k regex:icp_search_kernel -s 1 -c 1 -o captures/r02_icp_cold_combined_10m python tools/loop_run.py 10000000 combined 10 > /dev/null 2>&1
 FLUSH=1 $NCU -k regex:icp_cached_pipe_kernel -s 7 -c 1 -o captures/r02_icp_cached_combined_10m python tools/loop_run.py 10000000 combined 10 > /dev/null 2>&1
-FLUSH=1 $NCU -k regex:icp_search_kernel -s 8 -c 1 -o captures/r02_icp_warm_search_combined_10m python tools/loop_run.py 10000000 combined 10 > /dev/null 2>&1
 fi
 # (all of the above with the L2 flushed before every iteration, as in bench.py's value leg: FLUSH=1)
 # k-means 50 M x 1024, RANSAC 5 M x 1000 (the shipped kernels on the BASELINE configs)

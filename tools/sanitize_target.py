@@ -27,7 +27,7 @@ def main():
     oi, od = knn.query(oracle.transform_points(T, src), max_d2)
     assert np.array_equal(idx, oi), "1-NN"
     icp = capi.Icp(ctx, d_dst, d_src)
-    # device-resident loop (cold search kernel, cached pass, warm search kernel, device solve) and host loop
+    # device-resident loop (cold search kernel, cached pass with its searches, device solve) and host loop
     for kw in (dict(metric="p2p"), dict(metric="combined", w_pt=0.1, w_pl=1.0),
                dict(metric="combined", w_pt=0.1, w_pl=1.0, pt_rbf_sigma=0.01, pl_rbf_sigma=0.01)):
         want = oracle.icp(dst, src, knn, dst_n=nrm if kw["metric"] == "combined" else None, max_iter=5, tol=0.0, max_d2=max_d2, **kw)
