@@ -151,6 +151,10 @@ struct ChunkPair {
   float d2;  // the match's squared distance (correspondence value)
 };
 
+// Lanes per queued region in the wide search's pooled scan (warp_search_wide.cuh). The cold search keeps one lane per
+// region. The cached pass's search uses pairs of lanes: its region scan then needs fewer live registers, and the
+// pass's streaming loop, which holds the call site of search_chunk_far, spills less (DESIGN §4.2).
+constexpr unsigned int kColdGroup = 1, kWarmGroup = 2;
 // kCold: nothing cached yet (no warm seed, first-iteration slack). Otherwise the query failed the exclusion test:
 // its cached match seeds the search and its last motion sets the slack.
 template <bool kCold>
@@ -176,7 +180,7 @@ __device__ __forceinline__ ChunkPair search_chunk_body(const LoopArgs& a, const 
       sd = a.cache_pos[cp.i];
     }
   }
-  const WideBest wb = warp_grid_nearest_wide(a.dst, *wsm, act, cp.qx, cp.qy, cp.qz, a.max_d2, sd, slack);
+  const WideBest wb = warp_grid_nearest_wide<kCold ? kColdGroup : kWarmGroup>(a.dst, *wsm, act, cp.qx, cp.qy, cp.qz, a.max_d2, sd, slack);
   if (act) {
     cp.pos = (wb.idx >= 0 && wb.d2 < a.max_d2) ? wb.pos : -1;
     cp.d2 = wb.d2;

@@ -14,7 +14,7 @@
 // smallest distances are tracked instead of one, and D2 = min(second smallest scanned, the widened bound,
 // the squared distance to the boundary of the scanned 3x3x3 block).
 // The shared-memory arrays and item decode (warp_search.cuh), the 4-wide candidate loop and the termination test
-// (nn_search.cuh) are the narrow search's. Phase A keeps its own copy of the region enumeration (compared against
+// (nn_search.cuh) are the narrow search's; with kGroup > 1 lanes per region, phase B has its own interleaved loop. Phase A keeps its own copy of the region enumeration (compared against
 // wide2 instead of the best distance): calling queue_regions() here costs the <3,*> search kernels 4-12 B of spills.
 #pragma once
 #include "warp_search.cuh"
@@ -24,6 +24,8 @@ namespace cb {
 struct WideSearchSmem : WarpQueue {
   unsigned int sec[32];  // merged second-smallest d2 (float bits; non-negative floats order like uints)
 };
+// The cached pass of the ICP loop keeps 8 of these per block and is 176 B short of losing a resident block per SM.
+static_assert(sizeof(WideSearchSmem) <= 3456, "WideSearchSmem must not grow");
 
 struct WideBest {
   float d2;   // squared distance of the nearest point with d2 < max_d2 (else max_d2)
@@ -51,9 +53,27 @@ __device__ __forceinline__ void scan_range_two(const float4* __restrict__ pts, u
   });
 }
 
+// A region's two smallest distances (l1 at sorted position lp >= 0, l2) into the owner's merged (key, sec).
+__device__ __forceinline__ void merge_region(WideSearchSmem& sm, unsigned int owner, float l1, int lp, float l2,
+                                             float max_d2) {
+  constexpr float kInf = 3.402823466e+38f;
+  float loser = l1;  // what this region contributes to "second smallest" besides l2
+  if (l1 < max_d2) {
+    const unsigned long long key = pack_key(l1, (unsigned int)lp);
+    const unsigned long long old = atomicMin(&sm.key[owner], key);
+    const float od2 = __uint_as_float((unsigned int)(old >> 32));
+    // the loser of (previous best, this region's best) is a second-best candidate; the initial "none"
+    // sentinel is not a point
+    loser = ((unsigned int)(old & 0xffffffffull) == 0xffffffffu) ? kInf : fmaxf(od2, l1);
+  }
+  atomicMin(&sm.sec[owner], __float_as_uint(fminf(l2, loser)));
+}
+
 // All 32 lanes of the warp must call this (inactive lanes pass active = false).
+// kGroup: lanes per queued region in the pooled scan of phase B (1, 2, 4, ... 32).
 // warm_pos >= 0: sorted position of a point known to be close (the cached match); slack >= 0: widening of the
 // search radius beyond the nearest distance, in the units of the coordinates.
+template <unsigned int kGroup>
 __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, WideSearchSmem& sm, bool active, float qx,
                                                            float qy, float qz, float max_d2, int warm_pos, float slack) {
   const unsigned int lane = threadIdx.x & 31;
@@ -142,25 +162,61 @@ __device__ __forceinline__ WideBest warp_grid_nearest_wide(const GridView& g, Wi
   __syncwarp();
 
   // ---- phase B: pooled scan of the queued regions ----------------------------------------------------
-  for (unsigned int k = lane; k < count; k += 32) {
-    const QueueItem it = queue_item(g, sm, k);
-    if (it.b >= it.e) continue;
-    const unsigned long long cur = sm.key[it.lane];
-    float l1 = kInf, l2 = kInf;
-    int lp = -1;
-    // the only point that can be met twice is the warm seed, and only while it is the running best
-    scan_range_two(g.pts, it.b, it.e, it.q.x, it.q.y, it.q.z, l1, lp, l2, (int)(unsigned int)(cur & 0xffffffffull));
-    if (lp < 0) continue;
-    float loser = l1;  // what this region contributes to "second smallest" besides l2
-    if (l1 < max_d2) {
-      const unsigned long long key = pack_key(l1, (unsigned int)lp);
-      const unsigned long long old = atomicMin(&sm.key[it.lane], key);
-      const float od2 = __uint_as_float((unsigned int)(old >> 32));
-      // the loser of (previous best, this region's best) is a second-best candidate; the initial "none"
-      // sentinel is not a point
-      loser = ((unsigned int)(old & 0xffffffffull) == 0xffffffffu) ? kInf : fmaxf(od2, l1);
+  static_assert(kGroup >= 1 && kGroup <= 32 && (kGroup & (kGroup - 1)) == 0, "lanes per region: a power of two");
+  if constexpr (kGroup == 1) {
+    for (unsigned int k = lane; k < count; k += 32) {
+      const QueueItem it = queue_item(g, sm, k);
+      if (it.b >= it.e) continue;
+      const unsigned long long cur = sm.key[it.lane];
+      float l1 = kInf, l2 = kInf;
+      int lp = -1;
+      // the only point that can be met twice is the warm seed, and only while it is the running best
+      scan_range_two(g.pts, it.b, it.e, it.q.x, it.q.y, it.q.z, l1, lp, l2, (int)(unsigned int)(cur & 0xffffffffull));
+      if (lp < 0) continue;
+      merge_region(sm, it.lane, l1, lp, l2, max_d2);
     }
-    atomicMin(&sm.sec[it.lane], __float_as_uint(fminf(l2, loser)));
+  } else {
+    // kGroup neighbouring lanes share an item and read its points interleaved (two per lane per step). The group's
+    // two smallest distances are combined with shuffles, and its first lane merges them into the owner's (key, sec).
+    // The result is the same: the two smallest of the same candidates, the warm seed skipped on the same rule.
+    const unsigned int sub = lane & (kGroup - 1u);
+    for (unsigned int k0 = 0; k0 < count; k0 += 32u / kGroup) {
+      const unsigned int k = k0 + lane / kGroup;
+      float l1 = kInf, l2 = kInf;
+      int lp = -1;
+      unsigned int owner = 0;
+      if (k < count) {
+        const QueueItem it = queue_item(g, sm, k);
+        owner = it.lane;
+        // the only point that can be met twice is the warm seed, and only while it is the running best
+        const int skip = (int)(unsigned int)(sm.key[it.lane] & 0xffffffffull);
+        for (uint32_t j = it.b + sub; j < it.e; j += 2u * kGroup) {
+          const float4 p0 = __ldg(g.pts + j);
+          const bool has1 = j + kGroup < it.e;
+          float4 p1 = p0;
+          if (has1) p1 = __ldg(g.pts + j + kGroup);
+          const float r0 = rule::contract_d2(it.q.x, it.q.y, it.q.z, p0.x, p0.y, p0.z);
+          if ((int)j != skip) two_smallest(r0, (int)j, l1, lp, l2);
+          if (has1) {
+            const float r1 = rule::contract_d2(it.q.x, it.q.y, it.q.z, p1.x, p1.y, p1.z);
+            if ((int)(j + kGroup) != skip) two_smallest(r1, (int)(j + kGroup), l1, lp, l2);
+          }
+        }
+      }
+      // two smallest of the group: the larger of the two minima is a second-smallest candidate (a bit-equal pair
+      // leaves l2 == l1, which phase C reads as a tie)
+#pragma unroll
+      for (unsigned int m = 1; m < kGroup; m <<= 1) {
+        const float o1 = __shfl_xor_sync(0xffffffffu, l1, m), o2 = __shfl_xor_sync(0xffffffffu, l2, m);
+        const int op = __shfl_xor_sync(0xffffffffu, lp, m);
+        l2 = fminf(fmaxf(l1, o1), fminf(l2, o2));
+        if (o1 < l1 || (o1 == l1 && op > lp)) {
+          l1 = o1;
+          lp = op;
+        }
+      }
+      if (sub == 0 && lp >= 0) merge_region(sm, owner, l1, lp, l2, max_d2);
+    }
   }
   __syncwarp();
 
