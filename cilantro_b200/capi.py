@@ -169,6 +169,17 @@ class WarpResult(C.Structure):
     ]
 
 
+class McdParams(C.Structure):
+    _fields_ = [
+        ("num_trials", C.c_int32),
+        ("num_refinements", C.c_int32),
+        ("inlier_ratio", C.c_float),
+        ("chi_square_threshold", C.c_float),
+        ("min_sample_size", C.c_int32),
+        ("seed", C.c_uint32),
+    ]
+
+
 class SparseWarpParams(C.Structure):
     _fields_ = [("base", WarpParams), ("ctrl_coeff", C.c_float), ("reserved_", C.c_int32)]
 
@@ -209,7 +220,7 @@ EXPORTED = [
     "cb_comm_unique_id", "cb_context_init_comm", "cb_context_comm_info", "cb_comm_ipc_handle", "cb_comm_ipc_attach",
     "cb_comm_ipc_detach",
     "cb_cloud_create", "cb_cloud_create_pair", "cb_cloud_create_from_device", "cb_cloud_create_replicated", "cb_cloud_destroy", "cb_cloud_size", "cb_cloud_grid_info",
-    "cb_cloud_estimate_normals", "cb_grid_downsample", "cb_cloud_grid_downsample", "cb_cloud_download", "cb_cloud_segment",
+    "cb_cloud_estimate_normals", "cb_cloud_estimate_normals_mcd", "cb_grid_downsample", "cb_cloud_grid_downsample", "cb_cloud_download", "cb_cloud_segment",
     "cb_cloud_mean_shift",
     "cb_knn1_radius", "cb_knn_radius", "cb_radius_search", "cb_find_correspondences",
     "cb_icp_default_params", "cb_icp_create", "cb_icp_destroy", "cb_icp_estimate", "cb_icp_iteration_times",
@@ -385,6 +396,27 @@ class Cloud:
         _check(lib().cb_cloud_estimate_normals(self.ctx.h, self.h, C.c_int(k), C.c_float(radius2), _p(vp),
                                                C.c_int(int(use_current_as_ref)), _p(nrm), _p(curv), _p(cov), C.byref(ms)))
         return {"normals": nrm, "curvature": curv, "cov6": cov, "gpu_ms": ms.value}
+
+    def estimate_normals_mcd(self, k, radius2=0.0, view_point=None, use_current_as_ref=False, num_trials=6,
+                             num_refinements=3, inlier_ratio=0.75, chi_square_threshold=-1.0, min_sample_size=3, seed=0,
+                             want_curvature=True, want_cov=False, want_status=True, fetch=True):
+        """cb_cloud_estimate_normals_mcd: NormalEstimation with MinimumCovarianceDeterminant over kNN (radius2 <= 0)
+        or kNN-in-radius neighbourhoods, k in [1, 128]. Defaults are the reference's. Stores the normals in the cloud;
+        returns dict(normals, curvature, cov6, status, gpu_ms); status: 0 ok, 1 too few neighbours, 2 rejected by the
+        chi-square test, 3 no trial with a finite determinant."""
+        n = self.n
+        nrm = np.empty((n, 3), np.float32) if fetch else None
+        curv = np.empty(n, np.float32) if (fetch and want_curvature) else None
+        cov = np.empty((n, 6), np.float32) if (fetch and want_cov) else None
+        st = np.empty(n, np.uint8) if (fetch and want_status) else None
+        vp = None if view_point is None else np.ascontiguousarray(view_point, np.float32).reshape(3)
+        prm = McdParams(int(num_trials), int(num_refinements), float(inlier_ratio), float(chi_square_threshold),
+                        int(min_sample_size), int(seed) & 0xFFFFFFFF)
+        ms = C.c_float()
+        _check(lib().cb_cloud_estimate_normals_mcd(self.ctx.h, self.h, C.c_int(k), C.c_float(radius2), _p(vp),
+                                                   C.c_int(int(use_current_as_ref)), C.byref(prm), _p(nrm), _p(curv),
+                                                   _p(cov), _p(st), C.byref(ms)))
+        return {"normals": nrm, "curvature": curv, "cov6": cov, "status": st, "gpu_ms": ms.value}
 
     @classmethod
     def replicated(cls, ctx, xyz_block, normals_block, first_index, n_total):

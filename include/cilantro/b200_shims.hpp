@@ -1731,6 +1731,16 @@ struct PointCloud3f {
   }
   size_t size() const { return points.cols(); }
   bool hasNormals() const { return size() > 0 && normals.cols() == size(); }
+  // removeInvalidNormals() (utilities/point_cloud.hpp:210-219): remove() of the points whose normal is not finite
+  PointCloud3f& removeInvalidNormals() {
+    if (!hasNormals()) return *this;
+    std::vector<size_t> drop;
+    for (size_t i = 0; i < normals.cols(); i++) {
+      const float* v = normals.data() + 3 * i;
+      if (!(std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]))) drop.push_back(i);
+    }
+    return remove(drop);
+  }
   bool hasColors() const { return size() > 0 && colors.cols() == size(); }
   bool isEmpty() const { return size() == 0; }
   // per-point transforms (a warp field): points by transformPoints(tforms, ...), normals by the linear parts

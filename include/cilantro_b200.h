@@ -150,6 +150,34 @@ int cb_radius_search(cb_context* ctx, const cb_cloud* ref, const cb_cloud* qry, 
  * (the k-best lists live in shared memory; CB_ERR_UNSUPPORTED above). */
 int cb_cloud_estimate_normals(cb_context* ctx, cb_cloud* cloud, int k, float radius2, const float* view_point3,
                               int use_current_as_ref, float* normals, float* curvature, float* cov6, float* gpu_ms);
+
+/* ---- robust normal estimation (minimum covariance determinant) ---------------------------------
+ * Replaces NormalEstimation<float, 3, MinimumCovarianceDeterminant<float, 3>> (core/normal_estimation.hpp:279-421
+ * over MinimumCovarianceDeterminant::operator(), core/covariance.hpp:185-371). Per point, over its neighbourhood
+ * (size m, in ascending (d2, index) order): m < min_sample_size -> invalid; m == min_sample_size -> the plain
+ * covariance; else h = min(max(min_sample_size, llround(inlier_ratio * m)), m); h == m -> the plain covariance (bit
+ * for bit cb_cloud_estimate_normals'); else num_trials trials of min_sample_size draws with replacement, each refined
+ * num_refinements times (keep the h smallest Mahalanobis distances, recompute), and the trial of smallest finite
+ * determinant wins. With chi_square_threshold > 0, the neighbourhood's first point must lie within d_M^2 <= threshold.
+ * Normal, curvature and orientation then follow cb_cloud_estimate_normals. The random draws, the selection order
+ * and the 3x3 algebra follow the rule of DESIGN §4.15 (cilantro_b200/csrc/mcd_rule.hpp): every point runs
+ * std::minstd_rand0 seeded from `seed` and its index, so equal seeds give equal bits.
+ * Neighbourhoods: k in [1, 128], kNN (radius2 <= 0) or kNN-in-radius (radius2 > 0); radius-only (k == 0) gives
+ * CB_ERR_UNSUPPORTED. Rejected: num_trials < 1, num_refinements < 0 or a non-finite inlier_ratio (CB_ERR_INVALID);
+ * min_sample_size outside [2, 32] or k > 128 (CB_ERR_UNSUPPORTED). Outputs as cb_cloud_estimate_normals', plus
+ * status (n bytes, may be NULL): 0 ok, 1 too few neighbours, 2 rejected by the chi-square test, 3 no trial with a
+ * finite determinant; every status but 0 gives NaN normal, curvature and cov6. */
+typedef struct cb_mcd_params {
+  int num_trials;             /* 6 in the reference */
+  int num_refinements;        /* 3 */
+  float inlier_ratio;         /* 0.75 */
+  float chi_square_threshold; /* -1: no test */
+  int min_sample_size;        /* 3 (NormalEstimation's setMinValidSampleSize(3)) */
+  uint32_t seed;              /* replaces the reference's std::random_device */
+} cb_mcd_params;
+int cb_cloud_estimate_normals_mcd(cb_context* ctx, cb_cloud* cloud, int k, float radius2, const float* view_point3,
+                                  int use_current_as_ref, const cb_mcd_params* params, float* normals, float* curvature,
+                                  float* cov6, uint8_t* status, float* gpu_ms);
 /* ---- voxel-grid downsampling -------------------------------------------------------------------
  * Replaces PointCloud::gridDownsample / gridDownsampled (utilities/point_cloud.hpp:246-290) =
  * Points[Normals][Colors]GridDownsampler (core/grid_downsampler.hpp) over GridAccumulator::build_index_

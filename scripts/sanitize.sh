@@ -3,8 +3,9 @@
 #   bash scripts/sanitize.sh   -> captures/sanitize_{memcheck,racecheck,synccheck}.log
 # and a one-line verdict per tool on stdout; tools/sanitize_summary.py turns the logs into a summary).
 # memcheck: out-of-bounds / misaligned global, shared and local accesses, leaks of device allocations.
-# racecheck: shared-memory hazards between threads of a block (the warp-pooled search queues, the barrier-free
-#            block reduction). synccheck: divergent / invalid use of __syncthreads / __syncwarp / *_sync shuffles.
+# racecheck: shared-memory hazards between threads of a block (the warp-pooled search queues, the per-warp
+#            neighbourhood staging of the robust normals, the barrier-free block reduction).
+# synccheck: divergent / invalid use of __syncthreads / __syncwarp / *_sync shuffles.
 set -u
 cd "$(dirname "$0")/.."
 mkdir -p captures

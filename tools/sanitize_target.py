@@ -52,6 +52,10 @@ def main():
     ds = c.grid_downsample(0.03)
     ds.estimate_normals(k=8, view_point=[0.5, 0.5, 5.0])
     ds.estimate_normals(k=0, radius2=0.06 ** 2)
+    # robust (MCD) normals: trials with refinements, kNN-in-radius, and the largest neighbourhood
+    ds.estimate_normals_mcd(k=12, num_trials=2, num_refinements=1, chi_square_threshold=6.25, want_cov=True)
+    ds.estimate_normals_mcd(k=16, radius2=0.06 ** 2, want_cov=True)
+    ds.estimate_normals_mcd(k=128, inlier_ratio=0.5, min_sample_size=32)
     # connected-component segmentation: radius (all seeds, seed list) and kNN, with the normal / colour terms
     sheet_n = c.estimate_normals(k=8)["normals"]
     seg = capi.Cloud(ctx, sheet, sheet_n)
