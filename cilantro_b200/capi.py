@@ -282,7 +282,26 @@ def identity():
     return np.hstack([np.eye(3, dtype=np.float32), np.zeros((3, 1), np.float32)])
 
 
-class Context:
+class _Handle:
+    """An object of the library held through self.h; close() destroys it once (also when it is collected)."""
+
+    _destroy = None  # name of its cb_*_destroy entry
+
+    def close(self):
+        if self.h:
+            getattr(lib(), self._destroy)(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Context(_Handle):
+    _destroy = "cb_context_destroy"
+
     def __init__(self, device=0):
         h = C.c_void_p()
         _check(lib().cb_context_create(C.c_int(device), C.byref(h)))
@@ -297,14 +316,7 @@ class Context:
         if self.h:
             for child in list(self._children):
                 child.close()
-            lib().cb_context_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        super().close()
 
     def synchronize(self):
         _check(lib().cb_context_synchronize(self.h))
@@ -350,8 +362,10 @@ def comm_unique_id() -> bytes:
     return buf.raw
 
 
-class Cloud:
+class Cloud(_Handle):
     """Device-resident point set (+ optional normals); see cb_cloud_create."""
+
+    _destroy = "cb_cloud_destroy"
 
     def __init__(self, ctx, xyz=None, normals=None, index_offset=0, device_ptr=None, device_normals_ptr=None, n=None):
         self.ctx = ctx
@@ -371,17 +385,6 @@ class Cloud:
             self.n = xyz.shape[0]
         self.h = h
         ctx._adopt(self)
-
-    def close(self):
-        if self.h:
-            lib().cb_cloud_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def estimate_normals(self, k=0, radius2=0.0, view_point=None, use_current_as_ref=False, want_curvature=True,
                          want_cov=False, fetch=True):
@@ -639,8 +642,10 @@ def icp_params(metric="p2p", max_iter=15, tol=1e-5, max_d2=1e-4, w_pt=0.0, w_pl=
     return p
 
 
-class Icp:
+class Icp(_Handle):
     """cb_icp_*: SimplePointToPointMetricRigidICP3f / SimpleCombinedMetricRigidICP3f."""
+
+    _destroy = "cb_icp_destroy"
 
     def __init__(self, ctx, dst: Cloud, src: Cloud):
         self.ctx, self.dst, self.src = ctx, dst, src
@@ -648,17 +653,6 @@ class Icp:
         _check(lib().cb_icp_create(ctx.h, dst.h, src.h, C.byref(h)))
         self.h = h
         ctx._adopt(self)
-
-    def close(self):
-        if self.h:
-            lib().cb_icp_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def estimate(self, **kw):
         prm = kw.pop("params", None) or icp_params(**kw)
@@ -883,8 +877,40 @@ def _t_set(T, n):
     return T
 
 
-class WarpIcp:
+class _WarpIcpBase(_Handle):
+    """What WarpIcp and SparseWarpIcp share: the last estimate's correspondences and solve() on given ones."""
+
+    _entries = None  # the names of the object's cb_*_solve and cb_*_correspondences entries
+
+    def _solve(self, prm, first, second, T_src, m):
+        # m unknown blocks; T_src holds one transform per source point
+        f = np.ascontiguousarray(first, np.uint64)
+        s = np.ascontiguousarray(second, np.uint64)
+        T = np.empty((max(m, 1), 12), np.float32)
+        x = np.empty((max(m, 1), 6), np.float32)
+        res = WarpSolveResult()
+        _check(getattr(lib(), self._entries[0])(self.h, C.byref(prm), _p(_t_set(T_src, self.src.n)), _p(f), _p(s),
+                                                None, C.c_size_t(f.shape[0]), _p(T), _p(x), C.byref(res)))
+        return {"T": T[:m].reshape(m, 3, 4), "x": x[:m], "converged": bool(res.converged), "gn_steps": int(res.gn_steps),
+                "cg_iterations": int(res.cg_iterations), "cg_iterations_last": int(res.cg_iterations_last),
+                "cg_error": float(res.cg_error), "kernel_launches": int(res.kernel_launches)}
+
+    def correspondences(self):
+        n = max(self.src.n, 1)
+        i1 = np.empty(n, np.uint64)
+        i2 = np.empty(n, np.uint64)
+        v = np.empty(n, np.float32)
+        cnt = C.c_size_t()
+        _check(getattr(lib(), self._entries[1])(self.h, _p(i1), _p(i2), _p(v), C.byref(cnt)))
+        c = cnt.value
+        return i1[:c].astype(np.int64), i2[:c].astype(np.int64), v[:c]
+
+
+class WarpIcp(_WarpIcpBase):
     """cb_warp_icp_*: SimpleCombinedMetricDenseRigidWarpFieldICP3f. Transforms are (n_src, 3, 4) float32."""
+
+    _destroy = "cb_warp_icp_destroy"
+    _entries = ("cb_warp_icp_solve", "cb_warp_icp_correspondences")
 
     def __init__(self, ctx, dst: Cloud, src: Cloud, reg_offsets, reg_index, reg_value):
         self.ctx, self.dst, self.src = ctx, dst, src
@@ -896,17 +922,6 @@ class WarpIcp:
                                         C.c_size_t(max(off.shape[0] - 1, 0)), C.byref(h)))
         self.h = h
         ctx._adopt(self)
-
-    def close(self):
-        if self.h:
-            lib().cb_warp_icp_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def estimate(self, T_init=None, **kw):
         prm = kw.pop("params", None) or warp_params(**kw)
@@ -921,17 +936,7 @@ class WarpIcp:
 
     def solve(self, first, second, T_src=None, **kw):
         prm = kw.pop("params", None) or warp_params(**kw)
-        n = self.src.n
-        f = np.ascontiguousarray(first, np.uint64)
-        s = np.ascontiguousarray(second, np.uint64)
-        T = np.empty((max(n, 1), 12), np.float32)
-        x = np.empty((max(n, 1), 6), np.float32)
-        res = WarpSolveResult()
-        _check(lib().cb_warp_icp_solve(self.h, C.byref(prm), _p(_t_set(T_src, n)), _p(f), _p(s), None,
-                                       C.c_size_t(f.shape[0]), _p(T), _p(x), C.byref(res)))
-        return {"T": T[:n].reshape(n, 3, 4), "x": x[:n], "converged": bool(res.converged), "gn_steps": int(res.gn_steps),
-                "cg_iterations": int(res.cg_iterations), "cg_iterations_last": int(res.cg_iterations_last),
-                "cg_error": float(res.cg_error), "kernel_launches": int(res.kernel_launches)}
+        return self._solve(prm, first, second, T_src, self.src.n)
 
     def residuals(self, T, **kw):
         prm = kw.pop("params", None) or warp_params(**kw)
@@ -939,16 +944,6 @@ class WarpIcp:
         out = np.empty(max(n, 1), np.float32)
         _check(lib().cb_warp_icp_residuals(self.h, C.byref(prm), _p(_t_set(T, n)), _p(out)))
         return out[:n]
-
-    def correspondences(self):
-        n = max(self.src.n, 1)
-        i1 = np.empty(n, np.uint64)
-        i2 = np.empty(n, np.uint64)
-        v = np.empty(n, np.float32)
-        cnt = C.c_size_t()
-        _check(lib().cb_warp_icp_correspondences(self.h, _p(i1), _p(i2), _p(v), C.byref(cnt)))
-        c = cnt.value
-        return i1[:c].astype(np.int64), i2[:c].astype(np.int64), v[:c]
 
 
 def sparse_warp_params(ctrl_sigma=1.0, **kw):
@@ -960,10 +955,13 @@ def sparse_warp_params(ctrl_sigma=1.0, **kw):
     return p
 
 
-class SparseWarpIcp:
+class SparseWarpIcp(_WarpIcpBase):
     """cb_sparse_warp_icp_*: SimpleCombinedMetricSparseRigidWarpFieldICP3f. ctrl = (offsets, index, value), one list
     of (node, squared distance) per source point; reg = the node neighbourhoods' CSR. Node transforms are (n_ctrl, 3, 4)
     and dense transforms (n_src, 3, 4) float32."""
+
+    _destroy = "cb_sparse_warp_icp_destroy"
+    _entries = ("cb_sparse_warp_icp_solve", "cb_sparse_warp_icp_correspondences")
 
     def __init__(self, ctx, dst: Cloud, src: Cloud, ctrl, n_ctrl, reg):
         self.ctx, self.dst, self.src, self.n_ctrl = ctx, dst, src, int(n_ctrl)
@@ -980,17 +978,6 @@ class SparseWarpIcp:
                                                C.byref(h)))
         self.h = h
         ctx._adopt(self)
-
-    def close(self):
-        if self.h:
-            lib().cb_sparse_warp_icp_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def estimate(self, T_init=None, **kw):
         prm = kw.pop("params", None) or sparse_warp_params(**kw)
@@ -1009,17 +996,7 @@ class SparseWarpIcp:
 
     def solve(self, first, second, T_dense_src=None, **kw):
         prm = kw.pop("params", None) or sparse_warp_params(**kw)
-        n, m = self.src.n, self.n_ctrl
-        f = np.ascontiguousarray(first, np.uint64)
-        s = np.ascontiguousarray(second, np.uint64)
-        T = np.empty((max(m, 1), 12), np.float32)
-        x = np.empty((max(m, 1), 6), np.float32)
-        res = WarpSolveResult()
-        _check(lib().cb_sparse_warp_icp_solve(self.h, C.byref(prm), _p(_t_set(T_dense_src, n)), _p(f), _p(s), None,
-                                              C.c_size_t(f.shape[0]), _p(T), _p(x), C.byref(res)))
-        return {"T": T[:m].reshape(m, 3, 4), "x": x[:m], "converged": bool(res.converged), "gn_steps": int(res.gn_steps),
-                "cg_iterations": int(res.cg_iterations), "cg_iterations_last": int(res.cg_iterations_last),
-                "cg_error": float(res.cg_error), "kernel_launches": int(res.kernel_launches)}
+        return self._solve(prm, first, second, T_dense_src, self.n_ctrl)
 
     def resample(self, T_ctrl, **kw):
         prm = kw.pop("params", None) or sparse_warp_params(**kw)
@@ -1034,16 +1011,6 @@ class SparseWarpIcp:
         out = np.empty(max(n, 1), np.float32)
         _check(lib().cb_sparse_warp_icp_residuals(self.h, C.byref(prm), _p(_t_set(T_dense, n)), _p(out)))
         return out[:n]
-
-    def correspondences(self):
-        n = max(self.src.n, 1)
-        i1 = np.empty(n, np.uint64)
-        i2 = np.empty(n, np.uint64)
-        v = np.empty(n, np.float32)
-        cnt = C.c_size_t()
-        _check(lib().cb_sparse_warp_icp_correspondences(self.h, _p(i1), _p(i2), _p(v), C.byref(cnt)))
-        c = cnt.value
-        return i1[:c].astype(np.int64), i2[:c].astype(np.int64), v[:c]
 
 
 def mean_cov(ctx, pts: Cloud):

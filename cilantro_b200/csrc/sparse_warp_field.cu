@@ -23,16 +23,10 @@
 #include "warp_field_common.cuh"
 #include <cstring>
 
-struct cb_sparse_warp_icp {
-  explicit cb_sparse_warp_icp(cb_context* c) : ctx(c), mem(c) {}
-  cb_context* ctx = nullptr;
-  cb::DeviceScope mem;  // every buffer below (device and pinned host)
-  const cb_cloud* dst = nullptr;
-  const cb_cloud* src = nullptr;
-  uint32_t n = 0;        // source points
-  uint32_t m = 0;        // control nodes
-  uint32_t nnz = 0;      // control-list entries
-  uint32_t n_arcs = 0;   // regularisation arcs between nodes (self-arcs dropped)
+// The sparse field: the core's blocks are the m control nodes; the control lists and the per-point buffers here.
+struct cb_sparse_warp_icp : WarpCore {
+  using WarpCore::WarpCore;
+  uint32_t nnz = 0;  // control-list entries
   // control lists: per point entries ctrl_off[i] .. ctrl_off[i+1]-1, in the given order (resampling, W_i) and sorted
   // stably by node (the estimator: sidx[k] = node, sperm[k] = the given entry it came from)
   uint32_t* d_ctrl_off = nullptr;
@@ -47,33 +41,10 @@ struct cb_sparse_warp_icp {
   uint32_t* d_ninc_off = nullptr;
   uint32_t* d_ninc_pt = nullptr;
   uint32_t* d_ninc_slot = nullptr;
-  // arcs between nodes and their incidence by node (as the dense path)
-  uint32_t* d_arc_lo = nullptr;
-  uint32_t* d_arc_hi = nullptr;
-  float* d_arc_d2 = nullptr;
-  float* d_arc_c = nullptr;
-  uint32_t* d_inc_off = nullptr;
-  uint32_t* d_inc_arc = nullptr;
-  uint32_t* d_inc_other = nullptr;
-  // per node
-  float* d_T = nullptr;      // [m][12] control transforms
-  float* d_xs = nullptr;     // [m][6] unknowns of the running estimator call
-  float* d_b = nullptr;      // [m][6] At b
-  float* d_inv = nullptr;    // [m][6] Jacobi preconditioner
-  float* d_vec = nullptr;    // [5][m][6] CG vectors x, r, p, z, q
   // per point
-  float* d_Td = nullptr;      // [n][12] dense warp field
-  float4* d_warped = nullptr; // T_i s_i, .w = index bits
-  float* d_B = nullptr;       // [n][21] data block, upper triangle row-major
-  float* d_g = nullptr;       // [n][6]
-  float* d_y = nullptr;       // [n][6] B_i P_i of the running matvec
-  int* d_nn = nullptr;
-  float* d_nn_d2 = nullptr;
-  double* d_part = nullptr;
-  WarpStats* d_stats = nullptr;
-  WarpStats* h_stats = nullptr;  // pinned
-  int cg_grid = 0;
-  bool have_corr = false;
+  float* d_Td = nullptr;  // [n][12] dense warp field
+  float* d_g = nullptr;   // [n][6]
+  float* d_y = nullptr;   // [n][6] B_i P_i of the running matvec
 };
 
 namespace {
@@ -340,9 +311,7 @@ __global__ void node_incidence_fill_kernel(const uint64_t* __restrict__ keys, co
                                            uint32_t* __restrict__ inc_pt, uint32_t* __restrict__ inc_slot,
                                            uint32_t* __restrict__ off) {
   for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k <= total; k += gridDim.x * blockDim.x) {
-    const uint32_t cur = k < total ? (uint32_t)keys[k] : m;
-    const uint32_t first = k > 0 ? (uint32_t)keys[k - 1] + 1 : 0u;
-    for (uint32_t p = first; p <= cur && p <= m; p++) off[p] = k;
+    incidence_offsets(keys, k, total, m, off);
     if (k < total) {
       inc_slot[k] = vals[k];
       inc_pt[k] = slot_pt[vals[k]];
@@ -360,10 +329,7 @@ __global__ void node_keys_kernel(const uint32_t* __restrict__ sidx, uint32_t tot
 
 using Obj = cb_sparse_warp_icp;
 
-int check_params(const Obj* w, const cb_sparse_warp_params* p) {
-  CB_CHECK(w && p, CB_ERR_INVALID, "null argument");
-  return check_warp_params(w->ctx, w->dst, &p->base);
-}
+int check_params(const Obj* w, const cb_sparse_warp_params* p) { return check_params(w, p ? &p->base : nullptr); }
 
 // The control weights of this call's ctrl_coeff.
 int weights(Obj* w, const cb_sparse_warp_params* p) {
@@ -394,41 +360,17 @@ int resample(Obj* w, const int* nn) {
   if (w->n == 0) return CB_OK;
   sparse_resample_kernel<<<grid_for(w->ctx, w->n), kBlock, 0, w->ctx->stream>>>(
       w->n, w->d_ctrl_off, w->d_ctrl_idx, w->d_w, w->d_W, w->d_T, w->src->d_raw, w->d_Td, w->d_warped, nn,
-      (WarpStats*)w->d_stats);
+      w->d_stats);
   w->ctx->launches += 1;
   CB_CUDA(cudaGetLastError());
   return CB_OK;
 }
 
-// d_Td <- T_host (identities when NULL) and the warped points
-int set_dense(Obj* w, const float* T_host) {
-  if (w->n == 0) return CB_OK;
-  if (T_host)
-    CB_CUDA(cudaMemcpyAsync(w->d_Td, T_host, 12 * (size_t)w->n * sizeof(float), cudaMemcpyHostToDevice, w->ctx->stream));
-  warp_points_kernel<<<grid_for(w->ctx, w->n), kBlock, 0, w->ctx->stream>>>(w->n, w->src->d_raw, w->d_Td,
-                                                                             T_host == nullptr, w->d_warped);
-  w->ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
-}
-
-struct StepTimes {
-  double assemble = 0, cg = 0;
-};
-
-// One estimateSparseWarpFieldCombinedMetric call on the current warped points and correspondence slots (the node
-// unknowns start at zero, :1531-1532); the control weights of this call must be in place.
-int gauss_newton(Obj* w, const cb_sparse_warp_params* prm, const int* corr_dst, const uint32_t* corr_off,
-                 bool corr_known, bool has_corr, int* converged, uint64_t* steps, uint64_t* cg_total, uint64_t* cg_last,
-                 float* cg_err, StepTimes* times) {
+// One estimateSparseWarpFieldCombinedMetric call (gauss_newton) with the sparse assembly, node pass and CG; the
+// control weights of this call must be in place.
+int sparse_gauss_newton(Obj* w, const cb_warp_params* p, const int* corr_dst, const uint32_t* corr_off, bool no_corr,
+                        GnCounts* gn, StepTimer* timer) {
   cb_context* ctx = w->ctx;
-  const cb_warp_params* p = &prm->base;
-  WarpStats* hs = (WarpStats*)w->h_stats;
-  const size_t n = w->n, m = w->m;
-  *converged = 0;
-  CB_CUDA(cudaMemsetAsync(w->d_xs, 0, 6 * std::max<size_t>(m, 1) * sizeof(float), ctx->stream));
-  const bool use_pt = p->w_pt > 0.f, use_pl = p->w_pl > 0.f;
-  if ((!use_pt && !use_pl) || (corr_known && !has_corr) || n == 0 || m == 0) return CB_OK;  // :1427-1433
   SparseAssembleArgs aa{};
   aa.n = w->n;
   aa.dst_raw = w->dst->d_raw;
@@ -445,9 +387,9 @@ int gauss_newton(Obj* w, const cb_sparse_warp_params* prm, const int* corr_dst, 
   aa.g = w->d_g;
   aa.w_pt_sqrt = sqrtf(p->w_pt);
   aa.w_pl_sqrt = sqrtf(p->w_pl);
-  aa.use_pt = use_pt;
-  aa.use_pl = use_pl;
-  aa.stats = (WarpStats*)w->d_stats;
+  aa.use_pt = p->w_pt > 0.f;
+  aa.use_pl = p->w_pl > 0.f;
+  aa.stats = w->d_stats;
   SparseNodeArgs na{};
   na.m = w->m;
   na.ninc_off = w->d_ninc_off;
@@ -468,19 +410,6 @@ int gauss_newton(Obj* w, const cb_sparse_warp_params* prm, const int* corr_dst, 
   na.reg_coeff = p->reg_coeff;
   na.huber = p->huber;
   SparseCgArgs ca{};
-  ca.v.n = w->m;
-  ca.v.b = w->d_b;
-  ca.v.inv = w->d_inv;
-  ca.v.x = w->d_vec;
-  ca.v.r = w->d_vec + 6 * m;
-  ca.v.p = w->d_vec + 12 * m;
-  ca.v.z = w->d_vec + 18 * m;
-  ca.v.q = w->d_vec + 24 * m;
-  ca.v.xs = w->d_xs;
-  ca.v.part = w->d_part;
-  ca.v.max_iter = (unsigned int)std::min<uint64_t>(p->max_cg_iter, 0xffffffffu);
-  ca.v.tol = (double)p->cg_tol;
-  ca.v.stats = (WarpStats*)w->d_stats;
   ca.n = w->n;
   ca.ctrl_off = w->d_ctrl_off;
   ca.sidx = w->d_sidx;
@@ -494,67 +423,15 @@ int gauss_newton(Obj* w, const cb_sparse_warp_params* prm, const int* corr_dst, 
   ca.inc_arc = w->d_inc_arc;
   ca.inc_other = w->d_inc_other;
   ca.arc_c = w->d_arc_c;
-  ScopedEvents ev;
-  CB_TRY(ev.create());
-  cudaEvent_t e_mid = nullptr;
-  CB_CUDA(cudaEventCreate(&e_mid));
-  struct EventGuard {
-    cudaEvent_t e;
-    ~EventGuard() { cudaEventDestroy(e); }
-  } guard{e_mid};
-  const float tol2 = p->gn_tol * p->gn_tol;
-  for (uint64_t step = 0; step < p->max_gn_iter; step++) {
-    CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
-    CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
-    sparse_assemble_kernel<<<(unsigned)((n + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(aa);
+  auto assemble = [&]() -> int {
+    sparse_assemble_kernel<<<(unsigned)(((size_t)w->n + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(aa);
     CB_CUDA(cudaGetLastError());
-    sparse_node_kernel<<<(unsigned)((m + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(na);
+    sparse_node_kernel<<<(unsigned)(((size_t)w->m + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(na);
     CB_CUDA(cudaGetLastError());
-    CB_CUDA(cudaEventRecord(e_mid, ctx->stream));
-    void* args[] = {&ca};
-    CB_CUDA(cudaLaunchCooperativeKernel((const void*)sparse_cg_kernel, dim3(w->cg_grid), dim3(kBlock), args, 0,
-                                        ctx->stream));
-    CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
-    ctx->launches += 3;
-    CB_CUDA(cudaMemcpyAsync(hs, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    float ta = 0.f, tc = 0.f;
-    CB_CUDA(cudaEventElapsedTime(&ta, ev.e0, e_mid));
-    CB_CUDA(cudaEventElapsedTime(&tc, e_mid, ev.e1));
-    times->assemble += ta;
-    times->cg += tc;
-    // no correspondence: b = 0, so the step left xs at zero; the reference returns before any step
-    if (step == 0 && hs->num_corr == 0) return CB_OK;
-    ++*steps;
-    *cg_total += hs->cg_iters;
-    *cg_last = hs->cg_iters;
-    *cg_err = hs->cg_err;
-    float mx;
-    std::memcpy(&mx, &hs->max_delta_bits, sizeof(float));
-    if (mx < tol2) {
-      *converged = 1;
-      break;
-    }
-  }
-  return CB_OK;
-}
-
-// The estimator's output over the nodes (compose: preApply with projection, else the plain transforms) and the max of
-// |dR_j - I|_F^2 + |dt_j|^2.
-int apply_update(Obj* w, bool compose, float* last_delta_sq) {
-  cb_context* ctx = w->ctx;
-  WarpStats* hs = (WarpStats*)w->h_stats;
-  CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
-  if (w->m) {
-    warp_compose_kernel<<<grid_for(ctx, w->m), kBlock, 0, ctx->stream>>>(w->m, nullptr, w->d_xs, w->d_T, compose,
-                                                                        nullptr, nullptr, (WarpStats*)w->d_stats);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
-  }
-  CB_CUDA(cudaMemcpyAsync(hs, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
-  CB_CUDA(cudaStreamSynchronize(ctx->stream));
-  std::memcpy(last_delta_sq, &hs->last_delta_bits, sizeof(float));
-  return CB_OK;
+    ctx->launches += 2;
+    return CB_OK;
+  };
+  return gauss_newton(w, p, no_corr, assemble, (const void*)sparse_cg_kernel, ca, gn, timer);
 }
 
 int init(Obj* w, const std::vector<uint32_t>& ctrl_off, const std::vector<uint32_t>& ctrl_idx,
@@ -563,8 +440,7 @@ int init(Obj* w, const std::vector<uint32_t>& ctrl_off, const std::vector<uint32
          const std::vector<float>& d2) {
   cb_context* ctx = w->ctx;
   cudaStream_t s = ctx->stream;
-  const size_t nn = std::max<size_t>(w->n, 1), mm = std::max<size_t>(w->m, 1), kk = std::max<size_t>(w->nnz, 1),
-               aa = std::max<size_t>(w->n_arcs, 1);
+  const size_t nn = std::max<size_t>(w->n, 1), mm = std::max<size_t>(w->m, 1), kk = std::max<size_t>(w->nnz, 1);
   CB_TRY(w->mem.alloc(&w->d_ctrl_off, nn + 1));
   CB_TRY(w->mem.alloc(&w->d_ctrl_idx, kk));
   CB_TRY(w->mem.alloc(&w->d_ctrl_d2, kk));
@@ -576,34 +452,11 @@ int init(Obj* w, const std::vector<uint32_t>& ctrl_off, const std::vector<uint32
   CB_TRY(w->mem.alloc(&w->d_ninc_off, mm + 1));
   CB_TRY(w->mem.alloc(&w->d_ninc_pt, kk));
   CB_TRY(w->mem.alloc(&w->d_ninc_slot, kk));
-  CB_TRY(w->mem.alloc(&w->d_arc_lo, aa));
-  CB_TRY(w->mem.alloc(&w->d_arc_hi, aa));
-  CB_TRY(w->mem.alloc(&w->d_arc_d2, aa));
-  CB_TRY(w->mem.alloc(&w->d_arc_c, 6 * aa));
-  CB_TRY(w->mem.alloc(&w->d_inc_off, mm + 1));
-  CB_TRY(w->mem.alloc(&w->d_inc_arc, 2 * aa));
-  CB_TRY(w->mem.alloc(&w->d_inc_other, 2 * aa));
-  CB_TRY(w->mem.alloc(&w->d_T, 12 * mm));
-  CB_TRY(w->mem.alloc(&w->d_xs, 6 * mm));
-  CB_TRY(w->mem.alloc(&w->d_b, 6 * mm));
-  CB_TRY(w->mem.alloc(&w->d_inv, 6 * mm));
-  CB_TRY(w->mem.alloc(&w->d_vec, 30 * mm));
   CB_TRY(w->mem.alloc(&w->d_Td, 12 * nn));
-  CB_TRY(w->mem.alloc(&w->d_warped, nn));
-  CB_TRY(w->mem.alloc(&w->d_B, 21 * nn));
   CB_TRY(w->mem.alloc(&w->d_g, 6 * nn));
   CB_TRY(w->mem.alloc(&w->d_y, 6 * nn));
-  CB_TRY(w->mem.alloc(&w->d_nn, nn));
-  CB_TRY(w->mem.alloc(&w->d_nn_d2, nn));
-  CB_TRY(w->mem.alloc(&w->d_stats, 1));
-  CB_TRY(w->mem.alloc_host(&w->h_stats, 1));
-  // cooperative grid: every block resident; enough blocks for the larger of the point and node loops
-  int per_sm = 0;
-  CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sparse_cg_kernel, kBlock, 0));
-  CB_CHECK(per_sm >= 1, CB_ERR_CUDA, "the CG kernel cannot be resident");
-  w->cg_grid = (int)std::max<size_t>(
-      1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (std::max(nn, mm) + kBlock - 1) / kBlock));
-  CB_TRY(w->mem.alloc(&w->d_part, 5 * (size_t)w->cg_grid));
+  // the CG's loops run over the points and over the nodes
+  CB_TRY(alloc_core(w, (const void*)sparse_cg_kernel, std::max<size_t>(w->n, w->m)));
   CB_CUDA(cudaMemcpyAsync(w->d_ctrl_off, ctrl_off.data(), ctrl_off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
   DeviceScope scope(ctx);
   uint32_t* d_slot_pt = nullptr;
@@ -633,9 +486,7 @@ int init(Obj* w, const std::vector<uint32_t>& ctrl_off, const std::vector<uint32
                                                                                 w->d_ninc_off);
   ctx->launches += 1;
   CB_CUDA(cudaGetLastError());
-  CB_TRY(upload_arc_incidence(ctx, w->m, lo, hi, d2, w->d_arc_lo, w->d_arc_hi, w->d_arc_d2, w->d_inc_off,
-                              w->d_inc_arc, w->d_inc_other));  // synchronises the stream
-  return CB_OK;
+  return upload_arc_incidence(w, lo, hi, d2);  // synchronises the stream
 }
 
 int copy_out(Obj* w, float* T_out, float* T_dense_out) {
@@ -696,30 +547,13 @@ int cb_sparse_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_clo
   std::vector<uint32_t> lo, hi;
   std::vector<float> ad2;
   CB_TRY(build_arcs(m, reg_offsets, reg_index, reg_value, n_reg, lo, hi, ad2));
-  CB_CUDA(cudaSetDevice(ctx->device));
-  CB_TRY(ensure_index(const_cast<cb_cloud*>(dst)));
-  Obj* w = new Obj(ctx);
-  w->dst = dst;
-  w->src = src;
-  w->n = n;
-  w->m = m;
-  w->nnz = (uint32_t)total;
-  w->n_arcs = (uint32_t)lo.size();
-  const int rc = init(w, off, idx, d2, sidx, sperm, slot_pt, lo, hi, ad2);
-  if (rc != CB_OK) {
-    delete w;
-    return rc;
-  }
-  *out = w;
-  return CB_OK;
+  return create_object(ctx, dst, src, m, (uint32_t)lo.size(), out, [&](Obj* w) {
+    w->nnz = (uint32_t)total;
+    return init(w, off, idx, d2, sidx, sperm, slot_pt, lo, hi, ad2);
+  });
 }
 
-void cb_sparse_warp_icp_destroy(cb_sparse_warp_icp* w) {
-  if (!w) return;
-  cudaSetDevice(w->ctx->device);
-  cudaStreamSynchronize(w->ctx->stream);
-  delete w;
-}
+void cb_sparse_warp_icp_destroy(cb_sparse_warp_icp* w) { destroy_object(w); }
 
 int cb_sparse_warp_icp_estimate(cb_sparse_warp_icp* w, const cb_sparse_warp_params* prm, const float* T_init,
                                 float* T_out, float* T_dense_out, cb_sparse_warp_result* res) {
@@ -733,24 +567,22 @@ int cb_sparse_warp_icp_estimate(cb_sparse_warp_icp* w, const cb_sparse_warp_para
   CB_TRY(ev_r.create());
   std::memset(res, 0, sizeof(*res));
   double ms_search = 0, ms_resample = 0;
-  StepTimes times;
+  StepTimer times;
+  CB_TRY(times.create());
   CB_TRY(weights(w, prm));
   CB_TRY(set_nodes(w, T_init));  // transform_ = transform_init_ (icp_base.hpp:72)
   CB_TRY(resample(w, nullptr));  // initializeComputation (:202-205)
   float last_delta = INFINITY;
   int it = 0;
   uint32_t num_corr = 0;
+  GnCounts gn;
   while (it < p->max_iter) {
     CB_CUDA(cudaEventRecord(ev_s.e0, ctx->stream));
-    CB_TRY(warp_search(ctx, w->dst, w->d_warped, w->n, p->max_d2, w->d_nn, w->d_nn_d2));  // updateCorrespondences
+    CB_TRY(warp_search(w, p->max_d2));  // updateCorrespondences
     CB_CUDA(cudaEventRecord(ev_s.e1, ctx->stream));
-    int conv = 0;
-    uint64_t cg_last = 0;
-    float cg_err = 0.f;
-    CB_TRY(gauss_newton(w, prm, w->d_nn, nullptr, false, false, &conv, &res->gn_steps, &res->cg_iterations, &cg_last,
-                        &cg_err, &times));
+    CB_TRY(sparse_gauss_newton(w, p, w->d_nn, nullptr, false, &gn, &times));
     float ld2 = 0.f;
-    CB_TRY(apply_update(w, true, &ld2));  // preApply over the nodes + last_delta_norm_ (:227, :231-239)
+    CB_TRY(apply_update(w, true, false, &ld2, nullptr));  // preApply over the nodes + last_delta_norm_ (:227, :231-239)
     CB_CUDA(cudaEventRecord(ev_r.e0, ctx->stream));
     CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
     CB_TRY(resample(w, w->d_nn));  // :228-229
@@ -758,7 +590,7 @@ int cb_sparse_warp_icp_estimate(cb_sparse_warp_icp* w, const cb_sparse_warp_para
     CB_CUDA(cudaMemcpyAsync(w->h_stats, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaEventSynchronize(ev_r.e1));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    num_corr = ((WarpStats*)w->h_stats)->num_corr;
+    num_corr = w->h_stats->num_corr;
     float a = 0.f, b = 0.f;
     CB_CUDA(cudaEventElapsedTime(&a, ev_s.e0, ev_s.e1));
     CB_CUDA(cudaEventElapsedTime(&b, ev_r.e0, ev_r.e1));
@@ -774,6 +606,8 @@ int cb_sparse_warp_icp_estimate(cb_sparse_warp_icp* w, const cb_sparse_warp_para
   res->last_delta = last_delta;
   res->converged = it > 0 && last_delta < p->tol;
   res->num_corr = num_corr;
+  res->gn_steps = gn.steps;
+  res->cg_iterations = gn.cg_total;
   res->gpu_ms_search = ms_search;
   res->gpu_ms_resample = ms_resample;
   res->gpu_ms_assemble = times.assemble;
@@ -793,28 +627,24 @@ int cb_sparse_warp_icp_solve(cb_sparse_warp_icp* w, const cb_sparse_warp_params*
   cb_context* ctx = w->ctx;
   const uint64_t launches0 = ctx->launches;
   std::memset(res, 0, sizeof(*res));
-  std::vector<uint32_t> off;
-  std::vector<int> slot;
-  CB_TRY(corr_slots(w->dst->n, w->n, corr_first, corr_second, n_corr, off, slot));
-  DeviceScope scope(ctx);
-  uint32_t* d_off = nullptr;
-  int* d_slot = nullptr;
-  CB_TRY(scope.alloc(&d_off, off.size()));
-  CB_TRY(scope.alloc(&d_slot, slot.size()));
-  CB_CUDA(cudaMemcpyAsync(d_off, off.data(), off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  CB_CUDA(cudaMemcpyAsync(d_slot, slot.data(), slot.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+  CorrSlots cs(ctx);
+  CB_TRY(upload_corr_slots(w, corr_first, corr_second, n_corr, &cs));
   CB_TRY(weights(w, prm));
-  CB_TRY(set_dense(w, T_dense_src));
-  int conv = 0;
-  StepTimes times;
-  CB_TRY(gauss_newton(w, prm, d_slot, d_off, true, n_corr > 0, &conv, &res->gn_steps, &res->cg_iterations,
-                      &res->cg_iterations_last, &res->cg_error, &times));
+  CB_TRY(warp_points(w, w->d_Td, T_dense_src));
+  GnCounts gn;
+  StepTimer times;
+  CB_TRY(times.create());
+  CB_TRY(sparse_gauss_newton(w, &prm->base, cs.d_slot, cs.d_off, n_corr == 0, &gn, &times));
   float ld2 = 0.f;
-  CB_TRY(apply_update(w, false, &ld2));
+  CB_TRY(apply_update(w, false, false, &ld2, nullptr));
   if (w->m && x_out)
     CB_CUDA(cudaMemcpyAsync(x_out, w->d_xs, 6 * (size_t)w->m * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   CB_TRY(copy_out(w, T_out, nullptr));
-  res->converged = conv;
+  res->converged = gn.converged;
+  res->gn_steps = gn.steps;
+  res->cg_iterations = gn.cg_total;
+  res->cg_iterations_last = gn.cg_last;
+  res->cg_error = gn.cg_err;
   res->kernel_launches = ctx->launches - launches0;
   return CB_OK;
 }
@@ -834,15 +664,13 @@ int cb_sparse_warp_icp_residuals(cb_sparse_warp_icp* w, const cb_sparse_warp_par
   CB_TRY(check_params(w, prm));
   CB_CHECK(w->n == 0 || (T_dense && out), CB_ERR_INVALID, "null argument");
   if (w->n == 0) return CB_OK;
-  CB_TRY(set_dense(w, T_dense));
-  return warp_residuals(w->ctx, w->dst, w->d_warped, w->n, &prm->base, out);
+  CB_TRY(warp_points(w, w->d_Td, T_dense));
+  return warp_residuals(w, &prm->base, out);
 }
 
 int cb_sparse_warp_icp_correspondences(cb_sparse_warp_icp* w, uint64_t* index_first, uint64_t* index_second,
                                        float* value, size_t* count) {
-  CB_CHECK(w && count, CB_ERR_INVALID, "null argument");
-  CB_CHECK(w->have_corr, CB_ERR_INVALID, "no estimate() has run");
-  return warp_correspondences(w->ctx, w->n, w->d_nn, w->d_nn_d2, index_first, index_second, value, count);
+  return warp_correspondences(w, index_first, index_second, value, count);
 }
 
 }  // extern "C"

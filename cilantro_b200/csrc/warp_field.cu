@@ -24,37 +24,9 @@
 #include "warp_field_common.cuh"
 #include <cstring>
 
-struct cb_warp_icp {
-  explicit cb_warp_icp(cb_context* c) : ctx(c), mem(c) {}
-  cb_context* ctx = nullptr;
-  cb::DeviceScope mem;  // every buffer below (device and pinned host)
-  const cb_cloud* dst = nullptr;
-  const cb_cloud* src = nullptr;
-  uint32_t n = 0;        // source points
-  uint32_t n_arcs = 0;   // regularisation arcs (self-arcs dropped)
-  // arcs (lo < hi) and their incidence, sorted stably by point: entries inc_off[i] .. inc_off[i+1]-1 of point i
-  uint32_t* d_arc_lo = nullptr;
-  uint32_t* d_arc_hi = nullptr;
-  float* d_arc_d2 = nullptr;
-  float* d_arc_c = nullptr;  // [n_arcs][6] c_e of the current step
-  uint32_t* d_inc_off = nullptr;
-  uint32_t* d_inc_arc = nullptr;
-  uint32_t* d_inc_other = nullptr;
-  // per point
-  float* d_T = nullptr;       // [n][12] current transforms
-  float4* d_warped = nullptr; // T_i s_i, .w = index bits (the search's query layout)
-  float* d_xs = nullptr;      // [n][6] unknowns of the running estimator call
-  float* d_B = nullptr;       // [n][21] data block, upper triangle row-major
-  float* d_b = nullptr;       // [n][6] right-hand side At b
-  float* d_inv = nullptr;     // [n][6] Jacobi preconditioner
-  float* d_vec = nullptr;     // [5][n][6] CG vectors x, r, p, z, q
-  int* d_nn = nullptr;        // [n] last search: dst index or -1
-  float* d_nn_d2 = nullptr;
-  double* d_part = nullptr;   // CG reduction partials [5][grid]
-  WarpStats* d_stats = nullptr;
-  WarpStats* h_stats = nullptr;  // pinned
-  int cg_grid = 0;
-  bool have_corr = false;
+// The dense field: one block of unknowns per source point (m = n), nothing beyond the shared core.
+struct cb_warp_icp : WarpCore {
+  using WarpCore::WarpCore;
 };
 
 namespace {
@@ -173,23 +145,10 @@ __global__ void __launch_bounds__(kBlock) warp_cg_kernel(const CgArgs a) {
   });
 }
 
-int check_params(const cb_warp_icp* w, const cb_warp_params* p) {
-  CB_CHECK(w && p, CB_ERR_INVALID, "null argument");
-  return check_warp_params(w->ctx, w->dst, p);
-}
-
-// One estimateDenseWarpFieldCombinedMetric call on the current warped points and correspondence slots (the unknowns
-// start at zero, :460-461). Returns the estimator's flag through *converged and accumulates the step and CG counts.
-// corr_known: the host knows whether the list is empty (has_corr); else the first step's assembly counts it.
-int gauss_newton(cb_warp_icp* w, const cb_warp_params* p, const int* corr_dst, const uint32_t* corr_off, bool corr_known,
-                 bool has_corr, int* converged, uint64_t* steps, uint64_t* cg_total, uint64_t* cg_last, float* cg_err) {
+// One estimateDenseWarpFieldCombinedMetric call (gauss_newton) with the dense assembly and CG.
+int dense_gauss_newton(cb_warp_icp* w, const cb_warp_params* p, const int* corr_dst, const uint32_t* corr_off,
+                       bool no_corr, GnCounts* gn) {
   cb_context* ctx = w->ctx;
-  WarpStats* hs = (WarpStats*)w->h_stats;
-  const size_t n = w->n;
-  *converged = 0;
-  CB_CUDA(cudaMemsetAsync(w->d_xs, 0, 6 * std::max<size_t>(n, 1) * sizeof(float), ctx->stream));
-  const bool use_pt = p->w_pt > 0.f, use_pl = p->w_pl > 0.f;
-  if ((!use_pt && !use_pl) || (corr_known && !has_corr) || n == 0) return CB_OK;  // :398-408
   AssembleArgs aa{};
   aa.n = w->n;
   aa.dst_raw = w->dst->d_raw;
@@ -211,82 +170,22 @@ int gauss_newton(cb_warp_icp* w, const cb_warp_params* p, const int* corr_dst, c
   aa.reg_sqrt = sqrtf(p->stiffness);
   aa.reg_coeff = p->reg_coeff;
   aa.huber = p->huber;
-  aa.use_pt = use_pt;
-  aa.use_pl = use_pl;
-  aa.stats = (WarpStats*)w->d_stats;
+  aa.use_pt = p->w_pt > 0.f;
+  aa.use_pl = p->w_pl > 0.f;
+  aa.stats = w->d_stats;
   CgArgs ca{};
-  ca.v.n = w->n;
-  ca.v.b = w->d_b;
-  ca.v.inv = w->d_inv;
-  ca.v.x = w->d_vec;
-  ca.v.r = w->d_vec + 6 * n;
-  ca.v.p = w->d_vec + 12 * n;
-  ca.v.z = w->d_vec + 18 * n;
-  ca.v.q = w->d_vec + 24 * n;
-  ca.v.xs = w->d_xs;
-  ca.v.part = w->d_part;
-  ca.v.max_iter = (unsigned int)std::min<uint64_t>(p->max_cg_iter, 0xffffffffu);
-  ca.v.tol = (double)p->cg_tol;
-  ca.v.stats = (WarpStats*)w->d_stats;
   ca.B = w->d_B;
   ca.inc_off = w->d_inc_off;
   ca.inc_arc = w->d_inc_arc;
   ca.inc_other = w->d_inc_other;
   ca.arc_c = w->d_arc_c;
-  const float tol2 = p->gn_tol * p->gn_tol;
-  for (uint64_t step = 0; step < p->max_gn_iter; step++) {
-    CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
-    warp_assemble_kernel<<<(unsigned)((n + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(aa);
-    CB_CUDA(cudaGetLastError());
-    void* args[] = {&ca};
-    CB_CUDA(cudaLaunchCooperativeKernel((const void*)warp_cg_kernel, dim3(w->cg_grid), dim3(kBlock), args, 0, ctx->stream));
-    ctx->launches += 2;
-    CB_CUDA(cudaMemcpyAsync(hs, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    // no correspondence: b = 0, so the step left xs at zero; the reference returns before any step
-    if (step == 0 && hs->num_corr == 0) return CB_OK;
-    ++*steps;
-    *cg_total += hs->cg_iters;
-    *cg_last = hs->cg_iters;
-    *cg_err = hs->cg_err;
-    float mx;
-    std::memcpy(&mx, &hs->max_delta_bits, sizeof(float));
-    if (mx < tol2) {
-      *converged = 1;
-      break;
-    }
-  }
-  return CB_OK;
-}
-
-int apply_update(cb_warp_icp* w, bool compose, bool warp_next, float* last_delta_sq, uint32_t* num_corr) {
-  cb_context* ctx = w->ctx;
-  WarpStats* hs = (WarpStats*)w->h_stats;
-  CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
-  if (w->n) {
-    warp_compose_kernel<<<grid_for(ctx, w->n), kBlock, 0, ctx->stream>>>(
-        w->n, w->src->d_raw, w->d_xs, w->d_T, compose, warp_next ? w->d_warped : nullptr, warp_next ? w->d_nn : nullptr,
-        (WarpStats*)w->d_stats);
+  auto assemble = [&]() -> int {
+    warp_assemble_kernel<<<(unsigned)(((size_t)w->n + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(aa);
     ctx->launches += 1;
     CB_CUDA(cudaGetLastError());
-  }
-  CB_CUDA(cudaMemcpyAsync(hs, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
-  CB_CUDA(cudaStreamSynchronize(ctx->stream));
-  std::memcpy(last_delta_sq, &hs->last_delta_bits, sizeof(float));
-  *num_corr = hs->num_corr;
-  return CB_OK;
-}
-
-int warp_points(cb_warp_icp* w, const float* T_host) {
-  cb_context* ctx = w->ctx;
-  if (w->n == 0) return CB_OK;
-  if (T_host)
-    CB_CUDA(cudaMemcpyAsync(w->d_T, T_host, 12 * (size_t)w->n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  warp_points_kernel<<<grid_for(ctx, w->n), kBlock, 0, ctx->stream>>>(w->n, w->src->d_raw, w->d_T, T_host == nullptr,
-                                                                      w->d_warped);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+    return CB_OK;
+  };
+  return gauss_newton(w, p, no_corr, assemble, (const void*)warp_cg_kernel, ca, gn, nullptr);
 }
 
 }  // namespace
@@ -312,40 +211,6 @@ void cb_warp_default_params(cb_warp_params* p) {
   p->inlier_fraction = 1.0;
 }
 
-// Device buffers of a new warp-field ICP object: arcs (lo, hi, d2) uploaded and their incidence sorted by point.
-static int warp_init(cb_warp_icp* w, const std::vector<uint32_t>& lo, const std::vector<uint32_t>& hi,
-                     const std::vector<float>& d2) {
-  cb_context* ctx = w->ctx;
-  const uint32_t n = w->n;
-  const size_t nn = std::max<size_t>(n, 1), m = std::max<size_t>(w->n_arcs, 1);
-  CB_TRY(w->mem.alloc(&w->d_arc_lo, m));
-  CB_TRY(w->mem.alloc(&w->d_arc_hi, m));
-  CB_TRY(w->mem.alloc(&w->d_arc_d2, m));
-  CB_TRY(w->mem.alloc(&w->d_arc_c, 6 * m));
-  CB_TRY(w->mem.alloc(&w->d_inc_off, nn + 1));
-  CB_TRY(w->mem.alloc(&w->d_inc_arc, 2 * m));
-  CB_TRY(w->mem.alloc(&w->d_inc_other, 2 * m));
-  CB_TRY(w->mem.alloc(&w->d_T, 12 * nn));
-  CB_TRY(w->mem.alloc(&w->d_warped, nn));
-  CB_TRY(w->mem.alloc(&w->d_xs, 6 * nn));
-  CB_TRY(w->mem.alloc(&w->d_B, 21 * nn));
-  CB_TRY(w->mem.alloc(&w->d_b, 6 * nn));
-  CB_TRY(w->mem.alloc(&w->d_inv, 6 * nn));
-  CB_TRY(w->mem.alloc(&w->d_vec, 30 * nn));
-  CB_TRY(w->mem.alloc(&w->d_nn, nn));
-  CB_TRY(w->mem.alloc(&w->d_nn_d2, nn));
-  CB_TRY(w->mem.alloc(&w->d_stats, 1));
-  CB_TRY(w->mem.alloc_host(&w->h_stats, 1));
-  // cooperative grid: every block resident (occupancy API), no more blocks than points need
-  int per_sm = 0;
-  CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, warp_cg_kernel, kBlock, 0));
-  CB_CHECK(per_sm >= 1, CB_ERR_CUDA, "the CG kernel cannot be resident");
-  w->cg_grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (nn + kBlock - 1) / kBlock));
-  CB_TRY(w->mem.alloc(&w->d_part, 5 * (size_t)w->cg_grid));
-  return upload_arc_incidence(ctx, n, lo, hi, d2, w->d_arc_lo, w->d_arc_hi, w->d_arc_d2, w->d_inc_off, w->d_inc_arc,
-                              w->d_inc_other);
-}
-
 int cb_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const uint64_t* reg_offsets,
                        const int64_t* reg_index, const float* reg_value, size_t n_reg, cb_warp_icp** out) {
   CB_CHECK(ctx && dst && src && out, CB_ERR_INVALID, "null argument");
@@ -354,28 +219,13 @@ int cb_warp_icp_create(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src
   std::vector<uint32_t> lo, hi;
   std::vector<float> d2;
   CB_TRY(build_arcs(n, reg_offsets, reg_index, reg_value, n_reg, lo, hi, d2));
-  CB_CUDA(cudaSetDevice(ctx->device));
-  CB_TRY(ensure_index(const_cast<cb_cloud*>(dst)));
-  cb_warp_icp* w = new cb_warp_icp(ctx);
-  w->dst = dst;
-  w->src = src;
-  w->n = n;
-  w->n_arcs = (uint32_t)lo.size();
-  const int rc = warp_init(w, lo, hi, d2);
-  if (rc != CB_OK) {
-    delete w;
-    return rc;
-  }
-  *out = w;
-  return CB_OK;
+  return create_object(ctx, dst, src, n, (uint32_t)lo.size(), out, [&](cb_warp_icp* w) {
+    CB_TRY(alloc_core(w, (const void*)warp_cg_kernel, n));
+    return upload_arc_incidence(w, lo, hi, d2);
+  });
 }
 
-void cb_warp_icp_destroy(cb_warp_icp* w) {
-  if (!w) return;
-  cudaSetDevice(w->ctx->device);
-  cudaStreamSynchronize(w->ctx->stream);
-  delete w;
-}
+void cb_warp_icp_destroy(cb_warp_icp* w) { destroy_object(w); }
 
 int cb_warp_icp_estimate(cb_warp_icp* w, const cb_warp_params* p, const float* T_init, float* T_out,
                          cb_warp_result* res) {
@@ -388,20 +238,17 @@ int cb_warp_icp_estimate(cb_warp_icp* w, const cb_warp_params* p, const float* T
   CB_TRY(ev_v.create());
   std::memset(res, 0, sizeof(*res));
   double ms_search = 0, ms_solve = 0;
-  CB_TRY(warp_points(w, T_init));  // transform_ = transform_init_ (icp_base.hpp:72)
+  CB_TRY(warp_points(w, w->d_T, T_init));  // transform_ = transform_init_ (icp_base.hpp:72)
   float last_delta = INFINITY;
   int it = 0;
   uint32_t num_corr = 0;
+  GnCounts gn;
   while (it < p->max_iter) {
     CB_CUDA(cudaEventRecord(ev_s.e0, ctx->stream));
-    CB_TRY(warp_search(ctx, w->dst, w->d_warped, w->n, p->max_d2, w->d_nn, w->d_nn_d2));  // updateCorrespondences
+    CB_TRY(warp_search(w, p->max_d2));  // updateCorrespondences
     CB_CUDA(cudaEventRecord(ev_s.e1, ctx->stream));
     CB_CUDA(cudaEventRecord(ev_v.e0, ctx->stream));
-    int conv = 0;
-    uint64_t cg_last = 0;
-    float cg_err = 0.f;
-    CB_TRY(gauss_newton(w, p, w->d_nn, nullptr, false, false, &conv, &res->gn_steps, &res->cg_iterations, &cg_last,
-                        &cg_err));
+    CB_TRY(dense_gauss_newton(w, p, w->d_nn, nullptr, false, &gn));
     float ld2 = 0.f;
     CB_TRY(apply_update(w, true, true, &ld2, &num_corr));  // preApply + last_delta_norm_
     CB_CUDA(cudaEventRecord(ev_v.e1, ctx->stream));
@@ -422,6 +269,8 @@ int cb_warp_icp_estimate(cb_warp_icp* w, const cb_warp_params* p, const float* T
   res->last_delta = last_delta;
   res->converged = it > 0 && last_delta < p->tol;
   res->num_corr = num_corr;
+  res->gn_steps = gn.steps;
+  res->cg_iterations = gn.cg_total;
   res->gpu_ms_search = ms_search;
   res->gpu_ms_solve = ms_solve;
   res->kernel_launches = ctx->launches - launches0;
@@ -439,28 +288,22 @@ int cb_warp_icp_solve(cb_warp_icp* w, const cb_warp_params* p, const float* T_sr
   cb_context* ctx = w->ctx;
   const uint64_t launches0 = ctx->launches;
   std::memset(res, 0, sizeof(*res));
-  std::vector<uint32_t> off;
-  std::vector<int> slot;
-  CB_TRY(corr_slots(w->dst->n, w->n, corr_first, corr_second, n_corr, off, slot));
-  DeviceScope scope(ctx);
-  uint32_t* d_off = nullptr;
-  int* d_slot = nullptr;
-  CB_TRY(scope.alloc(&d_off, off.size()));
-  CB_TRY(scope.alloc(&d_slot, slot.size()));
-  CB_CUDA(cudaMemcpyAsync(d_off, off.data(), off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-  CB_CUDA(cudaMemcpyAsync(d_slot, slot.data(), slot.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-  CB_TRY(warp_points(w, T_src));
-  int conv = 0;
-  uint32_t nc = 0;
-  CB_TRY(gauss_newton(w, p, d_slot, d_off, true, n_corr > 0, &conv, &res->gn_steps, &res->cg_iterations,
-                      &res->cg_iterations_last, &res->cg_error));
+  CorrSlots cs(ctx);
+  CB_TRY(upload_corr_slots(w, corr_first, corr_second, n_corr, &cs));
+  CB_TRY(warp_points(w, w->d_T, T_src));
+  GnCounts gn;
+  CB_TRY(dense_gauss_newton(w, p, cs.d_slot, cs.d_off, n_corr == 0, &gn));
   float ld2 = 0.f;
-  CB_TRY(apply_update(w, false, false, &ld2, &nc));
+  CB_TRY(apply_update(w, false, false, &ld2, nullptr));
   if (w->n) CB_CUDA(cudaMemcpyAsync(T_out, w->d_T, 12 * (size_t)w->n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   if (w->n && x_out)
     CB_CUDA(cudaMemcpyAsync(x_out, w->d_xs, 6 * (size_t)w->n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
-  res->converged = conv;
+  res->converged = gn.converged;
+  res->gn_steps = gn.steps;
+  res->cg_iterations = gn.cg_total;
+  res->cg_iterations_last = gn.cg_last;
+  res->cg_error = gn.cg_err;
   res->kernel_launches = ctx->launches - launches0;
   return CB_OK;
 }
@@ -469,15 +312,13 @@ int cb_warp_icp_residuals(cb_warp_icp* w, const cb_warp_params* p, const float* 
   CB_TRY(check_params(w, p));
   CB_CHECK(w->n == 0 || (T && out), CB_ERR_INVALID, "null argument");
   if (w->n == 0) return CB_OK;
-  CB_TRY(warp_points(w, T));
-  return warp_residuals(w->ctx, w->dst, w->d_warped, w->n, p, out);
+  CB_TRY(warp_points(w, w->d_T, T));
+  return warp_residuals(w, p, out);
 }
 
 int cb_warp_icp_correspondences(cb_warp_icp* w, uint64_t* index_first, uint64_t* index_second, float* value,
                                 size_t* count) {
-  CB_CHECK(w && count, CB_ERR_INVALID, "null argument");
-  CB_CHECK(w->have_corr, CB_ERR_INVALID, "no estimate() has run");
-  return warp_correspondences(w->ctx, w->n, w->d_nn, w->d_nn_d2, index_first, index_second, value, count);
+  return warp_correspondences(w, index_first, index_second, value, count);
 }
 
 }  // extern "C"

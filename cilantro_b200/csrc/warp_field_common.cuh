@@ -1,7 +1,8 @@
 // Device and host pieces shared by the dense (warp_field.cu, DESIGN §4.13) and the sparse (sparse_warp_field.cu,
 // DESIGN §4.14) rigid warp-field ICP: the Huber rules, the rotation terms and data rows of the estimators, the block
 // and grid partial sums, the preconditioned CG loop, the compose step, the arc incidence and the 1-NN search on the
-// warped points. Product code (sm_90a).
+// warped points; on the host the object core both objects build on, their creation, checks and correspondence
+// uploads, the Gauss-Newton driver and the update step. Product code (sm_90a).
 //
 // Arithmetic: fp32 with every operation rounded on its own (no FMA contraction) wherever the oracles restate the
 // order; dot products and norms in fp64, summed in a fixed order; no float atomics.
@@ -14,6 +15,8 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstring>
+#include <memory>
 #include <vector>
 
 namespace {
@@ -452,16 +455,22 @@ __global__ void incidence_keys_kernel(const uint32_t* __restrict__ lo, const uin
   }
 }
 
+// Entry k (0 <= k <= total) of an incidence sorted by key (keys < n): off[p] = k for the keys p whose entries start
+// at k, so that off[p] = first entry of key p and off[n] = total.
+__device__ __forceinline__ void incidence_offsets(const uint64_t* __restrict__ keys, uint32_t k, uint32_t total,
+                                                  uint32_t n, uint32_t* __restrict__ off) {
+  const uint32_t cur = k < total ? (uint32_t)keys[k] : n;
+  const uint32_t first = k > 0 ? (uint32_t)keys[k - 1] + 1 : 0u;
+  for (uint32_t p = first; p <= cur && p <= n; p++) off[p] = k;
+}
+
 // after the sort: arc and other end per entry, and off[p] = first entry of point p (off[n] = total)
 __global__ void incidence_fill_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, uint32_t total,
                                       uint32_t n, const uint32_t* __restrict__ lo, const uint32_t* __restrict__ hi,
                                       uint32_t* __restrict__ inc_arc, uint32_t* __restrict__ inc_other,
                                       uint32_t* __restrict__ off) {
   for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k <= total; k += gridDim.x * blockDim.x) {
-    const uint32_t cur = k < total ? (uint32_t)keys[k] : n;
-    const uint32_t prev = k > 0 ? (uint32_t)keys[k - 1] : 0u;
-    const uint32_t first = k > 0 ? prev + 1 : 0u;
-    for (uint32_t p = first; p <= cur && p <= n; p++) off[p] = k;
+    incidence_offsets(keys, k, total, n, off);
     if (k < total) {
       const uint32_t e = vals[k] >> 1;
       inc_arc[k] = e;
@@ -470,16 +479,54 @@ __global__ void incidence_fill_kernel(const uint64_t* __restrict__ keys, const u
   }
 }
 
+// What both warp-field ICP objects hold (cb_warp_icp is this core; cb_sparse_warp_icp adds its control lists). The
+// unknowns come in m blocks of 6: one block per source point (dense, m = n) or per control node (sparse).
+struct WarpCore {
+  explicit WarpCore(cb_context* c) : ctx(c), mem(c) {}
+  cb_context* ctx = nullptr;
+  DeviceScope mem;  // every buffer of the object (device and pinned host)
+  const cb_cloud* dst = nullptr;
+  const cb_cloud* src = nullptr;
+  uint32_t n = 0;       // source points
+  uint32_t m = 0;       // unknown blocks
+  uint32_t n_arcs = 0;  // regularisation arcs between blocks (self-arcs dropped)
+  // arcs (lo < hi) and their incidence, sorted stably by block: entries inc_off[j] .. inc_off[j+1]-1 of block j
+  uint32_t* d_arc_lo = nullptr;
+  uint32_t* d_arc_hi = nullptr;
+  float* d_arc_d2 = nullptr;
+  float* d_arc_c = nullptr;  // [n_arcs][6] c_e of the current step
+  uint32_t* d_inc_off = nullptr;
+  uint32_t* d_inc_arc = nullptr;
+  uint32_t* d_inc_other = nullptr;
+  // per block
+  float* d_T = nullptr;    // [m][12] current transforms
+  float* d_xs = nullptr;   // [m][6] unknowns of the running estimator call
+  float* d_b = nullptr;    // [m][6] right-hand side At b
+  float* d_inv = nullptr;  // [m][6] Jacobi preconditioner
+  float* d_vec = nullptr;  // [5][m][6] CG vectors x, r, p, z, q
+  // per point
+  float* d_B = nullptr;        // [n][21] data block, upper triangle row-major
+  float4* d_warped = nullptr;  // T_i s_i, .w = index bits (the search's query layout)
+  int* d_nn = nullptr;         // [n] last search: dst index or -1
+  float* d_nn_d2 = nullptr;
+  double* d_part = nullptr;  // CG reduction partials [5][cg_grid]
+  WarpStats* d_stats = nullptr;
+  WarpStats* h_stats = nullptr;  // pinned
+  int cg_grid = 0;
+  bool have_corr = false;
+};
+
 int grid_for(cb_context* ctx, size_t n) {
   return (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + kBlock - 1) / kBlock));
 }
 
-int check_warp_params(cb_context* ctx, const cb_cloud* dst, const cb_warp_params* p) {
+int check_params(const WarpCore* w, const cb_warp_params* p) {
+  CB_CHECK(w && p, CB_ERR_INVALID, "null argument");
   CB_CHECK(p->search_dir == CB_SECOND_TO_FIRST && p->require_reciprocal == 0 && p->one_to_one == 0 &&
                !(p->inlier_fraction > 0.0 && p->inlier_fraction < 1.0),
            CB_ERR_UNSUPPORTED, "the warp-field ICP supports the default correspondence engine only");
-  CB_CHECK(!(p->w_pl > 0.f) || dst->d_raw_nrm, CB_ERR_INVALID, "w_pl > 0 needs a destination cloud with normals");
-  CB_CUDA(cudaSetDevice(ctx->device));
+  CB_CHECK(!(p->w_pl > 0.f) || w->dst->d_raw_nrm, CB_ERR_INVALID, "w_pl > 0 needs a destination cloud with normals");
+  CB_CUDA(cudaSetDevice(w->ctx->device));
   return CB_OK;
 }
 
@@ -526,17 +573,74 @@ int build_arcs(uint32_t n_nodes, const uint64_t* reg_offsets, const int64_t* reg
   return CB_OK;
 }
 
-// Uploads the arcs (lo, hi, d2: device buffers of max(m, 1) entries) and builds their incidence over n_nodes blocks,
-// sorted stably by block: entries inc_off[i] .. inc_off[i+1]-1 of block i, ascending arc.
-int upload_arc_incidence(cb_context* ctx, uint32_t n_nodes, const std::vector<uint32_t>& lo,
-                         const std::vector<uint32_t>& hi, const std::vector<float>& d2, uint32_t* d_lo, uint32_t* d_hi,
-                         float* d_d2, uint32_t* d_inc_off, uint32_t* d_inc_arc, uint32_t* d_inc_other) {
+// A new object on validated inputs: the destination's grid index, the core's sizes, then init(w), which allocates and
+// uploads; the object is freed again when a step fails.
+template <class Obj, class Init>
+int create_object(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, uint32_t m, uint32_t n_arcs, Obj** out,
+                  Init&& init) {
+  CB_CUDA(cudaSetDevice(ctx->device));
+  CB_TRY(ensure_index(const_cast<cb_cloud*>(dst)));
+  std::unique_ptr<Obj> w(new Obj(ctx));
+  w->dst = dst;
+  w->src = src;
+  w->n = (uint32_t)src->n;
+  w->m = m;
+  w->n_arcs = n_arcs;
+  CB_TRY(init(w.get()));
+  *out = w.release();
+  return CB_OK;
+}
+
+template <class Obj>
+void destroy_object(Obj* w) {
+  if (!w) return;
+  cudaSetDevice(w->ctx->device);
+  cudaStreamSynchronize(w->ctx->stream);
+  delete w;
+}
+
+// The core's buffers. The cooperative grid of cg_kernel: every block resident (occupancy API), no more blocks than
+// its grid-stride loops over loop_len entries need.
+int alloc_core(WarpCore* w, const void* cg_kernel, size_t loop_len) {
+  const size_t nn = std::max<size_t>(w->n, 1), mm = std::max<size_t>(w->m, 1), aa = std::max<size_t>(w->n_arcs, 1);
+  CB_TRY(w->mem.alloc(&w->d_arc_lo, aa));
+  CB_TRY(w->mem.alloc(&w->d_arc_hi, aa));
+  CB_TRY(w->mem.alloc(&w->d_arc_d2, aa));
+  CB_TRY(w->mem.alloc(&w->d_arc_c, 6 * aa));
+  CB_TRY(w->mem.alloc(&w->d_inc_off, mm + 1));
+  CB_TRY(w->mem.alloc(&w->d_inc_arc, 2 * aa));
+  CB_TRY(w->mem.alloc(&w->d_inc_other, 2 * aa));
+  CB_TRY(w->mem.alloc(&w->d_T, 12 * mm));
+  CB_TRY(w->mem.alloc(&w->d_xs, 6 * mm));
+  CB_TRY(w->mem.alloc(&w->d_b, 6 * mm));
+  CB_TRY(w->mem.alloc(&w->d_inv, 6 * mm));
+  CB_TRY(w->mem.alloc(&w->d_vec, 30 * mm));
+  CB_TRY(w->mem.alloc(&w->d_B, 21 * nn));
+  CB_TRY(w->mem.alloc(&w->d_warped, nn));
+  CB_TRY(w->mem.alloc(&w->d_nn, nn));
+  CB_TRY(w->mem.alloc(&w->d_nn_d2, nn));
+  CB_TRY(w->mem.alloc(&w->d_stats, 1));
+  CB_TRY(w->mem.alloc_host(&w->h_stats, 1));
+  int per_sm = 0;
+  CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cg_kernel, kBlock, 0));
+  CB_CHECK(per_sm >= 1, CB_ERR_CUDA, "the CG kernel cannot be resident");
+  w->cg_grid = (int)std::max<size_t>(
+      1, std::min<size_t>((size_t)w->ctx->sm_count * per_sm, (std::max<size_t>(loop_len, 1) + kBlock - 1) / kBlock));
+  return w->mem.alloc(&w->d_part, 5 * (size_t)w->cg_grid);
+}
+
+// Uploads the arcs (lo, hi, d2) and builds their incidence over the m blocks, sorted stably by block: entries
+// inc_off[j] .. inc_off[j+1]-1 of block j, ascending arc. Synchronises the stream.
+int upload_arc_incidence(WarpCore* w, const std::vector<uint32_t>& lo, const std::vector<uint32_t>& hi,
+                         const std::vector<float>& d2) {
+  cb_context* ctx = w->ctx;
   cudaStream_t s = ctx->stream;
-  const uint32_t m32 = (uint32_t)lo.size(), total = 2 * m32;
+  const uint32_t n_nodes = w->m, m32 = (uint32_t)lo.size(), total = 2 * m32;
+  uint32_t *d_lo = w->d_arc_lo, *d_hi = w->d_arc_hi;
   if (m32) {
     CB_CUDA(cudaMemcpyAsync(d_lo, lo.data(), m32 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     CB_CUDA(cudaMemcpyAsync(d_hi, hi.data(), m32 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-    CB_CUDA(cudaMemcpyAsync(d_d2, d2.data(), m32 * sizeof(float), cudaMemcpyHostToDevice, s));
+    CB_CUDA(cudaMemcpyAsync(w->d_arc_d2, d2.data(), m32 * sizeof(float), cudaMemcpyHostToDevice, s));
   }
   DeviceScope scope(ctx);
   uint64_t *keys = nullptr, *keys_tmp = nullptr;
@@ -554,38 +658,38 @@ int upload_arc_incidence(cb_context* ctx, uint32_t n_nodes, const std::vector<ui
     CB_TRY(radix_sort_pairs_u64(ctx, keys, vals, keys_tmp, vals_tmp, total, bits));
   }
   incidence_fill_kernel<<<grid_for(ctx, (size_t)total + 1), kBlock, 0, s>>>(keys, vals, total, n_nodes, d_lo, d_hi,
-                                                                           d_inc_arc, d_inc_other, d_inc_off);
+                                                                           w->d_inc_arc, w->d_inc_other, w->d_inc_off);
   ctx->launches += 1;
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaStreamSynchronize(s));
   return CB_OK;
 }
 
-// The grid 1-NN of the ICP pass kernel on the warped points: out_idx[i] = destination index within max_d2, or -1.
-int warp_search(cb_context* ctx, const cb_cloud* dst, const float4* warped, uint32_t n, float max_d2, int* out_idx,
-                float* out_d2) {
-  if (n == 0) return CB_OK;
+// The grid 1-NN of the ICP pass kernel on the warped points: nn[i] = destination index within max_d2, or -1.
+int warp_search(const WarpCore* w, float max_d2) {
+  if (w->n == 0) return CB_OK;
   IcpArgs a{};
-  a.dst = grid_view(dst);
-  a.src_pts = warped;
-  a.n_src = n;
+  a.dst = grid_view(w->dst);
+  a.src_pts = w->d_warped;
+  a.n_src = w->n;
   a.T = rigid_from_t12(nullptr);
   a.Tin = rigid_from_t12(nullptr);
   a.max_d2 = max_d2;
-  a.out_idx = out_idx;
-  a.out_d2 = out_d2;
-  return launch_icp_pass(ctx, a, kModeKnn, true, false, false);
+  a.out_idx = w->d_nn;
+  a.out_d2 = w->d_nn_d2;
+  return launch_icp_pass(w->ctx, a, kModeKnn, true, false, false);
 }
 
 // computeResiduals() of both warp-field ICP classes on the warped points (see cb_warp_icp_residuals).
-int warp_residuals(cb_context* ctx, const cb_cloud* dst, const float4* warped, uint32_t n, const cb_warp_params* p,
-                   float* out) {
+int warp_residuals(const WarpCore* w, const cb_warp_params* p, float* out) {
+  cb_context* ctx = w->ctx;
+  const uint32_t n = w->n;
   DeviceScope scope(ctx);
   float* d_out = nullptr;
   CB_TRY(scope.alloc(&d_out, n));
-  const bool normals = dst->d_raw_nrm != nullptr;
+  const bool normals = w->dst->d_raw_nrm != nullptr;
   // the combined residual reads the destination normals; without them (w_pl <= 0 here) it is w_pt |d - p|^2
-  CB_TRY(launch_residuals(ctx, grid_view(dst), warped, nullptr, n, rigid_from_t12(nullptr),
+  CB_TRY(launch_residuals(ctx, grid_view(w->dst), w->d_warped, nullptr, n, rigid_from_t12(nullptr),
                           normals ? CB_ICP_COMBINED : CB_ICP_POINT_TO_POINT, p->w_pt, p->w_pl, d_out));
   CB_CUDA(cudaMemcpyAsync(out, d_out, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -594,15 +698,19 @@ int warp_residuals(cb_context* ctx, const cb_cloud* dst, const float4* warped, u
   return CB_OK;
 }
 
-// getCorrespondences() from the last search (nn, nn_d2 on the device): ascending source index
-int warp_correspondences(cb_context* ctx, uint32_t n, const int* d_nn, const float* d_nn_d2, uint64_t* index_first,
-                         uint64_t* index_second, float* value, size_t* count) {
+// getCorrespondences() from the last search of estimate() (nn, nn_d2 on the device): ascending source index
+int warp_correspondences(const WarpCore* w, uint64_t* index_first, uint64_t* index_second, float* value,
+                         size_t* count) {
+  CB_CHECK(w && count, CB_ERR_INVALID, "null argument");
+  CB_CHECK(w->have_corr, CB_ERR_INVALID, "no estimate() has run");
+  cb_context* ctx = w->ctx;
+  const uint32_t n = w->n;
   CB_CUDA(cudaSetDevice(ctx->device));
   std::vector<int> idx(n);
   std::vector<float> d2(n);
   if (n) {
-    CB_CUDA(cudaMemcpyAsync(idx.data(), d_nn, n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaMemcpyAsync(d2.data(), d_nn_d2, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaMemcpyAsync(idx.data(), w->d_nn, n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaMemcpyAsync(d2.data(), w->d_nn_d2, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   }
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   size_t k = 0;
@@ -618,18 +726,150 @@ int warp_correspondences(cb_context* ctx, uint32_t n, const int* d_nn, const flo
 }
 
 // Caller-supplied correspondences grouped by source point (list order kept within a point): the slot CSR the
-// estimators' assembly reads. Validates the indices.
-int corr_slots(size_t n_dst, uint32_t n_src, const uint64_t* corr_first, const uint64_t* corr_second, size_t n_corr,
-               std::vector<uint32_t>& off, std::vector<int>& slot) {
-  off.assign((size_t)n_src + 1, 0u);
+// estimators' assembly reads (d_off[i] .. d_off[i+1]-1: the dst indices of point i), on the device for one call.
+struct CorrSlots {
+  explicit CorrSlots(cb_context* ctx) : scope(ctx) {}
+  DeviceScope scope;
+  std::vector<uint32_t> off;  // the host copies, kept until the call ends
+  std::vector<int> slot;
+  uint32_t* d_off = nullptr;
+  int* d_slot = nullptr;
+};
+
+// Validates the indices and uploads the slots.
+int upload_corr_slots(const WarpCore* w, const uint64_t* corr_first, const uint64_t* corr_second, size_t n_corr,
+                      CorrSlots* cs) {
+  const size_t n_dst = w->dst->n, n_src = w->n;
+  std::vector<uint32_t>& off = cs->off;
+  off.assign(n_src + 1, 0u);
   for (size_t c = 0; c < n_corr; c++) {
     CB_CHECK(corr_first[c] < n_dst && corr_second[c] < n_src, CB_ERR_INVALID, "correspondence index out of range");
     off[corr_second[c] + 1]++;
   }
   for (size_t i = 0; i < n_src; i++) off[i + 1] += off[i];
-  slot.assign(std::max<size_t>(n_corr, 1), 0);  // dst indices < 2^31 - 1 (checked at creation)
+  cs->slot.assign(std::max<size_t>(n_corr, 1), 0);  // dst indices < 2^31 - 1 (checked at creation)
   std::vector<uint32_t> fill(off.begin(), off.end() - 1);
-  for (size_t c = 0; c < n_corr; c++) slot[fill[corr_second[c]]++] = (int)corr_first[c];
+  for (size_t c = 0; c < n_corr; c++) cs->slot[fill[corr_second[c]]++] = (int)corr_first[c];
+  CB_TRY(cs->scope.alloc(&cs->d_off, off.size()));
+  CB_TRY(cs->scope.alloc(&cs->d_slot, cs->slot.size()));
+  cudaStream_t s = w->ctx->stream;
+  CB_CUDA(cudaMemcpyAsync(cs->d_off, off.data(), off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  CB_CUDA(cudaMemcpyAsync(cs->d_slot, cs->slot.data(), cs->slot.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  return CB_OK;
+}
+
+// T <- T_host ([n][12], identities when NULL; T one transform per source point) and warped_i = T_i s_i.
+int warp_points(WarpCore* w, float* T, const float* T_host) {
+  cb_context* ctx = w->ctx;
+  if (w->n == 0) return CB_OK;
+  if (T_host)
+    CB_CUDA(cudaMemcpyAsync(T, T_host, 12 * (size_t)w->n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  warp_points_kernel<<<grid_for(ctx, w->n), kBlock, 0, ctx->stream>>>(w->n, w->src->d_raw, T, T_host == nullptr,
+                                                                      w->d_warped);
+  ctx->launches += 1;
+  CB_CUDA(cudaGetLastError());
+  return CB_OK;
+}
+
+// What Gauss-Newton calls report: the flag of the last call, the steps and CG iterations summed over the calls, and
+// the last step's CG iterations and error.
+struct GnCounts {
+  int converged = 0;
+  uint64_t steps = 0, cg_total = 0, cg_last = 0;
+  float cg_err = 0.f;
+};
+
+// Device times of the Gauss-Newton steps, summed: the assembly launches and the CG launch.
+struct StepTimer {
+  ScopedEvents ev;  // ev.e0: assembly start, ev.e1: CG start
+  ScopedEvents end;  // end.e1: CG end
+  double assemble = 0, cg = 0;
+  int create() {
+    CB_TRY(ev.create());
+    return end.create();
+  }
+};
+
+// One estimator call (estimateDenseWarpFieldCombinedMetric, :368-715, or estimateSparseWarpFieldCombinedMetric,
+// :1388-1846) on the current warped points and correspondences: the unknowns start at zero (:460-461, :1531-1532) and
+// without a data term or a correspondence it returns before any step (:398-408, :1427-1433; no_corr: the caller
+// knows the list is empty, else the first step's assembly counts it). Per step, assemble() launches the caller's
+// assembly of b, inv and arc_c, then the cooperative cg_kernel(ca) runs the CG over the m blocks (ca.v is filled
+// here) and adds the solution to xs. timer, when given, takes the times of both.
+template <class CgArgs, class Assemble>
+int gauss_newton(WarpCore* w, const cb_warp_params* p, bool no_corr, Assemble&& assemble, const void* cg_kernel,
+                 CgArgs& ca, GnCounts* gn, StepTimer* timer) {
+  cb_context* ctx = w->ctx;
+  const size_t m = w->m;
+  gn->converged = 0;
+  CB_CUDA(cudaMemsetAsync(w->d_xs, 0, 6 * std::max<size_t>(m, 1) * sizeof(float), ctx->stream));
+  if ((!(p->w_pt > 0.f) && !(p->w_pl > 0.f)) || no_corr || w->n == 0 || m == 0) return CB_OK;
+  ca.v.n = w->m;
+  ca.v.b = w->d_b;
+  ca.v.inv = w->d_inv;
+  ca.v.x = w->d_vec;
+  ca.v.r = w->d_vec + 6 * m;
+  ca.v.p = w->d_vec + 12 * m;
+  ca.v.z = w->d_vec + 18 * m;
+  ca.v.q = w->d_vec + 24 * m;
+  ca.v.xs = w->d_xs;
+  ca.v.part = w->d_part;
+  ca.v.max_iter = (unsigned int)std::min<uint64_t>(p->max_cg_iter, 0xffffffffu);
+  ca.v.tol = (double)p->cg_tol;
+  ca.v.stats = w->d_stats;
+  const WarpStats* hs = w->h_stats;
+  const float tol2 = p->gn_tol * p->gn_tol;
+  for (uint64_t step = 0; step < p->max_gn_iter; step++) {
+    CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
+    if (timer) CB_CUDA(cudaEventRecord(timer->ev.e0, ctx->stream));
+    CB_TRY(assemble());
+    if (timer) CB_CUDA(cudaEventRecord(timer->ev.e1, ctx->stream));
+    void* args[] = {&ca};
+    CB_CUDA(cudaLaunchCooperativeKernel(cg_kernel, dim3(w->cg_grid), dim3(kBlock), args, 0, ctx->stream));
+    if (timer) CB_CUDA(cudaEventRecord(timer->end.e1, ctx->stream));
+    ctx->launches += 1;
+    CB_CUDA(cudaMemcpyAsync(w->h_stats, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (timer) {
+      float ta = 0.f, tc = 0.f;
+      CB_CUDA(cudaEventElapsedTime(&ta, timer->ev.e0, timer->ev.e1));
+      CB_CUDA(cudaEventElapsedTime(&tc, timer->ev.e1, timer->end.e1));
+      timer->assemble += ta;
+      timer->cg += tc;
+    }
+    // no correspondence: b = 0, so the step left xs at zero; the reference returns before any step
+    if (step == 0 && hs->num_corr == 0) return CB_OK;
+    ++gn->steps;
+    gn->cg_total += hs->cg_iters;
+    gn->cg_last = hs->cg_iters;
+    gn->cg_err = hs->cg_err;
+    float mx;
+    std::memcpy(&mx, &hs->max_delta_bits, sizeof(float));
+    if (mx < tol2) {
+      gn->converged = 1;
+      break;
+    }
+  }
+  return CB_OK;
+}
+
+// The estimator's output over the m blocks (:701-712, :1832-1843; compose: preApply with projection, else the plain
+// transforms) and the max of |dR_j - I|_F^2 + |dt_j|^2. warp_next (one block per point only): also the warped points
+// for the next search and, into *num_corr, the correspondences of the last search.
+int apply_update(WarpCore* w, bool compose, bool warp_next, float* last_delta_sq, uint32_t* num_corr) {
+  cb_context* ctx = w->ctx;
+  CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
+  if (w->m) {
+    warp_compose_kernel<<<grid_for(ctx, w->m), kBlock, 0, ctx->stream>>>(
+        w->m, w->src->d_raw, w->d_xs, w->d_T, compose, warp_next ? w->d_warped : nullptr,
+        warp_next ? w->d_nn : nullptr, w->d_stats);
+    ctx->launches += 1;
+    CB_CUDA(cudaGetLastError());
+  }
+  CB_CUDA(cudaMemcpyAsync(w->h_stats, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
+  CB_CUDA(cudaStreamSynchronize(ctx->stream));
+  std::memcpy(last_delta_sq, &w->h_stats->last_delta_bits, sizeof(float));
+  if (num_corr) *num_corr = w->h_stats->num_corr;
   return CB_OK;
 }
 

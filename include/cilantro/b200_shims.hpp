@@ -735,17 +735,183 @@ inline void transformPoints(const TransformSet<RigidTransform3f>& tforms, const 
   for (size_t i = 0; i < points.cols(); i++) result.setCol(i, tforms[i] * points.col(i));
 }
 
-// ---- SimpleCombinedMetricDenseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:99-144, 284-285) ----------
-// CombinedMetricDenseWarpFieldICP<RigidTransform<float,3>> (icp_warp_field_combined_metric_dense.hpp) with the Simple
-// instance's evaluators (unity data-term weights, RBFKernelWeightEvaluator<float, float, true> regularisation weights)
-// on cb_warp_icp_* (DESIGN §4.13). The correspondence engine takes the default settings only; another search
-// direction, reciprocity, one-to-one or fraction makes estimate() throw (CB_ERR_UNSUPPORTED).
-class SimpleCombinedMetricDenseRigidWarpFieldICP3f {
+namespace b200 {
+// The surface both warp-field ICP drop-ins share: IterativeClosestPointBase (registration/icp_base.hpp:40-106) and
+// CombinedMetric*WarpFieldICP over their cb_warp_params, the correspondence engine and evaluators, the dst/src cloud
+// pair and the last estimate's correspondences. Setters return Derived, so calls chain as in the reference. Result is
+// the C result record (iterations, last_delta, cg_iterations); the transforms are one per unknown block.
+template <class Derived, class Result>
+class WarpFieldICP {
 public:
   using Transform = TransformSet<RigidTransform3f>;
   using PointToPointCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
   using PointToPlaneCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
   using RegularizationWeightEvaluator = RBFKernelWeightEvaluator<float, float, true>;
+
+  WarpFieldICP(const WarpFieldICP&) = delete;
+  WarpFieldICP& operator=(const WarpFieldICP&) = delete;
+
+  CorrespondenceSearchEngineB200& correspondenceSearchEngine() { return engine_; }
+  PointToPointCorrespondenceWeightEvaluator& pointToPointCorrespondenceWeightEvaluator() { return pt_eval_; }
+  PointToPlaneCorrespondenceWeightEvaluator& pointToPlaneCorrespondenceWeightEvaluator() { return pl_eval_; }
+  RegularizationWeightEvaluator& regularizationWeightEvaluator() { return reg_eval_; }
+
+  // IterativeClosestPointBase surface
+  size_t getMaxNumberOfIterations() const { return (size_t)p_.max_iter; }
+  Derived& setMaxNumberOfIterations(size_t n) {
+    p_.max_iter = (int32_t)n;
+    return self();
+  }
+  float getConvergenceTolerance() const { return p_.tol; }
+  Derived& setConvergenceTolerance(float tol) {
+    p_.tol = tol;
+    return self();
+  }
+  const Transform& getInitialTransform() const { return transform_init_; }
+  Transform& initialTransform() { return transform_init_; }
+  Derived& setInitialTransform(const Transform& T) {
+    transform_init_ = T;
+    return self();
+  }
+  size_t getNumberOfPerformedIterations() const { return (size_t)res_.iterations; }
+  float getLastUpdateNorm() const { return res_.last_delta; }
+  bool hasConverged() const { return res_.last_delta < p_.tol; }  // icp_base.hpp:106
+  const Transform& getTransform() const { return transform_; }
+  Derived& estimate(size_t max_iter, float conv_tol) {
+    p_.max_iter = (int32_t)max_iter;
+    p_.tol = conv_tol;
+    return self().estimate();
+  }
+
+  // CombinedMetric*WarpFieldICP surface
+  float getPointToPointMetricWeight() const { return p_.w_pt; }
+  Derived& setPointToPointMetricWeight(float w) {
+    p_.w_pt = w;
+    return self();
+  }
+  float getPointToPlaneMetricWeight() const { return p_.w_pl; }
+  Derived& setPointToPlaneMetricWeight(float w) {
+    p_.w_pl = w;
+    return self();
+  }
+  float getStiffnessRegularizationWeight() const { return p_.stiffness; }
+  Derived& setStiffnessRegularizationWeight(float w) {
+    p_.stiffness = w;
+    return self();
+  }
+  size_t getMaxNumberOfGaussNewtonIterations() const { return (size_t)p_.max_gn_iter; }
+  Derived& setMaxNumberOfGaussNewtonIterations(size_t n) {
+    p_.max_gn_iter = n;
+    return self();
+  }
+  float getGaussNewtonConvergenceTolerance() const { return p_.gn_tol; }
+  Derived& setGaussNewtonConvergenceTolerance(float tol) {
+    p_.gn_tol = tol;
+    return self();
+  }
+  size_t getMaxNumberOfConjugateGradientIterations() const { return (size_t)p_.max_cg_iter; }
+  Derived& setMaxNumberOfConjugateGradientIterations(size_t n) {
+    p_.max_cg_iter = n;
+    return self();
+  }
+  float getConjugateGradientConvergenceTolerance() const { return p_.cg_tol; }
+  Derived& setConjugateGradientConvergenceTolerance(float tol) {
+    p_.cg_tol = tol;
+    return self();
+  }
+  float getHuberLossBoundary() const { return p_.huber; }
+  Derived& setHuberLossBoundary(float huber_boundary) {
+    p_.huber = huber_boundary;
+    return self();
+  }
+
+  uint64_t getNumberOfConjugateGradientIterations() const { return res_.cg_iterations; }  // over the last estimate()
+
+protected:
+  // p: the derived class's cb_warp_params (filled by it); n_blocks: the transforms' count
+  WarpFieldICP(cb_warp_params& p, const ConstVectorSetMatrixMap3f& dst_p, const ConstVectorSetMatrixMap3f& dst_n,
+               const ConstVectorSetMatrixMap3f& src_p, size_t n_blocks)
+      : n_src_(src_p.cols()), p_(p) {
+    const float* dn = (dst_n.cols() == dst_p.cols() && dst_p.cols() > 0) ? dst_n.data() : nullptr;
+    check(cb_cloud_create_pair(Context::get(), dst_p.data(), dn, dst_p.cols(), 0, src_p.data(), nullptr,
+                               src_p.cols(), 0, &dst_.h, &src_.h),
+          "cb_cloud_create_pair");
+    std::memset(&res_, 0, sizeof(res_));
+    res_.last_delta = std::numeric_limits<float>::infinity();
+    transform_init_.assign(n_blocks, RigidTransform3f());
+    transform_.assign(n_blocks, RigidTransform3f());
+  }
+  ~WarpFieldICP() = default;
+
+  Derived& self() { return static_cast<Derived&>(*this); }
+
+  // neighbourhood lists -> the (offsets, index, value) CSR of the C entries
+  template <typename IndexT>
+  static void csr(const std::vector<NeighborSet<float, IndexT>>& lists, std::vector<uint64_t>& off,
+                  std::vector<int64_t>& idx, std::vector<float>& val) {
+    off.assign(lists.size() + 1, 0);
+    for (size_t j = 0; j < lists.size(); j++) {
+      for (const auto& nb : lists[j]) {
+        idx.push_back(static_cast<int64_t>(nb.index));
+        val.push_back(nb.value);
+      }
+      off[j + 1] = idx.size();
+    }
+  }
+
+  // the engine's and the regularisation evaluator's settings into p_
+  void fill() {
+    cb_icp_params e;
+    cb_icp_default_params(&e);
+    engine_.fill(e);
+    p_.max_d2 = e.max_d2;
+    p_.search_dir = e.search_dir;
+    p_.inlier_fraction = e.inlier_fraction;
+    p_.require_reciprocal = e.require_reciprocal;
+    p_.one_to_one = e.one_to_one;
+    p_.reg_coeff = reg_eval_.b200_coeff();
+  }
+
+  // correspondenceSearchEngine().getCorrespondences() after estimate(): the last iteration's list, read through the
+  // object's cb_*_correspondences entry
+  template <class Handle>
+  const CorrespondenceSet<float, size_t>& correspondences(int (*entry)(Handle*, uint64_t*, uint64_t*, float*, size_t*),
+                                                          Handle* icp, const char* what) {
+    if (!corr_fresh_) {
+      std::vector<uint64_t> a(n_src_), b(n_src_);
+      std::vector<float> v(n_src_);
+      size_t cnt = 0;
+      check(entry(icp, a.data(), b.data(), v.data(), &cnt), what);
+      corr_.resize(cnt);
+      for (size_t i = 0; i < cnt; i++) corr_[i] = {(size_t)a[i], (size_t)b[i], v[i]};
+      corr_fresh_ = true;
+    }
+    return corr_;
+  }
+
+  size_t n_src_;
+  CloudHandle dst_, src_;
+  cb_warp_params& p_;
+  Result res_;
+  Transform transform_init_, transform_;
+  CorrespondenceSearchEngineB200 engine_;
+  PointToPointCorrespondenceWeightEvaluator pt_eval_;
+  PointToPlaneCorrespondenceWeightEvaluator pl_eval_;
+  RegularizationWeightEvaluator reg_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
+  CorrespondenceSet<float, size_t> corr_;
+  bool corr_fresh_ = false;
+};
+}  // namespace b200
+
+// ---- SimpleCombinedMetricDenseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:99-144, 284-285) ----------
+// CombinedMetricDenseWarpFieldICP<RigidTransform<float,3>> (icp_warp_field_combined_metric_dense.hpp) with the Simple
+// instance's evaluators (unity data-term weights, RBFKernelWeightEvaluator<float, float, true> regularisation weights)
+// on cb_warp_icp_* (DESIGN §4.13). The correspondence engine takes the default settings only; another search
+// direction, reciprocity, one-to-one or fraction makes estimate() throw (CB_ERR_UNSUPPORTED).
+class SimpleCombinedMetricDenseRigidWarpFieldICP3f
+    : public b200::WarpFieldICP<SimpleCombinedMetricDenseRigidWarpFieldICP3f, cb_warp_result> {
+public:
+  using WarpFieldICP::estimate;
 
   // regularization_neighborhoods: one list per neighbourhood, N[0] the centre (what KDTree3f<>::search returns)
   template <typename IndexT>
@@ -753,103 +919,18 @@ public:
                                                const ConstVectorSetMatrixMap3f& dst_n,
                                                const ConstVectorSetMatrixMap3f& src_p,
                                                const std::vector<NeighborSet<float, IndexT>>& regularization_neighborhoods)
-      : n_src_(src_p.cols()) {
-    const float* dn = (dst_n.cols() == dst_p.cols() && dst_p.cols() > 0) ? dst_n.data() : nullptr;
-    b200::check(cb_cloud_create_pair(b200::Context::get(), dst_p.data(), dn, dst_p.cols(), 0, src_p.data(), nullptr,
-                                     src_p.cols(), 0, &dst_.h, &src_.h),
-                "cb_cloud_create_pair");
-    std::vector<uint64_t> off(regularization_neighborhoods.size() + 1, 0);
+      : WarpFieldICP(prm_, dst_p, dst_n, src_p, src_p.cols()) {
+    std::vector<uint64_t> off;
     std::vector<int64_t> idx;
     std::vector<float> val;
-    for (size_t j = 0; j < regularization_neighborhoods.size(); j++) {
-      for (const auto& nb : regularization_neighborhoods[j]) {
-        idx.push_back(static_cast<int64_t>(nb.index));
-        val.push_back(nb.value);
-      }
-      off[j + 1] = idx.size();
-    }
+    csr(regularization_neighborhoods, off, idx, val);
     b200::check(cb_warp_icp_create(b200::Context::get(), dst_.h, src_.h, off.data(), idx.data(), val.data(),
                                    regularization_neighborhoods.size(), &icp_),
                 "cb_warp_icp_create");
     cb_warp_default_params(&prm_);
-    std::memset(&res_, 0, sizeof(res_));
-    res_.last_delta = std::numeric_limits<float>::infinity();
-    transform_init_.assign(n_src_, RigidTransform3f());
-    transform_.assign(n_src_, RigidTransform3f());
   }
   ~SimpleCombinedMetricDenseRigidWarpFieldICP3f() {
     if (icp_) cb_warp_icp_destroy(icp_);
-  }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f(const SimpleCombinedMetricDenseRigidWarpFieldICP3f&) = delete;
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& operator=(const SimpleCombinedMetricDenseRigidWarpFieldICP3f&) = delete;
-
-  CorrespondenceSearchEngineB200& correspondenceSearchEngine() { return engine_; }
-  PointToPointCorrespondenceWeightEvaluator& pointToPointCorrespondenceWeightEvaluator() { return pt_eval_; }
-  PointToPlaneCorrespondenceWeightEvaluator& pointToPlaneCorrespondenceWeightEvaluator() { return pl_eval_; }
-  RegularizationWeightEvaluator& regularizationWeightEvaluator() { return reg_eval_; }
-
-  // IterativeClosestPointBase surface (registration/icp_base.hpp:40-106)
-  size_t getMaxNumberOfIterations() const { return (size_t)prm_.max_iter; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setMaxNumberOfIterations(size_t n) {
-    prm_.max_iter = (int32_t)n;
-    return *this;
-  }
-  float getConvergenceTolerance() const { return prm_.tol; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setConvergenceTolerance(float tol) {
-    prm_.tol = tol;
-    return *this;
-  }
-  const Transform& getInitialTransform() const { return transform_init_; }
-  Transform& initialTransform() { return transform_init_; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setInitialTransform(const Transform& T) {
-    transform_init_ = T;
-    return *this;
-  }
-  size_t getNumberOfPerformedIterations() const { return (size_t)res_.iterations; }
-  float getLastUpdateNorm() const { return res_.last_delta; }
-  bool hasConverged() const { return res_.last_delta < prm_.tol; }  // icp_base.hpp:106
-  const Transform& getTransform() const { return transform_; }
-
-  // CombinedMetricDenseWarpFieldICP surface
-  float getPointToPointMetricWeight() const { return prm_.w_pt; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setPointToPointMetricWeight(float w) {
-    prm_.w_pt = w;
-    return *this;
-  }
-  float getPointToPlaneMetricWeight() const { return prm_.w_pl; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setPointToPlaneMetricWeight(float w) {
-    prm_.w_pl = w;
-    return *this;
-  }
-  float getStiffnessRegularizationWeight() const { return prm_.stiffness; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setStiffnessRegularizationWeight(float w) {
-    prm_.stiffness = w;
-    return *this;
-  }
-  size_t getMaxNumberOfGaussNewtonIterations() const { return (size_t)prm_.max_gn_iter; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setMaxNumberOfGaussNewtonIterations(size_t n) {
-    prm_.max_gn_iter = n;
-    return *this;
-  }
-  float getGaussNewtonConvergenceTolerance() const { return prm_.gn_tol; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setGaussNewtonConvergenceTolerance(float tol) {
-    prm_.gn_tol = tol;
-    return *this;
-  }
-  size_t getMaxNumberOfConjugateGradientIterations() const { return (size_t)prm_.max_cg_iter; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setMaxNumberOfConjugateGradientIterations(size_t n) {
-    prm_.max_cg_iter = n;
-    return *this;
-  }
-  float getConjugateGradientConvergenceTolerance() const { return prm_.cg_tol; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setConjugateGradientConvergenceTolerance(float tol) {
-    prm_.cg_tol = tol;
-    return *this;
-  }
-  float getHuberLossBoundary() const { return prm_.huber; }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& setHuberLossBoundary(float huber_boundary) {
-    prm_.huber = huber_boundary;
-    return *this;
   }
 
   SimpleCombinedMetricDenseRigidWarpFieldICP3f& estimate() {
@@ -863,11 +944,6 @@ public:
     corr_fresh_ = false;
     return *this;
   }
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& estimate(size_t max_iter, float conv_tol) {
-    prm_.max_iter = (int32_t)max_iter;
-    prm_.tol = conv_tol;
-    return estimate();
-  }
 
   // getResiduals() -> computeResiduals() (icp_warp_field_combined_metric_dense.hpp:216-236): 1 x N_src
   std::vector<float> getResiduals() {
@@ -878,47 +954,15 @@ public:
     return r;
   }
 
-  // correspondenceSearchEngine().getCorrespondences() after estimate(): the last iteration's list
   const CorrespondenceSet<float, size_t>& getCorrespondences() {
-    if (!corr_fresh_) {
-      std::vector<uint64_t> a(n_src_), b(n_src_);
-      std::vector<float> v(n_src_);
-      size_t cnt = 0;
-      b200::check(cb_warp_icp_correspondences(icp_, a.data(), b.data(), v.data(), &cnt), "cb_warp_icp_correspondences");
-      corr_.resize(cnt);
-      for (size_t i = 0; i < cnt; i++) corr_[i] = {(size_t)a[i], (size_t)b[i], v[i]};
-      corr_fresh_ = true;
-    }
-    return corr_;
+    return correspondences(cb_warp_icp_correspondences, icp_, "cb_warp_icp_correspondences");
   }
 
-  uint64_t getNumberOfConjugateGradientIterations() const { return res_.cg_iterations; }  // over the last estimate()
   double getLastEstimateDeviceMilliseconds() const { return res_.gpu_ms_search + res_.gpu_ms_solve; }
 
 private:
-  void fill() {
-    cb_icp_params e;
-    cb_icp_default_params(&e);
-    engine_.fill(e);
-    prm_.max_d2 = e.max_d2;
-    prm_.search_dir = e.search_dir;
-    prm_.inlier_fraction = e.inlier_fraction;
-    prm_.require_reciprocal = e.require_reciprocal;
-    prm_.one_to_one = e.one_to_one;
-    prm_.reg_coeff = reg_eval_.b200_coeff();
-  }
-  size_t n_src_;
-  b200::CloudHandle dst_, src_;
   cb_warp_icp* icp_ = nullptr;
   cb_warp_params prm_;
-  cb_warp_result res_;
-  Transform transform_init_, transform_;
-  CorrespondenceSearchEngineB200 engine_;
-  PointToPointCorrespondenceWeightEvaluator pt_eval_;
-  PointToPlaneCorrespondenceWeightEvaluator pl_eval_;
-  RegularizationWeightEvaluator reg_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
-  CorrespondenceSet<float, size_t> corr_;
-  bool corr_fresh_ = false;
 };
 
 // ---- SimpleCombinedMetricSparseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:146-199, 313-314) ---------
@@ -926,13 +970,11 @@ private:
 // instance's evaluators (unity data-term weights, RBFKernelWeightEvaluator<float, float, true> control and
 // regularisation weights) on cb_sparse_warp_icp_* (DESIGN §4.14). getTransform() holds one transform per control
 // node, getDenseWarpField() one per source point. The correspondence engine takes the default settings only.
-class SimpleCombinedMetricSparseRigidWarpFieldICP3f {
+class SimpleCombinedMetricSparseRigidWarpFieldICP3f
+    : public b200::WarpFieldICP<SimpleCombinedMetricSparseRigidWarpFieldICP3f, cb_sparse_warp_result> {
 public:
-  using Transform = TransformSet<RigidTransform3f>;
-  using PointToPointCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
-  using PointToPlaneCorrespondenceWeightEvaluator = UnityWeightEvaluator<float, float>;
   using ControlWeightEvaluator = RBFKernelWeightEvaluator<float, float, true>;
-  using RegularizationWeightEvaluator = RBFKernelWeightEvaluator<float, float, true>;
+  using WarpFieldICP::estimate;
 
   // src_to_control_nn: one list of (node, squared distance) per source point; regularization_nn: one list per node
   // neighbourhood, N[0] the centre (what KDTree<float, 3>::search over the nodes returns)
@@ -943,11 +985,7 @@ public:
                                                 const std::vector<NeighborSet<float, IndexT>>& src_to_control_nn,
                                                 size_t num_control_nodes,
                                                 const std::vector<NeighborSet<float, RegIndexT>>& regularization_nn)
-      : n_src_(src_p.cols()), n_ctrl_(num_control_nodes) {
-    const float* dn = (dst_n.cols() == dst_p.cols() && dst_p.cols() > 0) ? dst_n.data() : nullptr;
-    b200::check(cb_cloud_create_pair(b200::Context::get(), dst_p.data(), dn, dst_p.cols(), 0, src_p.data(), nullptr,
-                                     src_p.cols(), 0, &dst_.h, &src_.h),
-                "cb_cloud_create_pair");
+      : WarpFieldICP(prm_.base, dst_p, dst_n, src_p, num_control_nodes), n_ctrl_(num_control_nodes) {
     std::vector<uint64_t> coff, roff;
     std::vector<int64_t> cidx, ridx;
     std::vector<float> cval, rval;
@@ -958,88 +996,14 @@ public:
                                           regularization_nn.size(), &icp_),
                 "cb_sparse_warp_icp_create");
     cb_sparse_warp_default_params(&prm_);
-    std::memset(&res_, 0, sizeof(res_));
-    res_.last_delta = std::numeric_limits<float>::infinity();
-    transform_init_.assign(n_ctrl_, RigidTransform3f());
-    transform_.assign(n_ctrl_, RigidTransform3f());
     transform_dense_.assign(n_src_, RigidTransform3f());
   }
   ~SimpleCombinedMetricSparseRigidWarpFieldICP3f() {
     if (icp_) cb_sparse_warp_icp_destroy(icp_);
   }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f(const SimpleCombinedMetricSparseRigidWarpFieldICP3f&) = delete;
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& operator=(const SimpleCombinedMetricSparseRigidWarpFieldICP3f&) = delete;
 
-  CorrespondenceSearchEngineB200& correspondenceSearchEngine() { return engine_; }
-  PointToPointCorrespondenceWeightEvaluator& pointToPointCorrespondenceWeightEvaluator() { return pt_eval_; }
-  PointToPlaneCorrespondenceWeightEvaluator& pointToPlaneCorrespondenceWeightEvaluator() { return pl_eval_; }
   ControlWeightEvaluator& controlWeightEvaluator() { return ctrl_eval_; }
-  RegularizationWeightEvaluator& regularizationWeightEvaluator() { return reg_eval_; }
-
-  // IterativeClosestPointBase surface (registration/icp_base.hpp:40-106)
-  size_t getMaxNumberOfIterations() const { return (size_t)prm_.base.max_iter; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setMaxNumberOfIterations(size_t n) {
-    prm_.base.max_iter = (int32_t)n;
-    return *this;
-  }
-  float getConvergenceTolerance() const { return prm_.base.tol; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setConvergenceTolerance(float tol) {
-    prm_.base.tol = tol;
-    return *this;
-  }
-  const Transform& getInitialTransform() const { return transform_init_; }
-  Transform& initialTransform() { return transform_init_; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setInitialTransform(const Transform& T) {
-    transform_init_ = T;
-    return *this;
-  }
-  size_t getNumberOfPerformedIterations() const { return (size_t)res_.iterations; }
-  float getLastUpdateNorm() const { return res_.last_delta; }
-  bool hasConverged() const { return res_.last_delta < prm_.base.tol; }  // icp_base.hpp:106
-  const Transform& getTransform() const { return transform_; }
   const Transform& getDenseWarpField() const { return transform_dense_; }
-
-  // CombinedMetricSparseWarpFieldICP surface
-  float getPointToPointMetricWeight() const { return prm_.base.w_pt; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setPointToPointMetricWeight(float w) {
-    prm_.base.w_pt = w;
-    return *this;
-  }
-  float getPointToPlaneMetricWeight() const { return prm_.base.w_pl; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setPointToPlaneMetricWeight(float w) {
-    prm_.base.w_pl = w;
-    return *this;
-  }
-  float getStiffnessRegularizationWeight() const { return prm_.base.stiffness; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setStiffnessRegularizationWeight(float w) {
-    prm_.base.stiffness = w;
-    return *this;
-  }
-  size_t getMaxNumberOfGaussNewtonIterations() const { return (size_t)prm_.base.max_gn_iter; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setMaxNumberOfGaussNewtonIterations(size_t n) {
-    prm_.base.max_gn_iter = n;
-    return *this;
-  }
-  float getGaussNewtonConvergenceTolerance() const { return prm_.base.gn_tol; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setGaussNewtonConvergenceTolerance(float tol) {
-    prm_.base.gn_tol = tol;
-    return *this;
-  }
-  size_t getMaxNumberOfConjugateGradientIterations() const { return (size_t)prm_.base.max_cg_iter; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setMaxNumberOfConjugateGradientIterations(size_t n) {
-    prm_.base.max_cg_iter = n;
-    return *this;
-  }
-  float getConjugateGradientConvergenceTolerance() const { return prm_.base.cg_tol; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setConjugateGradientConvergenceTolerance(float tol) {
-    prm_.base.cg_tol = tol;
-    return *this;
-  }
-  float getHuberLossBoundary() const { return prm_.base.huber; }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& setHuberLossBoundary(float huber_boundary) {
-    prm_.base.huber = huber_boundary;
-    return *this;
-  }
 
   SimpleCombinedMetricSparseRigidWarpFieldICP3f& estimate() {
     if (transform_init_.size() != n_ctrl_) throw std::runtime_error("initial transform: one transform per control node expected");
@@ -1053,11 +1017,6 @@ public:
     corr_fresh_ = false;
     return *this;
   }
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& estimate(size_t max_iter, float conv_tol) {
-    prm_.base.max_iter = (int32_t)max_iter;
-    prm_.base.tol = conv_tol;
-    return estimate();
-  }
 
   // getResiduals() -> computeResiduals() (icp_warp_field_combined_metric_sparse.hpp:243-263) on the dense field
   std::vector<float> getResiduals() {
@@ -1068,64 +1027,24 @@ public:
     return r;
   }
 
-  // correspondenceSearchEngine().getCorrespondences() after estimate(): the last iteration's list
   const CorrespondenceSet<float, size_t>& getCorrespondences() {
-    if (!corr_fresh_) {
-      std::vector<uint64_t> a(n_src_), b(n_src_);
-      std::vector<float> v(n_src_);
-      size_t cnt = 0;
-      b200::check(cb_sparse_warp_icp_correspondences(icp_, a.data(), b.data(), v.data(), &cnt),
-                  "cb_sparse_warp_icp_correspondences");
-      corr_.resize(cnt);
-      for (size_t i = 0; i < cnt; i++) corr_[i] = {(size_t)a[i], (size_t)b[i], v[i]};
-      corr_fresh_ = true;
-    }
-    return corr_;
+    return correspondences(cb_sparse_warp_icp_correspondences, icp_, "cb_sparse_warp_icp_correspondences");
   }
 
-  uint64_t getNumberOfConjugateGradientIterations() const { return res_.cg_iterations; }  // over the last estimate()
   double getLastEstimateDeviceMilliseconds() const {
     return res_.gpu_ms_search + res_.gpu_ms_resample + res_.gpu_ms_assemble + res_.gpu_ms_cg;
   }
 
 private:
-  template <typename IndexT>
-  static void csr(const std::vector<NeighborSet<float, IndexT>>& lists, std::vector<uint64_t>& off,
-                  std::vector<int64_t>& idx, std::vector<float>& val) {
-    off.assign(lists.size() + 1, 0);
-    for (size_t j = 0; j < lists.size(); j++) {
-      for (const auto& nb : lists[j]) {
-        idx.push_back(static_cast<int64_t>(nb.index));
-        val.push_back(nb.value);
-      }
-      off[j + 1] = idx.size();
-    }
-  }
   void fill() {
-    cb_icp_params e;
-    cb_icp_default_params(&e);
-    engine_.fill(e);
-    prm_.base.max_d2 = e.max_d2;
-    prm_.base.search_dir = e.search_dir;
-    prm_.base.inlier_fraction = e.inlier_fraction;
-    prm_.base.require_reciprocal = e.require_reciprocal;
-    prm_.base.one_to_one = e.one_to_one;
-    prm_.base.reg_coeff = reg_eval_.b200_coeff();
+    WarpFieldICP::fill();
     prm_.ctrl_coeff = ctrl_eval_.b200_coeff();
   }
-  size_t n_src_, n_ctrl_;
-  b200::CloudHandle dst_, src_;
+  size_t n_ctrl_;
   cb_sparse_warp_icp* icp_ = nullptr;
   cb_sparse_warp_params prm_;
-  cb_sparse_warp_result res_;
-  Transform transform_init_, transform_, transform_dense_;
-  CorrespondenceSearchEngineB200 engine_;
-  PointToPointCorrespondenceWeightEvaluator pt_eval_;
-  PointToPlaneCorrespondenceWeightEvaluator pl_eval_;
-  ControlWeightEvaluator ctrl_eval_;        // sigma 1 (common_pair_evaluators.hpp:51)
-  RegularizationWeightEvaluator reg_eval_;  // sigma 1
-  CorrespondenceSet<float, size_t> corr_;
-  bool corr_fresh_ = false;
+  Transform transform_dense_;
+  ControlWeightEvaluator ctrl_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
 };
 
 // ---- KMeans3f<> -------------------------------------------------------------------------------------
