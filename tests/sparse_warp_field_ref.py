@@ -124,7 +124,8 @@ def system(dst, nrm, src, first, second, ctrl, m, reg, x, w_pt, w_pl, stiffness,
 
 
 def resample(T, ctrl, sigma):
-    """resampleTransforms in fp64: the weighted blend over each list in its order, then the nearest rotation (SVD)."""
+    """resampleTransforms in fp64: the weighted blend over each list in its order, then the nearest rotation (SVD,
+    a reflection repaired on the largest singular value)."""
     off, idx, d2 = (np.asarray(a) for a in ctrl)
     T = np.asarray(T, np.float64).reshape(-1, 3, 4)
     n = off.shape[0] - 1
@@ -137,8 +138,10 @@ def resample(T, ctrl, sigma):
     ok = W != 0
     L = L[ok] / W[ok, None, None]
     U, _, Vt = np.linalg.svd(L[:, :, :3])
+    # LinearTransform::rotation() (space_transformations.hpp:43-51) repairs a reflection on column 0 of U: the largest
+    # singular value's, as numpy's and Eigen's SVDs sort them descending
     D = np.ones((L.shape[0], 3))
-    D[:, 2] = np.sign(np.linalg.det(U @ Vt))
+    D[:, 0] = np.sign(np.linalg.det(U @ Vt))
     out[ok, :, :3] = (U * D[:, None, :]) @ Vt
     out[ok, :, 3] = L[:, :, 3]
     return out

@@ -96,12 +96,106 @@ def test_resample_statement_blends_and_projects():
     np.testing.assert_allclose(out[1, :, :3], U @ Vt, atol=1e-12)
 
 
+def test_resample_repairs_a_reflection_blend_on_the_largest_singular_value(swf):
+    """A blend of rotations far apart can have det < 0: weights (0, .45, .33, .22) on I, Rx(pi), Ry(pi), Rz(pi) give
+    diag(-.10, -.34, -.56). LinearTransform::rotation() (space_transformations.hpp:43-51) negates column 0 of U, the
+    largest singular value's (Eigen's JacobiSVD sorts them descending): the result is diag(-1, -1, 1) = Rz(pi), where
+    the Kabsch rule (column 2, the smallest) would give Rx(pi). Also conjugated by a random rotation Q, which keeps the
+    singular values and moves the answer to Q Rz(pi) Q^T."""
+    from scipy.spatial.transform import Rotation
+
+    rots = [np.eye(3), np.diag([1.0, -1.0, -1.0]), np.diag([-1.0, 1.0, -1.0]), np.diag([-1.0, -1.0, 1.0])]
+    w = np.array([0.45, 0.33, 0.22])
+    sigma = 1.0
+    # d2 = +inf is a zero weight; the others reproduce w up to a common factor
+    d2 = np.concatenate([[np.inf], -2.0 * sigma ** 2 * np.log(w)]).astype(np.float32)
+    t = np.array([[0.1, 0.2, 0.3], [-1.0, 0.5, 2.0], [0.3, -0.7, 0.0], [2.0, 1.0, -1.0]])
+    Q = Rotation.random(random_state=7).as_matrix()
+    ctrl = (np.array([0, 4, 8], np.uint64), np.array([0, 1, 2, 3, 4, 5, 6, 7], np.int64), np.concatenate([d2, d2]))
+    T = np.concatenate([np.concatenate([np.stack(rots), t[:, :, None]], 2),
+                        np.concatenate([Q @ np.stack(rots) @ Q.T, t[:, :, None]], 2)]).astype(np.float32)
+    A = np.einsum("k,kij->ij", ref.rbf(d2, sigma), T[:4, :, :3].astype(np.float64)) / ref.rbf(d2, sigma).sum()
+    np.testing.assert_allclose(A, np.diag([-0.10, -0.34, -0.56]), atol=1e-6)
+    assert np.linalg.det(A) < 0
+    want_R = [np.diag([-1.0, -1.0, 1.0]), Q @ np.diag([-1.0, -1.0, 1.0]) @ Q.T]  # sign(A) with the largest's flipped
+    w_all = ref.rbf(d2, sigma)
+    want_t = (w_all[:, None] * t).sum(0) / w_all.sum()
+    helper = ref.resample(T, ctrl, sigma)
+    orc = swf.resample(T, ctrl, 8, sigma)
+    for i in range(2):
+        np.testing.assert_allclose(helper[i, :, :3], want_R[i], atol=1e-6)
+        np.testing.assert_allclose(orc[i, :, :3], want_R[i], atol=1e-6)
+        np.testing.assert_allclose(helper[i, :, 3], want_t, atol=1e-6)
+        np.testing.assert_allclose(orc[i, :, 3], want_t, atol=1e-6)
+    np.testing.assert_allclose(orc, helper, atol=1e-6)
+
+
+def list_shape(P, shape):
+    """(ctrl, m, reg, first, second) of P with the control lists or the correspondence list in one of the shapes the
+    GPU edge tests run."""
+    ctrl, m, reg = P["ctrl"], P["m"], P["reg"]
+    first, second = corr_of(P)
+    off, idx, val = (np.asarray(a) for a in ctrl)
+    n = off.shape[0] - 1
+    lists = [(list(idx[off[i]:off[i + 1]]), list(val[off[i]:off[i + 1]])) for i in range(n)]
+    rng = np.random.default_rng(9)
+    if shape == "dups":
+        return with_duplicates(ctrl), m, reg, first, second
+    if shape == "multi-pair":  # 1-3 pairs per point, one exact duplicate, shuffled across points
+        import oracle
+
+        idx3, _, cnt3 = oracle.BruteKnn(P["dst"]).neighborhoods(P["src"], 3, 0.02 ** 2)
+        k = np.minimum(rng.integers(1, 4, n), cnt3)
+        f = [idx3[i, j] for i in range(n) for j in range(k[i])]
+        s = [i for i in range(n) for j in range(k[i])]
+        f.append(f[0])
+        s.append(s[0])
+        o = rng.permutation(len(s))
+        return ctrl, m, reg, np.array(f, np.int64)[o], np.array(s, np.int64)[o]
+    if shape == "ragged":  # K from 0 to the full list, every third list empty
+        for i in range(n):
+            k = 0 if i % 3 == 0 else int(rng.integers(1, len(lists[i][0]) + 1))
+            lists[i] = (lists[i][0][:k], lists[i][1][:k])
+    elif shape == "hub":  # node 0 last in every list, as heavy as the list's first node
+        lists = [(li + [0], lv + lv[:1]) for li, lv in lists]
+    elif shape == "m = 1":
+        lists = [([0], [float(np.sum((P["src"][i] - P["nodes"][0]) ** 2))]) for i in range(n)]
+        m, reg = 1, (np.zeros(2, np.uint64), np.zeros(0, np.int64), np.zeros(0, np.float32))
+    elif shape == "W = 0":  # every fourth list too far for its weights: they underflow to 0 in float and double
+        for i in range(0, n, 4):
+            lists[i] = (lists[i][0], [1.0] * len(lists[i][1]))
+    o = np.zeros(n + 1, np.uint64)
+    o[1:] = np.cumsum([len(a) for a, _ in lists])
+    c = (o, np.array(sum((a for a, _ in lists), []), np.int64), np.array(sum((b for _, b in lists), []), np.float32))
+    return c, m, reg, first, second
+
+
 @pytest.mark.parametrize("dups", [False, True])
 def test_oracle_normal_equations_match_the_reference_layout(swf, case, dups):
     P = dict(case)
     if dups:
         P["ctrl"] = with_duplicates(P["ctrl"])
     first, second = corr_of(P)
+    check_normal_equations(swf, P, first, second)
+
+
+@pytest.mark.parametrize("shape", ["multi-pair", "ragged", "hub", "m = 1", "W = 0"])
+def test_oracle_normal_equations_match_the_reference_layout_on_more_list_shapes(swf, case, shape):
+    """The list shapes the GPU edge tests judge the device on: several pairs per point (with a duplicate, in no
+    particular order), ragged and empty control lists, a hub node in every list, one node without arcs, and lists
+    whose weights all underflow (W_i = 0) on matched points."""
+    P = dict(case)
+    P["ctrl"], P["m"], P["reg"], first, second = list_shape(P, shape)
+    if shape == "W = 0":
+        _, _, _, W = ref.sorted_lists(P["ctrl"], KW["ctrl_sigma"])
+        assert (W == 0).sum() > 100 and np.isin(np.nonzero(W == 0)[0], second).sum() > 50
+    if shape == "ragged":
+        lens = np.diff(P["ctrl"][0].astype(np.int64))
+        assert (lens == 0).sum() > 100 and lens.max() > lens[lens > 0].min()
+    check_normal_equations(swf, P, first, second)
+
+
+def check_normal_equations(swf, P, first, second):
     m = P["m"]
     rng = np.random.default_rng(5)
     x = rng.normal(0, 0.01, (m, 6))
