@@ -224,7 +224,7 @@ EXPORTED = [
     "cb_cloud_mean_shift",
     "cb_knn1_radius", "cb_knn_radius", "cb_radius_search", "cb_find_correspondences",
     "cb_icp_default_params", "cb_icp_create", "cb_icp_destroy", "cb_icp_estimate", "cb_icp_iteration_times",
-    "cb_icp_correspondences", "cb_icp_residuals", "cb_icp_accumulate", "cb_icp_loop_cache",
+    "cb_icp_correspondences", "cb_icp_residuals", "cb_icp_accumulate", "cb_icp_loop_cache", "cb_icp_set_features",
     "cb_solve_kabsch_moments", "cb_solve_gauss_newton", "cb_solve_rotation", "cb_compose",
     "cb_kmeans_cluster", "cb_kmeans_assign", "cb_kmeans_seed_indices",
     "cb_ransac_score", "cb_ransac_residuals", "cb_ransac_rigid",
@@ -642,6 +642,9 @@ def icp_params(metric="p2p", max_iter=15, tol=1e-5, max_d2=1e-4, w_pt=0.0, w_pl=
     return p
 
 
+FEATURE_KINDS = {"point": 0, "point_normal": 1, "point_color": 2, "point_normal_color": 3}  # cb_feature_kind
+
+
 class Icp(_Handle):
     """cb_icp_*: SimplePointToPointMetricRigidICP3f / SimpleCombinedMetricRigidICP3f."""
 
@@ -701,6 +704,22 @@ class Icp(_Handle):
         out = np.empty(self.src.n, np.float32)
         _check(lib().cb_icp_residuals(self.h, C.byref(prm), _p(_T(T)), _p(out)))
         return out
+
+    def set_features(self, kind, dst_normals=None, dst_colors=None, src_normals=None, src_colors=None,
+                     normal_weight=1.0, color_weight=1.0):
+        """cb_icp_set_features: search correspondences on [p], [p, w_n n], [p, w_c c] or [p, w_n n, w_c c]
+        (kind "point", "point_normal", "point_color", "point_normal_color"); n x 3 arrays in cloud order."""
+        def arr(a, n):
+            if a is None:
+                return None
+            a = _f32(a)
+            assert a.shape[0] == n, (a.shape, n)
+            return a
+
+        dn, dc = arr(dst_normals, self.dst.n), arr(dst_colors, self.dst.n)
+        sn, sc = arr(src_normals, self.src.n), arr(src_colors, self.src.n)
+        _check(lib().cb_icp_set_features(self.h, C.c_int(FEATURE_KINDS[kind]), _p(dn), _p(dc), _p(sn), _p(sc),
+                                         C.c_float(normal_weight), C.c_float(color_weight)))
 
 
 def solve_kabsch_moments(sums16):

@@ -1,5 +1,7 @@
 // C ABI: context, clouds, nearest neighbour, rigid ICP (product code).
 #include "cb_internal.hpp"
+#include "feature_rule.hpp"
+#include "feature_search.cuh"
 #include "icp_kernels.cuh"
 #include "stats_kernels.cuh"
 #include "host_solve.hpp"
@@ -722,6 +724,11 @@ static int ensure_src_full(cb_icp* icp) {
 // the source cloud the engine modes work on: the whole cloud (replicated) with several ranks, else the caller's
 static const cb_cloud* esrc(const cb_icp* icp) { return (icp->ctx->world > 1 && icp->src_full) ? icp->src_full : icp->src; }
 
+// the correspondence list path (icp_engine.cu): non-default engine options, or features attached
+static bool icp_engine(const cb_icp* icp, const cb_icp_params* prm) {
+  return engine_mode(prm) || icp->feat.kind != CB_FEATURES_POINT;
+}
+
 // One estimator call of updateEstimate(): returns tform_iter (already un-centred), and the
 // correspondence count of the search pass. k0/k1 (nullable) are recorded around the search kernel.
 
@@ -730,13 +737,13 @@ static int icp_update(cb_icp* icp, const cb_icp_params* prm, const float* T, flo
   cb_context* ctx = icp->ctx;
   IcpArgs a;
   double sums[kMaxValues];
-  const bool engine = engine_mode(prm);
+  const bool engine = icp_engine(icp, prm);
   icp->engine_last = engine;
   if (engine) {
     // updateCorrespondences(): the explicit list (icp_engine.cu); the passes below accumulate over it
     if (k0) CB_CUDA(cudaEventRecord(k0, ctx->stream));
     CB_TRY(ensure_src_full(icp));
-    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, esrc(icp), prm, T, &icp->pairs));
+    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, esrc(icp), prm, T, &icp->pairs, &icp->feat));
     if (k1) CB_CUDA(cudaEventRecord(k1, ctx->stream));
   }
   if (prm->metric == CB_ICP_POINT_TO_POINT) {
@@ -818,7 +825,7 @@ int cb_icp_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res) {
     // device-resident loop (icp_loop.cu). prm->host_loop keeps the host-driven loop below; engine modes, inner
     // Gauss-Newton iterations and multi-rank runs without the fused exchange always use it.
     const bool one_step = prm->metric == CB_ICP_POINT_TO_POINT || prm->max_opt_iter == 1;
-    if (!prm->host_loop && !engine_mode(prm) && one_step && (ctx->world == 1 || exchange_available(ctx))) {
+    if (!prm->host_loop && !icp_engine(icp, prm) && one_step && (ctx->world == 1 || exchange_available(ctx))) {
       const int rc = icp_loop_estimate(icp, prm, res, &hand_over);
       if (rc != CB_OK || !hand_over) return rc;
       // the run is not converging: continue from the device loop's state with the host-driven loop below
@@ -929,9 +936,26 @@ int cb_icp_accumulate(cb_icp* icp, const cb_icp_params* prm, const float* T12, d
   cb_context* ctx = icp->ctx;
   CB_CUDA(cudaSetDevice(ctx->device));
   IcpArgs a;
-  CB_TRY(icp_fill_args(icp, prm, T12, nullptr, true, &a));
   double tmp[kMaxValues];
   int nv;
+  if (icp->feat.kind != CB_FEATURES_POINT) {
+    // the feature search's correspondence list (icp_engine.cu), accumulated like the list path's passes
+    const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
+    nv = p2p ? kP2PValues : kCombinedValues;
+    CB_CHECK(p2p || !(prm->w_pl > 0.f) || icp->dst->d_nrm, CB_ERR_INVALID, "dst has no normals");
+    CB_CHECK(cap >= nv, CB_ERR_INVALID, "sums buffer too small");
+    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, icp->src, prm, T12, &icp->pairs, &icp->feat));
+    CB_TRY(icp_fill_args(icp, prm, T12, nullptr, false, &a));
+    CB_TRY(launch_pairs_pass(ctx, a, icp->pairs, icp->dst, icp->src, p2p ? kModeP2P : kModeCombined,
+                             !p2p && prm->w_pt > 0.f, !p2p && prm->w_pl > 0.f));
+    CB_TRY(icp_fetch(ctx, nv, tmp, /*allreduce=*/false));
+    std::memcpy(sums, tmp, nv * sizeof(double));
+    icp->engine_last = true;
+    icp->nn_valid = true;
+    return nv;
+  }
+  CB_TRY(icp_fill_args(icp, prm, T12, nullptr, true, &a));
+  icp->engine_last = false;  // cb_icp_correspondences reads this pass's per-query result
   if (prm->metric == CB_ICP_POINT_TO_POINT) {
     nv = kP2PValues;
     CB_TRY(launch_icp_pass(ctx, a, kModeP2P, true, false, false));
@@ -1028,6 +1052,59 @@ int cb_icp_loop_cache(cb_icp* icp, float* T_search12, int64_t* nearest, uint64_t
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
     for (size_t i = 0; i < ns; i++) nearest[i] = first[i] < 0 ? -1 : (int64_t)first[i] + (int64_t)icp->dst->index_offset;
   }
+  return CB_OK;
+}
+
+// n x 3 host vectors weighted into one tail slot of an n x tails float4 array (the adaptors' constructors: one fp32
+// multiply per component)
+static void weight_tails(const float* v, size_t n, float w, int tails, int slot, std::vector<float4>& out) {
+  for (size_t i = 0; i < n; i++)
+    out[i * tails + slot] = make_float4(rule::mul_rn(w, v[3 * i]), rule::mul_rn(w, v[3 * i + 1]),
+                                        rule::mul_rn(w, v[3 * i + 2]), 0.f);
+}
+
+int cb_icp_set_features(cb_icp* icp, int kind, const float* dst_normals, const float* dst_colors,
+                        const float* src_normals, const float* src_colors, float normal_weight, float color_weight) {
+  CB_CHECK(icp, CB_ERR_INVALID, "null argument");
+  CB_CHECK(kind >= CB_FEATURES_POINT && kind <= CB_FEATURES_POINT_NORMAL_COLOR, CB_ERR_INVALID, "bad feature kind");
+  cb_context* ctx = icp->ctx;
+  CB_CHECK(ctx->world == 1, CB_ERR_UNSUPPORTED, "feature search with several ranks");
+  const bool nrm = kind == CB_FEATURES_POINT_NORMAL || kind == CB_FEATURES_POINT_NORMAL_COLOR;
+  const bool col = kind == CB_FEATURES_POINT_COLOR || kind == CB_FEATURES_POINT_NORMAL_COLOR;
+  CB_CHECK(!nrm || (dst_normals && src_normals), CB_ERR_INVALID, "the feature kind needs dst and src normals");
+  CB_CHECK(!col || (dst_colors && src_colors), CB_ERR_INVALID, "the feature kind needs dst and src colors");
+  CB_CHECK(!nrm || std::isfinite(normal_weight), CB_ERR_INVALID, "normal weight is not finite");
+  CB_CHECK(!col || std::isfinite(color_weight), CB_ERR_INVALID, "color weight is not finite");
+  CB_CUDA(cudaSetDevice(ctx->device));
+  FeatureSet& f = icp->feat;
+  for (float4* p : {f.dst_raw, f.dst_sorted, f.src_raw}) CB_TRY(icp->mem.free(p));
+  f = FeatureSet();
+  icp->nn_valid = false;
+  icp->engine_last = false;
+  if (kind == CB_FEATURES_POINT) return CB_OK;
+  const int tails = rule::feature_tails(kind);
+  const size_t nd = icp->dst->n, ns = icp->src->n;
+  std::vector<float4> hd(nd * tails), hs(ns * tails);
+  int slot = 0;
+  if (nrm) {
+    weight_tails(dst_normals, nd, normal_weight, tails, slot, hd);
+    weight_tails(src_normals, ns, normal_weight, tails, slot, hs);
+    ++slot;
+  }
+  if (col) {
+    weight_tails(dst_colors, nd, color_weight, tails, slot, hd);
+    weight_tails(src_colors, ns, color_weight, tails, slot, hs);
+  }
+  FeatureSet nf;
+  nf.kind = kind;
+  CB_TRY(icp->mem.alloc(&nf.dst_raw, nd * tails));
+  CB_TRY(icp->mem.alloc(&nf.dst_sorted, nd * tails));
+  CB_TRY(icp->mem.alloc(&nf.src_raw, ns * tails));
+  f = nf;  // owned by icp->mem from here on
+  CB_CUDA(cudaMemcpyAsync(f.dst_raw, hd.data(), hd.size() * sizeof(float4), cudaMemcpyHostToDevice, ctx->stream));
+  CB_CUDA(cudaMemcpyAsync(f.src_raw, hs.data(), hs.size() * sizeof(float4), cudaMemcpyHostToDevice, ctx->stream));
+  CB_TRY(launch_feature_gather(ctx, kind, icp->dst->d_pts, (uint32_t)nd, f.dst_raw, nullptr, f.dst_sorted));
+  CB_CUDA(cudaStreamSynchronize(ctx->stream));  // the host staging vectors go out of scope
   return CB_OK;
 }
 

@@ -261,11 +261,20 @@ inline bool engine_mode(const cb_icp_params* p) {
   return p->search_dir != CB_SECOND_TO_FIRST || p->one_to_one != 0 ||
          (p->inlier_fraction > 0.0 && p->inlier_fraction < 1.0);
 }
+// Feature tails attached to an ICP object (cb_icp_set_features, feature_rule.hpp): rule::feature_tails(kind) float4 per
+// point, already weighted.
+struct FeatureSet {
+  int kind = CB_FEATURES_POINT;  // cb_feature_kind; CB_FEATURES_POINT = no tails
+  float4* dst_raw = nullptr;     // destination tails, original order
+  float4* dst_sorted = nullptr;  // the same in the destination grid's cell order
+  float4* src_raw = nullptr;     // source tails, original order, untransformed
+};
 // findCorrespondences(tform) of CorrespondenceSearchKDTree (correspondence_search_kd_tree.hpp:107-229) for
 // the current estimate T: searches, union / intersection, fraction and one-to-one filters. Replaces *pairs, whose
-// buffers belong to `owner`.
+// buffers belong to `owner`. feat (nullable, or kind CB_FEATURES_POINT): search on the xyz distance; otherwise on the
+// feature distance (feature_search.cu), which is then the pairs' value.
 int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const cb_cloud* src,
-                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs);
+                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs, const FeatureSet* feat = nullptr);
 
 // nccl_dyn.cpp
 int nccl_unique_id(void* out128);

@@ -2,7 +2,8 @@
 // Replaces CorrespondenceSearchKDTree::findCorrespondences(tform) (correspondence_search/
 // correspondence_search_kd_tree.hpp:107-229) for search directions FIRST_TO_SECOND / BOTH, reciprocity,
 // inlier_fraction < 1 and one_to_one; the default configuration keeps the fused single-kernel path
-// (icp_kernels.cu) and never comes here.
+// (icp_kernels.cu) and never comes here. With feature tails attached (cb_icp_set_features) every configuration comes
+// here, and both searches run on the feature distance (feature_search.cu).
 //
 // Per ICP iteration the correspondence list is materialised on the device in the reference's own order:
 //   SECOND_TO_FIRST  q_j = T src_j searched in the dst grid          -> pairs (nn(j), j),   ascending j
@@ -18,6 +19,8 @@
 // the filter received (radix sorts are stable), and the oracle uses the same rule.
 // Sorting = radix_sort_pairs_u64 over (key, pair id); accumulation = one thread per pair over the raw
 // (original-order) arrays with the same per-pair arithmetic as the fused kernel (icp_accumulate.cuh).
+#include "feature_rule.hpp"
+#include "feature_search.cuh"
 #include "icp_accumulate.cuh"
 #include "icp_kernels.cuh"
 #include "reduce.cuh"
@@ -242,7 +245,7 @@ int launch_pairs_pass(cb_context* ctx, const IcpArgs& a, const EnginePairs& pair
 }
 
 int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const cb_cloud* src,
-                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs) {
+                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs, const FeatureSet* feat) {
   // (with several ranks the caller passes the whole source cloud, replicated: capi_core.cu, ensure_src_full)
   CB_CHECK(prm->search_dir >= CB_SECOND_TO_FIRST && prm->search_dir <= CB_BOTH, CB_ERR_INVALID, "bad search_dir");
   CB_TRY(owner.free(pairs->first));
@@ -254,10 +257,17 @@ int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, 
   if (n_src == 0 || n_dst == 0) return CB_OK;  // empty trees: no correspondences
   CB_TRY(ensure_index(const_cast<cb_cloud*>(dst)));
   CB_TRY(ensure_index(const_cast<cb_cloud*>(src)));
+  const bool features = feat && feat->kind != CB_FEATURES_POINT;
   Dev dev(ctx);
   int *s2f_idx = nullptr, *f2s_idx = nullptr;
   float *s2f_d2 = nullptr, *f2s_d2 = nullptr;
-  if (want_s2f) {
+  if (want_s2f && features) {
+    // queries = transformFeatures(T) of the source features, tree = the destination features
+    CB_TRY(dev.alloc(&s2f_idx, n_src));
+    CB_TRY(dev.alloc(&s2f_d2, n_src));
+    CB_TRY(launch_feature_nn(ctx, feat->kind, grid_view(dst), feat->dst_sorted, src->d_pts, n_src, feat->src_raw,
+                             rigid_of(T12), true, prm->max_d2, s2f_idx, s2f_d2));
+  } else if (want_s2f) {
     CB_TRY(dev.alloc(&s2f_idx, n_src));
     CB_TRY(dev.alloc(&s2f_d2, n_src));
     IcpArgs a;
@@ -279,17 +289,28 @@ int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, 
     CB_TRY(moved.mem.alloc(&moved.d_raw, 3 * (size_t)n_src));
     CB_TRY(launch_transform_points(ctx, rigid_of(T12), src->d_raw, n_src, moved.d_raw));
     CB_TRY(ensure_index(&moved));
-    IcpArgs a;
-    std::memset(&a, 0, sizeof(a));
-    a.dst = grid_view(&moved);
-    a.src_pts = dst->d_pts;
-    a.n_src = n_dst;
-    a.T = rigid_of(nullptr);
-    a.Tin = rigid_of(nullptr);
-    a.max_d2 = prm->max_d2;
-    a.out_idx = f2s_idx;
-    a.out_d2 = f2s_d2;
-    CB_TRY(launch_icp_pass(ctx, a, kModeKnn, true, false, false));
+    if (features) {
+      // the tree over transformFeatures(T) of the source: its tails in the new grid's cell order, queried with the
+      // destination features
+      const Rigid T = rigid_of(T12);
+      float4* moved_tails = nullptr;
+      CB_TRY(dev.alloc(&moved_tails, (size_t)n_src * rule::feature_tails(feat->kind)));
+      CB_TRY(launch_feature_gather(ctx, feat->kind, moved.d_pts, n_src, feat->src_raw, &T, moved_tails));
+      CB_TRY(launch_feature_nn(ctx, feat->kind, grid_view(&moved), moved_tails, dst->d_pts, n_dst, feat->dst_raw,
+                               rigid_of(nullptr), false, prm->max_d2, f2s_idx, f2s_d2));
+    } else {
+      IcpArgs a;
+      std::memset(&a, 0, sizeof(a));
+      a.dst = grid_view(&moved);
+      a.src_pts = dst->d_pts;
+      a.n_src = n_dst;
+      a.T = rigid_of(nullptr);
+      a.Tin = rigid_of(nullptr);
+      a.max_d2 = prm->max_d2;
+      a.out_idx = f2s_idx;
+      a.out_d2 = f2s_d2;
+      CB_TRY(launch_icp_pass(ctx, a, kModeKnn, true, false, false));
+    }
   }
   // pre-filter list
   Candidates c;

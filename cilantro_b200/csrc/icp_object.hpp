@@ -51,6 +51,7 @@ struct cb_icp {
   float max_d2_search = 0.f;
   cb::EnginePairs pairs;    // correspondence list of the last iteration in a non-default engine mode
   bool engine_last = false; // the last estimate() went through icp_engine.cu
+  cb::FeatureSet feat;      // cb_icp_set_features (tails owned by `mem`)
   double search_ms = 0;  // CUDA-event time of the fused search+accumulate kernels of the last estimate()
   std::vector<cudaEvent_t> events;
   std::vector<double> iter_ms;

@@ -271,3 +271,36 @@ def warp_pair(n, seed=1, spacing=0.005, bend=0.01, noise=0.0005):
     src = (dst + disp - c) @ R.T + c + 0.3 * bend * np.array([1.0, -1.0, 0.5]) + rng.normal(0.0, noise, (n, 3))
     return {"dst": np.ascontiguousarray(dst, np.float32), "dst_normals": np.ascontiguousarray(nrm, np.float32),
             "src": np.ascontiguousarray(src, np.float32), "spacing": float(spacing), "side": float(L)}
+
+
+def sheet_color(x, y):
+    """A smooth RGB texture over the plane (period ~0.2-0.35 along each axis), values in [0, 1]."""
+    tau = 2 * np.pi
+    return np.stack([0.5 + 0.5 * np.sin(tau * 4 * x) * np.cos(tau * 3 * y),
+                     0.5 + 0.5 * np.cos(tau * 5 * x + 1.0) * np.sin(tau * 3 * y + 0.5),
+                     0.5 + 0.5 * np.sin(tau * 3 * (x + y))], axis=1)
+
+
+def textured_sheet_pair(n, seed=1, offset=(0.03, -0.02), relief=0.002):
+    """Coloured-ICP stand-in: a low-relief sheet z = relief sin(7x) cos(6y) over [0,1)^2 with the colour texture
+    sheet_color, sampled twice (independent uniform samples). The source is the second sample shifted in-plane by
+    -offset, so the transform that registers it is a pure in-plane translation by +offset, which the geometry alone
+    barely constrains and the colours do. Returns dict(dst, dst_normals, dst_colors, src, src_normals, src_colors, T_ref)."""
+    rng = np.random.default_rng(seed)
+
+    def sample():
+        xy = rng.random((n, 2))
+        x, y = xy[:, 0], xy[:, 1]
+        z = relief * np.sin(7 * x) * np.cos(6 * y)
+        g = np.stack([-7 * relief * np.cos(7 * x) * np.cos(6 * y), 6 * relief * np.sin(7 * x) * np.sin(6 * y),
+                      np.ones(n)], axis=1)
+        g /= np.linalg.norm(g, axis=1, keepdims=True)
+        return np.stack([x, y, z], axis=1), g, sheet_color(x, y)
+
+    dp, dn, dc = sample()
+    sp, sn, sc = sample()
+    sp = sp - np.array([offset[0], offset[1], 0.0])
+    T_ref = np.hstack([np.eye(3), np.array([[offset[0]], [offset[1]], [0.0]])]).astype(np.float32)
+    f = lambda a: np.ascontiguousarray(a, np.float32)  # noqa: E731
+    return dict(dst=f(dp), dst_normals=f(dn), dst_colors=f(dc), src=f(sp), src_normals=f(sn), src_colors=f(sc),
+                T_ref=T_ref)

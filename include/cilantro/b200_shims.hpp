@@ -43,6 +43,8 @@
 #include <set>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../cilantro_b200.h"
@@ -594,6 +596,7 @@ public:
 
 protected:
   cb_icp_params& params() { return prm_; }
+  cb_icp* b200_icp() { return icp_; }
 
 private:
   // both clouds in one call: the source upload overlaps the destination's grid build (cb_cloud_create_pair)
@@ -704,6 +707,210 @@ public:
 private:
   PointToPointCorrWeightEvaluatorT& pt_;
   PointToPlaneCorrWeightEvaluatorT& pl_;
+};
+
+// ---- feature-space correspondence search (correspondence_search/common_transformable_feature_adaptors.hpp,
+// correspondence_search_kd_tree.hpp, registration/icp_common_instances.hpp:262-267 and the point-to-point twin) --------
+// The adaptors hold the reference constructors' inputs; the ICP objects hand them to cb_icp_set_features, whose device
+// search works on [p], [p, w_n n], [p, w_c c] or [p, w_n n, w_c c] exactly as the kd-tree over the adaptors would
+// (DESIGN §4.16). Only the 3-D float instances exist, like every other class here.
+
+// IdentityWeightEvaluator / DistanceEvaluator (core/common_pair_evaluators.hpp:13-27, :82): the correspondence value is
+// the squared feature distance itself (the only distance evaluator the device search implements)
+template <typename ValueT = float, typename WeightT = ValueT>
+class DistanceEvaluator {
+public:
+  using InputScalar = ValueT;
+  using OutputScalar = WeightT;
+  WeightT operator()(ValueT dist) const { return (WeightT)dist; }
+  WeightT operator()(size_t, size_t, ValueT dist) const { return (WeightT)dist; }
+};
+
+namespace b200 {
+// D x N column-major feature matrix, the pre-assembled form of the adaptors' first constructor
+template <int D>
+class ConstFeatureMatrixMap {
+public:
+  ConstFeatureMatrixMap(const float* data = nullptr, size_t n = 0) : p_(data), n_(n) {}
+  ConstFeatureMatrixMap(const std::vector<float>& s) : p_(s.data()), n_(s.size() / D) {}
+#ifdef CILANTRO_B200_HAS_EIGEN
+  ConstFeatureMatrixMap(const Eigen::Matrix<float, D, Eigen::Dynamic>& m) : p_(m.data()), n_((size_t)m.cols()) {}
+#endif
+  const float* data() const { return p_; }
+  size_t cols() const { return n_; }
+
+private:
+  const float* p_;
+  size_t n_;
+};
+
+template <int kKind>
+class FeaturesAdaptor3f {
+public:
+  using Scalar = float;
+  enum { FeatureDimension = kKind == CB_FEATURES_POINT_NORMAL_COLOR ? 9 : (kKind == CB_FEATURES_POINT ? 3 : 6) };
+  static constexpr int b200_kind() { return kKind; }
+
+  // pre-assembled [p; tails] (tails already weighted)
+  FeaturesAdaptor3f(const ConstFeatureMatrixMap<FeatureDimension>& data) : points_(3, data.cols()) {
+    constexpr bool nrm = kKind == CB_FEATURES_POINT_NORMAL || kKind == CB_FEATURES_POINT_NORMAL_COLOR;
+    constexpr bool col = kKind == CB_FEATURES_POINT_COLOR || kKind == CB_FEATURES_POINT_NORMAL_COLOR;
+    if (nrm) normals_.resize(3, data.cols());
+    if (col) colors_.resize(3, data.cols());
+    for (size_t i = 0; i < data.cols(); i++)
+      for (int k = 0; k < 3; k++) {
+        const float* c = data.data() + (size_t)FeatureDimension * i;
+        points_(k, i) = c[k];
+        if (nrm) normals_(k, i) = c[3 + k];
+        if (col) colors_(k, i) = c[(nrm ? 6 : 3) + k];
+      }
+  }
+  // PointFeaturesAdaptor (:13-17)
+  template <int K = kKind, typename std::enable_if<K == CB_FEATURES_POINT, int>::type = 0>
+  FeaturesAdaptor3f(const ConstVectorSetMatrixMap3f& points) : points_(copy(points)) {}
+  // PointNormalFeaturesAdaptor (:75-83) / PointColorFeaturesAdaptor (:175-183)
+  template <int K = kKind, typename std::enable_if<K == CB_FEATURES_POINT_NORMAL || K == CB_FEATURES_POINT_COLOR, int>::type = 0>
+  FeaturesAdaptor3f(const ConstVectorSetMatrixMap3f& points, const ConstVectorSetMatrixMap3f& tail, float weight)
+      : points_(copy(points)) {
+    (K == CB_FEATURES_POINT_NORMAL ? normals_ : colors_) = copy(tail);
+    (K == CB_FEATURES_POINT_NORMAL ? w_n_ : w_c_) = weight;
+  }
+  // PointNormalColorFeaturesAdaptor (:248-259)
+  template <int K = kKind, typename std::enable_if<K == CB_FEATURES_POINT_NORMAL_COLOR, int>::type = 0>
+  FeaturesAdaptor3f(const ConstVectorSetMatrixMap3f& points, const ConstVectorSetMatrixMap3f& normals,
+                    const ConstVectorSetMatrixMap3f& colors, float normal_weight, float color_weight)
+      : points_(copy(points)), normals_(copy(normals)), colors_(copy(colors)), w_n_(normal_weight), w_c_(color_weight) {}
+
+  size_t b200_size() const { return points_.cols(); }
+  const float* b200_normals() const { return normals_.cols() ? normals_.data() : nullptr; }
+  const float* b200_colors() const { return colors_.cols() ? colors_.data() : nullptr; }
+  float b200_normal_weight() const { return w_n_; }
+  float b200_color_weight() const { return w_c_; }
+
+private:
+  static VectorSet3f copy(const ConstVectorSetMatrixMap3f& m) {
+    VectorSet3f s(3, m.cols());
+    if (m.cols()) std::memcpy(s.data(), m.data(), 3 * m.cols() * sizeof(float));
+    return s;
+  }
+  VectorSet3f points_, normals_, colors_;
+  float w_n_ = 1.f, w_c_ = 1.f;  // the pre-assembled form carries weighted tails: 1 * x = x exactly
+};
+}  // namespace b200
+
+using PointFeaturesAdaptor3f = b200::FeaturesAdaptor3f<CB_FEATURES_POINT>;
+using PointNormalFeaturesAdaptor3f = b200::FeaturesAdaptor3f<CB_FEATURES_POINT_NORMAL>;
+using PointColorFeaturesAdaptor3f = b200::FeaturesAdaptor3f<CB_FEATURES_POINT_COLOR>;
+using PointNormalColorFeaturesAdaptor3f = b200::FeaturesAdaptor3f<CB_FEATURES_POINT_NORMAL_COLOR>;
+
+// CorrespondenceSearchKDTree<SearchFeatureAdaptorT> (correspondence_search_kd_tree.hpp:41-51, the 3-argument form): the
+// engine's fluent setters, and the two feature adaptors the ICP object searches on. The adaptors are held by reference,
+// as the reference does.
+template <class SearchFeatureAdaptorT, class EvaluatorT = DistanceEvaluator<float, float>>
+class CorrespondenceSearchKDTree : public CorrespondenceSearchEngineB200 {
+public:
+  using SearchResult = CorrespondenceSet<float, size_t>;
+  CorrespondenceSearchKDTree(SearchFeatureAdaptorT& dst_features, SearchFeatureAdaptorT& src_features,
+                             EvaluatorT& evaluator)
+      : dst_(dst_features), src_(src_features), eval_(evaluator) {}
+  SearchFeatureAdaptorT& b200_dst_features() { return dst_; }
+  SearchFeatureAdaptorT& b200_src_features() { return src_; }
+  EvaluatorT& evaluator() { return eval_; }
+  // after the ICP's estimate(), as the reference's engine holds them
+  const SearchResult& getCorrespondences() const { return feat_corr_; }
+  void b200_set_correspondences(const SearchResult& c) { feat_corr_ = c; }
+
+private:
+  SearchFeatureAdaptorT& dst_;
+  SearchFeatureAdaptorT& src_;
+  EvaluatorT& eval_;
+  SearchResult feat_corr_;
+};
+
+namespace b200 {
+// The engine-templated ICP classes: the reference's constructor order, the engine's settings and features read at every
+// estimate().
+template <class Engine, class Base>
+class EngineRigidICP3f : public Base {
+public:
+  template <class... Args>
+  EngineRigidICP3f(Engine& engine, Args&&... args) : Base(std::forward<Args>(args)...), engine_(engine) {}
+  Engine& correspondenceSearchEngine() { return engine_; }
+  const Engine& correspondenceSearchEngine() const { return engine_; }
+  EngineRigidICP3f& estimate() {
+    auto& dst = engine_.b200_dst_features();
+    auto& src = engine_.b200_src_features();
+    if (dst.b200_size() != n_dst_ || src.b200_size() != n_src_)
+      throw std::invalid_argument("cilantro_b200: the feature adaptors' sizes differ from the ICP's point sets");
+    check(cb_icp_set_features(this->b200_icp(), dst.b200_kind(), dst.b200_normals(), dst.b200_colors(),
+                              src.b200_normals(), src.b200_colors(), dst.b200_normal_weight(), dst.b200_color_weight()),
+          "cb_icp_set_features");
+    Base::correspondenceSearchEngine() = static_cast<const CorrespondenceSearchEngineB200&>(engine_);
+    Base::estimate();
+    return *this;
+  }
+  EngineRigidICP3f& estimate(size_t max_iter, float conv_tol) {
+    this->setMaxNumberOfIterations(max_iter);
+    this->setConvergenceTolerance(conv_tol);
+    return estimate();
+  }
+  const CorrespondenceSet<float, size_t>& getCorrespondences() {
+    engine_.b200_set_correspondences(Base::getCorrespondences());
+    return engine_.getCorrespondences();
+  }
+
+private:
+  Engine& engine_;
+
+protected:
+  size_t n_dst_ = 0, n_src_ = 0;
+};
+}  // namespace b200
+
+// PointToPointMetricRigidTransformICP3f<Engine> (icp_single_transform_point_to_point_metric.hpp:21-28, :96-98)
+template <class CorrespondenceSearchEngineT>
+class PointToPointMetricRigidTransformICP3f
+    : public b200::EngineRigidICP3f<CorrespondenceSearchEngineT, SimpleRigidICP3fB200<CB_ICP_POINT_TO_POINT>> {
+  using Base = b200::EngineRigidICP3f<CorrespondenceSearchEngineT, SimpleRigidICP3fB200<CB_ICP_POINT_TO_POINT>>;
+
+public:
+  PointToPointMetricRigidTransformICP3f(const ConstVectorSetMatrixMap3f& dst, const ConstVectorSetMatrixMap3f& src,
+                                        CorrespondenceSearchEngineT& corr_engine)
+      : Base(corr_engine, dst, src) {
+    this->n_dst_ = dst.cols();
+    this->n_src_ = src.cols();
+  }
+};
+
+// CombinedMetricRigidTransformICP3f<Engine, PtEval, PlEval> (icp_single_transform_combined_metric.hpp:33-40, :63-70;
+// icp_common_instances.hpp:262-267)
+template <class CorrespondenceSearchEngineT,
+          class PointToPointCorrWeightEvaluatorT = UnityWeightEvaluator<float, float>,
+          class PointToPlaneCorrWeightEvaluatorT = UnityWeightEvaluator<float, float>>
+class CombinedMetricRigidTransformICP3f
+    : public b200::EngineRigidICP3f<CorrespondenceSearchEngineT,
+                                    CombinedMetricRigidICP3f<PointToPointCorrWeightEvaluatorT, PointToPlaneCorrWeightEvaluatorT>> {
+  using Base = b200::EngineRigidICP3f<CorrespondenceSearchEngineT,
+                                      CombinedMetricRigidICP3f<PointToPointCorrWeightEvaluatorT, PointToPlaneCorrWeightEvaluatorT>>;
+
+public:
+  CombinedMetricRigidTransformICP3f(const ConstVectorSetMatrixMap3f& dst_p, const ConstVectorSetMatrixMap3f& dst_n,
+                                    const ConstVectorSetMatrixMap3f& src_p, CorrespondenceSearchEngineT& corr_engine,
+                                    PointToPointCorrWeightEvaluatorT& point_corr_eval,
+                                    PointToPlaneCorrWeightEvaluatorT& plane_corr_eval)
+      : Base(corr_engine, dst_p, dst_n, src_p, point_corr_eval, plane_corr_eval) {
+    this->n_dst_ = dst_p.cols();
+    this->n_src_ = src_p.cols();
+  }
+  CombinedMetricRigidTransformICP3f(const ConstVectorSetMatrixMap3f& dst_p, const ConstVectorSetMatrixMap3f& dst_n,
+                                    const ConstVectorSetMatrixMap3f& src_p, const ConstVectorSetMatrixMap3f& src_n,
+                                    CorrespondenceSearchEngineT& corr_engine,
+                                    PointToPointCorrWeightEvaluatorT& point_corr_eval,
+                                    PointToPlaneCorrWeightEvaluatorT& plane_corr_eval)
+      : Base(corr_engine, dst_p, dst_n, src_p, src_n, point_corr_eval, plane_corr_eval) {
+    this->n_dst_ = dst_p.cols();
+    this->n_src_ = src_p.cols();
+  }
 };
 
 // transformPoints(tform, in, out) — core/space_transformations.hpp:203-216

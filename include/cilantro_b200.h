@@ -383,6 +383,33 @@ int cb_icp_accumulate(cb_icp* icp, const cb_icp_params* prm, const float* T12, d
  * Returns CB_ERR_INVALID when the last estimate() did not run on the device loop. */
 int cb_icp_loop_cache(cb_icp* icp, float* T_search12, int64_t* nearest, uint64_t* searched_last);
 
+/* Feature-space correspondence search: CorrespondenceSearchKDTree<SearchFeatureAdaptorT> over the feature adaptors of
+ * correspondence_search/common_transformable_feature_adaptors.hpp, as CombinedMetricRigidTransformICP3f<Engine> /
+ * PointToPointMetricRigidTransformICP3f<Engine> take it (registration/icp_single_transform_combined_metric.hpp:262-267,
+ * icp_single_transform_point_to_point_metric.hpp:96-98):
+ *   CB_FEATURES_POINT               [p]                  PointFeaturesAdaptor3f (the default: xyz only)
+ *   CB_FEATURES_POINT_NORMAL        [p, w_n n]           PointNormalFeaturesAdaptor3f
+ *   CB_FEATURES_POINT_COLOR         [p, w_c c]           PointColorFeaturesAdaptor3f
+ *   CB_FEATURES_POINT_NORMAL_COLOR  [p, w_n n, w_c c]    PointNormalColorFeaturesAdaptor3f
+ * The arrays are host n x 3 (destination / source cloud order), copied and weighted at this call; the ones a kind
+ * does not use may be NULL. They are separate from the clouds' normals: source normals on the cloud make the metric
+ * symmetric, a feature adaptor does not. The source features are transformed with the estimate as transformFeatures
+ * does (normal part rotated, colour part copied). The correspondence search then runs on the feature distance (the
+ * correspondence value, the radius test, the weight evaluators and the engine filters all see the feature d2), while
+ * the estimator uses the 3-D points and destination normals as before; cb_icp_residuals stays a 3-D search, as the
+ * reference's computeResiduals. Every other kind than CB_FEATURES_POINT takes the list path of the non-default engine
+ * modes, whatever cb_icp_params says; CB_FEATURES_POINT drops the features and restores the default paths.
+ * CB_ERR_INVALID: an array the kind needs is NULL, or a weight the kind uses is not finite. Several ranks:
+ * CB_ERR_UNSUPPORTED. */
+typedef enum cb_feature_kind {
+  CB_FEATURES_POINT = 0,
+  CB_FEATURES_POINT_NORMAL = 1,
+  CB_FEATURES_POINT_COLOR = 2,
+  CB_FEATURES_POINT_NORMAL_COLOR = 3
+} cb_feature_kind;
+int cb_icp_set_features(cb_icp* icp, int kind, const float* dst_normals, const float* dst_colors,
+                        const float* src_normals, const float* src_colors, float normal_weight, float color_weight);
+
 /* Host-only O(1) solves (no device needed; exported so the N>1 logic is testable on CPU). */
 /* estimateTransformPointToPointMetric from moments — transform_estimation.hpp:25-47. Returns 1 if n>=3. */
 int cb_solve_kabsch_moments(const double* sums16, float* T12);

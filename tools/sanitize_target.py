@@ -44,6 +44,18 @@ def main():
                   dict(search_dir="first_to_second")):
         icp.estimate(metric="p2p", max_iter=2, tol=0.0, max_d2=max_d2, **extra)
         icp.correspondences()
+    # feature-space search (feature_search.cu): both directions, one and two tails, the unbounded far sweep
+    fs = synth.textured_sheet_pair(N, seed=4)
+    ficp = capi.Icp(ctx, capi.Cloud(ctx, fs["dst"], fs["dst_normals"]), capi.Cloud(ctx, fs["src"]))
+    for kind in ("point_color", "point_normal_color"):
+        ficp.set_features(kind, dst_normals=fs["dst_normals"], dst_colors=fs["dst_colors"],
+                          src_normals=fs["src_normals"], src_colors=fs["src_colors"], normal_weight=0.5, color_weight=5.0)
+        for extra in (dict(), dict(search_dir="both")):
+            ficp.estimate(metric="p2p", max_iter=2, tol=0.0, max_d2=max_d2, **extra)
+            ficp.correspondences()
+        ficp.estimate(metric="p2p", max_iter=1, tol=0.0, max_d2=np.float32(3e38), search_dir="first_to_second")
+    ficp.set_features("point")
+    ficp.close()
     # general-k kNN, radius lists, normals, downsample
     capi.knn_radius(ctx, d_dst, d_src, 8, T, np.float32(3e38))
     capi.radius_search(ctx, d_dst, d_src, np.float32(0.05 ** 2), T)
