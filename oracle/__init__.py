@@ -2,9 +2,12 @@
 
 ctypes bindings for the CPU restatement (oracle/libcilantro_oracle.so, built from
 cilantro_oracle.cpp) and, when present, for the reference's own vendored nanoflann compiled in
-place (oracle/_ref/libcilantro_ref_knn.so, built from nanoflann_ref.cpp against
-/root/reference). Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
+place (oracle/_ref/libcilantro_ref_knn.so, built from nanoflann_ref.cpp against the
+reference checkout). Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
 --impl reference legs may import this package; cilantro_b200 never does.
+
+oracle/Makefile builds every library of the package (build()); load() opens one for this module
+and each submodule. The ctypes helpers they share live here.
 
 All point sets are numpy float32 arrays of shape (n, 3), C-contiguous — byte-identical to the
 reference's column-major 3 x n Eigen layout (core/data_containers.hpp:155-156).
@@ -17,23 +20,39 @@ import subprocess
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB_PATH = os.path.join(_HERE, "libcilantro_oracle.so")
-_REF_PATH = os.path.join(_HERE, "_ref", "libcilantro_ref_knn.so")
 
 KNN_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_size_t, C.c_float, C.c_void_p, C.c_void_p)
+FLT_MAX = float(np.finfo(np.float32).max)
 
 
 def build(force=False):
-    """Compile the restatement (and the nanoflann-backed reference kNN where /root/reference exists)."""
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < os.path.getmtime(
-        os.path.join(_HERE, "cilantro_oracle.cpp")
-    ):
-        subprocess.check_call(["make", "-s", "-C", _HERE, "oracle"])
-    if os.path.exists("/root/reference/include/cilantro/3rd_party/nanoflann/nanoflann.hpp"):
-        if force or not os.path.exists(_REF_PATH) or os.path.getmtime(_REF_PATH) < os.path.getmtime(
-            os.path.join(_HERE, "nanoflann_ref.cpp")
-        ):
-            subprocess.check_call(["make", "-s", "-C", _HERE, "ref"])
+    """Compile every oracle library that is missing or stale (oracle/Makefile: the restatements, and the reference's
+    nanoflann into oracle/_ref where a reference checkout exists); force rebuilds them all."""
+    global _built
+    subprocess.check_call(["make", "-s", "-C", _HERE, f"-j{os.cpu_count() or 1}"] + (["-B"] if force else []))
+    _built = True
+
+
+_built = False
+_libs = {}
+
+
+def load(name, restype=None, argtypes=None):
+    """The library oracle/<name>, opened once per process after one build() (a no-op when nothing is stale), with the
+    given {function: restype} and {function: argtypes} set. None if the build leaves no such file (oracle/_ref without
+    a reference checkout)."""
+    if name not in _libs:
+        if not _built:
+            build()
+        path = os.path.join(_HERE, name)
+        h = C.CDLL(path) if os.path.exists(path) else None
+        if h is not None:
+            for fn, t in (restype or {}).items():
+                getattr(h, fn).restype = t
+            for fn, t in (argtypes or {}).items():
+                getattr(h, fn).argtypes = t
+        _libs[name] = h
+    return _libs[name]
 
 
 class IcpParams(C.Structure):
@@ -90,46 +109,33 @@ class BruteCtx(C.Structure):
     _fields_ = [("ref", C.c_void_p), ("nref", C.c_size_t)]
 
 
-_lib = None
-_ref = None
-
-
 def lib():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        _lib = C.CDLL(_LIB_PATH)
-        _lib.orc_kmeans.restype = C.c_size_t
-        _lib.orc_find_correspondences.restype = C.c_size_t
-        _lib.orc_num_threads.restype = C.c_int
-    return _lib
-
-
-def have_ref():
-    return os.path.exists(_REF_PATH)
+    return load("libcilantro_oracle.so", {"orc_kmeans": C.c_size_t, "orc_find_correspondences": C.c_size_t,
+                                          "orc_num_threads": C.c_int, "orc_engine_correspondences": C.c_size_t,
+                                          "orc_grid_downsample": C.c_size_t})
 
 
 def ref():
-    """The reference's own nanoflann (None if oracle/_ref was never built)."""
-    global _ref
-    if _ref is None:
-        if not os.path.exists(_REF_PATH):
-            build()
-        if not os.path.exists(_REF_PATH):
-            return None
-        _ref = C.CDLL(_REF_PATH)
-        _ref.ref_tree_build.restype = C.c_void_p
-        _ref.ref_knn_in_radius.restype = C.c_size_t
-        _ref.ref_nanoflann_version.restype = C.c_uint
-    return _ref
+    """The reference's own nanoflann (None without oracle/_ref)."""
+    return load("_ref/libcilantro_ref_knn.so", {"ref_tree_build": C.c_void_p, "ref_knn_in_radius": C.c_size_t,
+                                                "ref_nanoflann_version": C.c_uint})
+
+
+def have_ref():
+    return ref() is not None
 
 
 def _f32(a, shape_last=3):
+    """float32, C-contiguous; asserts the shape (n, shape_last) unless shape_last is None."""
     a = np.ascontiguousarray(a, dtype=np.float32)
     if shape_last is not None:
         assert a.ndim == 2 and a.shape[1] == shape_last, a.shape
     return a
+
+
+def _rows(a, cols=3):
+    """float32, C-contiguous, reshaped to (-1, cols)."""
+    return np.ascontiguousarray(a, np.float32).reshape(-1, cols)
 
 
 def _p(a):
@@ -143,6 +149,31 @@ def _T(T):
 
 def identity():
     return np.hstack([np.eye(3, dtype=np.float32), np.zeros((3, 1), np.float32)])
+
+
+def rbf_coeff(sigma):
+    """RBFKernelWeightEvaluator's coefficient in float: coeff_ = -(WeightT)(0.5) / (sigma * sigma)."""
+    sg = np.float32(sigma)
+    return float(np.float32(-0.5) / (sg * sg))
+
+
+def _icp_params(metric, max_iter, tol, max_d2, w_pt, w_pl, max_opt_iter, opt_tol, T_init, pt_rbf_sigma, pl_rbf_sigma,
+                **engine):
+    """The IcpParams of one ICP run (accum_double and parallel left 0); engine = _engine_fields' keywords."""
+    prm = IcpParams()
+    _engine_fields(prm, **engine)
+    prm.metric = 0 if metric == "p2p" else 1
+    prm.max_iter, prm.tol, prm.max_d2 = int(max_iter), tol, max_d2
+    prm.w_pt, prm.w_pl = w_pt, w_pl
+    prm.max_opt_iter, prm.opt_tol = int(max_opt_iter), opt_tol
+    if pt_rbf_sigma is not None:
+        prm.pt_weight_kind, prm.pt_weight_coeff = 1, rbf_coeff(pt_rbf_sigma)
+    if pl_rbf_sigma is not None:
+        prm.pl_weight_kind, prm.pl_weight_coeff = 1, rbf_coeff(pl_rbf_sigma)
+    Ti = identity() if T_init is None else _T(T_init)
+    for i, v in enumerate(Ti.reshape(-1)):
+        prm.T_init[i] = float(v)
+    return prm
 
 
 def num_threads():
@@ -195,7 +226,7 @@ class RefKnn:
     def __init__(self, ref_pts, max_leaf=10):
         r = ref()
         if r is None:
-            raise RuntimeError("oracle/_ref/libcilantro_ref_knn.so not built (needs /root/reference)")
+            raise RuntimeError("oracle/_ref/libcilantro_ref_knn.so not built (needs the reference checkout)")
         self.pts = _f32(ref_pts)
         self.h = C.c_void_p(r.ref_tree_build(_p(self.pts), C.c_size_t(self.pts.shape[0]), C.c_size_t(max_leaf)))
         self.fn = C.cast(r.ref_knn1_radius_cb, C.c_void_p)
@@ -315,25 +346,11 @@ def icp(dst_p, src_p, knn, metric="p2p", dst_n=None, src_n=None, max_iter=15, to
     dst_p, src_p = _f32(dst_p), _f32(src_p)
     dst_n = _f32(dst_n) if dst_n is not None else None
     src_n = _f32(src_n) if src_n is not None else None
-    prm = IcpParams()
-    _engine_fields(prm, search_dir, inlier_fraction, require_reciprocal, one_to_one, f2s_reference)
-    prm.metric = 0 if metric == "p2p" else 1
-    prm.max_iter = int(max_iter)
-    prm.tol = tol
-    prm.max_d2 = max_d2
-    prm.w_pt, prm.w_pl = w_pt, w_pl
-    prm.max_opt_iter = int(max_opt_iter)
-    prm.opt_tol = opt_tol
+    prm = _icp_params(metric, max_iter, tol, max_d2, w_pt, w_pl, max_opt_iter, opt_tol, T_init, pt_rbf_sigma,
+                      pl_rbf_sigma, search_dir=search_dir, inlier_fraction=inlier_fraction,
+                      require_reciprocal=require_reciprocal, one_to_one=one_to_one, f2s_reference=f2s_reference)
     prm.accum_double = int(accum_double)
     prm.parallel = int(parallel)
-    for kind, coeff, sigma in (("pt_weight_kind", "pt_weight_coeff", pt_rbf_sigma), ("pl_weight_kind", "pl_weight_coeff", pl_rbf_sigma)):
-        if sigma is not None:
-            sg = np.float32(sigma)
-            setattr(prm, kind, 1)
-            setattr(prm, coeff, float(np.float32(-0.5) / (sg * sg)))  # coeff_ = -(WeightT)(0.5) / (sigma * sigma), in float
-    Ti = identity() if T_init is None else _T(T_init)
-    for i, v in enumerate(Ti.reshape(-1)):
-        prm.T_init[i] = float(v)
     res = IcpResult()
     tlog = np.zeros((max(int(max_iter), 1), 3, 4), np.float32) if log else None
     if prm.metric == 1:
@@ -375,7 +392,6 @@ def engine_correspondences(dst_p, src_p, T, knn, max_d2, search_dir="second_to_f
     i1 = np.empty(cap, np.uint64)
     i2 = np.empty(cap, np.uint64)
     v = np.empty(cap, np.float32)
-    lib().orc_engine_correspondences.restype = C.c_size_t
     m = lib().orc_engine_correspondences(_p(dst_p), C.c_size_t(dst_p.shape[0]), _p(src_p), C.c_size_t(src_p.shape[0]),
                                          _p(_T(T)), C.byref(prm), knn.fn, knn.user, _p(i1), _p(i2), _p(v))
     return i1[:m].astype(np.int64), i2[:m].astype(np.int64), v[:m].copy()
@@ -464,9 +480,6 @@ def ransac_rigid(dst, src, seed, max_iter=100, thresh=0.01, inlier_count_thresh=
     }
 
 
-FLT_MAX = float(np.finfo(np.float32).max)
-
-
 def estimate_normals(pts, knn, k=0, radius2=None, view_point=None, ref_normals=None, neighbors=None):
     """NormalEstimation::estimateNormalsAndCurvature{KNN,Radius,KNNInRadius} (core/normal_estimation.hpp:83-232)
     on neighbourhoods from `knn` (RefKnn = the reference's nanoflann), or on precomputed `neighbors` = (idx, cnt).
@@ -500,7 +513,6 @@ def grid_downsample(pts, bin_size, normals=None, colors=None, min_points=1, orde
     o_p = np.empty((max(n, 1), 3), np.float32)
     o_n = np.empty((max(n, 1), 3), np.float32) if nrm is not None else None
     o_c = np.empty((max(n, 1), 3), np.float32) if col is not None else None
-    lib().orc_grid_downsample.restype = C.c_size_t
     m = lib().orc_grid_downsample(_p(pts), _p(nrm), _p(col), C.c_size_t(n), C.c_float(bin_size), C.c_size_t(min_points),
                                   C.c_int(order), _p(o_p), _p(o_n), _p(o_c))
     return o_p[:m].copy(), (o_n[:m].copy() if o_n is not None else None), (o_c[:m].copy() if o_c is not None else None)

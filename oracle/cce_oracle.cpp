@@ -1,7 +1,7 @@
 // ORACLE — test infrastructure, NOT product code.
 // Serial restatement of extractConnectedComponents in its neighbourhood-set form (clustering/
 // connected_component_extraction.hpp:21-118; the kd-tree form :163-265 runs the same logic on tree.search() results)
-// and of the proximity evaluators (core/common_pair_evaluators.hpp:88-259). Built by oracle/segment.py into
+// and of the proximity evaluators (core/common_pair_evaluators.hpp:88-259). Built by oracle/Makefile into
 // oracle/libcce_oracle.so; compile with -ffp-contract=off (the arithmetic contract of cilantro_oracle.cpp).
 //
 // Restated for ONE thread: the reference's OpenMP seed loop (:36-65) shares current_label without synchronisation.

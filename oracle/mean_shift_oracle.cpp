@@ -1,6 +1,6 @@
 // ORACLE — test infrastructure, NOT product code.
 // Serial restatement of MeanShift<float, 3>::cluster (clustering/mean_shift.hpp:37-115) for the fp32 arithmetic
-// contract of cilantro_oracle.cpp: built by oracle/mean_shift.py into oracle/libms_oracle.so with -ffp-contract=off.
+// contract of cilantro_oracle.cpp: built by oracle/Makefile into oracle/libms_oracle.so with -ffp-contract=off.
 //
 // Neighbourhoods: a brute-force radius search with BruteKnn's arithmetic (d2 = ((dx^2 + dy^2) + dz^2), dx = q - p,
 // strict d2 < r2), sorted on (d2, index), which pins the order the reference leaves to std::sort (DESIGN §6). The

@@ -4,7 +4,7 @@
 // PointNormalColorFeaturesAdaptor3f features (D = 6 / 9; D = 3 for PointFeaturesAdaptor3f), compiled in place from the
 // reference's OWN vendored nanoflann header (never copied into this repo), with the leaf size, build threads and
 // result adaptor of nanoflann_ref.cpp (that file is compiled into this library too). Output:
-// oracle/_ref/libcilantro_ref_feature_knn.so, built by oracle/feature_icp.py where the reference exists.
+// oracle/_ref/libcilantro_ref_feature_knn.so, built by oracle/Makefile where the reference exists.
 #include "nanoflann_ref.cpp"
 
 namespace {

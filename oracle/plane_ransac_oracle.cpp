@@ -1,7 +1,7 @@
 // ORACLE — test infrastructure, NOT product code.
 // Serial restatement of RandomSampleConsensusBase::estimate (model_estimation/ransac_base.hpp:64-131) with
 // HyperplaneRANSACEstimator<float, 3> (model_estimation/ransac_hyperplane_estimator.hpp), DESIGN §4.12: built by
-// oracle/ransac_plane.py into oracle/libplane_oracle.so with -ffp-contract=off.
+// oracle/Makefile into oracle/libplane_oracle.so with -ffp-contract=off.
 //
 // Hypothesis plane of a sample: the closed form pinned in DESIGN §4.12 (double, one rounding per operation). Residual:
 // |((n0 x) + ((n1 y) + (n2 z))) + d| in fp32. Re-estimation: the PCA of the kept hypothesis's inliers with the

@@ -1,5 +1,6 @@
 """ORACLE — test infrastructure, NOT product code: ctypes binding of the plane-RANSAC restatement
-(oracle/plane_ransac_oracle.cpp -> oracle/libplane_oracle.so, built on first use or by build()).
+(oracle/plane_ransac_oracle.cpp -> oracle/libplane_oracle.so, built by oracle/Makefile on first use or by
+oracle.build()).
 
     from oracle import ransac_plane
     ransac_plane.ransac_plane(pts, seed=3, max_iter=250, thresh=0.01, inlier_count_thresh=1500)
@@ -7,16 +8,12 @@
 Planes are float32 (n0, n1, n2, d). The result dict of ransac_plane() has the keys of capi.ransac_plane's.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "plane_ransac_oracle.cpp")
-_DEPS = (_SRC, os.path.join(_HERE, "small_linalg.hpp"))
-_LIB_PATH = os.path.join(_HERE, "libplane_oracle.so")
-_lib = None
+import oracle
+from oracle import _p, _rows
+from oracle import build  # noqa: F401 (oracle.build: every library, also callable as <submodule>.build)
 
 
 class PlaneResult(C.Structure):
@@ -29,32 +26,8 @@ class PlaneResult(C.Structure):
     ]
 
 
-def build(force=False):
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(d) for d in _DEPS):
-        env = dict(os.environ)
-        env.pop("CXX", None)
-        tmp = _LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fopenmp", "-fPIC",
-                               "-shared", "-fvisibility=hidden", "-Wall", "-o", tmp, _SRC], env=env)
-        os.replace(tmp, _LIB_PATH)
-
-
 def lib():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        _lib = C.CDLL(_LIB_PATH)
-        _lib.orc_plane_residuals.restype = C.c_size_t
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
-
-
-def _pts(pts):
-    return np.ascontiguousarray(pts, np.float32).reshape(-1, 3)
+    return oracle.load("libplane_oracle.so", {"orc_plane_residuals": C.c_size_t})
 
 
 def fit(sample_points):
@@ -69,7 +42,7 @@ def fit(sample_points):
 
 def residuals(pts, plane, thresh):
     """(residuals[n], ascending inlier indices) of one plane."""
-    pts = _pts(pts)
+    pts = _rows(pts)
     pl = np.ascontiguousarray(plane, np.float32).reshape(4)
     n = pts.shape[0]
     res = np.empty(max(n, 1), np.float32)
@@ -79,7 +52,7 @@ def residuals(pts, plane, thresh):
 
 
 def score(pts, planes, thresh):
-    pts = _pts(pts)
+    pts = _rows(pts)
     planes = np.ascontiguousarray(planes, np.float32).reshape(-1, 4)
     counts = np.empty(planes.shape[0], np.uint32)
     lib().orc_plane_score(_p(pts), C.c_size_t(pts.shape[0]), _p(planes), C.c_size_t(planes.shape[0]), C.c_float(thresh),
@@ -89,7 +62,7 @@ def score(pts, planes, thresh):
 
 def hypotheses(pts, seed, iters):
     """The loop's first `iters` samples (iters x min(3, n) indices) and their planes (iters x 4)."""
-    pts = _pts(pts)
+    pts = _rows(pts)
     n = pts.shape[0]
     samples = np.zeros((iters, 3), np.uint64)
     planes = np.empty((max(iters, 1), 4), np.float32)
@@ -99,7 +72,7 @@ def hypotheses(pts, seed, iters):
 
 def pca_plane(pts, idx, accum_double=False):
     """estimateModel(sample_ind): the PCA plane of the listed points."""
-    pts = _pts(pts)
+    pts = _rows(pts)
     idx = np.ascontiguousarray(idx, np.uint64)
     out = np.empty(4, np.float32)
     lib().orc_plane_pca(_p(pts), _p(idx), C.c_size_t(idx.size), C.c_int(int(accum_double)), _p(out))
@@ -108,7 +81,7 @@ def pca_plane(pts, idx, accum_double=False):
 
 def ransac_plane(pts, seed, max_iter=100, thresh=0.1, inlier_count_thresh=None, re_estimate=True, accum_double=False):
     """PlaneRANSACEstimator3f::estimate restated serially, the seed injected in place of std::random_device."""
-    pts = _pts(pts)
+    pts = _rows(pts)
     n = pts.shape[0]
     if inlier_count_thresh is None:
         inlier_count_thresh = n // 2 + n % 2  # ransac_hyperplane_estimator.hpp:18

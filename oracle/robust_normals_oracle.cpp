@@ -1,6 +1,6 @@
 // ORACLE — test infrastructure, NOT product code.
 // Serial restatement of NormalEstimation<float, 3, MinimumCovarianceDeterminant<float, 3>> (core/normal_estimation.hpp:
-// 279-421 over core/covariance.hpp:185-371) under the contract of DESIGN §4.15, built by oracle/robust_normals.py into
+// 279-421 over core/covariance.hpp:185-371) under the contract of DESIGN §4.15, built by oracle/Makefile into
 // oracle/librobust_normals_oracle.so with -ffp-contract=off. It does not include the product's rule header: the draws
 // come from the installed libstdc++ (std::minstd_rand0, std::uniform_int_distribution<size_t>), the kept subset from
 // std::sort on (key, position) with NaN as +inf, and the 3x3 algebra is written out again here, one rounding per

@@ -1,5 +1,5 @@
 """ORACLE — test infrastructure, NOT product code: ctypes binding of the connected-component restatement
-(oracle/cce_oracle.cpp -> oracle/libcce_oracle.so, built on first use or by build()).
+(oracle/cce_oracle.cpp -> oracle/libcce_oracle.so, built by oracle/Makefile on first use or by oracle.build()).
 
     from oracle import segment
     segment.connected_components(pts, k=0, radius2=r2, terms=2, max_angle=a, normals=nrm)
@@ -8,43 +8,16 @@ Neighbourhoods: BruteKnn (oracle/cilantro_oracle.cpp, ascending (d2, index)) by 
 same neighborhoods(qry, k, r2, stride) method whose rows are re-sorted on (d2, index) here (e.g. RefKnn).
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 import oracle
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "cce_oracle.cpp")
-_LIB_PATH = os.path.join(_HERE, "libcce_oracle.so")
-_lib = None
-
-FLT_MAX = float(np.finfo(np.float32).max)
-
-
-def build(force=False):
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < os.path.getmtime(_SRC):
-        env = dict(os.environ)
-        env.pop("CXX", None)
-        tmp = _LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fPIC", "-shared",
-                               "-fvisibility=hidden", "-Wall", "-o", tmp, _SRC], env=env)
-        os.replace(tmp, _LIB_PATH)
+from oracle import FLT_MAX, _p
+from oracle import build  # noqa: F401 (oracle.build: every library, also callable as <submodule>.build)
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        _lib = C.CDLL(_LIB_PATH)
-        _lib.orc_connected_components.restype = C.c_size_t
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
+    return oracle.load("libcce_oracle.so", {"orc_connected_components": C.c_size_t})
 
 
 def neighborhoods(pts, k=0, radius2=0.0, knn=None):

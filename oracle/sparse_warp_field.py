@@ -1,6 +1,6 @@
 """ORACLE — test infrastructure, NOT product code: ctypes binding of the sparse warp-field restatement
-(oracle/sparse_warp_field_oracle.cpp -> oracle/libsparse_warp_oracle.so, built on first use or by build()) and the
-serial ICP loop of CombinedMetricSparseWarpFieldICP on the oracle's brute-force 1-NN.
+(oracle/sparse_warp_field_oracle.cpp -> oracle/libsparse_warp_oracle.so, built by oracle/Makefile on first use or by
+oracle.build()) and the serial ICP loop of CombinedMetricSparseWarpFieldICP on the oracle's brute-force 1-NN.
 
     from oracle import sparse_warp_field
     sparse_warp_field.icp(dst, dst_n, src, ctrl, n_ctrl, reg, max_iter=5, w_pt=0.0, stiffness=200.0)
@@ -9,49 +9,18 @@ ctrl = (offsets, index, value): one control list of (node, squared distance) per
 neighbourhoods' CSR. Node transforms are (n_ctrl, 3, 4) float32, dense transforms (n_src, 3, 4).
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from oracle import warp_field as _dense
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "sparse_warp_field_oracle.cpp")
-_LIB_PATH = os.path.join(_HERE, "libsparse_warp_oracle.so")
-_lib = None
-
-
-def build(force=False):
-    deps = [_SRC, os.path.join(_HERE, "warp_field_oracle.cpp"), os.path.join(_HERE, "small_linalg.hpp")]
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(d) for d in deps):
-        env = dict(os.environ)
-        env.pop("CXX", None)
-        tmp = _LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fPIC", "-shared",
-                               "-fvisibility=hidden", "-Wall", "-o", tmp, _SRC], env=env)
-        os.replace(tmp, _LIB_PATH)
+import oracle
+from oracle import _p, _rows, rbf_coeff
+from oracle import build  # noqa: F401 (oracle.build: every library, also callable as <submodule>.build)
+from oracle.warp_field import _nbhd, apply, compose, residuals  # noqa: F401 (residuals: the dense one applies)
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        _lib = C.CDLL(_LIB_PATH)
-        _lib.orc_sparse_warp_solve.restype = C.c_int
-        _lib.orc_sparse_warp_system.restype = None
-        _lib.orc_sparse_warp_resample.restype = None
-    return _lib
-
-
-_p = _dense._p
-_f32 = _dense._f32
-_nbhd = _dense._nbhd
-rbf_coeff = _dense.rbf_coeff
-apply = _dense.apply
-compose = _dense.compose
-residuals = _dense.residuals
+    return oracle.load("libsparse_warp_oracle.so", {"orc_sparse_warp_solve": C.c_int,
+                                                    "orc_sparse_warp_system": None, "orc_sparse_warp_resample": None})
 
 
 def _ctrl_args(ctrl, n_ctrl, ctrl_sigma):
@@ -72,8 +41,8 @@ def resample(T_ctrl, ctrl, n_ctrl, ctrl_sigma=1.0):
 def system(dst, dst_n, src, first, second, ctrl, n_ctrl, reg, x, p, w_pt=0.0, w_pl=1.0, stiffness=1.0,
            huber_delta=1e-4, reg_sigma=1.0, ctrl_sigma=1.0):
     """The normal equations in double at the node unknowns x (m, 6): dict(b, diag, q = At At^T p), each (m, 6)."""
-    dst, src = _f32(dst), _f32(src)
-    dn = None if dst_n is None else _f32(dst_n)
+    dst, src = _rows(dst), _rows(src)
+    dn = None if dst_n is None else _rows(dst_n)
     m = int(n_ctrl)
     cargs, _ = _ctrl_args(ctrl, n_ctrl, ctrl_sigma)
     roff, ridx, rval = _nbhd(reg)
@@ -93,8 +62,8 @@ def solve(dst, dst_n, src, first, second, ctrl, n_ctrl, reg, w_pt=0.0, w_pl=1.0,
           reg_sigma=1.0, ctrl_sigma=1.0, max_gn_iter=10, gn_tol=1e-5, max_cg_iter=1000, cg_tol=1e-5, double=False):
     """estimateSparseWarpFieldCombinedMetric on src (already warped). Returns dict(T (m, 3, 4), x (m, 6), converged,
     gn_steps, cg_iterations, cg_iterations_last, cg_error)."""
-    dst, src = _f32(dst), _f32(src)
-    dn = None if dst_n is None else _f32(dst_n)
+    dst, src = _rows(dst), _rows(src)
+    dn = None if dst_n is None else _rows(dst_n)
     m = int(n_ctrl)
     cargs, _ = _ctrl_args(ctrl, n_ctrl, ctrl_sigma)
     roff, ridx, rval = _nbhd(reg)
@@ -120,9 +89,7 @@ def icp(dst, dst_n, src, ctrl, n_ctrl, reg, knn=None, T_init=None, max_iter=15, 
     then per iteration the 1-NN of T_i s_i within max_d2, the estimator (solve(), kw = its parameters), the nodes'
     T_j <- rotation(dT_j T_j) and the resampling again. Returns dict(T, T_dense, iterations, converged, last_delta,
     num_corr, gn_steps, cg_iterations, first, second)."""
-    import oracle
-
-    dst, src = _f32(dst), _f32(src)
+    dst, src = _rows(dst), _rows(src)
     knn = knn or oracle.BruteKnn(dst)
     n, m = src.shape[0], int(n_ctrl)
     T = np.tile(np.hstack([np.eye(3), np.zeros((3, 1))]).astype(np.float32), (m, 1, 1)) if T_init is None else \

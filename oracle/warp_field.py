@@ -1,6 +1,6 @@
 """ORACLE — test infrastructure, NOT product code: ctypes binding of the dense warp-field restatement
-(oracle/warp_field_oracle.cpp -> oracle/libwarp_oracle.so, built on first use or by build()) and the serial ICP loop
-of CombinedMetricDenseWarpFieldICP on the oracle's brute-force 1-NN.
+(oracle/warp_field_oracle.cpp -> oracle/libwarp_oracle.so, built by oracle/Makefile on first use or by oracle.build())
+and the serial ICP loop of CombinedMetricDenseWarpFieldICP on the oracle's brute-force 1-NN.
 
     from oracle import warp_field
     warp_field.icp(dst, dst_n, src, nbhd, max_iter=5, w_pt=0.1, stiffness=200.0)
@@ -9,56 +9,20 @@ Transforms are (n, 3, 4) float32 arrays, one [R | t] per source point. nbhd = (o
 cb_warp_icp_create.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "warp_field_oracle.cpp")
-_LIB_PATH = os.path.join(_HERE, "libwarp_oracle.so")
-_lib = None
-
-FLT_MAX = float(np.finfo(np.float32).max)
-
-
-def build(force=False):
-    deps = [_SRC, os.path.join(_HERE, "small_linalg.hpp")]
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(d) for d in deps):
-        env = dict(os.environ)
-        env.pop("CXX", None)
-        tmp = _LIB_PATH + f".{os.getpid()}.tmp"
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fPIC", "-shared",
-                               "-fvisibility=hidden", "-Wall", "-o", tmp, _SRC], env=env)
-        os.replace(tmp, _LIB_PATH)
+import oracle
+from oracle import FLT_MAX, _p, _rows, rbf_coeff
+from oracle import build  # noqa: F401 (oracle.build: every library, also callable as <submodule>.build)
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(_LIB_PATH):
-            build()
-        _lib = C.CDLL(_LIB_PATH)
-        _lib.orc_warp_solve.restype = C.c_int
-        _lib.orc_warp_system.restype = C.c_size_t
-        _lib.orc_warp_huber.restype = C.c_float
-        _lib.orc_warp_huber.argtypes = [C.c_float, C.c_float, C.c_int]
-        _lib.orc_warp_rotation_terms.argtypes = [C.c_double, C.c_double, C.c_double, C.c_void_p]
-        _lib.orc_warp_compose.restype = C.c_float
-    return _lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p) if a is not None else None
-
-
-def _f32(a):
-    return np.ascontiguousarray(a, np.float32).reshape(-1, 3)
-
-
-def rbf_coeff(sigma):
-    sg = np.float32(sigma)
-    return float(np.float32(-0.5) / (sg * sg))
+    return oracle.load("libwarp_oracle.so",
+                       {"orc_warp_solve": C.c_int, "orc_warp_system": C.c_size_t, "orc_warp_huber": C.c_float,
+                        "orc_warp_compose": C.c_float},
+                       {"orc_warp_huber": [C.c_float, C.c_float, C.c_int],
+                        "orc_warp_rotation_terms": [C.c_double, C.c_double, C.c_double, C.c_void_p]})
 
 
 def _nbhd(nbhd):
@@ -81,7 +45,7 @@ def rotation_terms(a, b, c):
 def apply(T, pts):
     """T_i p_i for every point, in the device's float order: (R_r0 x + (R_r1 y + R_r2 z)) + t_r."""
     T = np.asarray(T, np.float32).reshape(-1, 3, 4)
-    p = _f32(pts)
+    p = _rows(pts)
     x, y, z = p[:, 0], p[:, 1], p[:, 2]
     return np.stack([(T[:, r, 0] * x + (T[:, r, 1] * y + T[:, r, 2] * z)) + T[:, r, 3] for r in range(3)], 1)
 
@@ -89,8 +53,8 @@ def apply(T, pts):
 def system(dst, dst_n, src, first, second, nbhd, x, w_pt=0.0, w_pl=1.0, stiffness=1.0, huber_delta=1e-4,
            reg_sigma=1.0):
     """The normal equations in double at the unknowns x (n, 6): dict(B (n, 21), g (n, 6), diag (n, 6), arc_c, lo, hi)."""
-    dst, src = _f32(dst), _f32(src)
-    dn = None if dst_n is None else _f32(dst_n)
+    dst, src = _rows(dst), _rows(src)
+    dn = None if dst_n is None else _rows(dst_n)
     n = src.shape[0]
     off, idx, val = _nbhd(nbhd)
     f = np.ascontiguousarray(first, np.uint64)
@@ -110,8 +74,8 @@ def solve(dst, dst_n, src, first, second, nbhd, w_pt=0.0, w_pl=1.0, stiffness=1.
           max_gn_iter=10, gn_tol=1e-5, max_cg_iter=1000, cg_tol=1e-5, double=False):
     """estimateDenseWarpFieldCombinedMetric on src (already transformed). Returns dict(T (n, 3, 4), converged,
     gn_steps, cg_iterations, cg_iterations_last, cg_error, x (n, 6): the unknowns rounded to float)."""
-    dst, src = _f32(dst), _f32(src)
-    dn = None if dst_n is None else _f32(dst_n)
+    dst, src = _rows(dst), _rows(src)
+    dn = None if dst_n is None else _rows(dst_n)
     n = src.shape[0]
     off, idx, val = _nbhd(nbhd)
     f = np.ascontiguousarray(first, np.uint64)
@@ -141,9 +105,7 @@ def icp(dst, dst_n, src, nbhd, knn=None, T_init=None, max_iter=15, tol=1e-5, max
     """CombinedMetricDenseWarpFieldICP::estimate() (icp_base.hpp:68-87): per iteration the 1-NN of T_i s_i within
     max_d2, the estimator (solve(), kw = its parameters), then T_i <- rotation(dT_i T_i). Returns dict(T, iterations,
     converged, last_delta, num_corr, gn_steps, cg_iterations, first, second)."""
-    import oracle
-
-    dst, src = _f32(dst), _f32(src)
+    dst, src = _rows(dst), _rows(src)
     knn = knn or oracle.BruteKnn(dst)
     n = src.shape[0]
     T = np.tile(np.hstack([np.eye(3), np.zeros((3, 1))]).astype(np.float32), (n, 1, 1)) if T_init is None else \
@@ -171,9 +133,7 @@ def icp(dst, dst_n, src, nbhd, knn=None, T_init=None, max_iter=15, tol=1e-5, max
 def residuals(dst, dst_n, src, T, w_pt=0.0, w_pl=1.0):
     """computeResiduals (:216-236) in the device's float order: unbounded 1-NN of T_i s_i,
     w_pt |e|^2 + (w_pl pd) pd with e = d - p, |e|^2 = e0^2 + (e1^2 + e2^2), pd = n0 e0 + (n1 e1 + n2 e2)."""
-    import oracle
-
-    dst = _f32(dst)
+    dst = _rows(dst)
     q = apply(T, src)
     if dst.shape[0] == 0:
         return np.full(q.shape[0], np.nan, np.float32)
@@ -182,6 +142,6 @@ def residuals(dst, dst_n, src, T, w_pt=0.0, w_pl=1.0):
     sq = e[:, 0] * e[:, 0] + (e[:, 1] * e[:, 1] + e[:, 2] * e[:, 2])
     if dst_n is None:
         return np.float32(w_pt) * sq
-    nn = _f32(dst_n)[np.maximum(idx, 0)]
+    nn = _rows(dst_n)[np.maximum(idx, 0)]
     pd = nn[:, 0] * e[:, 0] + (nn[:, 1] * e[:, 1] + nn[:, 2] * e[:, 2])
     return np.float32(w_pt) * sq + (np.float32(w_pl) * pd) * pd

@@ -6,22 +6,17 @@ and an inflated radius that must be caught. No GPU involved; the device side of 
 tests/test_gpu_loop.py (cache equals a fresh exact search, loops bit-identical with the host-driven loop)."""
 import os
 import re
-import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "cilantro_b200", "csrc")
+import cxx
+
+ROOT, CSRC = cxx.ROOT, cxx.CSRC
 
 
 def test_cache_rule_against_brute_force_on_the_host(tmp_path):
-    exe = str(tmp_path / "test_cache_rule")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-frounding-math", "-ffp-contract=off", "-Wall", "-I", CSRC,
-                           os.path.join(ROOT, "tests", "cpp", "test_cache_rule.cpp"), "-o", exe], env=env)
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "all cache-rule checks passed" in out.stdout and "FAIL" not in out.stdout
+    exe = cxx.build(os.path.join(ROOT, "tests", "cpp", "test_cache_rule.cpp"), str(tmp_path / "test_cache_rule"),
+                    ["-O2", "-frounding-math", "-ffp-contract=off", "-Wall", "-I", CSRC], link=False)
+    out = cxx.run(exe, timeout=600)
+    assert "all cache-rule checks passed" in out and "FAIL" not in out
 
 
 def test_the_cached_pass_kernel_compiles_the_same_rule():

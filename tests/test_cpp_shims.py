@@ -1,62 +1,42 @@
 """The C++ drop-in surface (include/cilantro/*.hpp over the C ABI): compiles without Eigen on CPU;
 on the GPU box the reference-example calls in tests/cpp/test_shims.cpp run end to end."""
 import os
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import cxx
+
+ROOT = cxx.ROOT
 SRC = os.path.join(ROOT, "tests", "cpp", "test_shims.cpp")
-INC = os.path.join(ROOT, "include")
-LIBDIR = os.path.join(ROOT, "cilantro_b200")
-
-
-def _env():
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    return env
 
 
 def test_shim_headers_compile_without_eigen():
-    subprocess.check_call(["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-I", INC, SRC], env=_env())
+    r = cxx.syntax(SRC)
+    assert r.returncode == 0, r.stderr
 
 
 @pytest.mark.gpu
 def test_reference_examples_through_cpp_shims(cb, tmp_path):
-    exe = str(tmp_path / "test_shims")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, SRC, "-o", exe, "-L", LIBDIR, "-lcilantro_b200",
-                           f"-Wl,-rpath,{LIBDIR}"], env=_env())
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "all C++ shim checks passed" in out.stdout
+    out = cxx.run(cxx.build(SRC, str(tmp_path / "test_shims")))
+    assert "all C++ shim checks passed" in out
 
 
 def test_eigen_adapters_type_check(tmp_path):
     """The `#if __has_include(<Eigen/Dense>)` adapters (VectorSet / ConstVectorSetMatrixMap / RigidTransform <-> Eigen).
     Eigen3 is absent from this image: they are compiled against tests/cpp/eigen_stub (a minimal stand-in with Eigen's
     layout and accessor names), or against the real Eigen where one is installed; host-only, no device call."""
-    have_real = subprocess.run(["g++", "-std=c++17", "-E", "-x", "c++", "-"], input="#include <Eigen/Dense>\n", text=True,
-                               capture_output=True, env=_env()).returncode == 0
-    inc = ["-I", INC] + ([] if have_real else ["-I", os.path.join(ROOT, "tests", "cpp", "eigen_stub")])
-    exe = str(tmp_path / "test_eigen_adapters")
-    subprocess.check_call(["g++", "-std=c++17", "-Wall", *inc, os.path.join(ROOT, "tests", "cpp", "test_eigen_adapters.cpp"),
-                           "-o", exe, "-L", LIBDIR, "-lcilantro_b200", f"-Wl,-rpath,{LIBDIR}"], env=_env())
-    assert subprocess.run([exe]).returncode == 0
+    exe = cxx.build(os.path.join(ROOT, "tests", "cpp", "test_eigen_adapters.cpp"),
+                    str(tmp_path / "test_eigen_adapters"), ["-Wall", *cxx.eigen_flags()])
+    cxx.run(exe)
 
 
 def test_example_program_compiles():
-    subprocess.check_call(["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-I", INC,
-                           os.path.join(ROOT, "examples", "register_clouds.cpp")], env=_env())
+    r = cxx.syntax(os.path.join(ROOT, "examples", "register_clouds.cpp"))
+    assert r.returncode == 0, r.stderr
 
 
 @pytest.mark.gpu
 def test_example_program_registers_a_synthetic_pair(cb, tmp_path):
-    exe = str(tmp_path / "register_clouds")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, os.path.join(ROOT, "examples", "register_clouds.cpp"),
-                           "-o", exe, "-L", LIBDIR, "-lcilantro_b200", f"-Wl,-rpath,{LIBDIR}"], env=_env())
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=300, cwd=str(tmp_path))
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "wrote registered.ply" in out.stdout and os.path.exists(tmp_path / "registered.ply")
+    exe = cxx.build(os.path.join(ROOT, "examples", "register_clouds.cpp"), str(tmp_path / "register_clouds"))
+    out = cxx.run(exe, cwd=str(tmp_path))
+    assert "wrote registered.ply" in out and os.path.exists(tmp_path / "registered.ply")

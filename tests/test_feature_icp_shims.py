@@ -5,45 +5,22 @@ against the Eigen stub and against real Eigen where present; on the GPU the shim
 PointFeaturesAdaptor3f engine gives SimpleCombinedMetricRigidICP3f's, the pre-assembled feature matrix gives what the
 (points, colours, weight) form gives, and the example runs."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import cxx
 from cilantro_b200 import synth
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INC = os.path.join(ROOT, "include")
-LIBDIR = os.path.join(ROOT, "cilantro_b200")
+ROOT = cxx.ROOT
 SHIM = os.path.join(ROOT, "tests", "cpp", "test_feature_icp_shim.cpp")
 EXAMPLE = os.path.join(ROOT, "examples", "colored_icp_cloud.cpp")
 
 
-def _env():
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    return env
-
-
-def _have_real_eigen():
-    return subprocess.run(["g++", "-std=c++17", "-E", "-x", "c++", "-"], input="#include <Eigen/Dense>\n", text=True,
-                          capture_output=True, env=_env()).returncode == 0
-
-
-def _build(src, exe):
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, src, "-o", exe, "-L", LIBDIR, "-lcilantro_b200",
-                           f"-Wl,-rpath,{LIBDIR}"], env=_env())
-    return exe
-
-
 def test_shim_and_example_compile_with_and_without_eigen():
-    incs = [["-I", INC], ["-I", INC] + ([] if _have_real_eigen() else ["-I", os.path.join(ROOT, "tests", "cpp",
-                                                                                           "eigen_stub")])]
-    for inc in incs:
+    for flags in (["-Wall"], ["-Wall", *cxx.eigen_flags()]):
         for path in (SHIM, EXAMPLE):
-            r = subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-Wall", *inc, path], capture_output=True,
-                               text=True, env=_env())
+            r = cxx.syntax(path, flags=flags)
             assert r.returncode == 0, r.stderr
 
 
@@ -57,21 +34,16 @@ def test_adaptor_constructors_match_the_feature_kind(tmp_path):
                    "  cilantro::PointNormalFeaturesAdaptor3f f(p, n, c, 0.5f, 5.0f);\n"
                    "  return 0;\n"
                    "}\n")
-    r = subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-I", INC, str(src)], capture_output=True, text=True,
-                       env=_env())
-    assert r.returncode != 0
+    assert cxx.syntax(str(src), flags=()).returncode != 0
 
 
 def _run_shim(tmp_path, s):
     path = tmp_path / "scene.bin"
     np.concatenate([s[k].reshape(-1) for k in ("dst", "dst_normals", "dst_colors", "src", "src_normals",
                                                "src_colors")]).astype(np.float32).tofile(path)
-    exe = _build(SHIM, str(tmp_path / "shim"))
-    out = subprocess.run([exe, str(path), str(s["dst"].shape[0]), str(s["src"].shape[0])], capture_output=True,
-                         text=True, timeout=300)
-    assert out.returncode == 0, out.stdout + out.stderr
+    out = cxx.run(cxx.build(SHIM, str(tmp_path / "shim")), path, s["dst"].shape[0], s["src"].shape[0])
     runs = {}
-    for line in out.stdout.strip().splitlines():
+    for line in out.strip().splitlines():
         w = line.split()
         runs[w[0]] = (np.array(w[1:13], np.uint64).astype(np.uint32).view(np.float32).reshape(3, 4), int(w[13]),
                       int(w[14]))
@@ -103,7 +75,5 @@ def test_shim_matches_capi(cb, ctx, tmp_path):
 
 @pytest.mark.gpu
 def test_example_runs(tmp_path):
-    exe = _build(EXAMPLE, str(tmp_path / "colored_icp_cloud"))
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600, cwd=tmp_path)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "in-plane offset error" in out.stdout
+    out = cxx.run(cxx.build(EXAMPLE, str(tmp_path / "colored_icp_cloud")), timeout=600, cwd=tmp_path)
+    assert "in-plane offset error" in out

@@ -5,27 +5,22 @@ feature_d2 >= contract_d2(xyz part) that keeps the grid search exact, and for th
 float64. No GPU involved; the device side is tests/test_gpu_feature_icp.py."""
 import os
 import re
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "cilantro_b200", "csrc")
+import cxx
+
+ROOT, CSRC = cxx.ROOT, cxx.CSRC
 NANOFLANN = "/root/reference/include/cilantro/3rd_party/nanoflann"
 
 
 def _run(tmp_path, extra, args=()):
-    exe = str(tmp_path / "test_feature_rule")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-frounding-math", "-ffp-contract=off", "-Wall", "-I", CSRC]
-                          + extra + [os.path.join(ROOT, "tests", "cpp", "test_feature_rule.cpp"), "-o", exe], env=env)
-    out = subprocess.run([exe, *args], capture_output=True, text=True, timeout=600)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "all feature-rule checks passed" in out.stdout and "FAIL" not in out.stdout
-    return out.stdout
+    exe = cxx.build(os.path.join(ROOT, "tests", "cpp", "test_feature_rule.cpp"), str(tmp_path / "test_feature_rule"),
+                    ["-O2", "-frounding-math", "-ffp-contract=off", "-Wall", "-I", CSRC, *extra], link=False)
+    out = cxx.run(exe, *args, timeout=600)
+    assert "all feature-rule checks passed" in out and "FAIL" not in out
+    return out
 
 
 def test_feature_rule_inequality_and_rotation_on_the_host(tmp_path):
@@ -45,7 +40,6 @@ def test_feature_rule_matches_the_prebuilt_reference_bits(tmp_path, orc):
     the reference checkout itself is absent)."""
     from oracle import feature_icp
 
-    feature_icp.build()
     if not feature_icp.have_ref():
         pytest.skip("oracle/_ref was never built (no reference checkout when it was built)")
     path = tmp_path / "samples.bin"

@@ -31,7 +31,6 @@ W_N, W_C = 0.5, 5.0  # the reference example's PointNormalColorFeaturesAdaptor3f
 def F(orc):
     from oracle import feature_icp
 
-    feature_icp.build()
     return feature_icp
 
 

@@ -4,18 +4,16 @@ seeds and a seed list, plus its known answer), the far-query path, NaN / Inf poi
 thousands of coincident converged seeds, clustering chains, forced multi-batch runs and a downsampled cloud that
 never leaves the device; RBF weights within the stated bound; the error cases."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import cxx
 from cilantro_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INC = os.path.join(ROOT, "include")
-LIBDIR = os.path.join(ROOT, "cilantro_b200")
+ROOT = cxx.ROOT
 
 KEYS = ("offsets", "points", "point_to_cluster", "num_clusters", "iterations")
 
@@ -24,7 +22,6 @@ KEYS = ("offsets", "points", "point_to_cluster", "num_clusters", "iterations")
 def ms():
     from oracle import mean_shift
 
-    mean_shift.build()
     return mean_shift
 
 
@@ -212,28 +209,13 @@ def test_large_groups_of_coincident_seeds_are_deduplicated(cb, ctx, ms):
     assert got["gpu_ms"] < 1000.0, got["gpu_ms"]
 
 
-def _cpp_env():
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    return env
-
-
 def test_cpp_shim_runs(cb, tmp_path):
-    exe = str(tmp_path / "test_mean_shift_shim")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, os.path.join(ROOT, "tests", "cpp", "test_mean_shift_shim.cpp"),
-                           "-o", exe, "-L", LIBDIR, "-lcilantro_b200", f"-Wl,-rpath,{LIBDIR}"], env=_cpp_env())
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "all mean-shift shim checks passed" in out.stdout
+    out = cxx.run(cxx.build(os.path.join(ROOT, "tests", "cpp", "test_mean_shift_shim.cpp"),
+                            str(tmp_path / "test_mean_shift_shim")))
+    assert "all mean-shift shim checks passed" in out
 
 
 def test_example_program_finds_the_three_blobs(cb, tmp_path):
-    exe = str(tmp_path / "mean_shift_cloud")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, os.path.join(ROOT, "examples", "mean_shift_cloud.cpp"),
-                           "-o", exe, "-L", LIBDIR, "-lcilantro_b200", f"-Wl,-rpath,{LIBDIR}"], env=_cpp_env())
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=300, cwd=str(tmp_path))
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "clusters found" in out.stdout
+    out = cxx.run(cxx.build(os.path.join(ROOT, "examples", "mean_shift_cloud.cpp"), str(tmp_path / "mean_shift_cloud")),
+                  cwd=str(tmp_path))
+    assert "clusters found" in out

@@ -1,12 +1,11 @@
 """GPU parity of plane RANSAC (cb_plane_score, cb_plane_residuals, cb_ransac_plane) against the oracle
 (oracle/plane_ransac_oracle.cpp) and numpy, and device-versus-host bit identity of the hypothesis fit (plane_fit.hpp)."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
+import cxx
 from cilantro_b200 import synth
 from oracle import ransac_plane as orp
 from test_oracle_ransac_plane import fit_cases, np_residuals, same_bits
@@ -200,20 +199,10 @@ def test_rejected_inputs(cb, ctx):
 
 # ---- the fit header: device build == host build ----------------------------------------------------------------------
 def test_fit_device_bits_equal_host_bits(tmp_path):
-    sys.path.insert(0, ROOT)
-    from cilantro_b200 import build as cb_build
-
     src = os.path.join(ROOT, "tests", "cuda", "plane_fit_harness.cu")
-    inc = "-I" + os.path.join(ROOT, "cilantro_b200", "csrc")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    exe_d, exe_h = str(tmp_path / "fit_dev"), str(tmp_path / "fit_host")
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    for cmd in ([nvcc] + cb_build.NVCC_FLAGS + ["-ccbin", "g++", inc, "-o", exe_d, src],
-                ["g++", "-x", "c++", "-std=c++17", "-O2", inc, "-o", exe_h, src]):
-        r = subprocess.run(cmd, capture_output=True, text=True, env=env)
-        assert r.returncode == 0, r.stdout + r.stderr
+    inc = ["-I" + cxx.CSRC]
+    exe_d = cxx.harness(src, str(tmp_path / "fit_dev"), inc, device=True)
+    exe_h = cxx.harness(src, str(tmp_path / "fit_host"), inc, device=False)
     rng = np.random.default_rng(17)
     cases = fit_cases() + [rng.normal(size=(3, 3)) * 10.0 ** rng.integers(-20, 20) for _ in range(2000)]
     rec = np.zeros((len(cases), 10), F32)
@@ -224,8 +213,7 @@ def test_fit_device_bits_equal_host_bits(tmp_path):
     rec.tofile(tmp_path / "in.bin")
     outs = []
     for exe in (exe_d, exe_h):
-        r = subprocess.run([exe, str(tmp_path / "in.bin"), str(tmp_path / "out.bin")], capture_output=True, text=True)
-        assert r.returncode == 0, r.stdout + r.stderr
+        cxx.run(exe, tmp_path / "in.bin", tmp_path / "out.bin")
         outs.append(np.fromfile(tmp_path / "out.bin", F32).reshape(-1, 4))
     assert same_bits(outs[0], outs[1])
     for i, s in enumerate(cases):  # and both are the oracle's (and numpy's, test_oracle_ransac_plane.py) closed form

@@ -3,18 +3,16 @@ point -> cluster map, cluster count) for every neighbourhood spec x evaluator ki
 analytic answer of synth.segment_scene; a 1-2 M-point check against scipy on the cb_radius_search graph; a 1 M-point
 polyline (one component of diameter 10^6); determinism; the C++ shim and the example program."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import cxx
 import segment_ref as ref
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INC = os.path.join(ROOT, "include")
-LIBDIR = os.path.join(ROOT, "cilantro_b200")
+ROOT = cxx.ROOT
 
 SPECS = {"radius": (0, 1.0), "knn": (8, 0.0), "knn_in_radius": (8, 1.0)}  # radius2 in units of the spacing^2
 
@@ -23,7 +21,6 @@ SPECS = {"radius": (0, 1.0), "knn": (8, 0.0), "knn_in_radius": (8, 1.0)}  # radi
 def seg(orc):
     from oracle import segment
 
-    segment.build()
     return segment
 
 
@@ -215,28 +212,13 @@ def test_outputs_are_bit_identical_from_run_to_run(cb, ctx, scene):
             assert np.array_equal(a[key], b[key]), (kw, key)
 
 
-def _env():
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    return env
-
-
 def test_cpp_shim_runs(cb, tmp_path):
-    exe = str(tmp_path / "test_segment_shim")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, os.path.join(ROOT, "tests", "cpp", "test_segment_shim.cpp"),
-                           "-o", exe, "-L", LIBDIR, "-lcilantro_b200", f"-Wl,-rpath,{LIBDIR}"], env=_env())
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=300)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "all segmentation shim checks passed" in out.stdout
+    out = cxx.run(cxx.build(os.path.join(ROOT, "tests", "cpp", "test_segment_shim.cpp"),
+                            str(tmp_path / "test_segment_shim")))
+    assert "all segmentation shim checks passed" in out
 
 
 def test_example_program_segments_a_synthetic_scene(cb, tmp_path):
-    exe = str(tmp_path / "segment_cloud")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, os.path.join(ROOT, "examples", "segment_cloud.cpp"),
-                           "-o", exe, "-L", LIBDIR, "-lcilantro_b200", f"-Wl,-rpath,{LIBDIR}"], env=_env())
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=300, cwd=str(tmp_path))
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "components found" in out.stdout
+    out = cxx.run(cxx.build(os.path.join(ROOT, "examples", "segment_cloud.cpp"), str(tmp_path / "segment_cloud")),
+                  cwd=str(tmp_path))
+    assert "components found" in out

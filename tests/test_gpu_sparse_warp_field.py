@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import scipy.sparse.linalg as spla
 
+import cxx
 import sparse_warp_field_ref as ref
 from cilantro_b200 import synth
 
@@ -19,7 +20,6 @@ LOOP = dict(max_iter=15, tol=2.5e-3, max_d2=0.02 ** 2)
 def swf(orc):
     from oracle import sparse_warp_field
 
-    sparse_warp_field.build()
     return sparse_warp_field
 
 
@@ -216,32 +216,14 @@ def test_create_destroy_does_not_leak(cb, ctx, case):
     assert free0 - torch.cuda.mem_get_info()[0] < (8 << 20)
 
 
-def _build_and_run(src, exe, cwd):
-    import os
-    import subprocess
-
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    libdir = os.path.join(root, "cilantro_b200")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", os.path.join(root, "include"), src, "-o", exe, "-L",
-                           libdir, "-lcilantro_b200", f"-Wl,-rpath,{libdir}"], env=env)
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600, cwd=cwd)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    return out.stdout
-
-
 def test_cpp_shim_and_example_run(cb, tmp_path):
     import os
 
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = _build_and_run(os.path.join(root, "tests", "cpp", "test_sparse_warp_field_shim.cpp"),
-                         str(tmp_path / "test_sparse_warp_field_shim"), str(tmp_path))
+    out = cxx.run(cxx.build(os.path.join(cxx.ROOT, "tests", "cpp", "test_sparse_warp_field_shim.cpp"),
+                            str(tmp_path / "test_sparse_warp_field_shim")), timeout=600, cwd=str(tmp_path))
     assert "all sparse warp-field shim checks passed" in out
-    out = _build_and_run(os.path.join(root, "examples", "sparse_non_rigid_icp_cloud.cpp"),
-                         str(tmp_path / "sparse_non_rigid_icp_cloud"), str(tmp_path))
+    out = cxx.run(cxx.build(os.path.join(cxx.ROOT, "examples", "sparse_non_rigid_icp_cloud.cpp"),
+                            str(tmp_path / "sparse_non_rigid_icp_cloud")), timeout=600, cwd=str(tmp_path))
     line = [ln for ln in out.splitlines() if ln.startswith("mean residual")][0]
     r0, r1 = (float(v) for v in line.split()[2::2])
     assert r1 < 0.5 * r0, line

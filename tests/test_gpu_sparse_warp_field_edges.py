@@ -47,7 +47,6 @@ REPORT = []
 def swf(orc):
     from oracle import sparse_warp_field
 
-    sparse_warp_field.build()
     return sparse_warp_field
 
 

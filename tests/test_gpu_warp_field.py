@@ -1,17 +1,15 @@
 """Dense rigid warp-field ICP on the device (cb_warp_icp_*) against the serial oracle (oracle/warp_field_oracle.cpp,
 in fp32 and fp64) and scipy."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 import scipy.sparse.linalg as spla
 
+import cxx
 from cilantro_b200 import synth
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INC = os.path.join(ROOT, "include")
-LIBDIR = os.path.join(ROOT, "cilantro_b200")
+ROOT = cxx.ROOT
 
 pytestmark = pytest.mark.gpu
 
@@ -25,7 +23,6 @@ RECIPE = dict(w_pt=0.1, w_pl=1.0, stiffness=200.0, max_gn_iter=1, gn_tol=5e-4, m
 def wf(orc):
     from oracle import warp_field
 
-    warp_field.build()
     return warp_field
 
 
@@ -218,27 +215,15 @@ def test_non_finite_points_and_zero_cg_iterations(cb, ctx, orc, wf, pair):
     assert z["cg_iterations"] == 0 and np.array_equal(z["T"], identities(src.shape[0]))
 
 
-def _build_and_run(src, exe, cwd):
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, src, "-o", exe, "-L", LIBDIR, "-lcilantro_b200",
-                           f"-Wl,-rpath,{LIBDIR}"], env=env)
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600, cwd=cwd)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    return out.stdout
-
-
 def test_cpp_shim_runs(cb, tmp_path):
-    out = _build_and_run(os.path.join(ROOT, "tests", "cpp", "test_warp_field_shim.cpp"),
-                         str(tmp_path / "test_warp_field_shim"), str(tmp_path))
+    out = cxx.run(cxx.build(os.path.join(ROOT, "tests", "cpp", "test_warp_field_shim.cpp"),
+                            str(tmp_path / "test_warp_field_shim")), timeout=600, cwd=str(tmp_path))
     assert "all warp-field shim checks passed" in out
 
 
 def test_example_program_registers_the_synthetic_pair(cb, tmp_path):
-    out = _build_and_run(os.path.join(ROOT, "examples", "non_rigid_icp_cloud.cpp"), str(tmp_path / "non_rigid_icp_cloud"),
-                         str(tmp_path))
+    out = cxx.run(cxx.build(os.path.join(ROOT, "examples", "non_rigid_icp_cloud.cpp"),
+                            str(tmp_path / "non_rigid_icp_cloud")), timeout=600, cwd=str(tmp_path))
     line = [ln for ln in out.splitlines() if ln.startswith("mean residual")][0]
     r0, r1 = (float(v) for v in line.split()[2::2])
     assert r1 < 0.5 * r0, line

@@ -41,7 +41,6 @@ REPORT = []
 def wf(orc):
     from oracle import warp_field
 
-    warp_field.build()
     return warp_field
 
 

@@ -4,22 +4,17 @@ libstdc++ (std::minstd_rand0, std::uniform_int_distribution<size_t>), the select
 subset size and the 3x3 determinant and inverse against float64. No GPU involved."""
 import os
 import re
-import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "cilantro_b200", "csrc")
+import cxx
+
+ROOT, CSRC = cxx.ROOT, cxx.CSRC
 
 
 def test_mcd_rule_matches_libstdcxx_and_float64(tmp_path):
-    exe = str(tmp_path / "test_mcd_rule")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-Wall", "-I", CSRC,
-                           os.path.join(ROOT, "tests", "cpp", "test_mcd_rule.cpp"), "-o", exe], env=env)
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "all mcd-rule checks passed" in out.stdout and "FAIL" not in out.stdout
+    exe = cxx.build(os.path.join(ROOT, "tests", "cpp", "test_mcd_rule.cpp"), str(tmp_path / "test_mcd_rule"),
+                    ["-O2", "-ffp-contract=off", "-Wall", "-I", CSRC], link=False)
+    out = cxx.run(exe, timeout=600)
+    assert "all mcd-rule checks passed" in out and "FAIL" not in out
 
 
 def test_the_kernel_uses_the_shared_rule():

@@ -14,7 +14,6 @@ KINDS = ["point_normal", "point_color", "point_normal_color"]
 def F(orc):
     from oracle import feature_icp
 
-    feature_icp.build()
     return feature_icp
 
 

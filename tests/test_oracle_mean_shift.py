@@ -14,7 +14,6 @@ KEYS = ("offsets", "points", "point_to_cluster", "num_clusters", "iterations")
 def ms():
     from oracle import mean_shift
 
-    mean_shift.build()
     return mean_shift
 
 

@@ -11,7 +11,6 @@ import segment_ref as ref
 def seg(orc):
     from oracle import segment
 
-    segment.build()
     return segment
 
 

@@ -13,7 +13,6 @@ KW = dict(w_pt=0.1, w_pl=1.0, stiffness=200.0, huber=1e-2, reg_sigma=0.075, ctrl
 def swf():
     from oracle import sparse_warp_field
 
-    sparse_warp_field.build()
     return sparse_warp_field
 
 

@@ -13,7 +13,6 @@ from cilantro_b200 import synth
 def wf(orc):
     from oracle import warp_field
 
-    warp_field.build()
     return warp_field
 
 

@@ -1,23 +1,16 @@
 """Host-only: the PLY passthrough of the PointCloud3f shim (tests/cpp/test_ply.cpp) — round trips in ascii and
 binary, a hand-written file with another property layout and a face element, append / clear, a missing file."""
 import os
-import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import cxx
+
+ROOT = cxx.ROOT
+PLY = os.path.join(ROOT, "tests", "cpp", "test_ply.cpp")
 
 
 def test_ply_passthrough(tmp_path):
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    exe = str(tmp_path / "test_ply")
-    lib = os.path.join(ROOT, "cilantro_b200")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "test_ply.cpp"), "-o", exe, "-L", lib, "-lcilantro_b200",
-                           f"-Wl,-rpath,{lib}"], env=env)
-    out = subprocess.run([exe, str(tmp_path)], capture_output=True, text=True, timeout=120)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "PLY checks passed" in out.stdout
+    out = cxx.run(cxx.build(PLY, str(tmp_path / "test_ply"), ["-O1", "-Wall"]), tmp_path, timeout=120)
+    assert "PLY checks passed" in out
 
 
 def test_reads_the_reference_scans(tmp_path):
@@ -29,17 +22,8 @@ def test_reads_the_reference_scans(tmp_path):
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     from golden.make_config1_fixture import EXCERPT as scan, read_test_ply
 
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    exe = str(tmp_path / "test_ply")
-    lib = os.path.join(ROOT, "cilantro_b200")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "test_ply.cpp"), "-o", exe, "-L", lib, "-lcilantro_b200",
-                           f"-Wl,-rpath,{lib}"], env=env)
-    out = subprocess.run([exe, str(tmp_path), scan], capture_output=True, text=True, timeout=120)
-    assert out.returncode == 0, out.stdout + out.stderr
-    lines = out.stdout.strip().splitlines()
+    out = cxx.run(cxx.build(PLY, str(tmp_path / "test_ply"), ["-O1"]), tmp_path, scan, timeout=120)
+    lines = out.strip().splitlines()
     p, n, c = read_test_ply(scan)
     assert lines[0].split() == ["scan", str(p.shape[0]), "1", "1"]
     for ln in lines[1:]:

@@ -2,37 +2,21 @@
 PointCloud3f index subsets: they compile without Eigen, and on the GPU the shim gives what capi gives, estimateModel
 is cb_pca's plane, the subsets follow the reference's set semantics, and the example runs."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import cxx
 from cilantro_b200 import synth
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INC = os.path.join(ROOT, "include")
-LIBDIR = os.path.join(ROOT, "cilantro_b200")
+ROOT = cxx.ROOT
 SHIM = os.path.join(ROOT, "tests", "cpp", "test_ransac_plane_shim.cpp")
 EXAMPLE = os.path.join(ROOT, "examples", "ransac_plane_cloud.cpp")
 
 
-def _env():
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    return env
-
-
-def _build(src, exe):
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-I", INC, src, "-o", exe, "-L", LIBDIR, "-lcilantro_b200",
-                           f"-Wl,-rpath,{LIBDIR}"], env=_env())
-    return exe
-
-
 def test_shim_and_example_compile_without_eigen():
     for path in (SHIM, EXAMPLE):
-        r = subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-I", INC, path], capture_output=True, text=True,
-                           env=_env())
+        r = cxx.syntax(path)
         assert r.returncode == 0, r.stderr
 
 
@@ -65,10 +49,8 @@ def ref_remove(n, idx):
 def test_shim_matches_capi(cb, ctx, tmp_path):
     pts = synth.plane_scene(30000, seed=4)["points"]
     pts.tofile(tmp_path / "pts.bin")
-    exe = _build(SHIM, str(tmp_path / "shim"))
-    out = subprocess.run([exe, str(tmp_path / "pts.bin"), "6"], capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stdout + out.stderr
-    rows = {ln.split()[0]: ln.split()[1:] for ln in out.stdout.splitlines() if ln.strip()}
+    out = cxx.run(cxx.build(SHIM, str(tmp_path / "shim")), tmp_path / "pts.bin", 6)
+    rows = {ln.split()[0]: ln.split()[1:] for ln in out.splitlines() if ln.strip()}
     cloud = cb.Cloud(ctx, pts)
     got = cb.ransac_plane(ctx, cloud, 6, max_iter=250, thresh=0.01, inlier_count_thresh=int(0.15 * 30000),
                           re_estimate=False)
@@ -94,9 +76,7 @@ def test_shim_matches_capi(cb, ctx, tmp_path):
 
 @pytest.mark.gpu
 def test_example_runs(cb, tmp_path):
-    exe = _build(EXAMPLE, str(tmp_path / "ransac_plane_cloud"))
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=300, cwd=str(tmp_path))
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "RANSAC iterations:" in out.stdout and "left" in out.stdout
-    line = [ln for ln in out.stdout.splitlines() if ln.startswith("plane:")][0]
+    out = cxx.run(cxx.build(EXAMPLE, str(tmp_path / "ransac_plane_cloud")), cwd=str(tmp_path))
+    assert "RANSAC iterations:" in out and "left" in out
+    line = [ln for ln in out.splitlines() if ln.startswith("plane:")][0]
     assert abs(abs(float(line.split()[3])) - 1.0) < 1e-3  # the floor, z = 0

@@ -2,22 +2,13 @@
 connected_component_extraction.hpp) compiles without Eigen, together with the example program; the GPU run of both is
 in tests/test_gpu_segment.py."""
 import os
-import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INC = os.path.join(ROOT, "include")
-
-
-def _env():
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    return env
+from cxx import ROOT, syntax
 
 
 def test_segment_shim_compiles_without_eigen():
-    subprocess.check_call(["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-I", INC,
-                           os.path.join(ROOT, "tests", "cpp", "test_segment_shim.cpp")], env=_env())
+    r = syntax(os.path.join(ROOT, "tests", "cpp", "test_segment_shim.cpp"))
+    assert r.returncode == 0, r.stderr
 
 
 def test_evaluators_compile_from_the_reference_include_path():
@@ -26,14 +17,13 @@ def test_evaluators_compile_from_the_reference_include_path():
            "  cilantro::NormalsProximityEvaluator<float, 3> a(n, 0.1f); cilantro::ColorsProximityEvaluator<float> b(c, 0.1f);\n"
            "  cilantro::PointsNormalsColorsProximityEvaluator<float, 3> d(n, c, 1.f, 0.1f, 0.1f);\n"
            "  return cilantro::AlwaysTrueEvaluator<float>()(0, 1, 0.f) ? 0 : 1; }\n")
-    r = subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-I", INC, "-x", "c++", "-"], input=src, text=True,
-                       capture_output=True, env=_env())
+    r = syntax(src=src)
     assert r.returncode == 0, r.stderr
 
 
 def test_segment_example_compiles():
-    subprocess.check_call(["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-I", INC,
-                           os.path.join(ROOT, "examples", "segment_cloud.cpp")], env=_env())
+    r = syntax(os.path.join(ROOT, "examples", "segment_cloud.cpp"))
+    assert r.returncode == 0, r.stderr
 
 
 def test_an_evaluator_without_a_device_mapping_is_a_compile_error():
@@ -42,6 +32,5 @@ def test_an_evaluator_without_a_device_mapping_is_a_compile_error():
            "int main() { cilantro::VectorSet3f p(3, 4);\n"
            "  cilantro::ConnectedComponentExtraction3f<>(p).segment(cilantro::RadiusNeighborhoodSpecification<float>(1.f),"
            " MyEvaluator()); }\n")
-    r = subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-I", INC, "-x", "c++", "-"], input=src, text=True,
-                       capture_output=True, env=_env())
+    r = syntax(src=src, flags=())
     assert r.returncode != 0 and "segment_fill" in r.stderr

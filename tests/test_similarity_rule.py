@@ -4,22 +4,18 @@ compiles that header for the host and checks, over every float in [-1, 1], that 
 std::acos (and that acosf is monotone there, which the derivation relies on). No GPU involved."""
 import os
 import re
-import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "cilantro_b200", "csrc")
+import cxx
+
+ROOT, CSRC = cxx.ROOT, cxx.CSRC
 
 
 def test_angle_intervals_match_acos_on_every_float(tmp_path):
-    exe = str(tmp_path / "test_similarity_rule")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    subprocess.check_call(["g++", "-std=c++17", "-O3", "-march=x86-64-v3", "-ffp-contract=off", "-Wall", "-pthread", "-I", CSRC,
-                           os.path.join(ROOT, "tests", "cpp", "test_similarity_rule.cpp"), "-o", exe], env=env)
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=1200)
-    print(out.stdout)
-    assert out.returncode == 0, out.stdout + out.stderr
-    assert "all similarity-rule checks passed" in out.stdout and "FAIL" not in out.stdout
+    exe = cxx.build(os.path.join(ROOT, "tests", "cpp", "test_similarity_rule.cpp"),
+                    str(tmp_path / "test_similarity_rule"),
+                    ["-O3", "-march=x86-64-v3", "-ffp-contract=off", "-Wall", "-pthread", "-I", CSRC], link=False)
+    out = cxx.run(exe, timeout=1200)
+    assert "all similarity-rule checks passed" in out and "FAIL" not in out
 
 
 def test_the_kernel_uses_the_shared_rule():

@@ -14,12 +14,11 @@ cases sit where these solves branch or lose accuracy:
 Each GPU test prints its largest error against float64.
 """
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
+import cxx
 import icp_ref
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -31,23 +30,9 @@ EPS = np.finfo(np.float64).eps
 def build_harness(outdir, device, include_first=()):
     """Compile the harness: nvcc with the library's flags (device) or g++ (host). include_first: directories searched
     before the library's sources (to build the harness against another version of a header)."""
-    sys.path.insert(0, ROOT)
-    from cilantro_b200 import build as cb_build
-
     inc = [f"-I{d}" for d in include_first] + [f"-I{CSRC}"]
-    if device:
-        exe = os.path.join(outdir, "solve_harness_dev")
-        nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-        cmd = [nvcc] + cb_build.NVCC_FLAGS + ["-ccbin", "g++"] + inc + ["-o", exe, HARNESS]
-    else:
-        exe = os.path.join(outdir, "solve_harness_host")
-        cmd = ["g++", "-x", "c++", "-std=c++17", "-O2"] + inc + ["-o", exe, HARNESS]
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    r = subprocess.run(cmd, capture_output=True, text=True, env=env)
-    assert r.returncode == 0, r.stdout + r.stderr
-    return exe
+    exe = os.path.join(outdir, "solve_harness_dev" if device else "solve_harness_host")
+    return cxx.harness(HARNESS, exe, inc, device)
 
 
 def run(exe, mode, cases, tmpdir):
@@ -55,8 +40,7 @@ def run(exe, mode, cases, tmpdir):
     rec = {"rotation": 20, "kabsch": 13, "solve6": 14, "sym3": 7}[mode]
     src, dst = os.path.join(tmpdir, f"{mode}.in"), os.path.join(tmpdir, f"{mode}.out")
     np.ascontiguousarray(cases, dt).tofile(src)
-    r = subprocess.run([exe, mode, src, dst], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
+    cxx.run(exe, mode, src, dst)
     return np.fromfile(dst, dt).reshape(-1, rec)
 
 

@@ -12,7 +12,6 @@ import warp_field_ref
 def wf(orc):
     from oracle import warp_field
 
-    warp_field.build()
     return warp_field
 
 

@@ -2,24 +2,14 @@
 include/cilantro/registration/icp_common_instances.hpp) compiles without Eigen, together with the example program;
 the GPU runs of both are in tests/test_gpu_warp_field.py."""
 import os
-import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INC = os.path.join(ROOT, "include")
+import cxx
 
-
-def _env():
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    return env
+ROOT = cxx.ROOT
 
 
 def _syntax(src_path=None, src=None):
-    cmd = ["g++", "-std=c++17", "-fsyntax-only", "-Wall", "-Werror", "-I", INC]
-    if src is None:
-        return subprocess.run(cmd + [src_path], capture_output=True, text=True, env=_env())
-    return subprocess.run(cmd + ["-x", "c++", "-"], input=src, capture_output=True, text=True, env=_env())
+    return cxx.syntax(src_path, src, flags=("-Wall", "-Werror"))
 
 
 def test_warp_field_shim_and_example_compile_without_eigen():
