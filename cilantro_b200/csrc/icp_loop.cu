@@ -1,14 +1,16 @@
 // Device-resident rigid ICP loop (product code, sm_90a).
 //
 // IterativeClosestPointBase::estimate() (registration/icp_base.hpp:68-87) for the default correspondence engine:
-// ONE kernel per ICP iteration and NO host round trip between iterations. The kernel of iteration k
+// TWO kernels per ICP iteration and NO host round trip between iterations. In iteration k the first kernel
 //   1. reads the current estimate T_k from device memory (LoopState),
 //   2. finds every source point's correspondence under T_k (below),
-//   3. accumulates the estimator's moments and reduces them warp -> block -> grid in a fixed order,
-//   4. in the ONE warp that finishes the grid reduction: all-reduces the 16 / 28 totals with the peer ranks over
-//      NVLink peer memory (reduce.cuh, bounded wait), then solves on the device — Kabsch / one Gauss-Newton step,
-//      rotation() re-orthonormalisation, compose, update norm, convergence test (solve_core.hpp; the same code the
-//      host loop runs) — and writes T_{k+1} back to LoopState.
+//   3. accumulates the estimator's moments, reduces them warp -> block and writes one row per block (the cold search
+//      kernel of the first iteration goes on to the grid total, in rs.result);
+// the finish kernel (one block, launched behind it)
+//   4. folds the block rows into this GPU's 16 / 28 totals in a fixed order, all-reduces them with the peer ranks
+//      over NVLink peer memory (reduce.cuh, bounded wait), then solves on the device — Kabsch / one Gauss-Newton
+//      step, rotation() re-orthonormalisation, compose, update norm, convergence test (solve_core.hpp; the same code
+//      the host loop runs) — and writes T_{k+1} back to LoopState.
 // The host enqueues the launches back to back and reads LoopState once per batch; launches after convergence
 // return at once. With several ranks every rank solves the same totals redundantly -> bit-identical transforms.
 //
@@ -59,7 +61,9 @@ struct LoopArgs {
   float slack_first, slack_min, slack_max;  // widening of the search beyond the nearest distance (warp_search_wide.cuh)
   LoopState* st;
   ReduceScratch rs;
-  int trace;  // CB_LOOP_TRACE: fill LoopState::trace
+  uint32_t rows;  // block rows of the cached pass in rs.partials (its grid size); 0: the cold search kernel's totals
+                  // are in rs.result (enqueue_iteration)
+  int trace;      // CB_LOOP_TRACE: fill LoopState::trace
 };
 
 // per-block copy of the loop state; also the `Args` of accumulate_pair (T, dm, sm, w_pt, w_pl)
@@ -84,9 +88,10 @@ __device__ __forceinline__ Rigid rigid_from_t12_dev(const float* T12) {
 }
 
 // The serial epilogue of an iteration (one thread): totals -> update -> new state. It runs in a kernel of its own
-// (icp_finish_kernel, one warp): inside the search kernel its temporaries were spilled at that kernel's register
-// budget, and a spilled word of ONE thread lives in its own 128-byte line of local memory - after a 10 M-point pass
-// every one of them was a cold DRAM miss (in a %globaltimer trace the solve took many times its arithmetic).
+// (icp_finish_kernel): inside the search kernel its temporaries were spilled at that kernel's register budget, and a
+// local-memory word of ONE thread lives in its own 128-byte line - after a 10 M-point pass every one of them was a
+// cold DRAM miss (in a %globaltimer trace the solve took many times its arithmetic). So nothing here may be indexed
+// at run time (solve_core.hpp picks by selects): the solve keeps its temporaries in registers.
 template <int MODE>
 __device__ __forceinline__ void loop_solve(const LoopArgs* ap, const BlockCtx* cxp, const double* s, int late,
                                         unsigned long long seq) {
@@ -236,8 +241,8 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
 // PERSISTENT: the grid is a whole number of resident blocks per SM, a block walks the tiles blockIdx.x, + gridDim.x,
 // ... (static round-robin: every tile costs the same, and the assignment — hence, with the fixed queue order, the
 // summation order — is fixed), the next tiles' loads are in flight while the current tile is evaluated, and the
-// moments are reduced ONCE per block (a per-tile reduction cost as much as the tile itself). The block rows go through
-// one deterministic grid reduction per iteration into rs.result, read by the finish kernel.
+// moments are reduced ONCE per block (a per-tile reduction cost as much as the tile itself). Every block writes its row
+// to rs.partials (zeros included: the finish kernel folds every row) and is done.
 // The loads are not staged in registers: a register-staged version needed 128 registers -> 2 blocks/SM, few warp
 // slots occupied, long-scoreboard stalls on top - each thread can only keep the loads in flight that it has registers
 // for. Here every thread runs a private three-deep pipeline of cp.async copies into shared memory (LDGSTS: no
@@ -339,7 +344,7 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
   // The dependency wait comes BEFORE the first copies: the cache arrays are rewritten every iteration, their 4-byte
   // copies go through L1 (cp.async.ca), and only accesses after griddepcontrol.wait are guaranteed to see the previous
   // kernels' writes. What programmatic launch buys here: the blocks are resident when the finish kernel ends, and the
-  // one-warp finish kernel of this iteration, released at once, is resident and waiting when this grid drains.
+  // one-block finish kernel of this iteration, released at once, is resident and waiting when this grid drains.
   pdl_wait();
   pdl_launch_dependents();
   stage_a(t0, 0);           // group: A(0)
@@ -444,18 +449,17 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
   }
   if (a.trace && lane == 0) atomicMax(&a.st->trace[__ldcg(&a.st->iters) & 63][5], global_timer_ns());
   warp_sum_to_slot<NV, true>(acc, rsm);
-  double tot = 0;
-  if (!grid_reduce_slots_tail<NV>(a.rs, rsm, tot)) return;
-  // the last warp of the grid hands this GPU's totals to icp_finish_kernel
-  if (lane < NV) a.rs.result[lane] = tot;
-  if (a.trace && lane == 0) a.st->trace[__ldcg(&a.st->iters) & 63][1] = global_timer_ns();
+  double row;
+  if (block_row_from_slots<NV>(rsm, row) && lane < NV) a.rs.partials[(size_t)blockIdx.x * NV + lane] = row;
 }
 
 constexpr int kSearchMinBlocks = 4;  // resident blocks per SM the search kernel's register budget is set for
 
 // ---- the cold iteration (the first of a call: nothing cached yet): search, then the finish kernel -----------------
 // Every query is searched, one 256-query chunk per block, lane-dense; the searching thread accumulates its pair and
-// the last warp of the grid hands this GPU's totals to icp_finish_kernel.
+// the last warp of the grid hands this GPU's totals to icp_finish_kernel in rs.result. This kernel keeps the ticketed
+// grid reduction: its thousands of block rows (39 063 at 10 M queries) are folded group by group as its blocks finish,
+// spread over the SMs; one block folding them all after the grid took 138 us instead of 26 us at 10 M (DESIGN §4.2).
 template <int MODE>
 __global__ void __launch_bounds__(kBlock, kSearchMinBlocks) icp_search_kernel(const __grid_constant__ LoopArgs a) {
   constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
@@ -466,7 +470,7 @@ __global__ void __launch_bounds__(kBlock, kSearchMinBlocks) icp_search_kernel(co
   const unsigned int tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t base = blockIdx.x * kBlock;
   pdl_wait();               // the state of the previous finish kernel
-  pdl_launch_dependents();  // the one-warp finish kernel may be scheduled now and wait for this grid to drain
+  pdl_launch_dependents();  // the finish kernel may be scheduled now and wait for this grid to drain
   if (tid == 0) {
     rsm.arrived = 0u;
     load_block_ctx(a, cx);
@@ -496,32 +500,45 @@ __global__ void __launch_bounds__(kBlock, kSearchMinBlocks) icp_search_kernel(co
     }
   }
   if (a.trace && lane == 0) atomicMax(&a.st->trace[trace_slot][5], global_timer_ns());
-  double tot = 0;
-  if (!grid_reduce_async_tail<NV>(acc, a.rs, rsm, tot)) return;
+  warp_sum_to_slot<NV, false>(acc, rsm);
+  double row, tot = 0;
+  if (!block_row_from_slots<NV>(rsm, row) || !grid_reduce_rows_tail<NV>(row, a.rs, lane, tot)) return;
   if (lane < NV) a.rs.result[lane] = tot;
   if (a.trace && lane == 0) a.st->trace[trace_slot][1] = global_timer_ns();
 }
 
-// ---- kernel 3 of an iteration: exchange + solve (one warp) -------------------------------------------------------------
-// This GPU's totals -> all-reduce with the peer ranks over NVLink peer memory (reduce.cuh, bounded wait; every rank
-// sums the rows in rank order -> bit-identical totals) -> Kabsch / Gauss-Newton step, rotation(), compose,
-// convergence test -> LoopState for the next iteration's kernels.
+// ---- kernel 2 of an iteration: fold + exchange + solve (one block) -----------------------------------------------------
+// The cached pass's block rows (a.rows of them) -> this GPU's totals (block_fold_rows: the whole block, in the fixed
+// order of the grid reduction; after the cold search kernel the totals are read from rs.result) -> all-reduce with the
+// peer ranks over NVLink peer memory (reduce.cuh, bounded wait; every rank sums the rows in rank order ->
+// bit-identical totals) -> Kabsch / Gauss-Newton step, rotation(), compose, convergence test -> LoopState for the next
+// iteration's kernels. Everything after the fold runs in warp 0.
 template <int MODE>
-__global__ void __launch_bounds__(32, 1) icp_finish_kernel(const __grid_constant__ LoopArgs a) {
+__global__ void __launch_bounds__(kBlock, 1) icp_finish_kernel(const __grid_constant__ LoopArgs a) {
   constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
   __shared__ BlockCtx cx;
   __shared__ double sbuf[kCombinedValues + 8];
   static_assert(NV + 2 <= kExchangeVals, "row of the fused exchange");
   const unsigned int lane = threadIdx.x;
-  pdl_wait();               // this GPU's totals (cached pass or cold search kernel), the state of the previous iteration
+  // griddepcontrol.wait returns once the whole grid before (cached pass or cold search kernel) has completed and its
+  // rows are visible; it also orders this kernel after the state of the previous iteration
+  pdl_wait();
   pdl_launch_dependents();  // the next iteration's cached pass may start streaming
-  if (lane == 0) load_block_ctx(a, cx);
-  __syncwarp();
+  if (threadIdx.x == 0) load_block_ctx(a, cx);
+  __syncthreads();
   if (cx.done) return;
+  if (a.rows != 0) {
+    block_fold_rows<NV>(a.rs.partials, a.rows, sbuf);
+  } else if (threadIdx.x < NV) {
+    sbuf[threadIdx.x] = __ldcg(a.rs.result + threadIdx.x);
+  }
+  if (threadIdx.x >= 32) return;
+  __syncwarp();
   const int trace_slot = a.trace ? (__ldcg(&a.st->iters) & 63) : 0;
+  if (a.trace && lane == 0 && a.rows != 0) a.st->trace[trace_slot][1] = global_timer_ns();
   // lanes < NV: the moments; lane NV: queries this rank searched in this iteration; lane NV + 1: its source points
   // (both ride along so that every rank sees the same global search share: the hand-over decision of the host)
-  double tot = (lane < NV) ? __ldcg(a.rs.result + lane) : 0.0;
+  double tot = (lane < NV) ? sbuf[lane] : 0.0;
   if (lane == NV) tot = (double)__ldcg(&a.st->searched_cur);
   if (lane == NV + 1) tot = (double)a.n_src;
   bool late = false;
@@ -581,13 +598,15 @@ static cudaError_t launch_pdl(Kernel k, int blocks, int threads, size_t smem, cu
 // Enqueues the kernels of ICP iteration `it` of this call: the search kernel in the cold first iteration (nothing
 // cached yet), else the cached pass with its search of the flagged queries; then the finish kernel.
 template <int MODE>
-static int enqueue_iteration(cb_context* ctx, const LoopArgs& a, int it, int blocks_cold, int blocks_cached) {
+static int enqueue_iteration(cb_context* ctx, const LoopArgs& args, int it, int blocks_cold, int blocks_cached) {
+  LoopArgs a = args;
+  a.rows = (uint32_t)(it == 0 ? 0 : blocks_cached);  // each block of the cached pass writes one row
   if (it == 0)
     CB_CUDA(launch_pdl(icp_search_kernel<MODE>, blocks_cold, kBlock, 0, ctx->stream, a));
   else
     CB_CUDA(launch_pdl(icp_cached_pipe_kernel<MODE>, blocks_cached, kBlock, sizeof(PipeSmem<MODE == kModeCombined>),
                        ctx->stream, a));
-  CB_CUDA(launch_pdl(icp_finish_kernel<MODE>, 1, 32, 0, ctx->stream, a));
+  CB_CUDA(launch_pdl(icp_finish_kernel<MODE>, 1, kBlock, 0, ctx->stream, a));
   ctx->launches += 2;
   return CB_OK;
 }

@@ -287,10 +287,11 @@ __device__ __forceinline__ void warp_sum_to_slot(double (&acc)[NV], AsyncReduceS
   __syncwarp();
 }
 
-// Block and grid levels once every warp of the block has filled its slot (warp_sum_to_slot): same return value as
-// grid_reduce_async_tail.
+// Block level once every warp of the block has filled its slot (warp_sum_to_slot): returns true on exactly one warp
+// of the block - the last to arrive - with `row` = the block's total of value `lane` (lane < NV; zero on the other
+// lanes). Fixed order.
 template <int NV>
-__device__ __forceinline__ bool grid_reduce_slots_tail(const ReduceScratch& rs, AsyncReduceSmem<NV>& sm, double& tot) {
+__device__ __forceinline__ bool block_row_from_slots(AsyncReduceSmem<NV>& sm, double& row) {
   const int lane = threadIdx.x & 31;
   constexpr int kWarps = kReduceBlock / 32;
   unsigned int t = 0;
@@ -301,33 +302,85 @@ __device__ __forceinline__ bool grid_reduce_slots_tail(const ReduceScratch& rs, 
   t = __shfl_sync(0xffffffffu, t, 0);
   if (t != kWarps - 1) return false;
   __threadfence_block();
-  // last warp of the block: block row
-  double row = 0;
+  row = 0;
   if (lane < NV) {
 #pragma unroll
     for (int w = 0; w < kWarps; w++) row += ((volatile double*)sm.slot[w])[lane];
   }
-  return grid_reduce_rows_tail<NV>(row, rs, lane, tot);
+  return true;
 }
 
-// Returns true on exactly ONE warp of the grid - the last to arrive - with `tot` = this GPU's total of value
-// `lane` (lane < NV); every other warp returns false as soon as its part is done. The caller continues alone on
-// that warp (exchange, publication, the device-resident solve of icp_loop.cu).
-template <int NV>
-__device__ __forceinline__ bool grid_reduce_async_tail(double (&acc)[NV], const ReduceScratch& rs, AsyncReduceSmem<NV>& sm,
-                                                       double& tot) {
-  warp_sum_to_slot<NV, false>(acc, sm);
-  return grid_reduce_slots_tail<NV>(rs, sm, tot);
-}
-
-// ... -> (optional) fused all-reduce over NVLink peer memory -> device result + mapped host mailbox
+// warp -> block -> group -> grid without a barrier (the last warp of the grid carries on alone) -> (optional) fused
+// all-reduce over NVLink peer memory -> device result + mapped host mailbox
 template <int NV>
 __device__ __forceinline__ void grid_reduce_async(double (&acc)[NV], const ReduceScratch& rs, AsyncReduceSmem<NV>& sm) {
   const int lane = threadIdx.x & 31;
-  double tot = 0;
-  if (!grid_reduce_async_tail<NV>(acc, rs, sm, tot)) return;
+  warp_sum_to_slot<NV, false>(acc, sm);
+  double row, tot = 0;
+  if (!block_row_from_slots<NV>(sm, row)) return;
+  if (!grid_reduce_rows_tail<NV>(row, rs, lane, tot)) return;
   tot = exchange_and_publish<NV>(tot, rs, lane);
   if (lane < NV) rs.result[lane] = tot;
+}
+
+// ---- one block folds a whole grid's rows ------------------------------------------------------------------------
+// Sums rows 0 .. rows-1 of a [rows][NV] table (one row per block of the kernel that ran before; launched after it,
+// so no ticket is needed) with the kReduceBlock threads of ONE block, into out[NV] (shared memory). The result is
+// bit-identical to the two ticketed levels of grid_reduce_rows_tail: groups of kReduceGroup consecutive rows, each
+// summed by warp_sum_rows' rule (NV <= 16: even and odd rows separately in ascending order, then even + odd; else
+// ascending), then the group rows by the same rule.
+// Thread work item: (group, parity, pair of adjacent values); its rows are loaded 16 B at a time, kFoldBatch of them in
+// flight, and added in ascending order. A round covers the groups that one item per thread reaches; the round's
+// group rows go through shared memory to the threads that carry the grid-level sums, in ascending group order.
+template <int NV>
+__device__ __forceinline__ void block_fold_rows(const double* __restrict__ table, unsigned int rows, double* out) {
+  static_assert(NV % 2 == 0, "values are loaded in pairs");
+  constexpr int kPar = (NV <= 16) ? 2 : 1;                 // parities summed apart (warp_sum_rows)
+  constexpr int kPairs = NV / 2;
+  constexpr int kItemsPerGroup = kPar * kPairs;
+  constexpr int kRoundGroups = kReduceBlock / kItemsPerGroup;  // even: group parity = parity within the round
+  constexpr int kFoldBatch = 32;
+  static_assert(kRoundGroups % 2 == 0, "group parity");
+  __shared__ double part[kRoundGroups][kPar][NV];
+  __shared__ double grid_par[kPar][NV];
+  const unsigned int tid = threadIdx.x;
+  const unsigned int ngroups = (rows + kReduceGroup - 1) / kReduceGroup;
+  const unsigned int gl = tid / kItemsPerGroup, par = (tid % kItemsPerGroup) / kPairs, v = 2 * (tid % kPairs);
+  double acc = 0;  // grid level: thread tid < kPar * NV sums value tid % NV over the groups of parity tid / NV
+  for (unsigned int g0 = 0; g0 < ngroups; g0 += kRoundGroups) {
+    const unsigned int g = g0 + gl;
+    if (gl < kRoundGroups && g < ngroups) {
+      const unsigned int r1 = min(rows, (g + 1) * kReduceGroup);
+      double sx = 0, sy = 0;
+      for (unsigned int r = g * kReduceGroup + par; r < r1; r += kFoldBatch * kPar) {
+        double2 t[kFoldBatch];
+#pragma unroll
+        for (int u = 0; u < kFoldBatch; u++) {
+          const unsigned int b = r + u * kPar;
+          if (b < r1) t[u] = __ldcg(reinterpret_cast<const double2*>(table + (size_t)b * NV + v));
+        }
+#pragma unroll
+        for (int u = 0; u < kFoldBatch; u++)
+          if (r + u * kPar < r1) {
+            sx += t[u].x;
+            sy += t[u].y;
+          }
+      }
+      part[gl][par][v] = sx;
+      part[gl][par][v + 1] = sy;
+    }
+    __syncthreads();
+    if (tid < kPar * NV) {
+      const unsigned int p = tid / NV, i = tid % NV;
+      for (unsigned int k = p; k < kRoundGroups && g0 + k < ngroups; k += kPar)
+        acc += (kPar == 2) ? part[k][0][i] + part[k][kPar - 1][i] : part[k][0][i];
+    }
+    __syncthreads();
+  }
+  if (tid < kPar * NV) grid_par[tid / NV][tid % NV] = acc;
+  __syncthreads();
+  if (tid < NV) out[tid] = (kPar == 2) ? grid_par[0][tid] + grid_par[kPar - 1][tid] : grid_par[0][tid];
+  __syncthreads();
 }
 
 }  // namespace cb

@@ -91,22 +91,30 @@ CB_HD Svd svd_hestenes(const Mat3& A) {
     if (!rotated) break;
   }
   double nrm[3];
-  int order[3] = {0, 1, 2};
   for (int j = 0; j < 3; j++) nrm[j] = sqrt(G[0][j] * G[0][j] + G[1][j] * G[1][j] + G[2][j] * G[2][j]);
-  // stable descending order of three values (insertion)
-  for (int a = 1; a < 3; a++)
-    for (int b = a; b > 0 && nrm[order[b]] > nrm[order[b - 1]]; b--) {
-      const int t = order[b];
-      order[b] = order[b - 1];
-      order[b - 1] = t;
+  // stable descending order of three values (insertion sort as compare-exchanges). Columns are picked with selects,
+  // not indexed by the order: an array indexed at run time lives in local memory on the device.
+  int o0 = 0, o1 = 1, o2 = 2;
+  auto nrm_of = [&](int s) { return s == 0 ? nrm[0] : (s == 1 ? nrm[1] : nrm[2]); };
+  auto cmpx = [&](int& hi, int& lo) {
+    if (nrm_of(lo) > nrm_of(hi)) {
+      const int t = hi;
+      hi = lo;
+      lo = t;
     }
+  };
+  cmpx(o0, o1);
+  cmpx(o1, o2);
+  cmpx(o0, o1);  // (a no-op when the step before did not exchange)
   Svd r;
   for (int j = 0; j < 3; j++) {
-    const int s = order[j];
-    r.sv[j] = nrm[s];
+    const int s = j == 0 ? o0 : (j == 1 ? o1 : o2);
+    const double ns = nrm_of(s);
+    r.sv[j] = ns;
     for (int i = 0; i < 3; i++) {
-      r.V.m[i][j] = V[i][s];
-      r.U.m[i][j] = (nrm[s] > 0.0) ? G[i][s] / nrm[s] : 0.0;
+      const double g = s == 0 ? G[i][0] : (s == 1 ? G[i][1] : G[i][2]);
+      r.V.m[i][j] = s == 0 ? V[i][0] : (s == 1 ? V[i][1] : V[i][2]);
+      r.U.m[i][j] = (ns > 0.0) ? g / ns : 0.0;
     }
   }
   // complete U where singular values vanish (rank-deficient input)
@@ -116,11 +124,13 @@ CB_HD Svd svd_hestenes(const Mat3& A) {
   } else {
     if (r.sv[1] <= tiny) {  // pick any unit vector orthogonal to u0
       int k = 0;
+      double d = r.U.m[0][0];
       for (int i = 1; i < 3; i++)
-        if (fabs(r.U.m[i][0]) < fabs(r.U.m[k][0])) k = i;
-      double e[3] = {0, 0, 0};
-      e[k] = 1.0;
-      double d = r.U.m[k][0];
+        if (fabs(r.U.m[i][0]) < fabs(d)) {
+          k = i;
+          d = r.U.m[i][0];
+        }
+      const double e[3] = {k == 0 ? 1.0 : 0.0, k == 1 ? 1.0 : 0.0, k == 2 ? 1.0 : 0.0};
       double v[3] = {e[0] - d * r.U.m[0][0], e[1] - d * r.U.m[1][0], e[2] - d * r.U.m[2][0]};
       double n = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
       for (int i = 0; i < 3; i++) r.U.m[i][1] = v[i] / n;
