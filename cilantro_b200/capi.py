@@ -227,6 +227,8 @@ EXPORTED = [
     "cb_icp_correspondences", "cb_icp_residuals", "cb_icp_accumulate", "cb_icp_loop_cache", "cb_icp_set_features",
     "cb_solve_kabsch_moments", "cb_solve_gauss_newton", "cb_solve_rotation", "cb_compose",
     "cb_kmeans_cluster", "cb_kmeans_assign", "cb_kmeans_seed_indices",
+    "cb_vectors_create", "cb_vectors_create_from_device", "cb_vectors_destroy", "cb_vectors_size",
+    "cb_kmeans_cluster_vectors", "cb_kmeans_assign_vectors",
     "cb_ransac_score", "cb_ransac_residuals", "cb_ransac_rigid",
     "cb_plane_score", "cb_plane_residuals", "cb_ransac_plane",
     "cb_warp_default_params", "cb_warp_icp_create", "cb_warp_icp_destroy", "cb_warp_icp_estimate", "cb_warp_icp_solve",
@@ -252,6 +254,7 @@ def lib():
         _lib.cb_last_error.restype = C.c_char_p
         _lib.cb_version.restype = C.c_char_p
         _lib.cb_cloud_size.restype = C.c_size_t
+        _lib.cb_vectors_size.restype = C.c_size_t
         _lib.cb_context_kernel_launches.restype = C.c_uint64
         _lib.cb_context_kernel_launches.argtypes = [C.c_void_p]
     return _lib
@@ -533,6 +536,29 @@ class Cloud(_Handle):
         return {"cell_edge": edge.value, "dims": list(dims), "mean_occupancy": occ.value}
 
 
+class Vectors(_Handle):
+    """Device-resident n x D float32 rows for k-means (cb_vectors_create); array [n, D] on the host, or a device
+    pointer with n and D."""
+
+    _destroy = "cb_vectors_destroy"
+
+    def __init__(self, ctx, array=None, device_ptr=None, n=None, D=None):
+        self.ctx = ctx
+        h = C.c_void_p()
+        if device_ptr is not None:
+            _check(lib().cb_vectors_create_from_device(ctx.h, C.c_void_p(device_ptr), C.c_size_t(n), C.c_int(D),
+                                                       C.byref(h)))
+        else:
+            a = np.ascontiguousarray(array, dtype=np.float32)
+            if a.ndim != 2:
+                raise ValueError(f"Vectors wants an [n, D] array, got shape {a.shape}")
+            n, D = a.shape
+            _check(lib().cb_vectors_create(ctx.h, _p(a), C.c_size_t(n), C.c_int(D), C.byref(h)))
+        self.h = h
+        self.n, self.D = int(n), int(D)
+        ctx._adopt(self)
+
+
 def cloud_pair(ctx, xyz_a, normals_a, xyz_b, normals_b, offset_a=0, offset_b=0):
     """cb_cloud_create_pair: two indexed Clouds; the second upload overlaps the first grid build."""
     xa, xb = _f32(xyz_a), _f32(xyz_b)
@@ -757,22 +783,32 @@ def kmeans_seed_indices(n, k, seed):
     return out.astype(np.int64)
 
 
-def kmeans_assign(ctx, pts: Cloud, centroids, want_labels=True):
-    cent = _f32(centroids)
+def _kmeans_rows(pts):
+    """(entry-point suffix, row dimension) of a Cloud (xyz) or a Vectors set."""
+    return ("_vectors", pts.D) if isinstance(pts, Vectors) else ("", 3)
+
+
+def kmeans_assign(ctx, pts, centroids, want_labels=True):
+    """One assignment of a Cloud or a Vectors set: (labels, sums [k, D] float64, counts [k])."""
+    sfx, D = _kmeans_rows(pts)
+    cent = _f32(centroids, D)
     k = cent.shape[0]
     labels = np.empty(pts.n, np.uint64) if want_labels else None
-    sums = np.empty((k, 3), np.float64)
+    sums = np.empty((k, D), np.float64)
     counts = np.empty(k, np.uint64)
-    _check(lib().cb_kmeans_assign(ctx.h, pts.h, _p(cent), C.c_size_t(k), _p(labels), _p(sums), _p(counts)))
+    _check(getattr(lib(), "cb_kmeans_assign" + sfx)(ctx.h, pts.h, _p(cent), C.c_size_t(k), _p(labels), _p(sums),
+                                                     _p(counts)))
     return (labels.astype(np.int64) if want_labels else None), sums, counts.astype(np.int64)
 
 
-def kmeans_cluster(ctx, pts: Cloud, centroids0, max_iter=100, tol=float(np.finfo(np.float32).eps), want_labels=True):
-    cent = _f32(centroids0).copy()
+def kmeans_cluster(ctx, pts, centroids0, max_iter=100, tol=float(np.finfo(np.float32).eps), want_labels=True):
+    """Lloyd's k-means of a Cloud or a Vectors set from centroids0 [k, D]."""
+    sfx, D = _kmeans_rows(pts)
+    cent = _f32(centroids0, D).copy()
     labels = np.empty(pts.n, np.uint64) if want_labels else None
     res = KMeansResult()
-    _check(lib().cb_kmeans_cluster(ctx.h, pts.h, _p(cent), C.c_size_t(cent.shape[0]), C.c_size_t(max_iter),
-                                   C.c_float(tol), _p(labels), C.byref(res)))
+    _check(getattr(lib(), "cb_kmeans_cluster" + sfx)(ctx.h, pts.h, _p(cent), C.c_size_t(cent.shape[0]),
+                                                      C.c_size_t(max_iter), C.c_float(tol), _p(labels), C.byref(res)))
     return {
         "centroids": cent,
         "labels": labels.astype(np.int64) if want_labels else None,

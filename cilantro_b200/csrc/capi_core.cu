@@ -481,6 +481,47 @@ void cb_cloud_destroy(cb_cloud* c) {
 
 size_t cb_cloud_size(const cb_cloud* c) { return c ? c->n : 0; }
 
+// ---- D-dimensional vector sets --------------------------------------------------------------------
+static int vectors_create_common(cb_context* ctx, const float* data, size_t n, int D, cudaMemcpyKind kind,
+                                 cb_vectors** out) {
+  CB_CHECK(ctx && data && out, CB_ERR_INVALID, "null argument");
+  CB_CHECK(D > 0, CB_ERR_INVALID, "D must be >= 1");
+  CB_CHECK(n < (1ull << 31), CB_ERR_INVALID, "vector sets of >= 2^31 rows are not supported");
+  CB_CUDA(cudaSetDevice(ctx->device));
+  *out = nullptr;
+  cb_vectors* v = new cb_vectors(ctx, n, D);
+  auto fill = [&]() -> int {
+    CB_TRY(v->mem.alloc(&v->d_raw, n * (size_t)D));
+    if (n) CB_CUDA(cudaMemcpyAsync(v->d_raw, data, n * (size_t)D * sizeof(float), kind, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return CB_OK;
+  };
+  const int rc = fill();
+  if (rc != CB_OK) {
+    delete v;
+    return rc;
+  }
+  *out = v;
+  return CB_OK;
+}
+
+int cb_vectors_create(cb_context* ctx, const float* data, size_t n, int D, cb_vectors** out) {
+  return vectors_create_common(ctx, data, n, D, cudaMemcpyHostToDevice, out);
+}
+
+int cb_vectors_create_from_device(cb_context* ctx, const float* d_data, size_t n, int D, cb_vectors** out) {
+  return vectors_create_common(ctx, d_data, n, D, cudaMemcpyDeviceToDevice, out);
+}
+
+void cb_vectors_destroy(cb_vectors* v) {
+  if (!v) return;
+  cudaSetDevice(v->ctx->device);
+  cudaStreamSynchronize(v->ctx->stream);
+  delete v;
+}
+
+size_t cb_vectors_size(const cb_vectors* v) { return v ? v->n : 0; }
+
 int cb_cloud_grid_info(const cb_cloud* c, float* cell_edge, int* dims3, double* mean_occupancy) {
   CB_CHECK(c, CB_ERR_INVALID, "cloud is null");
   CB_TRY(ensure_index(const_cast<cb_cloud*>(c)));

@@ -176,7 +176,25 @@ struct cb_cloud {
   double mean_occ = 0;
 };
 
+// n x D fp32, point-major: the bytes a ConstVectorSetMatrixMap<float, D> wraps (at D = 3, the layout of
+// cb_cloud::d_raw).
+struct cb_vectors {
+  cb_vectors(cb_context* c, size_t n_, int d) : ctx(c), n(n_), D(d), mem(c) {}
+  cb_context* ctx = nullptr;
+  size_t n = 0;
+  int D = 0;
+  cb::DeviceScope mem;
+  float* d_raw = nullptr;
+};
+
 namespace cb {
+
+// k-means over D-dimensional rows (kmeans_features.cu), D != 3: labels, the changed flag and the K x (D + 1) double
+// sums (D coordinates, then the count) of one assignment, in one launch. sums and *changed must be zero on entry.
+int kmeans_features_assign(cb_context* ctx, const float* raw, size_t n, int D, const float* cent, size_t K,
+                           uint32_t* labels, double* sums, unsigned int* changed);
+// Per-cluster sums stay in shared memory while K x (D + 1) doubles fit in this many bytes (both assignment kernels).
+constexpr size_t kKMeansSmemSumsBytes = 184 * 1024;
 
 template <class T>
 int DeviceScope::alloc(T** p, size_t count) {

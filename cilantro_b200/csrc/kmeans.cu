@@ -12,6 +12,9 @@
 // A point with a NaN / Inf coordinate never satisfies d < best, so it keeps label 0; it adds nothing
 // to any sum or count and the empty-cluster repair never picks it (the reference leaves its label
 // uninitialised and sums it, so one such point would turn centroid 0 into NaN for good).
+// The Lloyd loop below runs on rows of any dimension D (KMeansData): clouds are D = 3, cb_vectors sets any D >= 1.
+// D = 3 assigns with kmeans_assign_kernel, other D with kmeans_features.cu; the distance of the repair and the tol
+// test is the right fold of DESIGN §4.17, which is dx*dx + (dy*dy + dz*dz) at D = 3.
 #include "cb_internal.hpp"
 #include "host_solve.hpp"
 #include <algorithm>
@@ -102,71 +105,104 @@ __global__ void __launch_bounds__(kBlock) kmeans_assign_kernel(const float* __re
   if (__syncthreads_or(any_changed) && threadIdx.x == 0) atomicOr(changed, 1u);
 }
 
-// farthest member of cluster `target` from point c (kmeans.hpp:151-169): packs (dist bits, ~index)
+// farthest member of cluster `target` from the D-vector c (kmeans.hpp:151-169) under the distance contract
+// (the right fold of DESIGN §4.17; at D = 3 it is dx*dx + (dy*dy + dz*dz)): packs (dist bits, ~index)
 // so that atomicMax picks the largest distance and, on ties, the LOWEST index (the serial order).
 // Members with a non-finite coordinate are skipped (they are in no sum).
-__global__ void farthest_member_kernel(const float* __restrict__ raw, size_t n, const uint32_t* __restrict__ labels,
-                                       uint32_t target, float cx, float cy, float cz,
+__global__ void farthest_member_kernel(const float* __restrict__ raw, size_t n, int D, const uint32_t* __restrict__ labels,
+                                       uint32_t target, const float* __restrict__ c,
                                        unsigned long long* __restrict__ out) {
   unsigned long long best = 0;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     if (labels[i] != target) continue;
-    const float x = raw[3 * i], y = raw[3 * i + 1], z = raw[3 * i + 2];
-    if (!(isfinite(x) && isfinite(y) && isfinite(z))) continue;
-    const float dx = __fsub_rn(cx, x), dy = __fsub_rn(cy, y), dz = __fsub_rn(cz, z);
-    const float d = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
+    const float* p = raw + i * (size_t)D;
+    bool finite = true;
+    float d2 = 0.f;  // 0 + d[D-1]^2 is d[D-1]^2 exactly
+    for (int j = D - 1; j >= 0; j--) {
+      const float x = p[j];
+      finite = finite && isfinite(x);
+      const float d = __fsub_rn(c[j], x);
+      d2 = __fadd_rn(__fmul_rn(d, d), d2);
+    }
+    if (!finite) continue;
     const unsigned long long key =
-        ((unsigned long long)__float_as_uint(d) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)i);
+        ((unsigned long long)__float_as_uint(d2) << 32) | (unsigned long long)(0xffffffffu - (uint32_t)i);
     best = max(best, key | (1ull << 63));  // bit 63 marks "a member exists" (d >= 0 so its sign bit is free)
   }
   for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
   if ((threadIdx.x & 31) == 0 && best) atomicMax(out, best);
 }
 
+// the right fold of the squared difference of two D-vectors on the host (the tol test, kmeans.hpp:186-188)
+float fold_d2(const float* a, const float* b, int D) {
+  float acc = 0.f;
+  for (int j = D - 1; j >= 0; j--) {
+    const float d = a[j] - b[j];
+    acc = d * d + acc;
+  }
+  return acc;
+}
+
+// the rows k-means runs on: a cloud's packed xyz (D = 3) or a cb_vectors set
+struct KMeansData {
+  const float* raw;  // n x D, point-major
+  size_t n;
+  int D;
+};
+
 struct KMeansBuffers {
-  float4* d_cent = nullptr;
+  float* d_cent = nullptr;  // K float4 at D = 3, else K x D
+  float* d_oc = nullptr;    // D: the repair's old centroid
   uint32_t* d_labels = nullptr;
-  double* d_sums = nullptr;
+  double* d_sums = nullptr;  // K x (D + 1)
   unsigned int* d_changed = nullptr;
   unsigned long long* d_far = nullptr;
 };
 
-int kmeans_step(cb_context* ctx, const cb_cloud* pts, const KMeansBuffers& b, const float* cent, size_t K,
+// one assignment: labels, changed flag and the K x (D + 1) sums, downloaded to h_sums
+int kmeans_step(cb_context* ctx, const KMeansData& x, const KMeansBuffers& b, const float* cent, size_t K,
                 std::vector<double>& h_sums, bool* changed) {
-  std::vector<float4> c4(K);
-  for (size_t j = 0; j < K; j++) c4[j] = make_float4(cent[3 * j], cent[3 * j + 1], cent[3 * j + 2], 0.f);
-  CB_CUDA(cudaMemcpyAsync(b.d_cent, c4.data(), K * sizeof(float4), cudaMemcpyHostToDevice, ctx->stream));
-  CB_CUDA(cudaMemsetAsync(b.d_sums, 0, K * 4 * sizeof(double), ctx->stream));
+  const size_t W = (size_t)x.D + 1;
+  CB_CUDA(cudaMemsetAsync(b.d_sums, 0, K * W * sizeof(double), ctx->stream));
   CB_CUDA(cudaMemsetAsync(b.d_changed, 0, sizeof(unsigned int), ctx->stream));
-  const size_t tile = (size_t)kBlock * kPts;
-  const size_t smem_sums = K * 4 * sizeof(double);
-  const bool use_smem = smem_sums + kChunk * sizeof(float4) <= 200 * 1024;
-  const size_t smem = kChunk * sizeof(float4) + (use_smem ? smem_sums : 0);
-  // persistent grid = SMs x resident blocks per SM (occupancy API with this launch's dynamic smem);
-  // a fixed 2 blocks/SM left most warp slots empty
-  int per_sm = 0;
-  if (use_smem) {
-    CB_CUDA(cudaFuncSetAttribute(kmeans_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kmeans_assign_kernel<true>, kBlock, smem));
+  if (x.D != 3) {
+    CB_CUDA(cudaMemcpyAsync(b.d_cent, cent, K * x.D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CB_TRY(kmeans_features_assign(ctx, x.raw, x.n, x.D, b.d_cent, K, b.d_labels, b.d_sums, b.d_changed));
   } else {
-    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kmeans_assign_kernel<false>, kBlock, smem));
+    std::vector<float4> c4(K);
+    for (size_t j = 0; j < K; j++) c4[j] = make_float4(cent[3 * j], cent[3 * j + 1], cent[3 * j + 2], 0.f);
+    float4* d_c4 = reinterpret_cast<float4*>(b.d_cent);
+    CB_CUDA(cudaMemcpyAsync(d_c4, c4.data(), K * sizeof(float4), cudaMemcpyHostToDevice, ctx->stream));
+    const size_t tile = (size_t)kBlock * kPts;
+    const size_t smem_sums = K * 4 * sizeof(double);
+    const bool use_smem = smem_sums <= kKMeansSmemSumsBytes;
+    const size_t smem = kChunk * sizeof(float4) + (use_smem ? smem_sums : 0);
+    // persistent grid = SMs x resident blocks per SM (occupancy API with this launch's dynamic smem);
+    // a fixed 2 blocks/SM left most warp slots empty
+    int per_sm = 0;
+    if (use_smem) {
+      CB_CUDA(cudaFuncSetAttribute(kmeans_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kmeans_assign_kernel<true>, kBlock, smem));
+    } else {
+      CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kmeans_assign_kernel<false>, kBlock, smem));
+    }
+    per_sm = std::max(1, std::min(per_sm, 6));
+    int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (x.n + tile - 1) / tile));
+    if (use_smem) {
+      kmeans_assign_kernel<true><<<blocks, kBlock, smem, ctx->stream>>>(x.raw, x.n, d_c4, (int)K, b.d_labels, b.d_sums,
+                                                                       b.d_changed);
+    } else {
+      kmeans_assign_kernel<false><<<blocks, kBlock, smem, ctx->stream>>>(x.raw, x.n, d_c4, (int)K, b.d_labels, b.d_sums,
+                                                                        b.d_changed);
+    }
+    ctx->launches += 1;
+    CB_CUDA(cudaGetLastError());
   }
-  per_sm = std::max(1, std::min(per_sm, 6));
-  int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (pts->n + tile - 1) / tile));
-  if (use_smem) {
-    kmeans_assign_kernel<true><<<blocks, kBlock, smem, ctx->stream>>>(pts->d_raw, pts->n, b.d_cent, (int)K, b.d_labels,
-                                                                     b.d_sums, b.d_changed);
-  } else {
-    kmeans_assign_kernel<false><<<blocks, kBlock, smem, ctx->stream>>>(pts->d_raw, pts->n, b.d_cent, (int)K,
-                                                                      b.d_labels, b.d_sums, b.d_changed);
-  }
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  // one all-reduce of K x 4 sums per iteration when sharded (SURVEY.md §8e)
-  if (ctx->world > 1) CB_TRY(nccl_allreduce_sum_f64(ctx, b.d_sums, K * 4));
-  h_sums.resize(K * 4);
+  // one all-reduce of K x 4 sums per iteration when sharded (SURVEY.md §8e; clouds only)
+  if (ctx->world > 1) CB_TRY(nccl_allreduce_sum_f64(ctx, b.d_sums, K * W));
+  h_sums.resize(K * W);
   unsigned int h_changed = 0;
-  CB_CUDA(cudaMemcpyAsync(h_sums.data(), b.d_sums, K * 4 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  CB_CUDA(cudaMemcpyAsync(h_sums.data(), b.d_sums, K * W * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaMemcpyAsync(&h_changed, b.d_changed, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   if (ctx->world > 1) {
@@ -183,11 +219,12 @@ int kmeans_step(cb_context* ctx, const cb_cloud* pts, const KMeansBuffers& b, co
   return CB_OK;
 }
 
-int alloc_buffers(cb_context* ctx, DeviceScope& scope, size_t n, size_t K, KMeansBuffers* b) {
-  CB_TRY(scope.alloc(&b->d_cent, K));
-  CB_TRY(scope.alloc(&b->d_labels, n));
-  CB_CUDA(cudaMemsetAsync(b->d_labels, 0, std::max<size_t>(n, 1) * sizeof(uint32_t), ctx->stream));  // kmeans.hpp:82
-  CB_TRY(scope.alloc(&b->d_sums, std::max<size_t>(K, 1) * 4));
+int alloc_buffers(cb_context* ctx, DeviceScope& scope, const KMeansData& x, size_t K, KMeansBuffers* b) {
+  CB_TRY(scope.alloc(&b->d_cent, K * (x.D == 3 ? 4 : x.D)));
+  CB_TRY(scope.alloc(&b->d_oc, (size_t)x.D));
+  CB_TRY(scope.alloc(&b->d_labels, x.n));
+  CB_CUDA(cudaMemsetAsync(b->d_labels, 0, std::max<size_t>(x.n, 1) * sizeof(uint32_t), ctx->stream));  // kmeans.hpp:82
+  CB_TRY(scope.alloc(&b->d_sums, std::max<size_t>(K, 1) * (x.D + 1)));
   CB_TRY(scope.alloc(&b->d_changed, 1));
   CB_TRY(scope.alloc(&b->d_far, 1));
   return CB_OK;
@@ -199,6 +236,116 @@ int download_labels(cb_context* ctx, const KMeansBuffers& b, size_t n, uint64_t*
   CB_CUDA(cudaMemcpyAsync(h.data(), b.d_labels, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
   for (size_t i = 0; i < n; i++) labels[i] = h[i];
+  return CB_OK;
+}
+
+int kmeans_assign(cb_context* ctx, const KMeansData& x, const float* centroids, size_t k, uint64_t* labels,
+                  double* sums, uint64_t* counts) {
+  CB_CUDA(cudaSetDevice(ctx->device));
+  DeviceScope scope(ctx);
+  KMeansBuffers b;
+  CB_TRY(alloc_buffers(ctx, scope, x, k, &b));
+  std::vector<double> h_sums;
+  bool changed = false;
+  CB_TRY(kmeans_step(ctx, x, b, centroids, k, h_sums, &changed));
+  CB_TRY(download_labels(ctx, b, x.n, labels));
+  const size_t D = x.D, W = D + 1;
+  for (size_t j = 0; j < k; j++) {
+    if (sums)
+      for (size_t r = 0; r < D; r++) sums[D * j + r] = h_sums[W * j + r];
+    if (counts) counts[j] = (uint64_t)(h_sums[W * j + D] + 0.5);
+  }
+  return CB_OK;
+}
+
+// the Lloyd loop of kmeans.hpp:67-194 over rows of any dimension
+int kmeans_cluster(cb_context* ctx, const KMeansData& x, float* centroids, size_t k, size_t max_iter, float tol,
+                   uint64_t* labels, cb_kmeans_result* res) {
+  CB_CUDA(cudaSetDevice(ctx->device));
+  const uint64_t launches0 = ctx->launches;
+  const size_t D = x.D, W = D + 1;
+  DeviceScope scope(ctx);
+  KMeansBuffers b;
+  CB_TRY(alloc_buffers(ctx, scope, x, k, &b));
+  ScopedEvents ev;
+  CB_TRY(ev.create());
+  const float tol_sq = tol * tol;
+  std::vector<float> old, oc(D), p(D);
+  std::vector<double> s;
+  size_t it = 0;
+  CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
+  while (it < max_iter) {
+    bool changed = false;
+    CB_TRY(kmeans_step(ctx, x, b, centroids, k, s, &changed));
+    if (!changed && it > 0) break;                              // kmeans.hpp:122
+    if (tol > 0.f) old.assign(centroids, centroids + D * k);   // :123
+    // :134-176 empty-cluster repair, on the reduced sums. The farthest-member search is a device
+    // reduction; in the sharded case every rank proposes its best and the global best is taken.
+    std::vector<double> cnt(k);
+    for (size_t j = 0; j < k; j++) cnt[j] = s[W * j + D];
+    for (size_t i = 0; i < k; i++) {
+      if (cnt[i] != 0.0) continue;
+      size_t max_ind = 0;
+      for (size_t j = 1; j < k; j++)
+        if (cnt[j] > cnt[max_ind]) max_ind = j;
+      // old_centroid = sum * (1 / count) in fp32 (:147-148)
+      const float inv = 1.0f / (float)cnt[max_ind];
+      for (size_t r = 0; r < D; r++) oc[r] = (float)s[W * max_ind + r] * inv;
+      if (ctx->world > 1) {
+        set_error("empty-cluster repair is not implemented for sharded k-means");
+        return CB_ERR_UNSUPPORTED;
+      }
+      CB_CUDA(cudaMemcpyAsync(b.d_oc, oc.data(), D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+      CB_CUDA(cudaMemsetAsync(b.d_far, 0, sizeof(unsigned long long), ctx->stream));
+      const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (x.n + 255) / 256));
+      farthest_member_kernel<<<blocks, 256, 0, ctx->stream>>>(x.raw, x.n, x.D, b.d_labels, (uint32_t)max_ind, b.d_oc,
+                                                              b.d_far);
+      ctx->launches += 1;
+      CB_CUDA(cudaGetLastError());
+      unsigned long long key = 0;
+      CB_CUDA(cudaMemcpyAsync(&key, b.d_far, sizeof(key), cudaMemcpyDeviceToHost, ctx->stream));
+      CB_CUDA(cudaStreamSynchronize(ctx->stream));
+      if (!key) continue;  // cannot happen: the largest cluster has members
+      const uint32_t far_idx = 0xffffffffu - (uint32_t)(key & 0xffffffffull);
+      // move the point to cluster i (:172-175); note the reference does NOT add it to cluster i's sum
+      const uint32_t new_label = (uint32_t)i;
+      CB_CUDA(cudaMemcpyAsync(b.d_labels + far_idx, &new_label, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+      CB_CUDA(cudaMemcpyAsync(p.data(), x.raw + D * far_idx, D * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+      CB_CUDA(cudaStreamSynchronize(ctx->stream));
+      for (size_t r = 0; r < D; r++) s[W * max_ind + r] -= (double)p[r];
+      cnt[max_ind] -= 1.0;
+      cnt[i] += 1.0;
+    }
+    for (size_t j = 0; j < k; j++) {  // :179-181  centroid = sum * (1 / count)
+      const float inv = 1.0f / (float)cnt[j];
+      for (size_t r = 0; r < D; r++) centroids[D * j + r] = (float)s[W * j + r] * inv;
+    }
+    it++;
+    if (tol > 0.f) {  // :186-188
+      float mx = 0.f;
+      for (size_t j = 0; j < k; j++) mx = std::max(mx, fold_d2(centroids + D * j, old.data() + D * j, x.D));
+      if (mx < tol_sq) break;
+    }
+  }
+  CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
+  CB_TRY(download_labels(ctx, b, x.n, labels));
+  CB_CUDA(cudaStreamSynchronize(ctx->stream));
+  float ms = 0.f;
+  CB_CUDA(cudaEventElapsedTime(&ms, ev.e0, ev.e1));
+  if (res) {
+    res->iterations = it;
+    res->gpu_ms_total = ms;
+    res->kernel_launches = ctx->launches - launches0;
+  }
+  return CB_OK;
+}
+
+// the checks of the cb_vectors entry points: single GPU, centroid sums indexable by int
+int check_vectors(cb_context* ctx, const cb_vectors* v, const float* centroids, size_t k) {
+  CB_CHECK(ctx && v && centroids && k > 0, CB_ERR_INVALID, "bad arguments");
+  CB_CHECK(v->ctx == ctx, CB_ERR_INVALID, "vector set belongs to another context");
+  CB_CHECK(k <= (size_t)INT32_MAX / (size_t)(v->D + 1), CB_ERR_INVALID, "k x (D + 1) too large");
+  CB_CHECK(ctx->world == 1, CB_ERR_UNSUPPORTED, "k-means over vector sets runs on one GPU");
   return CB_OK;
 }
 
@@ -226,105 +373,26 @@ int cb_kmeans_seed_indices(size_t n, size_t k, uint32_t seed, uint64_t* out_idx)
 int cb_kmeans_assign(cb_context* ctx, const cb_cloud* pts, const float* centroids, size_t k, uint64_t* labels,
                      double* sums, uint64_t* counts) {
   CB_CHECK(ctx && pts && centroids && k > 0, CB_ERR_INVALID, "bad arguments");
-  CB_CUDA(cudaSetDevice(ctx->device));
-  DeviceScope scope(ctx);
-  KMeansBuffers b;
-  CB_TRY(alloc_buffers(ctx, scope, pts->n, k, &b));
-  std::vector<double> h_sums;
-  bool changed = false;
-  CB_TRY(kmeans_step(ctx, pts, b, centroids, k, h_sums, &changed));
-  CB_TRY(download_labels(ctx, b, pts->n, labels));
-  for (size_t j = 0; j < k; j++) {
-    if (sums)
-      for (int r = 0; r < 3; r++) sums[3 * j + r] = h_sums[4 * j + r];
-    if (counts) counts[j] = (uint64_t)(h_sums[4 * j + 3] + 0.5);
-  }
-  return CB_OK;
+  return kmeans_assign(ctx, KMeansData{pts->d_raw, pts->n, 3}, centroids, k, labels, sums, counts);
 }
 
 int cb_kmeans_cluster(cb_context* ctx, const cb_cloud* pts, float* centroids, size_t k, size_t max_iter, float tol,
                       uint64_t* labels, cb_kmeans_result* res) {
   CB_CHECK(ctx && pts && centroids && k > 0, CB_ERR_INVALID, "bad arguments");
-  CB_CUDA(cudaSetDevice(ctx->device));
-  const uint64_t launches0 = ctx->launches;
-  DeviceScope scope(ctx);
-  KMeansBuffers b;
-  CB_TRY(alloc_buffers(ctx, scope, pts->n, k, &b));
-  ScopedEvents ev;
-  CB_TRY(ev.create());
-  const float tol_sq = tol * tol;
-  std::vector<float> old;
-  std::vector<double> s;
-  size_t it = 0;
-  CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
-  while (it < max_iter) {
-    bool changed = false;
-    CB_TRY(kmeans_step(ctx, pts, b, centroids, k, s, &changed));
-    if (!changed && it > 0) break;                              // kmeans.hpp:122
-    if (tol > 0.f) old.assign(centroids, centroids + 3 * k);   // :123
-    // :134-176 empty-cluster repair, on the reduced sums. The farthest-member search is a device
-    // reduction; in the sharded case every rank proposes its best and the global best is taken.
-    std::vector<double> cnt(k);
-    for (size_t j = 0; j < k; j++) cnt[j] = s[4 * j + 3];
-    for (size_t i = 0; i < k; i++) {
-      if (cnt[i] != 0.0) continue;
-      size_t max_ind = 0;
-      for (size_t j = 1; j < k; j++)
-        if (cnt[j] > cnt[max_ind]) max_ind = j;
-      // old_centroid = sum * (1 / count) in fp32 (:147-148)
-      const float inv = 1.0f / (float)cnt[max_ind];
-      const float oc[3] = {(float)s[4 * max_ind] * inv, (float)s[4 * max_ind + 1] * inv, (float)s[4 * max_ind + 2] * inv};
-      if (ctx->world > 1) {
-        set_error("empty-cluster repair is not implemented for sharded k-means");
-        return CB_ERR_UNSUPPORTED;
-      }
-      CB_CUDA(cudaMemsetAsync(b.d_far, 0, sizeof(unsigned long long), ctx->stream));
-      const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (pts->n + 255) / 256));
-      farthest_member_kernel<<<blocks, 256, 0, ctx->stream>>>(pts->d_raw, pts->n, b.d_labels, (uint32_t)max_ind, oc[0],
-                                                              oc[1], oc[2], b.d_far);
-      ctx->launches += 1;
-      CB_CUDA(cudaGetLastError());
-      unsigned long long key = 0;
-      CB_CUDA(cudaMemcpyAsync(&key, b.d_far, sizeof(key), cudaMemcpyDeviceToHost, ctx->stream));
-      CB_CUDA(cudaStreamSynchronize(ctx->stream));
-      if (!key) continue;  // cannot happen: the largest cluster has members
-      const uint32_t far_idx = 0xffffffffu - (uint32_t)(key & 0xffffffffull);
-      // move the point to cluster i (:172-175); note the reference does NOT add it to cluster i's sum
-      const uint32_t new_label = (uint32_t)i;
-      CB_CUDA(cudaMemcpyAsync(b.d_labels + far_idx, &new_label, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-      float p[3];
-      CB_CUDA(cudaMemcpyAsync(p, pts->d_raw + 3 * (size_t)far_idx, sizeof(p), cudaMemcpyDeviceToHost, ctx->stream));
-      CB_CUDA(cudaStreamSynchronize(ctx->stream));
-      for (int r = 0; r < 3; r++) s[4 * max_ind + r] -= (double)p[r];
-      cnt[max_ind] -= 1.0;
-      cnt[i] += 1.0;
-    }
-    for (size_t j = 0; j < k; j++) {  // :179-181  centroid = sum * (1 / count)
-      const float inv = 1.0f / (float)cnt[j];
-      for (int r = 0; r < 3; r++) centroids[3 * j + r] = (float)s[4 * j + r] * inv;
-    }
-    it++;
-    if (tol > 0.f) {  // :186-188
-      float mx = 0.f;
-      for (size_t j = 0; j < k; j++) {
-        const float dx = centroids[3 * j] - old[3 * j], dy = centroids[3 * j + 1] - old[3 * j + 1],
-                    dz = centroids[3 * j + 2] - old[3 * j + 2];
-        mx = std::max(mx, dx * dx + (dy * dy + dz * dz));
-      }
-      if (mx < tol_sq) break;
-    }
-  }
-  CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
-  CB_TRY(download_labels(ctx, b, pts->n, labels));
-  CB_CUDA(cudaStreamSynchronize(ctx->stream));
-  float ms = 0.f;
-  CB_CUDA(cudaEventElapsedTime(&ms, ev.e0, ev.e1));
-  if (res) {
-    res->iterations = it;
-    res->gpu_ms_total = ms;
-    res->kernel_launches = ctx->launches - launches0;
-  }
-  return CB_OK;
+  return kmeans_cluster(ctx, KMeansData{pts->d_raw, pts->n, 3}, centroids, k, max_iter, tol, labels, res);
+}
+
+int cb_kmeans_assign_vectors(cb_context* ctx, const cb_vectors* vectors, const float* centroids, size_t k,
+                             uint64_t* labels, double* sums, uint64_t* counts) {
+  CB_TRY(check_vectors(ctx, vectors, centroids, k));
+  return kmeans_assign(ctx, KMeansData{vectors->d_raw, vectors->n, vectors->D}, centroids, k, labels, sums, counts);
+}
+
+int cb_kmeans_cluster_vectors(cb_context* ctx, const cb_vectors* vectors, float* centroids, size_t k, size_t max_iter,
+                              float tol, uint64_t* labels, cb_kmeans_result* res) {
+  CB_TRY(check_vectors(ctx, vectors, centroids, k));
+  return kmeans_cluster(ctx, KMeansData{vectors->d_raw, vectors->n, vectors->D}, centroids, k, max_iter, tol, labels,
+                        res);
 }
 
 }  // extern "C"

@@ -15,6 +15,8 @@
 //   SimpleCombinedMetricSparseRigidWarpFieldICP3f           registration/icp_common_instances.hpp:146-199,313-314
 //   VectorSet<float,3>, KDTree<float,3>, NeighborhoodSet    core/data_containers.hpp, kd_tree.hpp, nearest_neighbors.hpp
 //   KMeans3f<>                                              clustering/kmeans.hpp:9-59,205-207
+//   KMeans<float, D>, KMeans2f<>, KMeansXf<>                clustering/kmeans.hpp:9-59,197-219
+//   VectorSet<float, D>, ConstVectorSetMatrixMap<float, D>  core/data_containers.hpp:73-112 (D != 3: k-means only)
 //   RigidTransformRANSACEstimator3f<>                       model_estimation/ransac_transform_estimator.hpp:9-122
 //   PrincipalComponentAnalysis3f                            core/principal_component_analysis.hpp:8-89
 //   NormalEstimation3f                                      core/normal_estimation.hpp:11-421
@@ -412,8 +414,8 @@ private:
   b200::CloudHandle cloud_;
 };
 
-// VectorSet<float, 3> and KDTree<float, 3> (core/data_containers.hpp, core/kd_tree.hpp): the 3-D float instances are
-// the only ones; any other scalar or dimension is a compile-time error.
+// KDTree<float, 3> (core/kd_tree.hpp): the 3-D float instance is the only one; any other scalar or dimension is a
+// compile-time error. VectorSet<float, 3> is VectorSet3f.
 namespace b200 {
 template <class ScalarT, long EigenDim>
 struct Instance3f {
@@ -425,8 +427,92 @@ struct Instance3f<float, 3> {
   using KDTree = KDTree3f<>;
 };
 }  // namespace b200
+
+// VectorSet<float, D> and ConstVectorSetMatrixMap<float, D> for D != 3 (D = -1 is Eigen::Dynamic, rows set at run
+// time): D x N column-major float rows, the layout of Eigen::Matrix<float, D, Dynamic> (core/data_containers.hpp:73-112).
+// Only k-means takes them (KMeans<float, D> below); other scalars are a compile-time error.
+namespace b200 {
+constexpr long kDynamic = -1;  // Eigen::Dynamic
+#ifdef CILANTRO_B200_HAS_EIGEN
+static_assert(Eigen::Dynamic == kDynamic, "Eigen::Dynamic");
+#endif
+
+template <long D>
+class VectorSetD {
+  static_assert(D > 0 || D == kDynamic, "dimension must be positive or Eigen::Dynamic");
+
+public:
+  VectorSetD() = default;
+  VectorSetD(size_t rows, size_t cols) : rows_(D > 0 ? D : rows), d_(rows_ * cols) {}
+  size_t rows() const { return rows_; }
+  size_t cols() const { return rows_ ? d_.size() / rows_ : 0; }
+  void resize(size_t rows, size_t cols) {
+    rows_ = D > 0 ? D : rows;
+    d_.resize(rows_ * cols);
+  }
+  float* data() { return d_.data(); }
+  const float* data() const { return d_.data(); }
+  float& operator()(size_t r, size_t c) { return d_[rows_ * c + r]; }
+  float operator()(size_t r, size_t c) const { return d_[rows_ * c + r]; }
+#ifdef CILANTRO_B200_HAS_EIGEN
+  using EigenMatrix = Eigen::Matrix<float, (int)D, Eigen::Dynamic>;
+  VectorSetD(const EigenMatrix& m) : rows_((size_t)m.rows()), d_(m.data(), m.data() + m.size()) {}
+  Eigen::Map<EigenMatrix> eigen() { return {d_.data(), (Eigen::Index)rows_, (Eigen::Index)cols()}; }
+  Eigen::Map<const EigenMatrix> eigen() const { return {d_.data(), (Eigen::Index)rows_, (Eigen::Index)cols()}; }
+  operator EigenMatrix() const { return eigen(); }
+#endif
+
+private:
+  size_t rows_ = D > 0 ? D : 0;
+  std::vector<float> d_;
+};
+
+template <long D>
+class ConstVectorSetMatrixMapD {
+  static_assert(D > 0 || D == kDynamic, "dimension must be positive or Eigen::Dynamic");
+
+public:
+  ConstVectorSetMatrixMapD(const float* data = nullptr, size_t n = 0) : p_(data), rows_(D > 0 ? D : 0), n_(n) {}
+  ConstVectorSetMatrixMapD(const float* data, size_t rows, size_t n) : p_(data), rows_(rows), n_(n) {}
+  ConstVectorSetMatrixMapD(const VectorSetD<D>& s) : p_(s.data()), rows_(s.rows()), n_(s.cols()) {}
+#ifdef CILANTRO_B200_HAS_EIGEN
+  using EigenMatrix = Eigen::Matrix<float, (int)D, Eigen::Dynamic>;
+  ConstVectorSetMatrixMapD(const EigenMatrix& m) : p_(m.data()), rows_((size_t)m.rows()), n_((size_t)m.cols()) {}
+  ConstVectorSetMatrixMapD(const Eigen::Map<EigenMatrix>& m)
+      : p_(m.data()), rows_((size_t)m.rows()), n_((size_t)m.cols()) {}
+  ConstVectorSetMatrixMapD(const Eigen::Map<const EigenMatrix>& m)
+      : p_(m.data()), rows_((size_t)m.rows()), n_((size_t)m.cols()) {}
+  Eigen::Map<const EigenMatrix> eigen() const { return {p_, (Eigen::Index)rows_, (Eigen::Index)n_}; }
+#endif
+  const float* data() const { return p_; }
+  size_t rows() const { return rows_; }
+  size_t cols() const { return n_; }
+
+private:
+  const float* p_;
+  size_t rows_;
+  size_t n_;
+};
+
 template <class ScalarT, long EigenDim>
-using VectorSet = typename b200::Instance3f<ScalarT, EigenDim>::VectorSet;
+struct VectorInstance {
+  static_assert(sizeof(ScalarT) == 0, "cilantro_b200 provides float vector sets only");
+};
+template <long EigenDim>
+struct VectorInstance<float, EigenDim> {
+  using VectorSet = VectorSetD<EigenDim>;
+  using ConstMap = ConstVectorSetMatrixMapD<EigenDim>;
+};
+template <>
+struct VectorInstance<float, 3> {
+  using VectorSet = VectorSet3f;
+  using ConstMap = ConstVectorSetMatrixMap3f;
+};
+}  // namespace b200
+template <class ScalarT, long EigenDim>
+using VectorSet = typename b200::VectorInstance<ScalarT, EigenDim>::VectorSet;
+template <class ScalarT, long EigenDim>
+using ConstVectorSetMatrixMap = typename b200::VectorInstance<ScalarT, EigenDim>::ConstMap;
 template <class ScalarT, long EigenDim, class... DistanceAdaptorT>
 using KDTree = typename b200::Instance3f<ScalarT, EigenDim>::KDTree;
 
@@ -1310,6 +1396,114 @@ private:
   PointToClusterIndexMap labels_;
   ClusterToPointIndicesMap lists_;
 };
+
+// ---- KMeans<float, D> / KMeans2f<> / KMeansXf<> ----------------------------------------------------------
+// The distance adaptors of core/kd_tree.hpp:40-61, as tags: k-means has a device path for L2 and L2Simple only.
+namespace KDTreeDistanceAdaptors {
+template <class DataAdaptor>
+struct L1 {};
+template <class DataAdaptor>
+struct L2 {};
+template <class DataAdaptor>
+struct L2Simple {};
+template <class DataAdaptor>
+struct SO2 {};
+template <class DataAdaptor>
+struct SO3 {};
+}  // namespace KDTreeDistanceAdaptors
+
+namespace b200 {
+template <template <class> class DistAdaptor>
+struct IsL2 : std::false_type {};
+template <>
+struct IsL2<KDTreeDistanceAdaptors::L2> : std::true_type {};
+template <>
+struct IsL2<KDTreeDistanceAdaptors::L2Simple> : std::true_type {};
+
+// n x D rows resident on the device (cb_vectors)
+struct VectorsHandle {
+  cb_vectors* h = nullptr;
+  VectorsHandle(const float* data, size_t n, size_t D) {
+    check(cb_vectors_create(Context::get(), data, n, (int)D, &h), "cb_vectors_create");
+  }
+  VectorsHandle(const VectorsHandle&) = delete;
+  VectorsHandle& operator=(const VectorsHandle&) = delete;
+  ~VectorsHandle() { cb_vectors_destroy(h); }
+};
+}  // namespace b200
+
+// KMeans<float, D, DistAdaptor> (clustering/kmeans.hpp:9-59,197-219) for any D, Eigen::Dynamic included: the
+// brute-force Lloyd loop of cb_kmeans_cluster_vectors, with the distance fold of DESIGN §4.17. use_kd_tree is ignored
+// (both branches of the reference compute the same assignment).
+template <typename ScalarT, long EigenDim, template <class> class DistAdaptor = KDTreeDistanceAdaptors::L2,
+          typename PointIndexT = size_t, typename ClusterIndexT = size_t>
+class KMeans {
+  static_assert(std::is_same<ScalarT, float>::value, "cilantro_b200 provides float k-means only");
+  static_assert(b200::IsL2<DistAdaptor>::value, "cilantro_b200 k-means supports the L2 / L2Simple adaptors only");
+
+public:
+  using Scalar = ScalarT;
+  using ClusterToPointIndicesMap = std::vector<std::vector<PointIndexT>>;
+  using PointToClusterIndexMap = std::vector<ClusterIndexT>;
+  enum { Dimension = EigenDim };
+
+  KMeans(const ConstVectorSetMatrixMap<ScalarT, EigenDim>& data)
+      : n_(data.cols()), dim_(data.rows()), host_(data), vectors_(data.data(), data.cols(), data.rows()) {}
+
+  KMeans& cluster(const ConstVectorSetMatrixMap<ScalarT, EigenDim>& centroids, size_t max_iter = 100,
+                  float tol = std::numeric_limits<float>::epsilon(), bool use_kd_tree = false) {
+    (void)use_kd_tree;
+    b200::check(centroids.rows() == dim_ ? CB_OK : CB_ERR_INVALID, "KMeans::cluster: centroids of another dimension");
+    centroids_.resize(dim_, centroids.cols());
+    std::memcpy(centroids_.data(), centroids.data(), dim_ * centroids.cols() * sizeof(float));
+    return run(max_iter, tol);
+  }
+  KMeans& cluster(size_t num_clusters, size_t max_iter = 100, float tol = std::numeric_limits<float>::epsilon(),
+                  bool use_kd_tree = false, uint32_t seed = b200::random_seed()) {
+    (void)use_kd_tree;
+    const size_t k = std::max<size_t>(1, std::min(num_clusters, n_));  // kmeans.hpp:34-36
+    std::vector<uint64_t> idx(k);
+    b200::check(cb_kmeans_seed_indices(n_, k, seed, idx.data()), "cb_kmeans_seed_indices");
+    centroids_.resize(dim_, k);
+    for (size_t j = 0; j < k; j++) std::memcpy(&centroids_(0, j), host_.data() + dim_ * idx[j], dim_ * sizeof(float));
+    return run(max_iter, tol);
+  }
+  const VectorSet<ScalarT, EigenDim>& getClusterCentroids() const { return centroids_; }
+  size_t getNumberOfPerformedIterations() const { return iterations_; }
+  const PointToClusterIndexMap& getPointToClusterIndexMap() const { return labels_; }
+  const ClusterToPointIndicesMap& getClusterToPointIndicesMap() const { return lists_; }
+  size_t getNumberOfClusters() const { return lists_.size(); }
+  size_t getNumberOfPoints() const { return labels_.size(); }
+
+private:
+  KMeans& run(size_t max_iter, float tol) {
+    std::vector<uint64_t> lab(n_);
+    cb_kmeans_result r;
+    b200::check(cb_kmeans_cluster_vectors(b200::Context::get(), vectors_.h, centroids_.data(), centroids_.cols(),
+                                          max_iter, tol, lab.data(), &r),
+                "cb_kmeans_cluster_vectors");
+    iterations_ = r.iterations;
+    labels_.assign(lab.begin(), lab.end());
+    lists_.assign(centroids_.cols(), {});  // clustering_base.hpp:22-32
+    for (size_t i = 0; i < labels_.size(); i++)
+      if ((size_t)labels_[i] < lists_.size()) lists_[labels_[i]].emplace_back((PointIndexT)i);
+    return *this;
+  }
+  size_t n_, dim_;
+  ConstVectorSetMatrixMap<ScalarT, EigenDim> host_;
+  b200::VectorsHandle vectors_;
+  VectorSet<ScalarT, EigenDim> centroids_;
+  size_t iterations_ = 0;
+  PointToClusterIndexMap labels_;
+  ClusterToPointIndicesMap lists_;
+};
+
+template <template <class> class DistAdaptor = KDTreeDistanceAdaptors::L2, typename PointIndexT = size_t,
+          typename ClusterIndexT = size_t>
+using KMeans2f = KMeans<float, 2, DistAdaptor, PointIndexT, ClusterIndexT>;
+template <template <class> class DistAdaptor = KDTreeDistanceAdaptors::L2, typename PointIndexT = size_t,
+          typename ClusterIndexT = size_t>
+using KMeansXf = KMeans<float, b200::kDynamic, DistAdaptor, PointIndexT, ClusterIndexT>;
 
 // ---- RigidTransformRANSACEstimator3f<> ----------------------------------------------------------------
 template <typename IndexT = size_t>

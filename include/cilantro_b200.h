@@ -43,6 +43,7 @@ typedef enum cb_status {
 
 typedef struct cb_context cb_context;
 typedef struct cb_cloud cb_cloud;
+typedef struct cb_vectors cb_vectors;
 typedef struct cb_icp cb_icp;
 
 const char* cb_last_error(void);
@@ -439,6 +440,25 @@ int cb_kmeans_assign(cb_context* ctx, const cb_cloud* pts, const float* centroid
                      double* sums, uint64_t* counts);
 /* KMeans::cluster(num_clusters,...) seeding (kmeans.hpp:32-49) with an injected seed. */
 int cb_kmeans_seed_indices(size_t n, size_t k, uint32_t seed, uint64_t* out_idx);
+
+/* ---- D-dimensional vector sets and k-means over them -------------------------------------------
+ * A cb_vectors holds n x D float32 rows in HBM, point-major: the bytes a ConstVectorSetMatrixMap<float, D>
+ * (core/data_containers.hpp:73-112) wraps. D >= 1; D <= 0 or a null pointer is CB_ERR_INVALID. */
+int cb_vectors_create(cb_context* ctx, const float* data, size_t n, int D, cb_vectors** out);
+int cb_vectors_create_from_device(cb_context* ctx, const float* d_data, size_t n, int D, cb_vectors** out);
+void cb_vectors_destroy(cb_vectors* v);
+size_t cb_vectors_size(const cb_vectors* v);
+/* KMeans<float, D, KDTreeDistanceAdaptors::L2>::cluster(centroids, max_iter, tol, use_kd_tree=false)
+ * (clustering/kmeans.hpp:9-59,67-194, brute-force branch) for any D: cb_kmeans_cluster over D-dimensional rows,
+ * with the distance d = c - p, acc = d[D-1]^2, acc = d[j]^2 + acc for j = D-2 .. 0 (fp32, no FMA; at D = 3 it is
+ * cb_kmeans_cluster's). centroids: in = initial (k x D), out = final. labels (may be NULL): n uint64. One GPU: a
+ * context with several ranks returns CB_ERR_UNSUPPORTED. */
+int cb_kmeans_cluster_vectors(cb_context* ctx, const cb_vectors* vectors, float* centroids, size_t k, size_t max_iter,
+                              float tol, uint64_t* labels, cb_kmeans_result* res);
+/* One assignment sweep (kmeans.hpp:100-131) over D-dimensional rows: labels n uint64, sums k x D doubles and
+ * counts k uint64 over the rows with D finite components, each when non-NULL. */
+int cb_kmeans_assign_vectors(cb_context* ctx, const cb_vectors* vectors, const float* centroids, size_t k,
+                             uint64_t* labels, double* sums, uint64_t* counts);
 
 /* ---- RANSAC ----------------------------------------------------------------------------------
  * Replaces TransformRANSACEstimator<RigidTransform3f>::computeResiduals + the inlier scan of

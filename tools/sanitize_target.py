@@ -12,6 +12,9 @@ sys.path.insert(0, ROOT)
 import oracle  # noqa: E402
 from cilantro_b200 import capi, synth  # noqa: E402
 
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import kmeans_features_ref  # noqa: E402
+
 N = int(os.environ.get("SANITIZE_N", "6000"))
 
 
@@ -88,6 +91,15 @@ def main():
     # k-means, RANSAC, PCA
     pts, cent = synth.kmeans_data(N, 16, seed=1)
     capi.kmeans_cluster(ctx, capi.Cloud(ctx, pts), cent, max_iter=3, tol=0.0)
+    # D-dimensional k-means: partial dimension chunks and tiles, both sums paths, a repair, a NaN row
+    rng = np.random.default_rng(4)
+    for D, n, k in ((6, 1001, 3365), (17, 777, 129), (40, 300, 7)):
+        rows = rng.standard_normal((n, D)).astype(np.float32)
+        rows[5, D - 1] = np.nan
+        c0 = np.vstack([rng.standard_normal((k - 1, D)), np.full((1, D), 50.0)]).astype(np.float32)
+        v = capi.Vectors(ctx, rows)
+        capi.kmeans_cluster(ctx, v, c0, max_iter=2, tol=0.0)
+        assert np.array_equal(capi.kmeans_assign(ctx, v, c0)[0], kmeans_features_ref.assign(rows, c0)), ("k-means", D)
     rd, rs, _, _ = synth.ransac_pairs(N, 0.4, seed=2)
     c_rd, c_rs = capi.Cloud(ctx, rd), capi.Cloud(ctx, rs)
     capi.ransac_rigid(ctx, c_rd, c_rs, seed=5, max_iter=64, thresh=0.01)
