@@ -484,7 +484,8 @@ size_t cb_cloud_size(const cb_cloud* c) { return c ? c->n : 0; }
 // ---- D-dimensional vector sets --------------------------------------------------------------------
 static int vectors_create_common(cb_context* ctx, const float* data, size_t n, int D, cudaMemcpyKind kind,
                                  cb_vectors** out) {
-  CB_CHECK(ctx && data && out, CB_ERR_INVALID, "null argument");
+  CB_CHECK(ctx && out, CB_ERR_INVALID, "null argument");
+  CB_CHECK(n == 0 || data, CB_ERR_INVALID, "data is null");
   CB_CHECK(D > 0, CB_ERR_INVALID, "D must be >= 1");
   CB_CHECK(n < (1ull << 31), CB_ERR_INVALID, "vector sets of >= 2^31 rows are not supported");
   CB_CUDA(cudaSetDevice(ctx->device));

@@ -14,8 +14,7 @@
 //   TransformSet<RigidTransform3f>, transformPoints         core/space_transformations.hpp:60-136,195-223
 //   SimpleCombinedMetricSparseRigidWarpFieldICP3f           registration/icp_common_instances.hpp:146-199,313-314
 //   VectorSet<float,3>, KDTree<float,3>, NeighborhoodSet    core/data_containers.hpp, kd_tree.hpp, nearest_neighbors.hpp
-//   KMeans3f<>                                              clustering/kmeans.hpp:9-59,205-207
-//   KMeans<float, D>, KMeans2f<>, KMeansXf<>                clustering/kmeans.hpp:9-59,197-219
+//   KMeans<float, D>, KMeans2f<>, KMeans3f<>, KMeansXf<>    clustering/kmeans.hpp:9-59,197-219
 //   VectorSet<float, D>, ConstVectorSetMatrixMap<float, D>  core/data_containers.hpp:73-112 (D != 3: k-means only)
 //   RigidTransformRANSACEstimator3f<>                       model_estimation/ransac_transform_estimator.hpp:9-122
 //   PrincipalComponentAnalysis3f                            core/principal_component_analysis.hpp:8-89
@@ -1340,64 +1339,7 @@ private:
   ControlWeightEvaluator ctrl_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
 };
 
-// ---- KMeans3f<> -------------------------------------------------------------------------------------
-template <typename PointIndexT = size_t, typename ClusterIndexT = size_t>
-class KMeans3f {
-public:
-  using ClusterToPointIndicesMap = std::vector<std::vector<PointIndexT>>;
-  using PointToClusterIndexMap = std::vector<ClusterIndexT>;
-
-  KMeans3f(const ConstVectorSetMatrixMap3f& data) : n_(data.cols()), host_(data), cloud_(data) {}
-
-  KMeans3f& cluster(const ConstVectorSetMatrixMap3f& centroids, size_t max_iter = 100,
-                    float tol = std::numeric_limits<float>::epsilon(), bool use_kd_tree = false) {
-    (void)use_kd_tree;  // both branches of the reference compute the same assignment; one GPU kernel here
-    centroids_.resize(3, centroids.cols());
-    std::memcpy(centroids_.data(), centroids.data(), 3 * centroids.cols() * sizeof(float));
-    return run(max_iter, tol);
-  }
-  KMeans3f& cluster(size_t num_clusters, size_t max_iter = 100, float tol = std::numeric_limits<float>::epsilon(),
-                    bool use_kd_tree = false, uint32_t seed = b200::random_seed()) {
-    (void)use_kd_tree;
-    const size_t k = std::max<size_t>(1, std::min(num_clusters, n_));  // kmeans.hpp:34-36
-    std::vector<uint64_t> idx(k);
-    b200::check(cb_kmeans_seed_indices(n_, k, seed, idx.data()), "cb_kmeans_seed_indices");
-    centroids_.resize(3, k);
-    for (size_t j = 0; j < k; j++) centroids_.setCol(j, host_.col(idx[j]));
-    return run(max_iter, tol);
-  }
-  const VectorSet3f& getClusterCentroids() const { return centroids_; }
-  size_t getNumberOfPerformedIterations() const { return iterations_; }
-  const PointToClusterIndexMap& getPointToClusterIndexMap() const { return labels_; }
-  const ClusterToPointIndicesMap& getClusterToPointIndicesMap() const { return lists_; }
-  size_t getNumberOfClusters() const { return lists_.size(); }
-  size_t getNumberOfPoints() const { return labels_.size(); }
-
-private:
-  struct std_seed_helper {};
-  KMeans3f& run(size_t max_iter, float tol) {
-    std::vector<uint64_t> lab(n_);
-    cb_kmeans_result r;
-    b200::check(cb_kmeans_cluster(b200::Context::get(), cloud_.h, centroids_.data(), centroids_.cols(), max_iter, tol,
-                                  lab.data(), &r),
-                "cb_kmeans_cluster");
-    iterations_ = r.iterations;
-    labels_.assign(lab.begin(), lab.end());
-    lists_.assign(centroids_.cols(), {});  // clustering_base.hpp:22-32
-    for (size_t i = 0; i < labels_.size(); i++)
-      if ((size_t)labels_[i] < lists_.size()) lists_[labels_[i]].emplace_back((PointIndexT)i);
-    return *this;
-  }
-  size_t n_;
-  ConstVectorSetMatrixMap3f host_;
-  b200::CloudHandle cloud_;
-  VectorSet3f centroids_;
-  size_t iterations_ = 0;
-  PointToClusterIndexMap labels_;
-  ClusterToPointIndicesMap lists_;
-};
-
-// ---- KMeans<float, D> / KMeans2f<> / KMeansXf<> ----------------------------------------------------------
+// ---- KMeans<float, D> / KMeans2f<> / KMeans3f<> / KMeansXf<> ---------------------------------------------
 // The distance adaptors of core/kd_tree.hpp:40-61, as tags: k-means has a device path for L2 and L2Simple only.
 namespace KDTreeDistanceAdaptors {
 template <class DataAdaptor>
@@ -1501,6 +1443,9 @@ private:
 template <template <class> class DistAdaptor = KDTreeDistanceAdaptors::L2, typename PointIndexT = size_t,
           typename ClusterIndexT = size_t>
 using KMeans2f = KMeans<float, 2, DistAdaptor, PointIndexT, ClusterIndexT>;
+template <template <class> class DistAdaptor = KDTreeDistanceAdaptors::L2, typename PointIndexT = size_t,
+          typename ClusterIndexT = size_t>
+using KMeans3f = KMeans<float, 3, DistAdaptor, PointIndexT, ClusterIndexT>;
 template <template <class> class DistAdaptor = KDTreeDistanceAdaptors::L2, typename PointIndexT = size_t,
           typename ClusterIndexT = size_t>
 using KMeansXf = KMeans<float, b200::kDynamic, DistAdaptor, PointIndexT, ClusterIndexT>;

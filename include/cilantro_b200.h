@@ -443,7 +443,8 @@ int cb_kmeans_seed_indices(size_t n, size_t k, uint32_t seed, uint64_t* out_idx)
 
 /* ---- D-dimensional vector sets and k-means over them -------------------------------------------
  * A cb_vectors holds n x D float32 rows in HBM, point-major: the bytes a ConstVectorSetMatrixMap<float, D>
- * (core/data_containers.hpp:73-112) wraps. D >= 1; D <= 0 or a null pointer is CB_ERR_INVALID. */
+ * (core/data_containers.hpp:73-112) wraps. D >= 1; D <= 0 or a null pointer is CB_ERR_INVALID, except a null data
+ * pointer with n = 0 (an empty set, as for clouds). */
 int cb_vectors_create(cb_context* ctx, const float* data, size_t n, int D, cb_vectors** out);
 int cb_vectors_create_from_device(cb_context* ctx, const float* d_data, size_t n, int D, cb_vectors** out);
 void cb_vectors_destroy(cb_vectors* v);

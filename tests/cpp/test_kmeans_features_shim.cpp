@@ -1,5 +1,5 @@
-// KMeans<float, 6>, KMeansXf<> and KMeans2f<> (include/cilantro/b200_shims.hpp) on rows read from a file, for
-// comparison with the C ABI's results (tests/test_kmeans_features_shims.py).
+// KMeans<float, 6>, KMeans3f<>, KMeansXf<> and KMeans2f<> (include/cilantro/b200_shims.hpp) on rows read from a file,
+// for comparison with the C ABI's results (tests/test_kmeans_features_shims.py), and on empty sets.
 //
 //   test_kmeans_features_shim in.bin out.bin
 //   in:  int64 n, D, k, max_iter, seed; float32 tol; float32 rows [n x D]; float32 centroids [k x D]
@@ -7,9 +7,14 @@
 //        int64 labels [n]
 #include <cilantro/clustering/kmeans.hpp>
 
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
+#include <type_traits>
 #include <vector>
+
+// the reference's alias (clustering/kmeans.hpp:205-207): the distance adaptor first, then the index types
+static_assert(std::is_same<cilantro::KMeans3f<>, cilantro::KMeans<float, 3>>::value, "KMeans3f<> is KMeans<float, 3>");
 
 template <class KM, class Map>
 static void run(FILE* o, const Map& data, const Map& cent, size_t k, size_t max_iter, float tol, uint32_t seed) {
@@ -33,6 +38,29 @@ static void run(FILE* o, const Map& data, const Map& cent, size_t k, size_t max_
   }
 }
 
+// An empty set (its data() may be null) in every dimension: one iteration in which every cluster is empty, so every
+// centroid is 0 * (1 / 0) = NaN, no labels and k empty member lists.
+template <class KM, class Set>
+static bool empty_set_clusters_to_nothing(const Set& cent) {
+  const Set empty;
+  KM km(empty);
+  km.cluster(cent, 10, 0.f);
+  const auto& c = km.getClusterCentroids();
+  bool ok = km.getNumberOfPerformedIterations() == 1 && km.getNumberOfPoints() == 0 && km.getNumberOfClusters() == 3;
+  for (size_t i = 0; i < c.rows() * c.cols(); i++) ok = ok && std::isnan(c.data()[i]);
+  for (const auto& m : km.getClusterToPointIndicesMap()) ok = ok && m.empty();
+  return ok;
+}
+
+static bool empty_sets_cluster_to_nothing() {
+  cilantro::VectorSet<float, 2> c2(2, 3);
+  cilantro::VectorSet3f c3(3, 3);
+  const bool ok = empty_set_clusters_to_nothing<cilantro::KMeans2f<>>(c2) &&
+                  empty_set_clusters_to_nothing<cilantro::KMeans3f<>>(c3);
+  if (!ok) std::fprintf(stderr, "k-means on an empty set\n");
+  return ok;
+}
+
 int main(int argc, char** argv) {
   if (argc != 3) return 2;
   FILE* f = std::fopen(argv[1], "rb");
@@ -52,6 +80,10 @@ int main(int argc, char** argv) {
     using Map = cilantro::ConstVectorSetMatrixMap<float, 6>;
     run<cilantro::KMeans<float, 6, cilantro::KDTreeDistanceAdaptors::L2>>(o, Map(rows.data(), n), Map(cent.data(), k),
                                                                            k, max_iter, tol, seed);
+  } else if (D == 3) {
+    using Map = cilantro::ConstVectorSetMatrixMap<float, 3>;
+    run<cilantro::KMeans3f<cilantro::KDTreeDistanceAdaptors::L2>>(o, Map(rows.data(), n), Map(cent.data(), k), k,
+                                                                   max_iter, tol, seed);
   } else if (D == 2) {
     using Map = cilantro::ConstVectorSetMatrixMap<float, 2>;
     run<cilantro::KMeans2f<cilantro::KDTreeDistanceAdaptors::L2Simple>>(o, Map(rows.data(), n), Map(cent.data(), k),
@@ -61,6 +93,7 @@ int main(int argc, char** argv) {
     run<cilantro::KMeansXf<>>(o, Map(rows.data(), D, n), Map(cent.data(), D, k), k, max_iter, tol, seed);
   }
   std::fclose(o);
+  if (!empty_sets_cluster_to_nothing()) return 1;
   std::printf("k-means shim: D = %zu done\n", D);
   return 0;
 }

@@ -1,14 +1,22 @@
-"""A numpy restatement of k-means over D-dimensional rows (cb_kmeans_*_vectors, DESIGN §4.17; tests only).
+"""A numpy restatement of what the product promises for k-means (cb_kmeans_*, DESIGN §4.3 and §4.17; tests only).
 
+The one restatement for every D: clouds are D = 3, cb_vectors sets any D >= 1. Not the reference's fp32 serial sums
+(the oracle restates those): the contracts of the device code.
   - distance: d = c - p per component in fp32, then the right fold without FMA,
     acc = d[D-1]^2; acc = d[j]^2 + acc for j = D-2 .. 0 (at D = 3: dx*dx + (dy*dy + dz*dz));
-  - assignment: strict '<' over ascending j from +inf (lowest j wins ties, label 0 when no d2 is below +inf);
-  - sums and counts in float64 over the rows whose D components are finite;
-  - the Lloyd loop of kmeans_ransac_ref.kmeans_lloyd (repair, division, stopping rules) with that distance.
+  - assignment: strict '<' over ascending j from +inf (lowest j wins ties; a row whose every d2 is NaN or +inf keeps
+    label 0);
+  - Lloyd loop (cb_kmeans_cluster, cb_kmeans_cluster_vectors): float64 sums and counts over the rows whose D
+    components are finite; the empty-cluster repair in ascending i from the largest count (first index on ties), the
+    old centroid f32(sum) * f32(1 / count), the farthest finite member by the fp32 distance (lowest index on ties), the
+    moved row leaving the sum of its cluster and not entering cluster i's; stop when no label changed (after the first
+    iteration) or, with tol > 0, when the largest fp32 centroid move is < tol^2.
 On dyadic inputs (multiples of 2^-10, |v| < 4) and n small enough, every float64 sum is exact in any order, so the
 device agrees with this restatement bit for bit over whole runs.
 """
 import numpy as np
+
+from kmeans_ransac_ref import dyadic
 
 F32 = np.float32
 
@@ -60,7 +68,7 @@ def sums(pts, labels, k):
 
 
 def lloyd(pts, cent0, max_iter, tol):
-    """cb_kmeans_cluster_vectors restated. Returns (centroids f32 [k, D], labels int64, iterations)."""
+    """cb_kmeans_cluster / cb_kmeans_cluster_vectors restated. Returns (centroids f32 [k, D], labels int64, iterations)."""
     pts = np.asarray(pts, F32)
     cent = np.array(cent0, F32)
     k = len(cent)
@@ -107,8 +115,6 @@ def lloyd(pts, cent0, max_iter, tol):
 
 def lloyd_cases(D, seed=0):
     """Small dyadic Lloyd runs {name: (pts, centroids0, max_iter, tol)} at the loop's edges in D dimensions."""
-    from kmeans_ransac_ref import dyadic
-
     rng = np.random.default_rng(seed + 31 * D)
     shifts = [np.full(D, v, F32) for v in (1.0, -2.0, 0.5)]
     blobs = np.vstack([dyadic(rng, (200, D), 0.25) + c for c in shifts]).astype(F32)
@@ -124,4 +130,28 @@ def lloyd_cases(D, seed=0):
         "max_iter_0": (few, dyadic(rng, (3, D), 2.0), 0, 0.0),
         "max_iter_1": (blobs, blobs[:7].copy(), 1, 0.0),
         "empty_set": (np.zeros((0, D), F32), dyadic(rng, (3, D), 2.0), 5, 0.0),
+    }
+
+
+def cloud_lloyd_cases():
+    """Small dyadic Lloyd runs {name: (pts [n, 3], centroids0, max_iter, tol)} at the loop's edges on clouds (n <= 1500,
+    so the oracle's fp32 sums are exact too)."""
+    rng = np.random.default_rng(20)
+    blobs = np.vstack([dyadic(rng, (300, 3), 0.25) + c for c in ((1, 1, 1), (-2, 0, 1), (0, -2, -1))]).astype(F32)
+    dup = np.repeat(dyadic(rng, (40, 3), 2.0), 5, axis=0)
+    few = dyadic(rng, (5, 3), 2.0)
+    far = dyadic(rng, (8, 3), 3.0)
+    return {
+        # uniform cloud, tol = 0, several iterations
+        "uniform": (dyadic(rng, (1500, 3), 3.0), dyadic(rng, (24, 3), 3.0), 4, 0.0),
+        # three blobs and a tol that stops the loop before the labels settle
+        "tol_stop": (blobs, blobs[[0, 1, 2, 300, 600]].copy(), 50, 0.05),
+        # several clusters empty in the first iteration (centroids far outside the cloud)
+        "many_empty": (dyadic(rng, (800, 3), 1.0), np.vstack([dyadic(rng, (4, 3), 1.0), far + 8.0]).astype(F32), 3, 0.0),
+        # duplicated points: farthest-member ties go to the lowest index
+        "duplicates": (dup, np.vstack([dup[:3], dup[:3] + 40.0]).astype(F32), 3, 0.0),
+        # n < K: repairs cascade, a cluster is emptied again after its turn
+        "n_lt_k": (few, dyadic(rng, (9, 3), 2.0), 3, 0.0),
+        "max_iter_0": (few, dyadic(rng, (3, 3), 2.0), 0, 0.0),
+        "max_iter_1": (blobs, blobs[:7].copy(), 1, 0.0),
     }

@@ -1,18 +1,12 @@
-"""A numpy restatement of what the product promises for k-means and rigid RANSAC scoring (tests only).
+"""A numpy restatement of what the product promises for rigid RANSAC scoring, and the inputs the k-means and RANSAC
+tests share (tests only). k-means is restated once, for every D, in kmeans_features_ref.py.
 
-Not the reference's fp32 serial sums (the oracle restates those): the contracts of the device code.
-  - k-means assignment: d = c - p, d2 = dx*dx + (dy*dy + dz*dz) in fp32 without FMA, j scanned ascending with a
-    strict '<' from +inf (lowest j wins ties; a point whose every d2 is NaN or +inf keeps label 0).
-  - Lloyd loop (cb_kmeans_cluster): float64 sums and counts over the points with three finite coordinates; the
-    empty-cluster repair in ascending i from the largest count (first index on ties), the old centroid
-    f32(sum) * f32(1 / count), the farthest finite member by the fp32 distance (lowest index on ties), the moved
-    point leaving the sum of its cluster and not entering cluster i's; stop when no label changed (after the
-    first iteration) or, with tol > 0, when the largest fp32 centroid move is < tol^2.
+Not the reference's fp32 serial sums (the oracle restates those): the contract of the device code.
   - RANSAC score: q_r = (R_r0 x + (R_r1 y + R_r2 z)) + t_r, e = q - d, x = e0^2 + (e1^2 + e2^2) in fp32, inlier
     iff sqrt_rn(x) <= thresh (numpy's correctly rounded fp32 sqrt: an independent check of the device's
     precomputed x bound).
-On "dyadic" inputs (multiples of 2^-10, |v| < 4) every float64 sum is exact in any order, so the device agrees
-with this restatement bit for bit over whole runs.
+On "dyadic" inputs (multiples of 2^-10, |v| < 4) every float64 sum is exact in any order: the device's double
+atomics then agree with a float64 restatement bit for bit over whole runs.
 """
 import numpy as np
 
@@ -25,115 +19,6 @@ def dyadic(rng, shape, lim=4.0):
     """Multiples of 2^-10 in (-lim, lim), as float32."""
     m = int(lim * 1024) - 1
     return (rng.integers(-m, m + 1, size=shape) / 1024.0).astype(F32)
-
-
-def finite_rows(pts):
-    return np.isfinite(np.asarray(pts, F32)).all(1)
-
-
-def _d2(c, p):
-    """fp32 contract distance between centroid(s) c [k, 3] and points p [n, 3] -> [n, k]."""
-    c = np.asarray(c, F32)
-    p = np.asarray(p, F32)
-    with np.errstate(invalid="ignore", over="ignore"):
-        dx = c[None, :, 0] - p[:, None, 0]
-        dy = c[None, :, 1] - p[:, None, 1]
-        dz = c[None, :, 2] - p[:, None, 2]
-        return dx * dx + (dy * dy + dz * dz)
-
-
-def kmeans_assign(pts, cent, chunk=1 << 22):
-    """Labels (int64) of the strict-'<' ascending scan."""
-    pts, cent = np.asarray(pts, F32).reshape(-1, 3), np.asarray(cent, F32).reshape(-1, 3)
-    n, k = len(pts), len(cent)
-    labels = np.zeros(n, np.int64)
-    step = max(1, chunk // max(k, 1))
-    for a in range(0, n, step):
-        d = _d2(cent, pts[a:a + step])
-        d[np.isnan(d)] = np.inf
-        best = d.argmin(1)
-        labels[a:a + step] = np.where(d[np.arange(len(d)), best] < np.inf, best, 0)
-    return labels
-
-
-def kmeans_sums(pts, labels, k):
-    """float64 per-cluster sums [k, 3] and counts [k] over the finite points."""
-    pts = np.asarray(pts, F32).reshape(-1, 3)
-    fin = finite_rows(pts)
-    s = np.zeros((k, 3))
-    np.add.at(s, labels[fin], pts[fin].astype(np.float64))
-    return s, np.bincount(labels[fin], minlength=k).astype(np.int64)
-
-
-def kmeans_lloyd(pts, cent0, max_iter, tol):
-    """cb_kmeans_cluster restated. Returns (centroids f32 [k, 3], labels int64, iterations)."""
-    pts = np.asarray(pts, F32).reshape(-1, 3)
-    cent = np.array(cent0, F32).reshape(-1, 3)
-    k = len(cent)
-    fin = finite_rows(pts)
-    labels = np.zeros(len(pts), np.int64)
-    tol_sq = F32(tol) * F32(tol)
-    it = 0
-    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
-        while it < max_iter:
-            new = kmeans_assign(pts, cent)
-            changed = bool((new != labels).any())
-            labels = new
-            if not changed and it > 0:
-                break
-            old = cent.copy()
-            s, cnt = kmeans_sums(pts, labels, k)
-            for i in range(k):
-                if cnt[i] != 0:
-                    continue
-                max_ind = int(np.argmax(cnt))
-                inv = F32(1.0) / F32(cnt[max_ind])
-                oc = s[max_ind].astype(F32) * inv
-                members = np.flatnonzero((labels == max_ind) & fin)
-                if len(members) == 0:
-                    continue
-                key = _d2(oc[None], pts[members])[:, 0].view(np.uint32)
-                j = int(members[int(np.argmax(key))])
-                labels[j] = i
-                s[max_ind] -= pts[j].astype(np.float64)
-                cnt[max_ind] -= 1
-                cnt[i] += 1
-            inv = F32(1.0) / cnt.astype(F32)
-            cent = s.astype(F32) * inv[:, None]
-            it += 1
-            if tol > 0:
-                mv = _d2(cent, old)[np.arange(k), np.arange(k)]
-                mx = F32(0.0)
-                for v in mv:  # std::max(mx, v)
-                    if mx < v:
-                        mx = v
-                if mx < tol_sq:
-                    break
-    return cent, labels, it
-
-
-def lloyd_cases():
-    """Small dyadic Lloyd runs {name: (pts, centroids0, max_iter, tol)} at the loop's edges (n <= 1500, so the
-    oracle's fp32 sums are exact too)."""
-    rng = np.random.default_rng(20)
-    blobs = np.vstack([dyadic(rng, (300, 3), 0.25) + c for c in ((1, 1, 1), (-2, 0, 1), (0, -2, -1))]).astype(np.float32)
-    dup = np.repeat(dyadic(rng, (40, 3), 2.0), 5, axis=0)
-    few = dyadic(rng, (5, 3), 2.0)
-    far = dyadic(rng, (8, 3), 3.0)
-    return {
-        # uniform cloud, tol = 0, several iterations
-        "uniform": (dyadic(rng, (1500, 3), 3.0), dyadic(rng, (24, 3), 3.0), 4, 0.0),
-        # three blobs and a tol that stops the loop before the labels settle
-        "tol_stop": (blobs, blobs[[0, 1, 2, 300, 600]].copy(), 50, 0.05),
-        # several clusters empty in the first iteration (centroids far outside the cloud)
-        "many_empty": (dyadic(rng, (800, 3), 1.0), np.vstack([dyadic(rng, (4, 3), 1.0), far + 8.0]).astype(np.float32), 3, 0.0),
-        # duplicated points: farthest-member ties go to the lowest index
-        "duplicates": (dup, np.vstack([dup[:3], dup[:3] + 40.0]).astype(np.float32), 3, 0.0),
-        # n < K: repairs cascade, a cluster is emptied again after its turn
-        "n_lt_k": (few, dyadic(rng, (9, 3), 2.0), 3, 0.0),
-        "max_iter_0": (few, dyadic(rng, (3, 3), 2.0), 0, 0.0),
-        "max_iter_1": (blobs, blobs[:7].copy(), 1, 0.0),
-    }
 
 
 def ransac_x(dst, src, T_h):

@@ -99,9 +99,9 @@ def test_non_finite_rows_change_nothing_else(cb, ctx, D):
     assert rit == res["iterations"] and np.array_equal(res["labels"], rl) and _same_f32(res["centroids"], rc)
 
 
-@pytest.mark.parametrize("case", list(kr.lloyd_cases()))
+@pytest.mark.parametrize("case", list(kf.cloud_lloyd_cases()))
 def test_d3_vectors_equal_cloud(cb, ctx, case):
-    pts, cent0, max_iter, tol = kr.lloyd_cases()[case]
+    pts, cent0, max_iter, tol = kf.cloud_lloyd_cases()[case]
     a = cb.kmeans_cluster(ctx, cb.Cloud(ctx, pts), cent0, max_iter=max_iter, tol=tol)
     b = cb.kmeans_cluster(ctx, cb.Vectors(ctx, pts), cent0, max_iter=max_iter, tol=tol)
     assert a["iterations"] == b["iterations"] and a["kernel_launches"] == b["kernel_launches"]

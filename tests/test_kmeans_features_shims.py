@@ -1,7 +1,7 @@
-"""The C++ drop-ins for D-dimensional k-means (KMeans<float, D>, KMeans2f<>, KMeansXf<>, VectorSet<float, D>,
+"""The C++ drop-ins for k-means (KMeans<float, D>, KMeans2f<>, KMeans3f<>, KMeansXf<>, VectorSet<float, D>,
 ConstVectorSetMatrixMap<float, D>): they compile without Eigen and with the Eigen stub (or a real Eigen), the
 combinations the device path does not cover stay compile-time errors, and on the GPU the shim program gives the C ABI's
-results bit for bit and the coloured k-means example runs."""
+results bit for bit, clusters empty sets, and the coloured k-means example runs."""
 import os
 
 import numpy as np
@@ -51,7 +51,7 @@ def _case(D, seed):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("D", [6, 2, 5])
+@pytest.mark.parametrize("D", [6, 2, 3, 5])
 def test_shim_program_equals_capi(cb, ctx, tmp_path, D):
     pts, cent0 = _case(D, D)
     n, k, max_iter, seed, tol = len(pts), len(cent0), 20, 7, 1e-4

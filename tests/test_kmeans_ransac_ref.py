@@ -1,4 +1,5 @@
-"""Pins the numpy restatement of k-means and RANSAC scoring (kmeans_ransac_ref.py) against the oracle on the CPU.
+"""Pins the numpy restatements of k-means at D = 3 (kmeans_features_ref.py) and of RANSAC scoring (kmeans_ransac_ref.py)
+against the oracle on the CPU.
 
 On small dyadic inputs the oracle's fp32 serial sums are exact, so its Lloyd loop (the reference's) and the
 restatement's float64 one must agree bit for bit, repairs and tol stops included. The oracle's RANSAC scan is the
@@ -6,6 +7,7 @@ reference's sqrt(x) <= thresh, which the restatement states independently."""
 import numpy as np
 import pytest
 
+import kmeans_features_ref as kf
 import kmeans_ransac_ref as kr
 
 
@@ -14,11 +16,11 @@ def _same_f32(a, b):
     return a.shape == b.shape and bool(np.all((a.view(np.uint32) == b.view(np.uint32)) | (np.isnan(a) & np.isnan(b))))
 
 
-@pytest.mark.parametrize("case", list(kr.lloyd_cases()))
+@pytest.mark.parametrize("case", list(kf.cloud_lloyd_cases()))
 def test_lloyd_restatement_equals_oracle_on_dyadic_inputs(orc, case):
-    pts, cent0, max_iter, tol = kr.lloyd_cases()[case]
+    pts, cent0, max_iter, tol = kf.cloud_lloyd_cases()[case]
     oc, ol, oit = orc.kmeans(pts, cent0, max_iter=max_iter, tol=tol)
-    rc, rl, rit = kr.kmeans_lloyd(pts, cent0, max_iter, tol)
+    rc, rl, rit = kf.lloyd(pts, cent0, max_iter, tol)
     assert rit == oit
     assert np.array_equal(rl, ol)
     assert _same_f32(rc, oc)
@@ -33,12 +35,21 @@ def test_assign_restatement_equals_oracle(orc):
     pts = kr.dyadic(rng, (3000, 3), 3.0)
     cent = np.vstack([kr.dyadic(rng, (300, 3), 3.0)] * 2)  # every point ties between j and j + 300
     want, _ = orc.kmeans_assign(pts, cent)
-    got = kr.kmeans_assign(pts, cent)
+    got = kf.assign(pts, cent)
     assert np.array_equal(got, want.astype(np.int64)) and got.max() < 300
     # a finite point whose every squared distance overflows keeps label 0
     big = np.array([[3e19, 0, 0], [-3e19, 3e19, 0]], np.float32)
     want, _ = orc.kmeans_assign(big, cent)
-    assert not kr.kmeans_assign(big, cent).any() and not want.any()
+    assert not kf.assign(big, cent).any() and not want.any()
+    # non-finite rows keep label 0, and a duplicated centroid loses every tie to its first copy
+    rng = np.random.default_rng(1)
+    pts = rng.standard_normal((5000, 3)).astype(np.float32)
+    pts[::97] = kr.BAD_ROWS[np.arange(len(pts[::97])) % len(kr.BAD_ROWS)]
+    cent = rng.standard_normal((77, 3)).astype(np.float32)
+    cent[5] = cent[3]
+    want, _ = orc.kmeans_assign(pts, cent)
+    got = kf.assign(pts, cent)
+    assert np.array_equal(got, want.astype(np.int64)) and not got[::97].any() and not (got == 5).any()
 
 
 @pytest.mark.parametrize("n", [1, 31, 1025])
