@@ -17,6 +17,7 @@
 // (4) one thread per bin replays the reference's sequential accumulation; (5) optional re-ordering of
 // the bins by their first point index, compaction by min_points_in_bin, emit.
 #include "cb_internal.hpp"
+#include "launch.cuh"
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -33,10 +34,6 @@ struct BinGrid {
   uint64_t ny, nz;
   uint64_t none;            // key of a point with a non-finite coordinate: one past the largest bin key
 };
-
-inline int blocks_for(const cb_context* ctx, size_t n) {
-  return (int)std::max<size_t>(1, std::min<size_t>((n + kThreads - 1) / kThreads, (size_t)ctx->sm_count * 16));
-}
 
 // (ptrdiff_t)std::floor(point[i] * bin_size_inv_[i]) relative to the cloud's minimum bin. The bounding box
 // covers every finite coordinate, so a finite point's bin lies inside the grid.
@@ -222,12 +219,10 @@ int downsample_device(cb_context* ctx, DeviceScope& out, const float* d_raw, con
   CB_TRY(bufs.alloc(&d_vals, n));
   CB_TRY(bufs.alloc(&d_vals2, n));
   CB_TRY(bufs.alloc(&d_flags, n + 2));
-  const int nb = blocks_for(ctx, n);
-  bin_key_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_raw, n, g, d_keys, d_vals);
-  ctx->launches += 1;
+  const int nb = grid_for(ctx, n, kThreads, 16);
+  CB_TRY(launch(ctx, bin_key_kernel, nb, kThreads, 0, d_raw, n, g, d_keys, d_vals));
   CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_vals, d_keys2, d_vals2, n, key_bits));
-  head_flag_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_keys, n, g.none, d_flags);
-  ctx->launches += 1;
+  CB_TRY(launch(ctx, head_flag_kernel, nb, kThreads, 0, d_keys, n, g.none, d_flags));
   CB_TRY(exclusive_scan_u32(ctx, d_flags, n + 1, 0u));  // flags[n] = number of bins; flags[n + 1] = sentinel
   uint32_t nbins = 0;
   CB_CUDA(cudaMemcpyAsync(&nbins, d_flags + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -235,7 +230,7 @@ int downsample_device(cb_context* ctx, DeviceScope& out, const float* d_raw, con
   CB_CHECK(nbins <= n, CB_ERR_CUDA, "internal: inconsistent bin count");
   if (nbins == 0) return CB_OK;  // no point with three finite coordinates
   CB_TRY(bufs.alloc(&d_start, (size_t)nbins + 1));
-  bin_start_kernel<<<nb, kThreads, 0, ctx->stream>>>(d_keys, n, g.none, d_flags, d_start);
+  CB_TRY(launch(ctx, bin_start_kernel, nb, kThreads, 0, d_keys, n, g.none, d_flags, d_start));
   BinOut o;
   o.nrm = nullptr;
   o.col = nullptr;
@@ -244,22 +239,18 @@ int downsample_device(cb_context* ctx, DeviceScope& out, const float* d_raw, con
   if (d_col) CB_TRY(bufs.alloc(&o.col, 3 * (size_t)nbins));
   CB_TRY(bufs.alloc(&o.cnt, nbins));
   CB_TRY(bufs.alloc(&o.first, nbins));
-  const int bb = blocks_for(ctx, nbins);
-  bin_reduce_kernel<<<bb, kThreads, 0, ctx->stream>>>(d_raw, d_nrm, d_col, d_vals, d_start, nbins, o);
-  ctx->launches += 2;
-  CB_CUDA(cudaGetLastError());
+  const int bb = grid_for(ctx, nbins, kThreads, 16);
+  CB_TRY(launch(ctx, bin_reduce_kernel, bb, kThreads, 0, d_raw, d_nrm, d_col, d_vals, d_start, nbins, o));
   // output order
   uint32_t* d_rank_bin = nullptr;
   if (order == 1 && nbins > 1) {  // first-occurrence order (serial build): sort the bins by their first index
-    first_key_kernel<<<bb, kThreads, 0, ctx->stream>>>(o.first, nbins, d_keys, d_vals);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, first_key_kernel, bb, kThreads, 0, o.first, nbins, d_keys, d_vals));
     CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_vals, d_keys2, d_vals2, nbins, bits_for(n)));
     d_rank_bin = d_vals;
   }
   size_t m = nbins;
   const uint32_t minp = (uint32_t)std::min<size_t>(min_points, 0xffffffffu);
-  valid_flag_kernel<<<bb, kThreads, 0, ctx->stream>>>(d_rank_bin, o.cnt, nbins, minp, d_flags);
-  ctx->launches += 1;
+  CB_TRY(launch(ctx, valid_flag_kernel, bb, kThreads, 0, d_rank_bin, o.cnt, nbins, minp, d_flags));
   CB_TRY(exclusive_scan_u32(ctx, d_flags, (size_t)nbins + 1, 0u));
   if (minp > 1) {
     uint32_t mm = 0;
@@ -273,9 +264,7 @@ int downsample_device(cb_context* ctx, DeviceScope& out, const float* d_raw, con
   CB_TRY(out.alloc(&r_pts, 3 * m));
   if (d_nrm && out_nrm) CB_TRY(out.alloc(&r_nrm, 3 * m));
   if (d_col && out_col) CB_TRY(out.alloc(&r_col, 3 * m));
-  emit_kernel<<<bb, kThreads, 0, ctx->stream>>>(d_rank_bin, d_flags, o, nbins, minp, r_pts, r_nrm, r_col);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, emit_kernel, bb, kThreads, 0, d_rank_bin, d_flags, o, nbins, minp, r_pts, r_nrm, r_col));
   *out_pts = r_pts;
   if (r_nrm) *out_nrm = r_nrm;
   if (r_col) *out_col = r_col;

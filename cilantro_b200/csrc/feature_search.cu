@@ -13,16 +13,13 @@
 #include "feature_rule.hpp"
 #include "feature_search.cuh"
 #include "grid_sweep.cuh"
+#include "launch.cuh"
 
 namespace cb {
 
 namespace {
 
 constexpr int kThreads = 256;
-
-inline int blocks_for(const cb_context* ctx, size_t n) {
-  return (int)std::max<size_t>(1, std::min<size_t>((n + kThreads - 1) / kThreads, (size_t)ctx->sm_count * 16));
-}
 
 template <int NT>
 __device__ __forceinline__ void load_tails(const float4* __restrict__ tails, uint32_t i, int kind, const Rigid* T,
@@ -100,30 +97,17 @@ int launch_feature_gather(cb_context* ctx, int kind, const float4* pts, uint32_t
                           float4* out) {
   if (n == 0) return CB_OK;
   const Rigid Tv = T ? *T : rigid_from_t12(nullptr);
-  const int nb = blocks_for(ctx, n);
-  if (rule::feature_tails(kind) == 2)
-    feature_gather_kernel<2><<<nb, kThreads, 0, ctx->stream>>>(kind, pts, n, raw, Tv, T != nullptr, out);
-  else
-    feature_gather_kernel<1><<<nb, kThreads, 0, ctx->stream>>>(kind, pts, n, raw, Tv, T != nullptr, out);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  auto kernel = rule::feature_tails(kind) == 2 ? feature_gather_kernel<2> : feature_gather_kernel<1>;
+  return launch(ctx, kernel, grid_for(ctx, n, kThreads, 16), kThreads, 0, kind, pts, n, raw, Tv, T != nullptr, out);
 }
 
 int launch_feature_nn(cb_context* ctx, int kind, const GridView& g, const float4* g_tails, const float4* q_pts,
                       uint32_t n_q, const float4* q_tails, const Rigid& T, bool rotate, float max_d2, int* out_idx,
                       float* out_d2) {
   if (n_q == 0) return CB_OK;
-  const int nb = blocks_for(ctx, n_q);
-  if (rule::feature_tails(kind) == 2)
-    feature_nn_kernel<2><<<nb, kThreads, 0, ctx->stream>>>(kind, g, g_tails, q_pts, n_q, q_tails, T, rotate, max_d2,
-                                                          out_idx, out_d2);
-  else
-    feature_nn_kernel<1><<<nb, kThreads, 0, ctx->stream>>>(kind, g, g_tails, q_pts, n_q, q_tails, T, rotate, max_d2,
-                                                          out_idx, out_d2);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  auto kernel = rule::feature_tails(kind) == 2 ? feature_nn_kernel<2> : feature_nn_kernel<1>;
+  return launch(ctx, kernel, grid_for(ctx, n_q, kThreads, 16), kThreads, 0, kind, g, g_tails, q_pts, n_q, q_tails, T,
+                rotate, max_d2, out_idx, out_d2);
 }
 
 }  // namespace cb

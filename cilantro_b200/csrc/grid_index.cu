@@ -9,6 +9,7 @@
 //   holds more than kHugeCell points, one stable radix sort of (cell, index)) -> gather into the
 //   cell-sorted float4 arrays. Either way every cell lists its points in ascending original index.
 #include "cb_internal.hpp"
+#include "launch.cuh"
 #include "nn_search.cuh"
 #include <cfloat>
 #include <cmath>
@@ -333,12 +334,6 @@ __global__ void block_emit_kernel(const uint32_t* __restrict__ cnt, const uint32
   }
 }
 
-inline int grid_blocks(const cb_context* ctx, size_t n, int per_sm = 8) {
-  size_t want = (n + kThreads - 1) / kThreads;
-  size_t cap = (size_t)ctx->sm_count * per_sm;
-  return (int)std::max<size_t>(1, std::min(want, cap));
-}
-
 }  // namespace
 
 int exclusive_scan_u32(cb_context* ctx, uint32_t* d_data, size_t n, uint32_t total) {
@@ -347,11 +342,9 @@ int exclusive_scan_u32(cb_context* ctx, uint32_t* d_data, size_t n, uint32_t tot
   DeviceScope scope(ctx);
   uint32_t* d_sums = nullptr;
   CB_TRY(scope.alloc(&d_sums, nblocks));
-  scan_block_kernel<<<(unsigned)nblocks, kThreads, 0, ctx->stream>>>(d_data, n, d_sums);
-  scan_sums_kernel<<<1, 1024, 0, ctx->stream>>>(d_sums, nblocks);
-  scan_add_kernel<<<(unsigned)nblocks, kThreads, 0, ctx->stream>>>(d_data, n, d_sums, total);
-  ctx->launches += 3;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, scan_block_kernel, (unsigned)nblocks, kThreads, 0, d_data, n, d_sums));
+  CB_TRY(launch(ctx, scan_sums_kernel, 1, 1024, 0, d_sums, nblocks));
+  CB_TRY(launch(ctx, scan_add_kernel, (unsigned)nblocks, kThreads, 0, d_data, n, d_sums, total));
   return CB_OK;
 }
 
@@ -359,9 +352,8 @@ int points_bbox(cb_context* ctx, const float* d_raw, size_t n, float mn[3], floa
   DeviceScope scope(ctx);
   int* d_bb = nullptr;
   CB_TRY(scope.alloc(&d_bb, 6));
-  bbox_init_kernel<<<1, 32, 0, ctx->stream>>>(d_bb);
-  bbox_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_raw, n, d_bb);
-  ctx->launches += 2;
+  CB_TRY(launch(ctx, bbox_init_kernel, 1, 32, 0, d_bb));
+  CB_TRY(launch(ctx, bbox_kernel, grid_for(ctx, n, kThreads), kThreads, 0, d_raw, n, d_bb));
   int h_bb[6];
   CB_CUDA(cudaMemcpyAsync(h_bb, d_bb, sizeof(h_bb), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -441,9 +433,8 @@ int ensure_index(cb_cloud* c) {
     CB_TRY(scope.alloc(&d_hist, ncells + 1));
     CB_CUDA(cudaMemsetAsync(d_hist, 0, (ncells + 1) * sizeof(uint32_t), ctx->stream));
     CB_CUDA(cudaMemsetAsync(d_stats, 0, 2 * sizeof(unsigned long long), ctx->stream));
-    hist_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(c->d_raw, n, gp, d_cell_id, d_hist);
-    occupancy_kernel<<<grid_blocks(ctx, ncells), kThreads, 0, ctx->stream>>>(d_hist, ncells, d_stats);
-    ctx->launches += 2;
+    CB_TRY(launch(ctx, hist_kernel, grid_for(ctx, n, kThreads), kThreads, 0, c->d_raw, n, gp, d_cell_id, d_hist));
+    CB_TRY(launch(ctx, occupancy_kernel, grid_for(ctx, ncells, kThreads), kThreads, 0, d_hist, ncells, d_stats));
     unsigned long long h_stats[2];
     CB_CUDA(cudaMemcpyAsync(h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -486,11 +477,11 @@ int ensure_index(cb_cloud* c) {
     CB_TRY(scope.alloc(&d_big, big_cap + 1));
     CB_CUDA(cudaMemsetAsync(d_big, 0, sizeof(uint32_t), ctx->stream));
     CB_TRY(scope.alloc(&d_tmp, n));
-    scatter_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_cell_id, n, d_hist, d_cursor, d_perm);
-    sort_small_cells_kernel<<<grid_blocks(ctx, ncells), kThreads, 0, ctx->stream>>>(d_hist, ncells, d_perm,
-                                                                                   d_big + 1, d_big);
-    sort_big_cells_kernel<<<ctx->sm_count * 2, kThreads, 0, ctx->stream>>>(d_hist, d_big + 1, d_big, d_perm, d_tmp);
-    ctx->launches += 3;
+    CB_TRY(launch(ctx, scatter_kernel, grid_for(ctx, n, kThreads), kThreads, 0, d_cell_id, n, d_hist, d_cursor,
+                  d_perm));
+    CB_TRY(launch(ctx, sort_small_cells_kernel, grid_for(ctx, ncells, kThreads), kThreads, 0, d_hist, ncells, d_perm,
+                  d_big + 1, d_big));
+    CB_TRY(launch(ctx, sort_big_cells_kernel, ctx->sm_count * 2, kThreads, 0, d_hist, d_big + 1, d_big, d_perm, d_tmp));
   } else {
     // a rank sort of a cell this large would cost O(m^2): sort (cell, index) pairs of the whole cloud instead
     uint64_t* d_keys = nullptr;
@@ -499,8 +490,7 @@ int ensure_index(cb_cloud* c) {
     CB_TRY(scope.alloc(&d_keys, n));
     CB_TRY(scope.alloc(&d_keys_tmp, n));
     CB_TRY(scope.alloc(&d_vals_tmp, n));
-    cell_keys_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(d_cell_id, n, d_keys, d_perm);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, cell_keys_kernel, grid_for(ctx, n, kThreads), kThreads, 0, d_cell_id, n, d_keys, d_perm));
     int bits = 1;
     while (bits < 32 && ((ncells - 1) >> bits) != 0) ++bits;
     CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_perm, d_keys_tmp, d_vals_tmp, n, bits));
@@ -509,9 +499,8 @@ int ensure_index(cb_cloud* c) {
   float4 *d_pts = nullptr, *d_nrm = nullptr;
   CB_TRY(scope.alloc(&d_pts, n));
   if (c->d_raw_nrm) CB_TRY(scope.alloc(&d_nrm, n));
-  gather_kernel<<<grid_blocks(ctx, n), kThreads, 0, ctx->stream>>>(c->d_raw, c->d_raw_nrm, d_perm, n, d_pts, d_nrm);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, gather_kernel, grid_for(ctx, n, kThreads), kThreads, 0, c->d_raw, c->d_raw_nrm, d_perm, n, d_pts,
+                d_nrm));
   // 6. coarse occupancy: the list of non-empty 8x8x8-cell blocks for the far-query path
   uint4* d_blocks = nullptr;
   {
@@ -521,15 +510,14 @@ int ensure_index(cb_cloud* c) {
     uint32_t* d_cnt = nullptr;
     CB_TRY(scope.alloc(&d_cnt, 2 * nb + 2));
     uint32_t* d_flag = d_cnt + nb;  // nb + 2 entries
-    block_count_kernel<<<grid_blocks(ctx, (nb + 1) * 32), kThreads, 0, ctx->stream>>>(d_hist, gp.nx, gp.ny, gp.nz, bx, by, bz,
-                                                                         d_cnt, d_flag);
+    CB_TRY(launch(ctx, block_count_kernel, grid_for(ctx, (nb + 1) * 32, kThreads), kThreads, 0, d_hist, gp.nx, gp.ny,
+                  gp.nz, bx, by, bz, d_cnt, d_flag));
     CB_TRY(exclusive_scan_u32(ctx, d_flag, nb + 1, 0u));
     // at most min(nb, n) blocks are non-empty: sized without waiting for the count, which is read back at
     // the final synchronise below
     CB_TRY(scope.alloc(&d_blocks, std::min(nb, n)));
-    block_emit_kernel<<<grid_blocks(ctx, nb), kThreads, 0, ctx->stream>>>(d_cnt, d_flag, bx, by, bz, d_blocks);
-    ctx->launches += 2;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, block_emit_kernel, grid_for(ctx, nb, kThreads), kThreads, 0, d_cnt, d_flag, bx, by, bz,
+                  d_blocks));
     CB_CUDA(cudaMemcpyAsync(&c->nblocks, d_flag + nb, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   }
   CB_CUDA(cudaStreamSynchronize(ctx->stream));

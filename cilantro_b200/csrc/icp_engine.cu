@@ -23,6 +23,7 @@
 #include "feature_search.cuh"
 #include "icp_accumulate.cuh"
 #include "icp_kernels.cuh"
+#include "launch.cuh"
 #include "reduce.cuh"
 #include <algorithm>
 #include <cmath>
@@ -33,10 +34,6 @@ namespace cb {
 namespace {
 
 constexpr int kThreads = 256;
-
-inline int blocks_for(const cb_context* ctx, size_t n) {
-  return (int)std::max<size_t>(1, std::min<size_t>((n + kThreads - 1) / kThreads, (size_t)ctx->sm_count * 16));
-}
 
 using Dev = DeviceScope;  // scoped stream-ordered allocations (cb_internal.hpp)
 
@@ -163,15 +160,12 @@ struct PairBufs {
 
 int sort_pairs(cb_context* ctx, PairBufs& b, uint32_t m, int kind, int high_bits, int low_bits) {
   if (m <= 1) return CB_OK;
-  const int nb = blocks_for(ctx, m);
-  pair_key_kernel<<<nb, kThreads, 0, ctx->stream>>>(b.f[b.cur], b.s[b.cur], b.d[b.cur], m, kind, low_bits, b.keys[0],
-                                                   b.vals[0]);
-  ctx->launches += 1;
+  const int nb = grid_for(ctx, m, kThreads, 16);
+  CB_TRY(launch(ctx, pair_key_kernel, nb, kThreads, 0, b.f[b.cur], b.s[b.cur], b.d[b.cur], m, kind, low_bits, b.keys[0],
+                b.vals[0]));
   CB_TRY(radix_sort_pairs_u64(ctx, b.keys[0], b.vals[0], b.keys[1], b.vals[1], m, high_bits + low_bits));
-  pair_gather_kernel<<<nb, kThreads, 0, ctx->stream>>>(b.vals[0], m, b.f[b.cur], b.s[b.cur], b.d[b.cur],
-                                                      b.f[b.cur ^ 1], b.s[b.cur ^ 1], b.d[b.cur ^ 1]);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, pair_gather_kernel, nb, kThreads, 0, b.vals[0], m, b.f[b.cur], b.s[b.cur], b.d[b.cur],
+                b.f[b.cur ^ 1], b.s[b.cur ^ 1], b.d[b.cur ^ 1]));
   b.cur ^= 1;
   return CB_OK;
 }
@@ -221,27 +215,18 @@ __global__ void __launch_bounds__(kReduceBlock) pairs_pass_kernel(const IcpArgs 
 
 int launch_pairs_pass(cb_context* ctx, const IcpArgs& a, const EnginePairs& pairs, const cb_cloud* dst,
                       const cb_cloud* src, int mode, bool has_pt, bool has_pl) {
-  const int blocks = std::max(1, std::min(ctx->sm_count * 4, (int)((pairs.count + kReduceBlock - 1) / kReduceBlock)));
+  const int blocks = grid_for(ctx, pairs.count, kReduceBlock, 4);
   IcpArgs args = a;
   CB_TRY(get_reduce_scratch(ctx, blocks, kMaxValues, &args.rs));
   args.rs.ex.enabled = 0;
   ctx->pass_armed = false;
   const float* src_nrm = (mode == kModeCombined) ? src->d_raw_nrm : nullptr;
-  if (mode == kModeP2PCentered)
-    pairs_pass_kernel<kModeP2PCentered><<<blocks, kReduceBlock, 0, ctx->stream>>>(args, pairs.first, pairs.second, pairs.d2,
-                                                                                pairs.count, dst->d_raw, dst->d_raw_nrm, src->d_raw,
-                                                                                src_nrm, false, false);
-  else if (mode == kModeP2P)
-    pairs_pass_kernel<kModeP2P><<<blocks, kReduceBlock, 0, ctx->stream>>>(args, pairs.first, pairs.second, pairs.d2,
-                                                                        pairs.count, dst->d_raw, dst->d_raw_nrm, src->d_raw, src_nrm,
-                                                                        false, false);
-  else
-    pairs_pass_kernel<kModeCombined><<<blocks, kReduceBlock, 0, ctx->stream>>>(
-        args, pairs.first, pairs.second, pairs.d2, pairs.count, dst->d_raw, dst->d_raw_nrm, src->d_raw, src_nrm, has_pt,
-        has_pl);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  auto kernel = mode == kModeP2PCentered ? pairs_pass_kernel<kModeP2PCentered>
+                : mode == kModeP2P       ? pairs_pass_kernel<kModeP2P>
+                                         : pairs_pass_kernel<kModeCombined>;
+  // only the combined metric reads has_pt / has_pl
+  return launch(ctx, kernel, blocks, kReduceBlock, 0, args, pairs.first, pairs.second, pairs.d2, pairs.count,
+                dst->d_raw, dst->d_raw_nrm, src->d_raw, src_nrm, has_pt, has_pl);
 }
 
 int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const cb_cloud* src,
@@ -332,12 +317,10 @@ int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, 
     CB_TRY(dev.alloc(&b.vals[k], total));
   }
   CB_TRY(dev.alloc(&b.flags, (size_t)total + 2));
-  const int nb = blocks_for(ctx, total);
-  candidate_flag_kernel<<<nb, kThreads, 0, ctx->stream>>>(c, total, b.flags);
+  const int nb = grid_for(ctx, total, kThreads, 16);
+  CB_TRY(launch(ctx, candidate_flag_kernel, nb, kThreads, 0, c, total, b.flags));
   CB_TRY(exclusive_scan_u32(ctx, b.flags, (size_t)total + 1, 0u));
-  candidate_compact_kernel<<<nb, kThreads, 0, ctx->stream>>>(c, total, b.flags, b.f[0], b.s[0], b.d[0]);
-  ctx->launches += 2;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, candidate_compact_kernel, nb, kThreads, 0, c, total, b.flags, b.f[0], b.s[0], b.d[0]));
   uint32_t m = 0;
   CB_TRY(read_u32(ctx, b.flags + total, &m));
   const int idx_bits = bits_of(std::max(n_src, n_dst));
@@ -358,13 +341,11 @@ int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, 
     const bool by_first = prm->search_dir == CB_SECOND_TO_FIRST;
     CB_TRY(sort_pairs(ctx, b, m, by_first ? kKeyFirstValue : kKeySecondValue, idx_bits, val_bits));
     const uint32_t* index = by_first ? b.f[b.cur] : b.s[b.cur];
-    const int mb = blocks_for(ctx, m);
-    group_head_flag_kernel<<<mb, kThreads, 0, ctx->stream>>>(index, m, b.flags);
+    const int mb = grid_for(ctx, m, kThreads, 16);
+    CB_TRY(launch(ctx, group_head_flag_kernel, mb, kThreads, 0, index, m, b.flags));
     CB_TRY(exclusive_scan_u32(ctx, b.flags, (size_t)m + 1, 0u));
-    flagged_compact_kernel<<<mb, kThreads, 0, ctx->stream>>>(index, m, b.flags, b.f[b.cur], b.s[b.cur], b.d[b.cur],
-                                                            b.f[b.cur ^ 1], b.s[b.cur ^ 1], b.d[b.cur ^ 1]);
-    ctx->launches += 2;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, flagged_compact_kernel, mb, kThreads, 0, index, m, b.flags, b.f[b.cur], b.s[b.cur], b.d[b.cur],
+                  b.f[b.cur ^ 1], b.s[b.cur ^ 1], b.d[b.cur ^ 1]));
     CB_TRY(read_u32(ctx, b.flags + m, &m));
     b.cur ^= 1;
   }

@@ -14,6 +14,7 @@
 // correspondence list is only materialised when a caller asks for it.
 #include "icp_accumulate.cuh"
 #include "icp_kernels.cuh"
+#include "launch.cuh"
 #include "reduce.cuh"
 #include "warp_search.cuh"
 #include <algorithm>
@@ -169,15 +170,12 @@ __global__ void translate_matches_kernel(const int* __restrict__ nn_pos, const f
 int launch_translate_matches(cb_context* ctx, const int* nn_pos, const float* nn_d2, const float4* src_pts,
                              const float4* dst_pts, uint32_t n_src, int* out_first, float* out_val) {
   if (n_src == 0) return CB_OK;
-  const int blocks = (int)std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)ctx->sm_count * 8, (n_src + 255) / 256));
-  translate_matches_kernel<<<blocks, 256, 0, ctx->stream>>>(nn_pos, nn_d2, src_pts, dst_pts, n_src, out_first, out_val);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, translate_matches_kernel, grid_for(ctx, n_src, 256), 256, 0, nn_pos, nn_d2, src_pts, dst_pts,
+                n_src, out_first, out_val);
 }
 
-int icp_grid_blocks(const cb_context* ctx) {
-  // persistent-style launch: a whole number of waves of resident CTAs
+// resident blocks per SM of the pass kernel: the residual kernel's grid is at most one wave of them
+static int icp_blocks_per_sm() {
   static int per_sm = -1;
   if (per_sm < 0) {
     int v = 0;
@@ -187,7 +185,7 @@ int icp_grid_blocks(const cb_context* ctx) {
       v = 2;
     per_sm = v;
   }
-  return ctx->sm_count * per_sm;
+  return per_sm;
 }
 
 int launch_icp_pass(cb_context* ctx, const IcpArgs& a, int mode, bool search, bool has_pt, bool has_pl) {
@@ -199,43 +197,27 @@ int launch_icp_pass(cb_context* ctx, const IcpArgs& a, int mode, bool search, bo
   // reduction passes carry the fused NVLink all-reduce + host mailbox epilogue when the context has it
   ctx->pass_armed = (mode != kModeKnn) && arm_exchange(ctx, &args.rs.ex);
   args.prefetch_blocks = (uint32_t)(2 * ctx->sm_count * kIcpMinBlocks);  // ~2 waves of resident blocks
-  if (mode == kModeKnn) {
-    icp_pass_kernel<kModeKnn, true><<<blocks, kBlock, 0, ctx->stream>>>(args, false, false);
-  } else if (mode == kModeP2P) {
-    if (search)
-      icp_pass_kernel<kModeP2P, true><<<blocks, kBlock, 0, ctx->stream>>>(args, false, false);
-    else
-      icp_pass_kernel<kModeP2P, false><<<blocks, kBlock, 0, ctx->stream>>>(args, false, false);
-  } else if (mode == kModeP2PCentered) {  // Kabsch moments about the pivots a.dm / a.sm (the ICP loop; always a search pass)
-    icp_pass_kernel<kModeP2PCentered, true><<<blocks, kBlock, 0, ctx->stream>>>(args, false, false);
-  } else {
-    if (search)
-      icp_pass_kernel<kModeCombined, true><<<blocks, kBlock, 0, ctx->stream>>>(args, has_pt, has_pl);
-    else
-      icp_pass_kernel<kModeCombined, false><<<blocks, kBlock, 0, ctx->stream>>>(args, has_pt, has_pl);
-  }
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  auto kernel = search ? icp_pass_kernel<kModeCombined, true> : icp_pass_kernel<kModeCombined, false>;
+  if (mode == kModeKnn)
+    kernel = icp_pass_kernel<kModeKnn, true>;
+  else if (mode == kModeP2P)
+    kernel = search ? icp_pass_kernel<kModeP2P, true> : icp_pass_kernel<kModeP2P, false>;
+  else if (mode == kModeP2PCentered)  // Kabsch moments about the pivots a.dm / a.sm (the ICP loop, a search pass)
+    kernel = icp_pass_kernel<kModeP2PCentered, true>;
+  // only the combined metric reads has_pt / has_pl
+  return launch(ctx, kernel, blocks, kBlock, 0, args, has_pt, has_pl);
 }
 
 int launch_residuals(cb_context* ctx, const GridView& dst, const float4* src_pts, const float4* src_nrm,
                      uint32_t n_src, const Rigid& T, int metric, float w_pt, float w_pl, float* d_out) {
   if (n_src == 0) return CB_OK;
-  int blocks = std::max(1, std::min(icp_grid_blocks(ctx), (int)((n_src + kBlock - 1) / kBlock)));
-  residual_kernel<<<blocks, kBlock, 0, ctx->stream>>>(dst, src_pts, src_nrm, n_src, T, metric, w_pt, w_pl, d_out);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, residual_kernel, grid_for(ctx, n_src, kBlock, icp_blocks_per_sm()), kBlock, 0, dst, src_pts,
+                src_nrm, n_src, T, metric, w_pt, w_pl, d_out);
 }
 
 int launch_transform_points(cb_context* ctx, const Rigid& T, const float* d_in, size_t n, float* d_out) {
   if (n == 0) return CB_OK;
-  int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + 255) / 256));
-  transform_points_kernel<<<blocks, 256, 0, ctx->stream>>>(T, d_in, n, d_out);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, transform_points_kernel, grid_for(ctx, n, 256), 256, 0, T, d_in, n, d_out);
 }
 
 }  // namespace cb

@@ -56,8 +56,6 @@ int launch_residuals(cb_context* ctx, const GridView& dst, const float4* src_pts
 
 int launch_transform_points(cb_context* ctx, const Rigid& T, const float* d_in, size_t n, float* d_out);
 
-int icp_grid_blocks(const cb_context* ctx);
-
 // Per sorted source position p: out_first[orig(p)] = original index of dst point nn_pos[p] (or -1),
 // out_val[orig(p)] = nn_d2[p] (nullable) - the getters' translation from sorted positions to caller indices.
 int launch_translate_matches(cb_context* ctx, const int* nn_pos, const float* nn_d2, const float4* src_pts,

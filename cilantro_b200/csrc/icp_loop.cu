@@ -29,6 +29,7 @@
 #include "icp_accumulate.cuh"
 #include "icp_kernels.cuh"
 #include "icp_object.hpp"
+#include "launch.cuh"
 #include "reduce.cuh"
 #include "solve_core.hpp"
 #include "solve_warp.cuh"
@@ -578,37 +579,19 @@ constexpr int kFirstBatch = 4;
 constexpr int kBridgeBatch = 2;  // enqueued behind the first batch: covers the host's look at the first batch's state
 constexpr double kGiveUpShare = 0.15;
 
-// launch with programmatic stream serialization (see pdl_wait above)
-template <class Kernel>
-static cudaError_t launch_pdl(Kernel k, int blocks, int threads, size_t smem, cudaStream_t stream, const LoopArgs& a) {
-  cudaLaunchConfig_t cfg;
-  std::memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)blocks);
-  cfg.blockDim = dim3((unsigned)threads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, k, a);
-}
-
-// Enqueues the kernels of ICP iteration `it` of this call: the search kernel in the cold first iteration (nothing
-// cached yet), else the cached pass with its search of the flagged queries; then the finish kernel.
+// Enqueues the kernels of ICP iteration `it` of this call, with programmatic stream serialization (see pdl_wait
+// above): the search kernel in the cold first iteration (nothing cached yet), else the cached pass with its search of
+// the flagged queries; then the finish kernel.
 template <int MODE>
 static int enqueue_iteration(cb_context* ctx, const LoopArgs& args, int it, int blocks_cold, int blocks_cached) {
   LoopArgs a = args;
   a.rows = (uint32_t)(it == 0 ? 0 : blocks_cached);  // each block of the cached pass writes one row
   if (it == 0)
-    CB_CUDA(launch_pdl(icp_search_kernel<MODE>, blocks_cold, kBlock, 0, ctx->stream, a));
+    CB_TRY(launch_pdl(ctx, icp_search_kernel<MODE>, blocks_cold, kBlock, 0, a));
   else
-    CB_CUDA(launch_pdl(icp_cached_pipe_kernel<MODE>, blocks_cached, kBlock, sizeof(PipeSmem<MODE == kModeCombined>),
-                       ctx->stream, a));
-  CB_CUDA(launch_pdl(icp_finish_kernel<MODE>, 1, kBlock, 0, ctx->stream, a));
-  ctx->launches += 2;
-  return CB_OK;
+    CB_TRY(launch_pdl(ctx, icp_cached_pipe_kernel<MODE>, blocks_cached, kBlock, sizeof(PipeSmem<MODE == kModeCombined>),
+                      a));
+  return launch_pdl(ctx, icp_finish_kernel<MODE>, 1, kBlock, 0, a);
 }
 
 int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res, int* hand_over) {
@@ -685,7 +668,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
   const int per_sm = std::max(1, resident[p2p ? 0 : 1]);
   const size_t tile = (size_t)pipe_qpt(!p2p) * kBlock;
-  const int blocks_cached = std::max(1, std::min(ctx->sm_count * per_sm, (int)((ns + tile - 1) / tile)));
+  const int blocks_cached = grid_for(ctx, ns, tile, per_sm);
   CB_TRY(get_reduce_scratch(ctx, blocks_cold, kMaxValues, &a.rs));
   Exchange ex;
   std::memset(&ex, 0, sizeof(ex));
@@ -725,7 +708,6 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
         CB_TRY(enqueue_iteration<kModeCombined>(ctx, a, issued + k, blocks_cold, blocks_cached));
       if (timing) CB_CUDA(cudaEventRecord(icp->events[2 * (issued + k) + 1], ctx->stream));
     }
-    CB_CUDA(cudaGetLastError());
     issued += n;
     CB_CUDA(cudaMemcpyAsync(hbuf[enq & 1], icp->d_state, sizeof(LoopState), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaEventRecord(icp->batch_ev[enq & 1], ctx->stream));

@@ -17,6 +17,7 @@
 // test is the right fold of DESIGN §4.17, which is dx*dx + (dy*dy + dz*dz) at D = 3.
 #include "cb_internal.hpp"
 #include "host_solve.hpp"
+#include "launch.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -179,24 +180,13 @@ int kmeans_step(cb_context* ctx, const KMeansData& x, const KMeansBuffers& b, co
     const size_t smem = kChunk * sizeof(float4) + (use_smem ? smem_sums : 0);
     // persistent grid = SMs x resident blocks per SM (occupancy API with this launch's dynamic smem);
     // a fixed 2 blocks/SM left most warp slots empty
+    auto kern = use_smem ? kmeans_assign_kernel<true> : kmeans_assign_kernel<false>;
+    if (use_smem) CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    if (use_smem) {
-      CB_CUDA(cudaFuncSetAttribute(kmeans_assign_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kmeans_assign_kernel<true>, kBlock, smem));
-    } else {
-      CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kmeans_assign_kernel<false>, kBlock, smem));
-    }
+    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kBlock, smem));
     per_sm = std::max(1, std::min(per_sm, 6));
-    int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (x.n + tile - 1) / tile));
-    if (use_smem) {
-      kmeans_assign_kernel<true><<<blocks, kBlock, smem, ctx->stream>>>(x.raw, x.n, d_c4, (int)K, b.d_labels, b.d_sums,
-                                                                       b.d_changed);
-    } else {
-      kmeans_assign_kernel<false><<<blocks, kBlock, smem, ctx->stream>>>(x.raw, x.n, d_c4, (int)K, b.d_labels, b.d_sums,
-                                                                        b.d_changed);
-    }
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, kern, grid_for(ctx, x.n, tile, per_sm), kBlock, smem, x.raw, x.n, d_c4, (int)K, b.d_labels,
+                  b.d_sums, b.d_changed));
   }
   // one all-reduce of K x 4 sums per iteration when sharded (SURVEY.md §8e; clouds only)
   if (ctx->world > 1) CB_TRY(nccl_allreduce_sum_f64(ctx, b.d_sums, K * W));
@@ -297,11 +287,8 @@ int kmeans_cluster(cb_context* ctx, const KMeansData& x, float* centroids, size_
       }
       CB_CUDA(cudaMemcpyAsync(b.d_oc, oc.data(), D * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
       CB_CUDA(cudaMemsetAsync(b.d_far, 0, sizeof(unsigned long long), ctx->stream));
-      const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (x.n + 255) / 256));
-      farthest_member_kernel<<<blocks, 256, 0, ctx->stream>>>(x.raw, x.n, x.D, b.d_labels, (uint32_t)max_ind, b.d_oc,
-                                                              b.d_far);
-      ctx->launches += 1;
-      CB_CUDA(cudaGetLastError());
+      CB_TRY(launch(ctx, farthest_member_kernel, grid_for(ctx, x.n, 256), 256, 0, x.raw, x.n, x.D, b.d_labels,
+                    (uint32_t)max_ind, b.d_oc, b.d_far));
       unsigned long long key = 0;
       CB_CUDA(cudaMemcpyAsync(&key, b.d_far, sizeof(key), cudaMemcpyDeviceToHost, ctx->stream));
       CB_CUDA(cudaStreamSynchronize(ctx->stream));

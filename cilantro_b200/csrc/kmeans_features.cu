@@ -10,6 +10,7 @@
 // per dimension from chunks of 16 dimensions staged transposed in shared memory, highest chunk first.
 // A row with a non-finite component gets label 0 (no d2 of it is below +inf) and adds to no sum or count.
 #include "cb_internal.hpp"
+#include "launch.cuh"
 #include <algorithm>
 
 using namespace cb;
@@ -168,12 +169,8 @@ int kmeans_features_assign(cb_context* ctx, const float* raw, size_t n, int D, c
   int per_sm = 0;
   CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
   per_sm = std::max(1, per_sm);
-  const size_t ntiles = (n + kTile - 1) / kTile;
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, ntiles));
-  kern<<<blocks, kThreads, smem, ctx->stream>>>(raw, n, D, cent, (int)K, labels, sums, changed);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, kern, grid_for(ctx, n, kTile, per_sm), kThreads, smem, raw, n, D, cent, (int)K, labels, sums,
+                changed);
 }
 
 }  // namespace cb

@@ -6,6 +6,7 @@
 #include "cb_internal.hpp"
 #include "grid_sweep.cuh"
 #include "kbest.cuh"
+#include "launch.cuh"
 #include "radius_lists.cuh"
 #include <algorithm>
 #include <vector>
@@ -68,22 +69,19 @@ extern "C" int cb_knn_radius(cb_context* ctx, const cb_cloud* ref, const cb_clou
   CB_TRY(scope.alloc(&d_idx, nq * k));
   CB_TRY(scope.alloc(&d_d2, nq * k));
   CB_TRY(scope.alloc(&d_cnt, nq));
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (nq + kBlock - 1) / kBlock));
-  const GridView g = grid_view(ref);
+  auto kernel = knn_k_kernel<256>;
   if (k <= 4)
-    knn_k_kernel<4><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, k, max_d2, d_idx, d_d2, d_cnt);
+    kernel = knn_k_kernel<4>;
   else if (k <= 16)
-    knn_k_kernel<16><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, k, max_d2, d_idx, d_d2, d_cnt);
+    kernel = knn_k_kernel<16>;
   else if (k <= 32)
-    knn_k_kernel<32><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, k, max_d2, d_idx, d_d2, d_cnt);
+    kernel = knn_k_kernel<32>;
   else if (k <= 64)
-    knn_k_kernel<64><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, k, max_d2, d_idx, d_d2, d_cnt);
+    kernel = knn_k_kernel<64>;
   else if (k <= 128)
-    knn_k_kernel<128><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, k, max_d2, d_idx, d_d2, d_cnt);
-  else
-    knn_k_kernel<256><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, k, max_d2, d_idx, d_d2, d_cnt);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+    kernel = knn_k_kernel<128>;
+  CB_TRY(launch(ctx, kernel, grid_for(ctx, nq, kBlock), kBlock, 0, grid_view(ref), qry->d_pts, (uint32_t)nq, T, k,
+                max_d2, d_idx, d_d2, d_cnt));
   std::vector<int> h_idx(nq * k);
   CB_CUDA(cudaMemcpyAsync(h_idx.data(), d_idx, nq * k * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaMemcpyAsync(d2, d_d2, nq * k * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
@@ -112,11 +110,10 @@ extern "C" int cb_radius_search(cb_context* ctx, const cb_cloud* ref, const cb_c
   uint32_t* d_off = nullptr;
   CB_TRY(scope.alloc(&d_off, nq + 2));
   CB_CUDA(cudaMemsetAsync(d_off, 0, (nq + 2) * sizeof(uint32_t), ctx->stream));
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (nq + kBlock - 1) / kBlock));
+  const int blocks = grid_for(ctx, nq, kBlock);
   const GridView g = grid_view(ref);
-  radius_kernel<false><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, radius2, d_off, nullptr,
-                                                          nullptr, nullptr);
-  ctx->launches += 1;
+  CB_TRY(launch(ctx, radius_kernel<false>, blocks, kBlock, 0, g, qry->d_pts, (uint32_t)nq, T, radius2, d_off, nullptr,
+                nullptr, nullptr));
   // counts are 32-bit: sum them on the host in 64 bits before trusting the 32-bit scan
   std::vector<uint32_t> h_cnt(nq);
   CB_CUDA(cudaMemcpyAsync(h_cnt.data(), d_off, nq * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -136,11 +133,9 @@ extern "C" int cb_radius_search(cb_context* ctx, const cb_cloud* ref, const cb_c
   float* d_d2 = nullptr;
   CB_TRY(scope.alloc(&d_idx, sum));
   CB_TRY(scope.alloc(&d_d2, sum));
-  radius_kernel<true><<<blocks, kBlock, 0, ctx->stream>>>(g, qry->d_pts, (uint32_t)nq, T, radius2, nullptr, d_off, d_idx,
-                                                         d_d2);
-  segment_heapsort_kernel<<<blocks, kBlock, 0, ctx->stream>>>(d_off, (uint32_t)nq, d_idx, d_d2);
-  ctx->launches += 2;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, radius_kernel<true>, blocks, kBlock, 0, g, qry->d_pts, (uint32_t)nq, T, radius2, nullptr, d_off,
+                d_idx, d_d2));
+  CB_TRY(launch(ctx, segment_heapsort_kernel, blocks, kBlock, 0, d_off, (uint32_t)nq, d_idx, d_d2));
   std::vector<int> h_idx(sum);
   CB_CUDA(cudaMemcpyAsync(h_idx.data(), d_idx, sum * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaMemcpyAsync(d2, d_d2, sum * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));

@@ -18,6 +18,7 @@
 // mode serially in seed order (the reference's order), so that pass costs as much as the largest cluster.
 #include "cb_internal.hpp"
 #include "grid_sweep.cuh"
+#include "launch.cuh"
 #include "radius_lists.cuh"
 #include <algorithm>
 #include <cstdlib>
@@ -276,9 +277,6 @@ uint64_t pair_budget() {
   return std::min<uint64_t>(b, 0xffffffffull);
 }
 
-inline int blocks_for(const cb_context* ctx, size_t n, int block) {
-  return (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + block - 1) / block));
-}
 
 }  // namespace
 
@@ -328,7 +326,7 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
   CB_TRY(scope.alloc(&d_off, (size_t)ns + 1));
   CB_TRY(scope.alloc(&d_counter, 1));
   CB_TRY(scope.alloc(&d_xyz, 3 * (size_t)ns));
-  const int eb = blocks_for(ctx, ns, 256);
+  const int eb = grid_for(ctx, ns, 256);
 
   ScopedEvents ev, ev2;  // ev2.e0: end of the shift loop
   if (gpu_ms || gpu_ms_shift) {
@@ -339,9 +337,7 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
   if (seeds) {
     CB_CUDA(cudaMemcpyAsync(d_xyz, seeds, 3 * (size_t)ns * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   }
-  init_seeds_kernel<<<eb, 256, 0, ctx->stream>>>(seeds ? d_xyz : cloud->d_raw, ns, d_seeds, d_act);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, init_seeds_kernel, eb, 256, 0, seeds ? d_xyz : cloud->d_raw, ns, d_seeds, d_act));
 
   // ---- shift (mean_shift.hpp:55-82) ----
   const GridView g = grid_view(cloud);
@@ -354,17 +350,14 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
   uint64_t iters = 0;
   while (iters < max_iter) {
     CB_CUDA(cudaMemsetAsync(d_counter, 0, sizeof(uint32_t), ctx->stream));
-    queries_kernel<<<blocks_for(ctx, n_act, 256), 256, 0, ctx->stream>>>(d_seeds, d_act, n_act, d_q);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, queries_kernel, grid_for(ctx, n_act, 256), 256, 0, d_seeds, d_act, n_act, d_q));
     // list sizes of every active seed (r2 <= 0 or NaN: every list is empty, nothing to search)
     if (r2 > 0.f) {
-      radius_kernel<false><<<blocks_for(ctx, n_act, kRadiusBlock), kRadiusBlock, 0, ctx->stream>>>(
-          g, d_q, n_act, I, r2, d_cnt, nullptr, nullptr, nullptr);
-      ctx->launches += 1;
+      CB_TRY(launch(ctx, radius_kernel<false>, grid_for(ctx, n_act, kRadiusBlock), kRadiusBlock, 0, g, d_q, n_act, I,
+                    r2, d_cnt, nullptr, nullptr, nullptr));
     } else {
       CB_CUDA(cudaMemsetAsync(d_cnt, 0, n_act * sizeof(uint32_t), ctx->stream));
     }
-    CB_CUDA(cudaGetLastError());
     h_cnt.resize(n_act);
     CB_CUDA(cudaMemcpyAsync(h_cnt.data(), d_cnt, n_act * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -386,16 +379,14 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
       uint32_t* off = d_off + b0;
       CB_CUDA(cudaMemcpyAsync(off, d_cnt + b0, nb * sizeof(uint32_t), cudaMemcpyDeviceToDevice, ctx->stream));
       CB_TRY(exclusive_scan_u32(ctx, off, nb, (uint32_t)pairs));
-      const int qb = blocks_for(ctx, nb, kRadiusBlock);
+      const int qb = grid_for(ctx, nb, kRadiusBlock);
       if (pairs > 0) {
-        radius_kernel<true><<<qb, kRadiusBlock, 0, ctx->stream>>>(g, d_q + b0, nb, I, r2, nullptr, d_off, d_idx, d_d2);
-        segment_heapsort_kernel<<<qb, kRadiusBlock, 0, ctx->stream>>>(off, nb, d_idx, d_d2);
-        ctx->launches += 2;
+        CB_TRY(launch(ctx, radius_kernel<true>, qb, kRadiusBlock, 0, g, d_q + b0, nb, I, r2, nullptr, d_off, d_idx,
+                      d_d2));
+        CB_TRY(launch(ctx, segment_heapsort_kernel, qb, kRadiusBlock, 0, off, nb, d_idx, d_d2));
       }
-      shift_kernel<<<blocks_for(ctx, nb, kBlock), kBlock, 0, ctx->stream>>>(
-          cloud->d_raw, d_act + b0, nb, off, d_idx, d_d2, rbf, prm->weight_coeff, tol2, d_seeds, d_next, d_counter);
-      ctx->launches += 1;
-      CB_CUDA(cudaGetLastError());
+      CB_TRY(launch(ctx, shift_kernel, grid_for(ctx, nb, kBlock), kBlock, 0, cloud->d_raw, d_act + b0, nb, off, d_idx,
+                    d_d2, rbf, prm->weight_coeff, tol2, d_seeds, d_next, d_counter));
       b0 = b1;
     }
     CB_CUDA(cudaMemcpyAsync(&n_act, d_counter, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -407,8 +398,7 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
 
   // ---- cluster (mean_shift.hpp:84-100) ----
   if (ev2.e0) CB_CUDA(cudaEventRecord(ev2.e0, ctx->stream));
-  pack_kernel<<<eb, 256, 0, ctx->stream>>>(d_seeds, ns, d_xyz);
-  ctx->launches += 1;
+  CB_TRY(launch(ctx, pack_kernel, eb, 256, 0, d_seeds, ns, d_xyz));
   uint32_t *d_rep, *d_flag;
   CB_TRY(scope.alloc(&d_rep, ns));
   CB_TRY(scope.alloc(&d_flag, (size_t)ns + 1));
@@ -419,8 +409,7 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
   CB_TRY(scope.alloc(&d_vals, ns));
   CB_TRY(scope.alloc(&d_vals_tmp, ns));
   if (!(ctol2 > 0.f)) {  // every seed is a singleton
-    seed_rep_kernel<<<eb, 256, 0, ctx->stream>>>(nullptr, nullptr, ns, d_rep, d_flag);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, seed_rep_kernel, eb, 256, 0, nullptr, nullptr, ns, d_rep, d_flag));
   } else {
     // groups of bit-identical seeds (see key_z_kernel)
     uint32_t *d_head, *d_grp, *d_state, *d_rep_id;
@@ -428,29 +417,22 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
     CB_TRY(scope.alloc(&d_head, ns));
     CB_TRY(scope.alloc(&d_grp, ns));
     CB_TRY(scope.alloc(&d_hxyz, 3 * (size_t)ns));
-    key_z_kernel<<<eb, 256, 0, ctx->stream>>>(d_seeds, ns, d_keys, d_vals);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, key_z_kernel, eb, 256, 0, d_seeds, ns, d_keys, d_vals));
     CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_vals, d_keys_tmp, d_vals_tmp, ns, 32));
-    key_xy_kernel<<<eb, 256, 0, ctx->stream>>>(d_seeds, d_vals, ns, d_keys);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, key_xy_kernel, eb, 256, 0, d_seeds, d_vals, ns, d_keys));
     CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_vals, d_keys_tmp, d_vals_tmp, ns, 64));
-    start_kernel<<<eb, 256, 0, ctx->stream>>>(d_seeds, d_vals, ns, d_flag);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, start_kernel, eb, 256, 0, d_seeds, d_vals, ns, d_flag));
     uint32_t last_start = 0, ng = 0;
     CB_CUDA(cudaMemcpyAsync(&last_start, d_flag + ns - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CB_TRY(exclusive_scan_u32(ctx, d_flag, ns, 0u));
     CB_CUDA(cudaMemcpyAsync(&ng, d_flag + ns - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    group_kernel<<<eb, 256, 0, ctx->stream>>>(d_seeds, d_vals, d_flag, ns, d_head, d_hxyz, d_grp);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, group_kernel, eb, 256, 0, d_seeds, d_vals, d_flag, ns, d_head, d_hxyz, d_grp));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
     ng += last_start;
     CB_TRY(scope.alloc(&d_state, ng));
     CB_TRY(scope.alloc(&d_rep_id, ng));
-    const int gb = blocks_for(ctx, ng, 256);
-    state_init_kernel<<<gb, 256, 0, ctx->stream>>>(d_hxyz, ng, d_state);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    const int gb = grid_for(ctx, ng, 256);
+    CB_TRY(launch(ctx, state_init_kernel, gb, 256, 0, d_hxyz, ng, d_state));
     cb_cloud* sc = nullptr;  // grid over the group heads (non-finite ones are inert in it)
     CB_TRY(cb_cloud_create_from_device(ctx, d_hxyz, nullptr, ng, 0, &sc));
     struct CloudGuard {
@@ -459,22 +441,18 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
     } guard{sc};
     CB_TRY(ensure_index(sc));
     const GridView sg = grid_view(sc);
-    const int rb = blocks_for(ctx, ng, kBlock);
+    const int rb = grid_for(ctx, ng, kBlock);
     for (;;) {
       CB_CUDA(cudaMemsetAsync(d_counter, 0, sizeof(uint32_t), ctx->stream));
-      round_kernel<<<rb, kBlock, 0, ctx->stream>>>(sg, d_hxyz, d_head, ng, ctol2, d_state, d_counter);
-      ctx->launches += 1;
-      CB_CUDA(cudaGetLastError());
+      CB_TRY(launch(ctx, round_kernel, rb, kBlock, 0, sg, d_hxyz, d_head, ng, ctol2, d_state, d_counter));
       uint32_t undecided = 0;
       CB_CUDA(cudaMemcpyAsync(&undecided, d_counter, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
       CB_CUDA(cudaStreamSynchronize(ctx->stream));
       if (undecided == 0) break;
     }
-    rep_kernel<<<rb, kBlock, 0, ctx->stream>>>(sg, d_hxyz, d_head, ng, ctol2, d_state, d_rep_id);
-    seed_rep_kernel<<<eb, 256, 0, ctx->stream>>>(d_grp, d_rep_id, ns, d_rep, d_flag);
-    ctx->launches += 2;
+    CB_TRY(launch(ctx, rep_kernel, rb, kBlock, 0, sg, d_hxyz, d_head, ng, ctol2, d_state, d_rep_id));
+    CB_TRY(launch(ctx, seed_rep_kernel, eb, 256, 0, d_grp, d_rep_id, ns, d_rep, d_flag));
   }
-  CB_CUDA(cudaGetLastError());
   // clusters numbered by representative index
   uint32_t last_flag = 0;
   CB_CUDA(cudaMemcpyAsync(&last_flag, d_flag + ns - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -489,15 +467,11 @@ extern "C" int cb_cloud_mean_shift(cb_context* ctx, cb_cloud* cloud, const cb_me
   CB_TRY(scope.alloc(&d_size, (size_t)m + 1));
   CB_TRY(scope.alloc(&d_modes, 3 * (size_t)m));
   CB_CUDA(cudaMemsetAsync(d_size, 0, ((size_t)m + 1) * sizeof(uint32_t), ctx->stream));
-  cluster_kernel<<<eb, 256, 0, ctx->stream>>>(d_rep, d_flag, ns, d_size, d_keys, d_vals);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, cluster_kernel, eb, 256, 0, d_rep, d_flag, ns, d_size, d_keys, d_vals));
   // cluster -> seeds: stable sort of (cluster, seed) in seed order
   CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_vals, d_keys_tmp, d_vals_tmp, ns, bits_for(m)));
   CB_TRY(exclusive_scan_u32(ctx, d_size, m, ns));
-  modes_kernel<<<blocks_for(ctx, m, kBlock), kBlock, 0, ctx->stream>>>(d_seeds, d_size, d_vals, m, d_modes);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, modes_kernel, grid_for(ctx, m, kBlock), kBlock, 0, d_seeds, d_size, d_vals, m, d_modes));
   if (ev.e1) CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
 
   std::vector<uint32_t> h_pts(ns), h_off((size_t)m + 1);

@@ -14,6 +14,7 @@
 // so this mode agrees to fp32 rounding, not bit for bit.
 #include "cb_internal.hpp"
 #include "grid_sweep.cuh"
+#include "launch.cuh"
 #include "normals_out.cuh"
 #include <algorithm>
 #include <cmath>
@@ -190,31 +191,29 @@ extern "C" int cb_cloud_estimate_normals(cb_context* ctx, cb_cloud* cloud, int k
   set_orientation(o, view_point3, use_ref);
   const float max_d2 = radius2 > 0.f ? radius2 : 3.402823466e38f;
   const GridView g = grid_view(cloud);
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + kBlock - 1) / kBlock));
+  const int blocks = grid_for(ctx, n, kBlock);
   ScopedEvents ev;
   if (gpu_ms) {
     CB_TRY(ev.create());
     CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
   }
-  if (k == 0)
-    normals_radius_kernel<<<blocks, kBlock, 0, ctx->stream>>>(g, max_d2, o);
-  else if (k <= 8)
-    normals_knn_kernel<8><<<blocks, kBlock, 8 * kBlock * 8, ctx->stream>>>(g, k, max_d2, o);
-  else if (k <= 16)
-    normals_knn_kernel<16><<<blocks, kBlock, 16 * kBlock * 8, ctx->stream>>>(g, k, max_d2, o);
-  else if (k <= 32)
-    normals_knn_kernel<32><<<blocks, kBlock, 32 * kBlock * 8, ctx->stream>>>(g, k, max_d2, o);
-  else if (k <= 64) {
-    // (per call, not once per process: function attributes belong to the device the context is on)
-    CB_CUDA(cudaFuncSetAttribute(normals_knn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * kBlock * 8));
-    normals_knn_kernel<64><<<blocks, kBlock, 64 * kBlock * 8, ctx->stream>>>(g, k, max_d2, o);
+  if (k == 0) {
+    CB_TRY(launch(ctx, normals_radius_kernel, blocks, kBlock, 0, g, max_d2, o));
   } else {
-    CB_CUDA(cudaFuncSetAttribute(normals_knn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * kBlock * 8));
-    normals_knn_kernel<128><<<blocks, kBlock, 128 * kBlock * 8, ctx->stream>>>(g, k, max_d2, o);
+    // the kernel for the smallest K >= k, with its k-best lists as dynamic shared memory (8 B x K x kBlock)
+    constexpr int kKs[] = {8, 16, 32, 64, 128};  // k <= kMaxK = 128
+    void (*const kernels[])(GridView, int, float, NormalOut) = {normals_knn_kernel<8>, normals_knn_kernel<16>,
+                                                                normals_knn_kernel<32>, normals_knn_kernel<64>,
+                                                                normals_knn_kernel<128>};
+    int v = 0;
+    while (k > kKs[v]) v++;
+    const int smem = kKs[v] * kBlock * 8;
+    // above 48 KB (per call, not once per process: function attributes belong to the device the context is on)
+    if (kKs[v] > 32)
+      CB_CUDA(cudaFuncSetAttribute(kernels[v], cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CB_TRY(launch(ctx, kernels[v], blocks, kBlock, smem, g, k, max_d2, o));
   }
-  ctx->launches += 1;
   if (gpu_ms) CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
-  CB_CUDA(cudaGetLastError());
   if (normals)
     CB_CUDA(cudaMemcpyAsync(normals, cloud->d_raw_nrm, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   if (curvature)

@@ -12,6 +12,7 @@
 // digits is the input order (stable), which the downsampler relies on: points of one bin stay sorted by
 // their original index.
 #include "cb_internal.hpp"
+#include "launch.cuh"
 #include <algorithm>
 
 namespace cb {
@@ -105,12 +106,9 @@ int radix_sort_pairs_u64(cb_context* ctx, uint64_t* d_keys, uint32_t* d_vals, ui
   const int passes = (std::min(bits, 64) + 7) / 8;
   for (int p = 0; p < passes; p++) {
     const int shift = 8 * p;
-    radix_hist_kernel<<<ntiles, kSortThreads, 0, ctx->stream>>>(kin, n, shift, d_hist, ntiles);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, radix_hist_kernel, ntiles, kSortThreads, 0, kin, n, shift, d_hist, ntiles));
     CB_TRY(exclusive_scan_u32(ctx, d_hist, hn, (uint32_t)n));
-    radix_scatter_kernel<<<ntiles, kSortThreads, 0, ctx->stream>>>(kin, vin, n, shift, d_hist, ntiles, kout, vout);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, radix_scatter_kernel, ntiles, kSortThreads, 0, kin, vin, n, shift, d_hist, ntiles, kout, vout));
     std::swap(kin, kout);
     std::swap(vin, vout);
   }

@@ -14,6 +14,7 @@
 // evaluated as x <= x_max with x_max = max{x : sqrt_rn(x) <= thresh} found on the host (sqrt_rn is
 // monotone), which is bit-equivalent and keeps the MUFU pipe out of the inner loop.
 #include "cb_internal.hpp"
+#include "launch.cuh"
 #include "nn_search.cuh"
 #include "reduce.cuh"
 #include "host_solve.hpp"
@@ -176,18 +177,15 @@ int score_batch(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const
   int per_sm = 0;  // resident blocks per SM for this launch's dynamic shared memory (a fixed 2 left most warp slots empty)
   CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ransac_score_kernel, kBlock, smem));
   per_sm = std::max(1, std::min(per_sm, 6));
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (dst->n + tile - 1) / tile));
-  ransac_score_kernel<<<blocks, kBlock, smem, ctx->stream>>>(dst->d_raw, src->d_raw, dst->n, d_T, H, x_max, d_counts);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, ransac_score_kernel, grid_for(ctx, dst->n, tile, per_sm), kBlock, smem, dst->d_raw, src->d_raw,
+                dst->n, d_T, H, x_max, d_counts));
   if (ctx->world > 1) {
     DeviceScope scope(ctx);
     double* d_tmp = nullptr;
     CB_TRY(scope.alloc(&d_tmp, (size_t)H));
-    u32_to_f64_kernel<<<(H + 255) / 256, 256, 0, ctx->stream>>>(d_counts, d_tmp, H);
+    CB_TRY(launch(ctx, u32_to_f64_kernel, (H + 255) / 256, 256, 0, d_counts, d_tmp, H));
     CB_TRY(nccl_allreduce_sum_f64(ctx, d_tmp, (size_t)H));
-    f64_to_u32_kernel<<<(H + 255) / 256, 256, 0, ctx->stream>>>(d_tmp, d_counts, H);
-    ctx->launches += 2;
+    CB_TRY(launch(ctx, f64_to_u32_kernel, (H + 255) / 256, 256, 0, d_tmp, d_counts, H));
   }
   return CB_OK;
 }
@@ -203,11 +201,8 @@ Rigid rigid_of(const float* T12) {
 
 int residuals_device(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const float* T12, float* d_out) {
   if (dst->n == 0) return CB_OK;
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (dst->n + 255) / 256));
-  ransac_residual_kernel<<<blocks, 256, 0, ctx->stream>>>(dst->d_raw, src->d_raw, dst->n, rigid_of(T12), d_out);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, ransac_residual_kernel, grid_for(ctx, dst->n, 256), 256, 0, dst->d_raw, src->d_raw, dst->n,
+                rigid_of(T12), d_out);
 }
 
 }  // namespace
@@ -303,9 +298,8 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
     // estimateModel(sample) (:94, ransac_transform_estimator.hpp:72-82): Kabsch on the sample
     if (sample_size > 0) {
       CB_CUDA(cudaMemcpyAsync(d_idx, h_idx.data(), nb * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-      gather_pairs_kernel<<<(int)((nb * 3 + 255) / 256), 256, 0, ctx->stream>>>(dst->d_raw, src->d_raw, d_idx, nb * 3,
-                                                                              d_pairs);
-      ctx->launches += 1;
+      CB_TRY(launch(ctx, gather_pairs_kernel, (int)((nb * 3 + 255) / 256), 256, 0, dst->d_raw, src->d_raw, d_idx,
+                    nb * 3, d_pairs));
       CB_CUDA(cudaMemcpyAsync(h_pairs.data(), d_pairs, nb * 18 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
       CB_CUDA(cudaStreamSynchronize(ctx->stream));
     }
@@ -346,11 +340,11 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
   // no hypothesis ever reached sample_size inliers: model_inliers_ is empty, so the re-estimation
   // is a Kabsch over zero pairs = identity (transform_estimation.hpp:20-23)
   if (re_estimate && have_best) {  // :118-128
-    const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 4, (n + kReduceBlock - 1) / kReduceBlock));
+    const int blocks = grid_for(ctx, n, kReduceBlock, 4);
     ReduceScratch rs;
     CB_TRY(get_reduce_scratch(ctx, blocks, 16, &rs));
-    inlier_moments_kernel<<<blocks, kReduceBlock, 0, ctx->stream>>>(dst->d_raw, src->d_raw, n, rigid_of(best_T), x_max, rs);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, inlier_moments_kernel, blocks, kReduceBlock, 0, dst->d_raw, src->d_raw, n, rigid_of(best_T),
+                  x_max, rs));
     double m[16];
     CB_CUDA(cudaMemcpyAsync(ctx->h_result, ctx->d_result, sizeof(m), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));

@@ -15,6 +15,7 @@
 // carries no bounds test.
 #include "cb_internal.hpp"
 #include "host_solve.hpp"
+#include "launch.cuh"
 #include "plane_fit.hpp"
 #include "ransac_sampler.hpp"
 #include "reduce.cuh"
@@ -175,19 +176,13 @@ int score_planes(cb_context* ctx, const cb_cloud* cloud, const float4* d_planes,
     per_sm = v;
   }
   const size_t ntiles = (cloud->n + kWarpTile - 1) / kWarpTile;
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * per_sm, (ntiles + kWarps - 1) / kWarps));
-  plane_score_kernel<<<blocks, kBlock, 0, ctx->stream>>>(cloud->d_raw, cloud->n, d_planes, H, thresh, d_counts);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, plane_score_kernel, grid_for(ctx, ntiles, kWarps, per_sm), kBlock, 0, cloud->d_raw, cloud->n,
+                d_planes, H, thresh, d_counts);
 }
 
 int fit_planes(cb_context* ctx, const cb_cloud* cloud, const uint32_t* d_idx, int H, int sample_size, float4* d_planes) {
   if (H == 0) return CB_OK;
-  plane_fit_kernel<<<(H + 127) / 128, 128, 0, ctx->stream>>>(cloud->d_raw, d_idx, H, sample_size, d_planes);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, plane_fit_kernel, (H + 127) / 128, 128, 0, cloud->d_raw, d_idx, H, sample_size, d_planes);
 }
 
 // final residuals + stable compaction of the inliers; synchronises the stream
@@ -203,10 +198,8 @@ int residuals_and_inliers(cb_context* ctx, const cb_cloud* cloud, const float* p
     CB_TRY(scope.alloc(&d_flags, n + 2));
     if (residuals) CB_TRY(scope.alloc(&d_res, n));
     const float4 P = make_float4(plane4[0], plane4[1], plane4[2], plane4[3]);
-    const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + 256) / 256));
-    plane_residual_kernel<<<blocks, 256, 0, ctx->stream>>>(cloud->d_raw, n, P, thresh, d_res, d_flags);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    const int blocks = grid_for(ctx, n + 1, 256);  // n + 1 items: the kernel also writes flags[n]
+    CB_TRY(launch(ctx, plane_residual_kernel, blocks, 256, 0, cloud->d_raw, n, P, thresh, d_res, d_flags));
     CB_TRY(exclusive_scan_u32(ctx, d_flags, n + 1, 0u));
     uint32_t cnt = 0;
     CB_CUDA(cudaMemcpyAsync(&cnt, d_flags + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -215,9 +208,7 @@ int residuals_and_inliers(cb_context* ctx, const cb_cloud* cloud, const float* p
     k = cnt;
     if (inliers && k > 0) {
       CB_TRY(scope.alloc(&d_inl, k));
-      inlier_scatter_kernel<<<blocks, 256, 0, ctx->stream>>>(d_flags, n, d_inl);
-      ctx->launches += 1;
-      CB_CUDA(cudaGetLastError());
+      CB_TRY(launch(ctx, inlier_scatter_kernel, blocks, 256, 0, d_flags, n, d_inl));
       CB_CUDA(cudaMemcpyAsync(inliers, d_inl, k * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
       CB_CUDA(cudaStreamSynchronize(ctx->stream));
     }
@@ -230,14 +221,11 @@ int residuals_and_inliers(cb_context* ctx, const cb_cloud* cloud, const float* p
 int plane_moments(cb_context* ctx, const cb_cloud* cloud, const float* plane4, float thresh, const float* c,
                   double* m) {
   const size_t n = cloud->n;
-  const int blocks = (int)std::max<size_t>(
-      1, std::min<size_t>((size_t)ctx->sm_count * 4, (n + kReduceBlock - 1) / kReduceBlock));
+  const int blocks = grid_for(ctx, n, kReduceBlock, 4);
   ReduceScratch rs;
   CB_TRY(get_reduce_scratch(ctx, blocks, kMomentValues, &rs));
   const float4 P = make_float4(plane4[0], plane4[1], plane4[2], plane4[3]);
-  plane_moments_kernel<<<blocks, kReduceBlock, 0, ctx->stream>>>(cloud->d_raw, n, P, thresh, c[0], c[1], c[2], rs);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, plane_moments_kernel, blocks, kReduceBlock, 0, cloud->d_raw, n, P, thresh, c[0], c[1], c[2], rs));
   return fetch_result(ctx, kMomentValues, false, m);
 }
 

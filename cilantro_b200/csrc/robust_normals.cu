@@ -12,6 +12,7 @@
 #include "cb_internal.hpp"
 #include "grid_sweep.cuh"
 #include "kbest.cuh"
+#include "launch.cuh"
 #include "mcd_rule.hpp"
 #include "normals_out.cuh"
 #include <algorithm>
@@ -169,11 +170,6 @@ __global__ void __launch_bounds__(kBlock) mcd_kernel(const GridView g, const flo
   }
 }
 
-template <int K>
-void launch_search(const GridView& g, int k, float max_d2, int* nbr, uint8_t* cnt, int blocks, cudaStream_t s) {
-  mcd_search_kernel<K><<<blocks, kBlock, 0, s>>>(g, k, max_d2, nbr, cnt);
-}
-
 }  // namespace
 
 extern "C" int cb_cloud_estimate_normals_mcd(cb_context* ctx, cb_cloud* cloud, int k, float radius2,
@@ -224,27 +220,24 @@ extern "C" int cb_cloud_estimate_normals_mcd(cb_context* ctx, cb_cloud* cloud, i
   a.seed = params->seed;
   const float max_d2 = radius2 > 0.f ? radius2 : 3.402823466e38f;
   const GridView g = grid_view(cloud);
-  const int sblocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + kBlock - 1) / kBlock));
-  const int mblocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 16, (n + kWarps - 1) / kWarps));
+  auto search = mcd_search_kernel<128>;
+  if (k <= 8)
+    search = mcd_search_kernel<8>;
+  else if (k <= 16)
+    search = mcd_search_kernel<16>;
+  else if (k <= 32)
+    search = mcd_search_kernel<32>;
+  else if (k <= 64)
+    search = mcd_search_kernel<64>;
   ScopedEvents ev;
   if (gpu_ms) {
     CB_TRY(ev.create());
     CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
   }
-  if (k <= 8)
-    launch_search<8>(g, k, max_d2, d_nbr, d_cnt, sblocks, ctx->stream);
-  else if (k <= 16)
-    launch_search<16>(g, k, max_d2, d_nbr, d_cnt, sblocks, ctx->stream);
-  else if (k <= 32)
-    launch_search<32>(g, k, max_d2, d_nbr, d_cnt, sblocks, ctx->stream);
-  else if (k <= 64)
-    launch_search<64>(g, k, max_d2, d_nbr, d_cnt, sblocks, ctx->stream);
-  else
-    launch_search<128>(g, k, max_d2, d_nbr, d_cnt, sblocks, ctx->stream);
-  mcd_kernel<<<mblocks, kBlock, 0, ctx->stream>>>(g, cloud->d_raw, d_nbr, d_cnt, k, a, o, d_status);
-  ctx->launches += 2;
+  CB_TRY(launch(ctx, search, grid_for(ctx, n, kBlock), kBlock, 0, g, k, max_d2, d_nbr, d_cnt));
+  CB_TRY(launch(ctx, mcd_kernel, grid_for(ctx, n, kWarps, 16), kBlock, 0, g, cloud->d_raw, d_nbr, d_cnt, k, a, o,
+                d_status));
   if (gpu_ms) CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
-  CB_CUDA(cudaGetLastError());
   if (normals)
     CB_CUDA(cudaMemcpyAsync(normals, cloud->d_raw_nrm, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
   if (curvature)

@@ -19,6 +19,7 @@
 #include "cb_internal.hpp"
 #include "grid_sweep.cuh"
 #include "kbest.cuh"
+#include "launch.cuh"
 #include "similarity_rule.hpp"
 #include <algorithm>
 #include <cmath>
@@ -296,25 +297,21 @@ int bits_for(uint64_t v) {
 
 template <bool kBfs>
 int launch_sweep(cb_context* ctx, const SegArgs& a, uint32_t nq) {
-  const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * kBlocksPerSm, (nq + kBlock - 1) / kBlock));
   const int k = a.k;
+  auto kernel = segment_kernel<256, kBfs>;
   if (k == 0)
-    segment_kernel<0, kBfs><<<blocks, kBlock, 0, ctx->stream>>>(a);
+    kernel = segment_kernel<0, kBfs>;
   else if (k <= 4)
-    segment_kernel<4, kBfs><<<blocks, kBlock, 0, ctx->stream>>>(a);
+    kernel = segment_kernel<4, kBfs>;
   else if (k <= 16)
-    segment_kernel<16, kBfs><<<blocks, kBlock, 0, ctx->stream>>>(a);
+    kernel = segment_kernel<16, kBfs>;
   else if (k <= 32)
-    segment_kernel<32, kBfs><<<blocks, kBlock, 0, ctx->stream>>>(a);
+    kernel = segment_kernel<32, kBfs>;
   else if (k <= 64)
-    segment_kernel<64, kBfs><<<blocks, kBlock, 0, ctx->stream>>>(a);
+    kernel = segment_kernel<64, kBfs>;
   else if (k <= 128)
-    segment_kernel<128, kBfs><<<blocks, kBlock, 0, ctx->stream>>>(a);
-  else
-    segment_kernel<256, kBfs><<<blocks, kBlock, 0, ctx->stream>>>(a);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+    kernel = segment_kernel<128, kBfs>;
+  return launch(ctx, kernel, grid_for(ctx, nq, kBlock, kBlocksPerSm), kBlock, 0, a);
 }
 
 }  // namespace
@@ -365,7 +362,7 @@ extern "C" int cb_cloud_segment(cb_context* ctx, cb_cloud* cloud, const cb_segme
   if ((prm->terms & (CB_SEG_NORMALS | CB_SEG_COLORS)) && (normals || colors)) CB_TRY(scope.alloc(&d_host_in, 3 * n));
   float4* d_col = nullptr;
   float4* d_nrm = cloud->d_nrm;
-  const int eb = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + 255) / 256));
+  const int eb = grid_for(ctx, n, 256);
 
   ScopedEvents ev;
   if (gpu_ms) {
@@ -376,20 +373,17 @@ extern "C" int cb_cloud_segment(cb_context* ctx, cb_cloud* cloud, const cb_segme
   const unsigned long long zero[5] = {0, 0, 0, 0, 0};
   CB_CUDA(cudaMemcpyToSymbolAsync(g_uf_counts, zero, sizeof(zero), 0, cudaMemcpyHostToDevice, ctx->stream));
 #endif
-  rank_kernel<<<eb, 256, 0, ctx->stream>>>(cloud->d_pts, n32, d_rank);
-  iota_kernel<<<eb, 256, 0, ctx->stream>>>(d_parent, n32);
-  ctx->launches += 2;
+  CB_TRY(launch(ctx, rank_kernel, eb, 256, 0, cloud->d_pts, n32, d_rank));
+  CB_TRY(launch(ctx, iota_kernel, eb, 256, 0, d_parent, n32));
   if ((prm->terms & CB_SEG_NORMALS) && normals) {
     CB_TRY(scope.alloc(&d_nrm, n));
     CB_CUDA(cudaMemcpyAsync(d_host_in, normals, 3 * n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    gather_kernel<<<eb, 256, 0, ctx->stream>>>(d_host_in, cloud->d_pts, n32, d_nrm);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, gather_kernel, eb, 256, 0, d_host_in, cloud->d_pts, n32, d_nrm));
   }
   if (prm->terms & CB_SEG_COLORS) {
     CB_TRY(scope.alloc(&d_col, n));
     CB_CUDA(cudaMemcpyAsync(d_host_in, colors, 3 * n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    gather_kernel<<<eb, 256, 0, ctx->stream>>>(d_host_in, cloud->d_pts, n32, d_col);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, gather_kernel, eb, 256, 0, d_host_in, cloud->d_pts, n32, d_col));
   }
   a.nrm = (prm->terms & CB_SEG_NORMALS) ? d_nrm : nullptr;
   a.col = d_col;
@@ -414,10 +408,8 @@ extern "C" int cb_cloud_segment(cb_context* ctx, cb_cloud* cloud, const cb_segme
       for (size_t i = 0; i < n_seeds; i++) h_seeds[i] = (uint32_t)seeds[i];
       CB_TRY(scope.alloc(&d_seeds, n_seeds));
       CB_CUDA(cudaMemcpyAsync(d_seeds, h_seeds.data(), n_seeds * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-      const int sb = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n_seeds + 255) / 256));
-      seed_kernel<<<sb, 256, 0, ctx->stream>>>(d_seeds, (uint32_t)n_seeds, d_visited, d_front, d_cnt);
-      ctx->launches += 1;
-      CB_CUDA(cudaGetLastError());
+      const int sb = grid_for(ctx, n_seeds, 256);
+      CB_TRY(launch(ctx, seed_kernel, sb, 256, 0, d_seeds, (uint32_t)n_seeds, d_visited, d_front, d_cnt));
     }
     a.visited = d_visited;
     a.next_count = d_cnt + 1;
@@ -436,18 +428,15 @@ extern "C" int cb_cloud_segment(cb_context* ctx, cb_cloud* cloud, const cb_segme
     }
     CB_CUDA(cudaMemsetAsync(d_tie, 0xff, n * sizeof(uint32_t), ctx->stream));
     CB_CUDA(cudaMemsetAsync(d_size, 0, n * sizeof(uint32_t), ctx->stream));
-    compress_kernel<<<eb, 256, 0, ctx->stream>>>(d_parent, d_visited, n32, d_root, d_size);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, compress_kernel, eb, 256, 0, d_parent, d_visited, n32, d_root, d_size));
     if (n_seeds) {
-      const int sb = (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n_seeds + 255) / 256));
-      seed_tie_kernel<<<sb, 256, 0, ctx->stream>>>(d_seeds, (uint32_t)n_seeds, d_root, d_tie);
-      ctx->launches += 1;
+      const int sb = grid_for(ctx, n_seeds, 256);
+      CB_TRY(launch(ctx, seed_tie_kernel, sb, 256, 0, d_seeds, (uint32_t)n_seeds, d_root, d_tie));
     }
   }
   if (!seeded) {
     CB_CUDA(cudaMemsetAsync(d_size, 0, n * sizeof(uint32_t), ctx->stream));
-    compress_kernel<<<eb, 256, 0, ctx->stream>>>(d_parent, nullptr, n32, d_root, d_size);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, compress_kernel, eb, 256, 0, d_parent, nullptr, n32, d_root, d_size));
   }
 
   // kept segments, sorted on (size desc, tie key asc)
@@ -460,11 +449,8 @@ extern "C" int cb_cloud_segment(cb_context* ctx, cb_cloud* cloud, const cb_segme
   CB_TRY(scope.alloc(&d_cid, n));
   CB_TRY(scope.alloc(&d_p2c, n));
   CB_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(uint32_t), ctx->stream));
-  segments_kernel<<<eb, 256, 0, ctx->stream>>>(d_root, d_size, seeded ? d_tie : nullptr, n32,
-                                               (uint64_t)prm->min_segment_size, (uint64_t)prm->max_segment_size, d_keys,
-                                               d_vals, d_cnt);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, segments_kernel, eb, 256, 0, d_root, d_size, seeded ? d_tie : nullptr, n32,
+                (uint64_t)prm->min_segment_size, (uint64_t)prm->max_segment_size, d_keys, d_vals, d_cnt));
   uint32_t m = 0;
   CB_CUDA(cudaMemcpyAsync(&m, d_cnt, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -472,12 +458,9 @@ extern "C" int cb_cloud_segment(cb_context* ctx, cb_cloud* cloud, const cb_segme
   CB_CUDA(cudaMemsetAsync(d_cid, 0xff, n * sizeof(uint32_t), ctx->stream));
   uint32_t* d_sizes = d_size;  // (the per-root sizes are no longer needed: reused for the sorted segment sizes)
   if (m) {
-    cluster_id_kernel<<<eb, 256, 0, ctx->stream>>>(d_keys, d_vals, m, d_cid, d_sizes);
-    ctx->launches += 1;
+    CB_TRY(launch(ctx, cluster_id_kernel, eb, 256, 0, d_keys, d_vals, m, d_cid, d_sizes));
   }
-  label_kernel<<<eb, 256, 0, ctx->stream>>>(d_root, d_cid, n32, m, d_p2c, d_keys, d_vals);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, label_kernel, eb, 256, 0, d_root, d_cid, n32, m, d_p2c, d_keys, d_vals));
   // cluster -> points: stable sort of (cluster, point) in point order; unlabelled points (key m) sort last
   CB_TRY(radix_sort_pairs_u64(ctx, d_keys, d_vals, d_keys_tmp, d_vals_tmp, n, bits_for(m)));
   if (gpu_ms) CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));

@@ -334,12 +334,8 @@ int check_params(const Obj* w, const cb_sparse_warp_params* p) { return check_pa
 // The control weights of this call's ctrl_coeff.
 int weights(Obj* w, const cb_sparse_warp_params* p) {
   if (w->n == 0) return CB_OK;
-  ctrl_weights_kernel<<<grid_for(w->ctx, w->n), kBlock, 0, w->ctx->stream>>>(w->n, w->d_ctrl_off, w->d_ctrl_d2,
-                                                                              w->d_sperm, p->ctrl_coeff, w->d_w,
-                                                                              w->d_ws, w->d_W);
-  w->ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(w->ctx, ctrl_weights_kernel, grid_for(w->ctx, w->n, kBlock), kBlock, 0, w->n, w->d_ctrl_off,
+                w->d_ctrl_d2, w->d_sperm, p->ctrl_coeff, w->d_w, w->d_ws, w->d_W);
 }
 
 // d_T <- T_host (identities when NULL)
@@ -358,12 +354,8 @@ int set_nodes(Obj* w, const float* T_host) {
 
 int resample(Obj* w, const int* nn) {
   if (w->n == 0) return CB_OK;
-  sparse_resample_kernel<<<grid_for(w->ctx, w->n), kBlock, 0, w->ctx->stream>>>(
-      w->n, w->d_ctrl_off, w->d_ctrl_idx, w->d_w, w->d_W, w->d_T, w->src->d_raw, w->d_Td, w->d_warped, nn,
-      w->d_stats);
-  w->ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(w->ctx, sparse_resample_kernel, grid_for(w->ctx, w->n, kBlock), kBlock, 0, w->n, w->d_ctrl_off,
+                w->d_ctrl_idx, w->d_w, w->d_W, w->d_T, w->src->d_raw, w->d_Td, w->d_warped, nn, w->d_stats);
 }
 
 // One estimateSparseWarpFieldCombinedMetric call (gauss_newton) with the sparse assembly, node pass and CG; the
@@ -424,11 +416,8 @@ int sparse_gauss_newton(Obj* w, const cb_warp_params* p, const int* corr_dst, co
   ca.inc_other = w->d_inc_other;
   ca.arc_c = w->d_arc_c;
   auto assemble = [&]() -> int {
-    sparse_assemble_kernel<<<(unsigned)(((size_t)w->n + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(aa);
-    CB_CUDA(cudaGetLastError());
-    sparse_node_kernel<<<(unsigned)(((size_t)w->m + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(na);
-    CB_CUDA(cudaGetLastError());
-    ctx->launches += 2;
+    CB_TRY(launch(ctx, sparse_assemble_kernel, (unsigned)(((size_t)w->n + kBlock - 1) / kBlock), kBlock, 0, aa));
+    CB_TRY(launch(ctx, sparse_node_kernel, (unsigned)(((size_t)w->m + kBlock - 1) / kBlock), kBlock, 0, na));
     return CB_OK;
   };
   return gauss_newton(w, p, no_corr, assemble, (const void*)sparse_cg_kernel, ca, gn, timer);
@@ -474,18 +463,13 @@ int init(Obj* w, const std::vector<uint32_t>& ctrl_off, const std::vector<uint32
     CB_CUDA(cudaMemcpyAsync(w->d_sidx, sidx.data(), total * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     CB_CUDA(cudaMemcpyAsync(w->d_sperm, sperm.data(), total * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     CB_CUDA(cudaMemcpyAsync(d_slot_pt, slot_pt.data(), total * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-    node_keys_kernel<<<grid_for(ctx, total), kBlock, 0, s>>>(w->d_sidx, total, keys, vals);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, node_keys_kernel, grid_for(ctx, total, kBlock), kBlock, 0, w->d_sidx, total, keys, vals));
     int bits = 1;
     while (bits < 32 && (1ull << bits) < (uint64_t)mm) bits++;
     CB_TRY(radix_sort_pairs_u64(ctx, keys, vals, keys_tmp, vals_tmp, total, bits));
   }
-  node_incidence_fill_kernel<<<grid_for(ctx, (size_t)total + 1), kBlock, 0, s>>>(keys, vals, total, w->m, d_slot_pt,
-                                                                                w->d_ninc_pt, w->d_ninc_slot,
-                                                                                w->d_ninc_off);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, node_incidence_fill_kernel, grid_for(ctx, (size_t)total + 1, kBlock), kBlock, 0, keys, vals, total,
+                w->m, d_slot_pt, w->d_ninc_pt, w->d_ninc_slot, w->d_ninc_off));
   return upload_arc_incidence(w, lo, hi, d2);  // synchronises the stream
 }
 

@@ -3,6 +3,7 @@
 // rowwise().mean() of the ICP constructors (icp_single_transform_combined_metric.hpp:51-58) with one
 // streaming pass over the packed xyz array: HBM-bound, 12 B/point.
 #include "cb_internal.hpp"
+#include "launch.cuh"
 #include "reduce.cuh"
 #include "stats_kernels.cuh"
 #include <algorithm>
@@ -61,12 +62,12 @@ __global__ void __launch_bounds__(kReduceBlock) moments_kernel(const float* __re
 
 int launch_moments(cb_context* ctx, const float* d_raw, size_t n, const float* shift3, bool finite_only) {
   // persistent grid: a whole number of resident blocks per SM (occupancy API), 8 points per thread and trip
+  auto kernel = finite_only ? moments_kernel<true> : moments_kernel<false>;
   static int per_sm[2] = {0, 0};
   int& psm = per_sm[finite_only ? 1 : 0];
   if (psm == 0) {
     int v = 0;
-    const cudaError_t e = finite_only ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, moments_kernel<true>, kReduceBlock, 0)
-                                      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, moments_kernel<false>, kReduceBlock, 0);
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kernel, kReduceBlock, 0);
     if (e != cudaSuccess || v < 1) v = 4;
     psm = v;
   }
@@ -74,13 +75,7 @@ int launch_moments(cb_context* ctx, const float* d_raw, size_t n, const float* s
       1, std::min<size_t>((size_t)ctx->sm_count * psm, (n / 8 + kReduceBlock - 1) / kReduceBlock + 1));
   ReduceScratch rs;
   CB_TRY(get_reduce_scratch(ctx, blocks, kMomentValues, &rs));
-  if (finite_only)
-    moments_kernel<true><<<blocks, kReduceBlock, 0, ctx->stream>>>(d_raw, n, shift3[0], shift3[1], shift3[2], rs);
-  else
-    moments_kernel<false><<<blocks, kReduceBlock, 0, ctx->stream>>>(d_raw, n, shift3[0], shift3[1], shift3[2], rs);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, kernel, blocks, kReduceBlock, 0, d_raw, n, shift3[0], shift3[1], shift3[2], rs);
 }
 
 }  // namespace cb

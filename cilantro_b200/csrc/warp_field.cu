@@ -180,10 +180,7 @@ int dense_gauss_newton(cb_warp_icp* w, const cb_warp_params* p, const int* corr_
   ca.inc_other = w->d_inc_other;
   ca.arc_c = w->d_arc_c;
   auto assemble = [&]() -> int {
-    warp_assemble_kernel<<<(unsigned)(((size_t)w->n + kBlock - 1) / kBlock), kBlock, 0, ctx->stream>>>(aa);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
-    return CB_OK;
+    return launch(ctx, warp_assemble_kernel, (unsigned)(((size_t)w->n + kBlock - 1) / kBlock), kBlock, 0, aa);
   };
   return gauss_newton(w, p, no_corr, assemble, (const void*)warp_cg_kernel, ca, gn, nullptr);
 }

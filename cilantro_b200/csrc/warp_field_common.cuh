@@ -11,6 +11,7 @@
 
 #include "cb_internal.hpp"
 #include "icp_kernels.cuh"
+#include "launch.cuh"
 #include "solve_core.hpp"
 #include <algorithm>
 #include <cfloat>
@@ -516,10 +517,6 @@ struct WarpCore {
   bool have_corr = false;
 };
 
-int grid_for(cb_context* ctx, size_t n) {
-  return (int)std::max<size_t>(1, std::min<size_t>((size_t)ctx->sm_count * 8, (n + kBlock - 1) / kBlock));
-}
-
 int check_params(const WarpCore* w, const cb_warp_params* p) {
   CB_CHECK(w && p, CB_ERR_INVALID, "null argument");
   CB_CHECK(p->search_dir == CB_SECOND_TO_FIRST && p->require_reciprocal == 0 && p->one_to_one == 0 &&
@@ -624,8 +621,7 @@ int alloc_core(WarpCore* w, const void* cg_kernel, size_t loop_len) {
   int per_sm = 0;
   CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cg_kernel, kBlock, 0));
   CB_CHECK(per_sm >= 1, CB_ERR_CUDA, "the CG kernel cannot be resident");
-  w->cg_grid = (int)std::max<size_t>(
-      1, std::min<size_t>((size_t)w->ctx->sm_count * per_sm, (std::max<size_t>(loop_len, 1) + kBlock - 1) / kBlock));
+  w->cg_grid = grid_for(w->ctx, loop_len, kBlock, per_sm);
   return w->mem.alloc(&w->d_part, 5 * (size_t)w->cg_grid);
 }
 
@@ -650,17 +646,13 @@ int upload_arc_incidence(WarpCore* w, const std::vector<uint32_t>& lo, const std
   CB_TRY(scope.alloc(&vals, total));
   CB_TRY(scope.alloc(&vals_tmp, total));
   if (m32) {
-    incidence_keys_kernel<<<grid_for(ctx, m32), kBlock, 0, s>>>(d_lo, d_hi, m32, keys, vals);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, incidence_keys_kernel, grid_for(ctx, m32, kBlock), kBlock, 0, d_lo, d_hi, m32, keys, vals));
     int bits = 1;
     while (bits < 32 && (1ull << bits) < (uint64_t)std::max<uint32_t>(n_nodes, 1)) bits++;
     CB_TRY(radix_sort_pairs_u64(ctx, keys, vals, keys_tmp, vals_tmp, total, bits));
   }
-  incidence_fill_kernel<<<grid_for(ctx, (size_t)total + 1), kBlock, 0, s>>>(keys, vals, total, n_nodes, d_lo, d_hi,
-                                                                           w->d_inc_arc, w->d_inc_other, w->d_inc_off);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(launch(ctx, incidence_fill_kernel, grid_for(ctx, (size_t)total + 1, kBlock), kBlock, 0, keys, vals, total,
+                n_nodes, d_lo, d_hi, w->d_inc_arc, w->d_inc_other, w->d_inc_off));
   CB_CUDA(cudaStreamSynchronize(s));
   return CB_OK;
 }
@@ -764,11 +756,8 @@ int warp_points(WarpCore* w, float* T, const float* T_host) {
   if (w->n == 0) return CB_OK;
   if (T_host)
     CB_CUDA(cudaMemcpyAsync(T, T_host, 12 * (size_t)w->n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-  warp_points_kernel<<<grid_for(ctx, w->n), kBlock, 0, ctx->stream>>>(w->n, w->src->d_raw, T, T_host == nullptr,
-                                                                      w->d_warped);
-  ctx->launches += 1;
-  CB_CUDA(cudaGetLastError());
-  return CB_OK;
+  return launch(ctx, warp_points_kernel, grid_for(ctx, w->n, kBlock), kBlock, 0, w->n, w->src->d_raw, T,
+                T_host == nullptr, w->d_warped);
 }
 
 // What Gauss-Newton calls report: the flag of the last call, the steps and CG iterations summed over the calls, and
@@ -825,9 +814,8 @@ int gauss_newton(WarpCore* w, const cb_warp_params* p, bool no_corr, Assemble&& 
     CB_TRY(assemble());
     if (timer) CB_CUDA(cudaEventRecord(timer->ev.e1, ctx->stream));
     void* args[] = {&ca};
-    CB_CUDA(cudaLaunchCooperativeKernel(cg_kernel, dim3(w->cg_grid), dim3(kBlock), args, 0, ctx->stream));
+    CB_TRY(launch_cooperative(ctx, cg_kernel, w->cg_grid, kBlock, args));
     if (timer) CB_CUDA(cudaEventRecord(timer->end.e1, ctx->stream));
-    ctx->launches += 1;
     CB_CUDA(cudaMemcpyAsync(w->h_stats, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
     CB_CUDA(cudaStreamSynchronize(ctx->stream));
     if (timer) {
@@ -860,11 +848,8 @@ int apply_update(WarpCore* w, bool compose, bool warp_next, float* last_delta_sq
   cb_context* ctx = w->ctx;
   CB_CUDA(cudaMemsetAsync(w->d_stats, 0, sizeof(WarpStats), ctx->stream));
   if (w->m) {
-    warp_compose_kernel<<<grid_for(ctx, w->m), kBlock, 0, ctx->stream>>>(
-        w->m, w->src->d_raw, w->d_xs, w->d_T, compose, warp_next ? w->d_warped : nullptr,
-        warp_next ? w->d_nn : nullptr, w->d_stats);
-    ctx->launches += 1;
-    CB_CUDA(cudaGetLastError());
+    CB_TRY(launch(ctx, warp_compose_kernel, grid_for(ctx, w->m, kBlock), kBlock, 0, w->m, w->src->d_raw, w->d_xs,
+                  w->d_T, compose, warp_next ? w->d_warped : nullptr, warp_next ? w->d_nn : nullptr, w->d_stats));
   }
   CB_CUDA(cudaMemcpyAsync(w->h_stats, w->d_stats, sizeof(WarpStats), cudaMemcpyDeviceToHost, ctx->stream));
   CB_CUDA(cudaStreamSynchronize(ctx->stream));
