@@ -20,9 +20,9 @@
 // (triangle inequality); if the cached match's distance under T_{k+1} — evaluated with the contract arithmetic,
 // i.e. the very number the search would compute for it — is below that, the match is provably still the unique
 // nearest neighbour and its (index, d2) is what the full search would return, bit for bit. Only the queries
-// that fail the test are searched again, inside the same pass: each warp queues the ones it flagged, so the search
-// runs on dense warps. All bounds are rounded conservatively (directed rounding + 2^-18 relative margins, far above the
-// 6-ulp error of the fp32 distance evaluation); an exact tie can never pass the strict test.
+// that fail the test are searched again, inside the same pass: each warp lists the ones it flagged and searches them
+// after its last tile, on dense warps. All bounds are rounded conservatively (directed rounding + 2^-18 relative
+// margins, far above the 6-ulp error of the fp32 distance evaluation); an exact tie can never pass the strict test.
 // As ICP converges the per-iteration motion shrinks geometrically and almost every query takes the cached path:
 // the iteration becomes one streaming pass (16 B query + 8 B cache + one 16 B gather per source point).
 #include "cache_rule.hpp"
@@ -60,6 +60,8 @@ struct LoopArgs {
   int* cache_pos;      // per sorted query: sorted dst position of its match (-1 none)
   float* cache_r;      // per sorted query: every OTHER dst point is at least this far away (<= 0: unknown)
   float slack_first, slack_min, slack_max;  // widening of the search beyond the nearest distance (warp_search_wide.cuh)
+  uint32_t* flagged;       // cached pass: per warp of its grid, the queries it flagged, ascending (flagged_per_warp each)
+  uint32_t flagged_per_warp;
   LoopState* st;
   ReduceScratch rs;
   uint32_t rows;  // block rows of the cached pass in rs.partials (its grid size); 0: the cold search kernel's totals
@@ -158,8 +160,7 @@ struct ChunkPair {
 };
 
 // Lanes per queued region in the wide search's pooled scan (warp_search_wide.cuh). The cold search keeps one lane per
-// region. The cached pass's search uses pairs of lanes: its region scan then needs fewer live registers, and the
-// pass's streaming loop, which holds the call site of search_chunk_far, spills less (DESIGN §4.2).
+// region. The cached pass's search uses pairs of lanes: its region scan then needs fewer live registers (DESIGN §4.2).
 constexpr unsigned int kColdGroup = 1, kWarmGroup = 2;
 // kCold: nothing cached yet (no warm seed, first-iteration slack). Otherwise the query failed the exclusion test:
 // its cached match seeds the search and its last motion sets the slack.
@@ -196,15 +197,6 @@ __device__ __forceinline__ ChunkPair search_chunk_body(const LoopArgs& a, const 
   return cp;
 }
 
-// Out-of-line search of the cached pass: called from inside its tile loop, where the streaming registers and the
-// moment accumulators are live. Inlined there, the search's loop-invariant parameter loads were hoisted into
-// registers and the streaming loop spilled; behind the call only the call site saves and restores registers, once per
-// warp search.
-__device__ __noinline__ void search_chunk_far(const LoopArgs* ap, const BlockCtx* cxp, WideSearchSmem* wsm, bool act,
-                                              uint32_t i, ChunkPair* out) {
-  *out = search_chunk_body<false>(*ap, *cxp, wsm, act, i);
-}
-
 // Programmatic dependent launch (sm_90+): a kernel launched with the programmatic-stream-serialization attribute may
 // be scheduled while its predecessor in the stream is still running; it must execute pdl_wait() before it touches
 // anything the predecessor (or, transitively, earlier kernels: the predecessor passed its own pdl_wait first) wrote.
@@ -234,34 +226,37 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
 // ---- kernel 1 of a warm iteration: the cached pass and the search of what it could not decide ---------------------
 // Elementwise over the source cloud: per query 16 B (point) + 8 B (cache) streamed and one 16 B gather of the cached
 // match (+ 16 B normal for the plane term). Queries that pass the exclusion test accumulate their pair at once. The
-// others are searched by the warp that flagged them: after each 32-query slot the warp's ballot appends the flagged
-// query indices, in ascending order, to a warp-private queue; as soon as 32 are queued the warp searches them
-// lane-dense (search_chunk_far: same slack rule, warm seed and cache update as the cold search), and at the end of its
-// tiles it searches what is left. Only __syncwarp is involved, so a searching warp holds up no other warp of its
-// block, and the searching lane adds its pair to the same accumulators.
+// others are searched by the warp that flagged them, after its last tile: after each 32-query slot the warp's ballot
+// appends the flagged query indices, in ascending order, to the warp's list in global memory (a.flagged); once the
+// warp's copies have drained it searches the list lane-dense, 32 at a time (search_chunk_body: same slack rule, warm
+// seed and cache update as the cold search), in its own pipeline buffers, and the searching lane adds its pair to the
+// warp's sums. Only __syncwarp is involved, so a searching warp holds up no other warp of its block. A converged
+// iteration flags a few dozen of 10^6 queries: the search gets no shared memory of its own and no call site inside the
+// streaming loop, whose registers it would otherwise share.
 // PERSISTENT: the grid is a whole number of resident blocks per SM, a block walks the tiles blockIdx.x, + gridDim.x,
-// ... (static round-robin: every tile costs the same, and the assignment — hence, with the fixed queue order, the
+// ... (static round-robin: every tile costs the same, and the assignment — hence, with the fixed list order, the
 // summation order — is fixed), the next tiles' loads are in flight while the current tile is evaluated, and the
 // moments are reduced ONCE per block (a per-tile reduction cost as much as the tile itself). Every block writes its row
 // to rs.partials (zeros included: the finish kernel folds every row) and is done.
 // The loads are not staged in registers: a register-staged version needed 128 registers -> 2 blocks/SM, few warp
 // slots occupied, long-scoreboard stalls on top - each thread can only keep the loads in flight that it has registers
-// for. Here every thread runs a private three-deep pipeline of cp.async copies into shared memory (LDGSTS: no
-// destination register, no scoreboard slot):
-//   stage A (tile k+2)  the streamed arrays: its queries' point (16 B), exclusion radius (4 B), cached match (4 B)
-//   stage B (tile k+1)  the gathers, once A has landed: the matched destination point (+ normal for the plane term)
-//   stage C (tile k)    evaluation from shared memory
+// for. Here every thread runs a private pipeline of cp.async copies into shared memory (LDGSTS: no destination
+// register, no scoreboard slot), kDepthA tiles of stage A and kDepthB of stage B:
+//   stage A (tile k+kDepthA-1)  the streamed arrays: its queries' point (16 B), exclusion radius (4 B), cached match (4 B)
+//   stage B (tile k+kDepthB-1)  the gathers, once A has landed: the matched destination point (+ normal for the plane
+//                               term)
+//   stage C (tile k)            evaluation from shared memory
 // Each thread only ever reads what it copied itself, so cp.async.wait_group is all the synchronisation there is -
-// no block barrier inside the tile loop.
-// Shared memory per block: the pipeline (three A buffers, two B buffers) and one WideSearchSmem per warp (27.6 KB,
-// the queue included), 1 KB of reduction slots and state.
-//   p2p: 256-query tiles (one query per thread): 26 KB of pipeline, 56 KB per block -> 4 blocks per SM in the 228 KB
-//        of an H100 SM, 64 registers. (512-query tiles would need 82 KB per block: 2 blocks per SM.)
-//   combined: 512-query tiles: 68 KB of pipeline, 98 KB per block -> 2 blocks per SM, 128 registers. At 3 blocks
-//        (80 registers, 256-query tiles) the exclusion test and the 28 accumulators spilled on every query, and with
-//        3 x 65 KB of shared memory the L1 left for those spills was too small: the 10 M pass ran 3x slower.
-// Both keep 1024 queries per SM in flight in the pipeline.
+// no block barrier inside the tile loop. The buffers are laid out warp by warp (WarpPipe), so a warp whose copies have
+// drained owns one contiguous region, and its search buffer (WideSearchSmem) lives there.
+//   p2p: 256-query tiles (one query per thread), stage A 4 deep and stage B 3 deep: each gather is issued two tiles
+//        ahead of its evaluation. 36 KB of pipeline, 4 blocks per SM (64 registers).
+//   combined: 512-query tiles, stage A 3 deep and stage B 2 deep: 68 KB of pipeline, 2 blocks per SM (128 registers).
+//        At 3 blocks (80 registers, 256-query tiles) the exclusion test and the 28 accumulators spilled on every query.
+// (DESIGN §4.2 has the measured alternatives.)
 __host__ __device__ constexpr int pipe_qpt(bool normals) { return normals ? 2 : 1; }
+__host__ __device__ constexpr int pipe_depth_a(bool normals) { return normals ? 3 : 4; }
+__host__ __device__ constexpr int pipe_depth_b(bool normals) { return normals ? 2 : 3; }
 __host__ __device__ constexpr int pipe_min_blocks(bool normals) { return normals ? 2 : 4; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -280,31 +275,38 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
+// One warp's pipeline buffers: entry k * 32 + lane belongs to the warp's k-th query of a tile on that lane.
+template <bool kNormals>
+struct WarpPipe {
+  static constexpr int kA = pipe_depth_a(kNormals), kB = pipe_depth_b(kNormals);
+  static constexpr int kW = pipe_qpt(kNormals) * 32;  // the warp's queries per tile
+  float4 src[kA][kW];
+  float r[kA][kW];
+  int seed[kA][kW];
+  float4 pt[kB][kW];
+  float4 nr[kNormals ? kB : 1][kNormals ? kW : 1];
+};
 template <bool kNormals>
 struct PipeSmem {
-  static constexpr int kT = pipe_qpt(kNormals) * kBlock;  // queries per tile
-  float4 src[3][kT];
-  float r[3][kT];
-  int seed[3][kT];
-  float4 pt[2][kT];
-  float4 nr[kNormals ? 2 : 1][kNormals ? kT : 1];
+  WarpPipe<kNormals> warp[kBlock / 32];
 };
+static_assert(sizeof(WideSearchSmem) <= sizeof(WarpPipe<false>) && sizeof(WideSearchSmem) <= sizeof(WarpPipe<true>),
+              "a warp's search buffer lives in its drained pipeline region");
 
 template <int MODE>
 __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)) icp_cached_pipe_kernel(const __grid_constant__ LoopArgs a) {
   constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
   constexpr bool kNormals = (MODE == kModeCombined);
   constexpr int kQpt = pipe_qpt(kNormals), kTile = kQpt * kBlock;
+  // stage A of tile n + kLeadA and stage B of tile n + kLeadB are issued while tile n is evaluated
+  constexpr int kDepthA = pipe_depth_a(kNormals), kDepthB = pipe_depth_b(kNormals);
+  constexpr int kLeadA = kDepthA - 1, kLeadB = kDepthB - 1;
+  static_assert(kLeadB >= 1 && kLeadA > kLeadB, "a gather needs its stream landed one step earlier");
   extern __shared__ __align__(16) unsigned char pipe_raw[];
-  PipeSmem<kNormals>& ps = *reinterpret_cast<PipeSmem<kNormals>*>(pipe_raw);
   __shared__ BlockCtx cx;
   __shared__ AsyncReduceSmem<NV> rsm;
-  __shared__ WideSearchSmem wsm[kBlock / 32];
   const unsigned int tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-  // per warp: flagged query indices waiting for a search, ascending. The queue lives in the warp's search buffer: it
-  // is only filled between searches, and each lane reads its entry before the search overwrites the buffer. (A queue
-  // of its own, 1 KB per block, would leave the p2p pass 176 B short of 4 blocks per SM.)
-  uint32_t* wq = wsm[warp].sec;
+  WarpPipe<kNormals>& wp = reinterpret_cast<PipeSmem<kNormals>*>(pipe_raw)->warp[warp];
   const uint32_t ntiles = (a.n_src + kTile - 1) / kTile;
   const bool want_nrm = kNormals && a.has_pl != 0;
 
@@ -313,11 +315,11 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
     if (tile < ntiles) {
 #pragma unroll
       for (int k = 0; k < kQpt; k++) {
-        const uint32_t slot = k * kBlock + tid, i = tile * kTile + slot;
+        const uint32_t i = tile * kTile + k * kBlock + tid;
         if (i < a.n_src) {
-          cp_async_16_cg(&ps.src[buf][slot], a.src_pts + i);
-          cp_async_4(&ps.r[buf][slot], a.cache_r + i);
-          cp_async_4(&ps.seed[buf][slot], a.cache_pos + i);
+          cp_async_16_cg(&wp.src[buf][k * 32 + lane], a.src_pts + i);
+          cp_async_4(&wp.r[buf][k * 32 + lane], a.cache_r + i);
+          cp_async_4(&wp.seed[buf][k * 32 + lane], a.cache_pos + i);
         }
       }
     }
@@ -328,12 +330,12 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
     if (tile < ntiles) {
 #pragma unroll
       for (int k = 0; k < kQpt; k++) {
-        const uint32_t slot = k * kBlock + tid, i = tile * kTile + slot;
+        const uint32_t e = k * 32 + lane, i = tile * kTile + k * kBlock + tid;
         if (i < a.n_src) {
-          const int sd = ps.seed[abuf][slot];
-          if (sd >= 0 && ps.r[abuf][slot] > 0.f) {
-            cp_async_16_ca(&ps.pt[bbuf][slot], a.dst.pts + sd);
-            if (kNormals && want_nrm) cp_async_16_ca(&ps.nr[bbuf][slot], a.dst.nrm + sd);
+          const int sd = wp.seed[abuf][e];
+          if (sd >= 0 && wp.r[abuf][e] > 0.f) {
+            cp_async_16_ca(&wp.pt[bbuf][e], a.dst.pts + sd);
+            if (kNormals && want_nrm) cp_async_16_ca(&wp.nr[bbuf][e], a.dst.nrm + sd);
           }
         }
       }
@@ -342,14 +344,21 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
   };
 
   const uint32_t t0 = blockIdx.x, stride = gridDim.x;
+  // Step n of the block (n = -kLeadA, -kLeadA + 1, ...) commits two groups, A(n + kLeadA) then B(n + kLeadB) (either
+  // may be empty), and evaluates tile n once it is >= 0. With that fixed order, A(n + kLeadB) has landed when at most
+  // 2 (kLeadA - kLeadB) groups are pending after A(n + kLeadA), and B(n) when at most 2 kLeadB are pending after
+  // B(n + kLeadB).
   // The dependency wait comes BEFORE the first copies: the cache arrays are rewritten every iteration, their 4-byte
   // copies go through L1 (cp.async.ca), and only accesses after griddepcontrol.wait are guaranteed to see the previous
   // kernels' writes. What programmatic launch buys here: the blocks are resident when the finish kernel ends, and the
   // one-block finish kernel of this iteration, released at once, is resident and waiting when this grid drains.
   pdl_wait();
   pdl_launch_dependents();
-  stage_a(t0, 0);           // group: A(0)
-  stage_a(t0 + stride, 1);  // group: A(1)
+#pragma unroll
+  for (int n = 0; n < kLeadA - kLeadB; n++) {  // steps -kLeadA .. -kLeadB - 1: no gather due yet
+    stage_a(t0 + n * stride, n);
+    cp_async_commit();
+  }
   if (tid == 0) {
     rsm.arrived = 0u;
     load_block_ctx(a, cx);
@@ -364,92 +373,93 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
     a.st->trace[slot][0] = global_timer_ns();
     a.st->trace[slot][4] = 0ull;
   }
-  cp_async_wait<1>();   // A(0) has landed
-  stage_b(t0, 0, 0);    // group: B(0)
+#pragma unroll
+  for (int n = kLeadA - kLeadB; n < kLeadA; n++) {  // steps -kLeadB .. -1
+    stage_a(t0 + n * stride, n);
+    cp_async_wait<2 * (kLeadA - kLeadB)>();
+    stage_b(t0 + (n - (kLeadA - kLeadB)) * stride, n - (kLeadA - kLeadB), n - (kLeadA - kLeadB));
+  }
   double acc[NV];
 #pragma unroll
   for (int v = 0; v < NV; v++) acc[v] = 0.0;
-  // the warp's row of the block reduction: what the warp folded before each search (and, at the end, the rest)
+  // the warp's row of the block reduction: what the warp folded before its searches, then their pairs. (The fold adds
+  // value by value: the transposing butterfly of warp_sum_to_slot<16, false> keeps acc[] in local memory.)
   if (lane < NV) rsm.slot[warp][lane] = 0.0;
-  __syncwarp();  // (lane 0 adds to the whole row)
-  // The warp searches the queries queued in wq[0, n) on lanes < n; the searching lane accumulates its pair. The
-  // accumulators are folded into the warp's row first and restart from zero, so that no register of the streaming
-  // loop is live across the search call (held there, all of acc[] was kept in local memory for the whole loop).
-  unsigned int queued = 0, searched = 0;  // warp-uniform
-  auto search_queued = [&](unsigned int n) {
-    __syncwarp();
+  // the warp's flagged queries, ascending; `flagged` is warp-uniform
+  uint32_t* const list = a.flagged + (size_t)(blockIdx.x * (kBlock / 32) + warp) * a.flagged_per_warp;
+  unsigned int flagged = 0;
+  // step n evaluates tile t0 + n*stride from A buffer n % kDepthA and B buffer n % kDepthB
+  int abuf = 0, bbuf = 0;
+#pragma unroll 1
+  for (uint32_t tile = t0; tile < ntiles; tile += stride) {
+    const int abuf_next = (abuf == kDepthA - 1) ? 0 : abuf + 1, bbuf_next = (bbuf == kDepthB - 1) ? 0 : bbuf + 1;
+    // A(n + kLeadA) goes where tile n - 1 was, A(n + kLeadB) is in buffer (n + kLeadB) % kDepthA, and B(n + kLeadB)
+    // goes where tile n - 1's gathers were
+    const int abuf_prev = (abuf == 0) ? kDepthA - 1 : abuf - 1, bbuf_prev = (bbuf == 0) ? kDepthB - 1 : bbuf - 1;
+    const int abuf_b = (abuf + kLeadB) % kDepthA;
+    stage_a(tile + kLeadA * stride, abuf_prev);
+    cp_async_wait<2 * (kLeadA - kLeadB)>();
+    stage_b(tile + kLeadB * stride, abuf_b, bbuf_prev);
+    cp_async_wait<2 * kLeadB>();
+    const uint32_t base = tile * kTile;
+#pragma unroll
+    for (int k = 0; k < kQpt; k++) {
+      const uint32_t e = k * 32 + lane, i = base + k * kBlock + tid;
+      const bool active = i < a.n_src;
+      bool miss = active;
+      if (active) {
+        const float rc = wp.r[abuf][e];
+        const int sd = wp.seed[abuf][e];
+        if (rc > 0.f) {
+          const float4 sc = wp.src[abuf][e];
+          // the exclusion test (cache_rule.hpp): hit -> the cached match is this iteration's exact search result
+          rule::Verdict v;
+          float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
+          rule::cached_match_test(cx.T, cx.Tp, sc.x, sc.y, sc.z, rc, sd, a.max_d2, [&] { return wp.pt[bbuf][e]; }, p, v);
+          miss = v.miss;
+          if (!miss) a.cache_r[i] = v.r2;
+          if (v.pair) {
+            accumulate_pair<MODE, true>(
+                acc, cx, a.has_pt != 0, a.has_pl != 0, p, v.qx, v.qy, v.qz, a.src_nrm != nullptr,
+                [&] { return kNormals ? wp.nr[kNormals ? bbuf : 0][kNormals ? e : 0] : make_float4(0.f, 0.f, 0.f, 0.f); },
+                [&] { return __ldg(a.src_nrm + i); }, v.d2);
+          }
+        }
+      }
+      // flagged queries -> the warp's list, in ascending order
+      const unsigned int mm = __ballot_sync(0xffffffffu, miss);
+      if (miss) list[flagged + __popc(mm & ((1u << lane) - 1u))] = i;
+      flagged += __popc(mm);
+    }
+    abuf = abuf_next;
+    bbuf = bbuf_next;
+  }
+  cp_async_wait<0>();
+  // the warp's copies have drained (its pipeline region is free for the search) and its list entries are visible to
+  // all of its lanes
+  __syncwarp();
+  // The warp searches its list, 32 queries at a time; the searching lane accumulates its pair. Before each search the
+  // accumulators are folded into the warp's row and restart from zero, so that none of them is live across it.
+  WideSearchSmem* wsm = reinterpret_cast<WideSearchSmem*>(&wp);
+  for (unsigned int c = 0; c < flagged; c += 32u) {
     warp_sum_to_slot<NV, true>(acc, rsm);
 #pragma unroll
     for (int v = 0; v < NV; v++) acc[v] = 0.0;
-    const bool act = lane < n;
-    ChunkPair cp;
-    search_chunk_far(&a, &cx, &wsm[warp], act, act ? wq[lane] : 0u, &cp);
+    const bool act = c + lane < flagged;
+    const ChunkPair cp = search_chunk_body<false>(a, cx, wsm, act, act ? list[c + lane] : 0u);
     if (cp.pos >= 0) {
       const float4 dp = __ldg(a.dst.pts + cp.pos);
       accumulate_pair<MODE, true>(
           acc, cx, a.has_pt != 0, a.has_pl != 0, dp, cp.qx, cp.qy, cp.qz, a.src_nrm != nullptr,
           [&] { return __ldg(a.dst.nrm + cp.pos); }, [&] { return __ldg(a.src_nrm + cp.i); }, cp.d2);
     }
-    searched += n;
-    __syncwarp();  // every lane has read its entry before the queue is refilled
-  };
-  // iteration n evaluates tile t0 + n*stride; on entry the committed groups are ... A(n+1), B(n)
-  int abuf = 0, bbuf = 0;
-#pragma unroll 1
-  for (uint32_t tile = t0; tile < ntiles; tile += stride) {
-    const int abuf1 = (abuf == 2) ? 0 : abuf + 1, abuf2 = (abuf1 == 2) ? 0 : abuf1 + 1;
-    stage_a(tile + 2 * stride, abuf2);             // group: A(n+2)
-    cp_async_wait<2>();                            // pending at most {B(n), A(n+2)}: A(n+1) has landed
-    stage_b(tile + stride, abuf1, bbuf ^ 1);       // group: B(n+1)
-    cp_async_wait<2>();                            // pending at most {A(n+2), B(n+1)}: B(n) has landed
-    const uint32_t base = tile * kTile;
-#pragma unroll
-    for (int k = 0; k < kQpt; k++) {
-      const uint32_t slot = k * kBlock + tid, i = base + slot;
-      const bool active = i < a.n_src;
-      bool miss = active;
-      if (active) {
-        const float rc = ps.r[abuf][slot];
-        const int sd = ps.seed[abuf][slot];
-        if (rc > 0.f) {
-          const float4 sc = ps.src[abuf][slot];
-          // the exclusion test (cache_rule.hpp): hit -> the cached match is this iteration's exact search result
-          rule::Verdict v;
-          float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
-          rule::cached_match_test(cx.T, cx.Tp, sc.x, sc.y, sc.z, rc, sd, a.max_d2, [&] { return ps.pt[bbuf][slot]; }, p, v);
-          miss = v.miss;
-          if (!miss) a.cache_r[i] = v.r2;
-          if (v.pair) {
-            accumulate_pair<MODE, true>(
-                acc, cx, a.has_pt != 0, a.has_pl != 0, p, v.qx, v.qy, v.qz, a.src_nrm != nullptr,
-                [&] { return kNormals ? ps.nr[kNormals ? bbuf : 0][kNormals ? slot : 0] : make_float4(0.f, 0.f, 0.f, 0.f); },
-                [&] { return __ldg(a.src_nrm + i); }, v.d2);
-          }
-        }
-      }
-      // flagged queries -> the warp's queue; the ones that do not fit wait in their lane's register (i) until the
-      // 32 queued ones have been searched
-      const unsigned int mm = __ballot_sync(0xffffffffu, miss);
-      const unsigned int at = queued + __popc(mm & ((1u << lane) - 1u));
-      if (miss && at < 32u) wq[at] = i;
-      queued += __popc(mm);
-      if (queued >= 32u) {
-        search_queued(32u);
-        queued -= 32u;
-        if (miss && at >= 32u) wq[at - 32u] = i;
-      }
-    }
-    abuf = abuf1;
-    bbuf ^= 1;
   }
-  cp_async_wait<0>();
-  if (queued > 0u) search_queued(queued);
-  if (lane == 0 && searched > 0u) {
-    atomicAdd(&a.st->searched_cur, (unsigned long long)searched);
-    if (a.trace) atomicAdd(&a.st->trace[__ldcg(&a.st->iters) & 63][4], (unsigned long long)searched);
+  if (lane == 0 && flagged > 0u) {
+    atomicAdd(&a.st->searched_cur, (unsigned long long)flagged);
+    if (a.trace) atomicAdd(&a.st->trace[__ldcg(&a.st->iters) & 63][4], (unsigned long long)flagged);
   }
-  if (a.trace && lane == 0) atomicMax(&a.st->trace[__ldcg(&a.st->iters) & 63][5], global_timer_ns());
   warp_sum_to_slot<NV, true>(acc, rsm);
+  if (a.trace && lane == 0) atomicMax(&a.st->trace[__ldcg(&a.st->iters) & 63][5], global_timer_ns());
   double row;
   if (block_row_from_slots<NV>(rsm, row) && lane < NV) a.rs.partials[(size_t)blockIdx.x * NV + lane] = row;
 }
@@ -640,10 +650,10 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   static const bool trace = getenv("CB_LOOP_TRACE") != nullptr;
   a.trace = trace ? 1 : 0;
   // cold iteration (first launch: nothing cached): search kernel, one 256-query chunk per block; warm iterations:
-  // the persistent cached pass (PipeSmem::kT queries per tile), which also searches the queries it flags
+  // the persistent cached pass (pipe_qpt x kBlock queries per tile), which also searches the queries it flags
   const int blocks_cold = std::max(1, (int)((ns + kBlock - 1) / kBlock));
   // once per device (function attributes belong to the device the context is on, not to the process): the pipeline's
-  // dynamic shared memory, the whole shared-memory carveout (4 / 2 blocks of 56 / 98 KB per SM), and how many blocks
+  // dynamic shared memory, the whole shared-memory carveout, and how many blocks
   // of the cached pass are resident per SM
   static bool attr_set_dev[64] = {};
   static int resident_dev[64][2] = {};
@@ -669,6 +679,18 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   const int per_sm = std::max(1, resident[p2p ? 0 : 1]);
   const size_t tile = (size_t)pipe_qpt(!p2p) * kBlock;
   const int blocks_cached = grid_for(ctx, ns, tile, per_sm);
+  // the cached pass's flagged-query lists: per warp, room for every query of its block's tiles (about n_src in all)
+  const size_t per_warp = ((ns + tile - 1) / tile + blocks_cached - 1) / blocks_cached * (tile / (kBlock / 32));
+  const size_t flagged_need = per_warp * (size_t)blocks_cached * (kBlock / 32);
+  if (icp->loop_flagged_cap < flagged_need) {
+    if (icp->d_loop_flagged) CB_TRY(icp->mem.free(icp->d_loop_flagged));
+    icp->d_loop_flagged = nullptr;
+    icp->loop_flagged_cap = 0;
+    CB_TRY(icp->mem.alloc(&icp->d_loop_flagged, flagged_need));
+    icp->loop_flagged_cap = flagged_need;
+  }
+  a.flagged = icp->d_loop_flagged;
+  a.flagged_per_warp = (uint32_t)per_warp;
   CB_TRY(get_reduce_scratch(ctx, blocks_cold, kMaxValues, &a.rs));
   Exchange ex;
   std::memset(&ex, 0, sizeof(ex));

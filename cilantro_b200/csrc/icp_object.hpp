@@ -60,6 +60,8 @@ struct cb_icp {
   cb::LoopState* h_state = nullptr;  // pinned
   cb::LoopState* h_state2 = nullptr; // pinned: the batches' states alternate between the two
   cudaEvent_t batch_ev[2] = {nullptr, nullptr};  // end of a batch + its state copy
+  uint32_t* d_loop_flagged = nullptr;  // the cached pass's per-warp lists of flagged queries (icp_loop.cu)
+  size_t loop_flagged_cap = 0;         // in entries
   cb_cloud* src_full = nullptr;      // world > 1, engine modes: the whole source cloud replicated on this rank (owned)
   bool loop_last = false;            // the last estimate() ran on the device loop
   uint64_t searched_last = 0;        // queries its last iteration searched again (CB_LOOP_TRACE / cb_icp_loop_cache)

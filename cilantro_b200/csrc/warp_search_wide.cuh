@@ -24,8 +24,6 @@ namespace cb {
 struct WideSearchSmem : WarpQueue {
   unsigned int sec[32];  // merged second-smallest d2 (float bits; non-negative floats order like uints)
 };
-// The cached pass of the ICP loop keeps 8 of these per block and is 176 B short of losing a resident block per SM.
-static_assert(sizeof(WideSearchSmem) <= 3456, "WideSearchSmem must not grow");
 
 struct WideBest {
   float d2;   // squared distance of the nearest point with d2 < max_d2 (else max_d2)
