@@ -4,8 +4,7 @@
 // TWO kernels per ICP iteration and NO host round trip between iterations. In iteration k the first kernel
 //   1. reads the current estimate T_k from device memory (LoopState),
 //   2. finds every source point's correspondence under T_k (below),
-//   3. accumulates the estimator's moments, reduces them warp -> block and writes one row per block (the cold search
-//      kernel of the first iteration goes on to the grid total, in rs.result);
+//   3. accumulates the estimator's moments, reduces them warp -> block and writes one row per block;
 // the finish kernel (one block, launched behind it)
 //   4. folds the block rows into this GPU's 16 / 28 totals in a fixed order, all-reduces them with the peer ranks
 //      over NVLink peer memory (reduce.cuh, bounded wait), then solves on the device — Kabsch / one Gauss-Newton
@@ -64,8 +63,7 @@ struct LoopArgs {
   uint32_t flagged_per_warp;
   LoopState* st;
   ReduceScratch rs;
-  uint32_t rows;  // block rows of the cached pass in rs.partials (its grid size); 0: the cold search kernel's totals
-                  // are in rs.result (enqueue_iteration)
+  uint32_t rows;  // block rows of the pass in rs.partials (its grid size)
   int trace;      // CB_LOOP_TRACE: fill LoopState::trace
 };
 
@@ -159,12 +157,10 @@ struct ChunkPair {
   float d2;  // the match's squared distance (correspondence value)
 };
 
-// Lanes per queued region in the wide search's pooled scan (warp_search_wide.cuh). The cold search keeps one lane per
+// Lanes per queued region in the wide search's pooled scan (warp_search_wide.cuh). The cold pass keeps one lane per
 // region. The cached pass's search uses pairs of lanes: its region scan then needs fewer live registers (DESIGN §4.2).
 constexpr unsigned int kColdGroup = 1, kWarmGroup = 2;
-// kCold: nothing cached yet (no warm seed, first-iteration slack). Otherwise the query failed the exclusion test:
-// its cached match seeds the search and its last motion sets the slack.
-template <bool kCold>
+// The query failed the exclusion test: its cached match seeds the search and its last motion sets the slack.
 __device__ __forceinline__ ChunkPair search_chunk_body(const LoopArgs& a, const BlockCtx& cx, WideSearchSmem* wsm,
                                                        bool act, uint32_t i) {
   ChunkPair cp;
@@ -177,17 +173,15 @@ __device__ __forceinline__ ChunkPair search_chunk_body(const LoopArgs& a, const 
   if (act) {
     const float4 s = __ldg(a.src_pts + cp.i);
     rule::transform_point(cx.T, s.x, s.y, s.z, cp.qx, cp.qy, cp.qz);
-    if (!kCold) {
-      float ox, oy, oz;
-      rule::transform_point(cx.Tp, s.x, s.y, s.z, ox, oy, oz);
-      const float ex = __fsub_rn(cp.qx, ox), ey = __fsub_rn(cp.qy, oy), ez = __fsub_rn(cp.qz, oz);
-      const float dl = __fsqrt_ru(__fmaf_ru(ez, ez, __fmaf_ru(ey, ey, __fmul_ru(ex, ex))));
-      // the next step is expected to be about half of this one, and a hit needs r - (motion) > d: widen by 2 x
-      slack = fminf(fmaxf(__fmul_rn(2.f, dl), a.slack_min), a.slack_max);
-      sd = a.cache_pos[cp.i];
-    }
+    float ox, oy, oz;
+    rule::transform_point(cx.Tp, s.x, s.y, s.z, ox, oy, oz);
+    const float ex = __fsub_rn(cp.qx, ox), ey = __fsub_rn(cp.qy, oy), ez = __fsub_rn(cp.qz, oz);
+    const float dl = __fsqrt_ru(__fmaf_ru(ez, ez, __fmaf_ru(ey, ey, __fmul_ru(ex, ex))));
+    // the next step is expected to be about half of this one, and a hit needs r - (motion) > d: widen by 2 x
+    slack = fminf(fmaxf(__fmul_rn(2.f, dl), a.slack_min), a.slack_max);
+    sd = a.cache_pos[cp.i];
   }
-  const WideBest wb = warp_grid_nearest_wide<kCold ? kColdGroup : kWarmGroup>(a.dst, *wsm, act, cp.qx, cp.qy, cp.qz, a.max_d2, sd, slack);
+  const WideBest wb = warp_grid_nearest_wide<kWarmGroup>(a.dst, *wsm, act, cp.qx, cp.qy, cp.qz, a.max_d2, sd, slack);
   if (act) {
     cp.pos = (wb.idx >= 0 && wb.d2 < a.max_d2) ? wb.pos : -1;
     cp.d2 = wb.d2;
@@ -446,7 +440,7 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
 #pragma unroll
     for (int v = 0; v < NV; v++) acc[v] = 0.0;
     const bool act = c + lane < flagged;
-    const ChunkPair cp = search_chunk_body<false>(a, cx, wsm, act, act ? list[c + lane] : 0u);
+    const ChunkPair cp = search_chunk_body(a, cx, wsm, act, act ? list[c + lane] : 0u);
     if (cp.pos >= 0) {
       const float4 dp = __ldg(a.dst.pts + cp.pos);
       accumulate_pair<MODE, true>(
@@ -464,24 +458,36 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
   if (block_row_from_slots<NV>(rsm, row) && lane < NV) a.rs.partials[(size_t)blockIdx.x * NV + lane] = row;
 }
 
-constexpr int kSearchMinBlocks = 4;  // resident blocks per SM the search kernel's register budget is set for
+// ---- kernel 1 of the cold iteration (the first of a call: nothing cached yet): every query searched -------------
+// PERSISTENT, like the cached pass: the grid is a whole number of resident blocks per SM, and each warp walks the
+// 32-query chunks of the cell-sorted source round-robin (warp w of the grid takes chunks w, w + W, ..., W = the grid's
+// warps), so the assignment and the summation order are fixed. Each chunk is one lane-dense wide search (kColdGroup
+// lanes per region); the searching lane updates the cache and accumulates its pair, and the warp folds its pairs into
+// its row of the block reduction after every chunk, so none of the accumulators is live across a search. The next
+// chunk's source points are loaded before the current chunk's search. The last warp of the block writes the block row
+// to rs.partials, which the finish kernel folds: a few hundred rows instead of one per 256 queries.
+// Register budget: p2p 64 registers, 4 blocks per SM. The combined metric's 28 accumulators spilled at 64 registers
+// (its 10 M cold iteration took 1.97 ms against 1.69 ms at 80 registers, 3 blocks per SM; DESIGN §4.2).
+__host__ __device__ constexpr int cold_min_blocks(bool combined) { return combined ? 3 : 4; }
 
-// ---- the cold iteration (the first of a call: nothing cached yet): search, then the finish kernel -----------------
-// Every query is searched, one 256-query chunk per block, lane-dense; the searching thread accumulates its pair and
-// the last warp of the grid hands this GPU's totals to icp_finish_kernel in rs.result. This kernel keeps the ticketed
-// grid reduction: its thousands of block rows (39 063 at 10 M queries) are folded group by group as its blocks finish,
-// spread over the SMs; one block folding them all after the grid took 138 us instead of 26 us at 10 M (DESIGN §4.2).
 template <int MODE>
-__global__ void __launch_bounds__(kBlock, kSearchMinBlocks) icp_search_kernel(const __grid_constant__ LoopArgs a) {
+__global__ void __launch_bounds__(kBlock, cold_min_blocks(MODE == kModeCombined))
+    icp_search_kernel(const __grid_constant__ LoopArgs a) {
   constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
   __shared__ BlockCtx cx;
   __shared__ WideSearchSmem wsm[kBlock / 32];
   __shared__ AsyncReduceSmem<NV> rsm;
-
   const unsigned int tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-  const uint32_t base = blockIdx.x * kBlock;
+  const uint32_t nchunks = (a.n_src + 31u) / 32u;
+  const uint32_t c0 = blockIdx.x * (kBlock / 32) + warp, stride = gridDim.x * (kBlock / 32);
+  auto load_src = [&](uint32_t chunk) {
+    const uint32_t i = chunk * 32u + lane;
+    return (chunk < nchunks && i < a.n_src) ? __ldg(a.src_pts + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+  };
+
   pdl_wait();               // the state of the previous finish kernel
   pdl_launch_dependents();  // the finish kernel may be scheduled now and wait for this grid to drain
+  float4 s_next = load_src(c0);
   if (tid == 0) {
     rsm.arrived = 0u;
     load_block_ctx(a, cx);
@@ -493,34 +499,46 @@ __global__ void __launch_bounds__(kBlock, kSearchMinBlocks) icp_search_kernel(co
     a.st->trace[trace_slot][0] = global_timer_ns();
     a.st->trace[trace_slot][4] = 0ull;
   }
-  const unsigned int total = (base < a.n_src) ? min((uint32_t)kBlock, a.n_src - base) : 0u;
-  if (tid == 0 && total > 0) {
-    atomicAdd(&a.st->searched_cur, (unsigned long long)total);
-    if (a.trace) atomicAdd(&a.st->trace[trace_slot][4], (unsigned long long)total);
-  }
-  double acc[NV];
+  if (lane < NV) rsm.slot[warp][lane] = 0.0;
+  unsigned int searched = 0;
+#pragma unroll 1
+  for (uint32_t chunk = c0; chunk < nchunks; chunk += stride) {
+    const uint32_t i = chunk * 32u + lane;
+    const bool act = i < a.n_src;
+    const float4 s = s_next;
+    s_next = load_src(chunk + stride);
+    float qx = 0.f, qy = 0.f, qz = 0.f;
+    if (act) rule::transform_point(cx.T, s.x, s.y, s.z, qx, qy, qz);
+    const WideBest wb = warp_grid_nearest_wide<kColdGroup>(a.dst, wsm[warp], act, qx, qy, qz, a.max_d2, -1, a.slack_first);
+    double acc[NV];
 #pragma unroll
-  for (int v = 0; v < NV; v++) acc[v] = 0.0;
-  if ((tid & ~31u) < total) {
-    const ChunkPair cp = search_chunk_body<true>(a, cx, &wsm[warp], tid < total, base + tid);
-    if (cp.pos >= 0) {
-      const float4 dp = __ldg(a.dst.pts + cp.pos);
-      accumulate_pair<MODE, true>(
-          acc, cx, a.has_pt != 0, a.has_pl != 0, dp, cp.qx, cp.qy, cp.qz, a.src_nrm != nullptr,
-          [&] { return __ldg(a.dst.nrm + cp.pos); }, [&] { return __ldg(a.src_nrm + cp.i); }, cp.d2);
+    for (int v = 0; v < NV; v++) acc[v] = 0.0;
+    if (act) {
+      const int pos = (wb.idx >= 0 && wb.d2 < a.max_d2) ? wb.pos : -1;
+      a.cache_pos[i] = pos;
+      a.cache_r[i] = rule::cache_radius(wb.D2);
+      if (pos >= 0) {
+        const float4 dp = __ldg(a.dst.pts + pos);
+        accumulate_pair<MODE, true>(
+            acc, cx, a.has_pt != 0, a.has_pl != 0, dp, qx, qy, qz, a.src_nrm != nullptr,
+            [&] { return __ldg(a.dst.nrm + pos); }, [&] { return __ldg(a.src_nrm + i); }, wb.d2);
+      }
     }
+    warp_sum_to_slot<NV, true>(acc, rsm);
+    searched += (uint32_t)__popc(__ballot_sync(0xffffffffu, act));
+  }
+  if (lane == 0 && searched > 0u) {
+    atomicAdd(&a.st->searched_cur, (unsigned long long)searched);
+    if (a.trace) atomicAdd(&a.st->trace[trace_slot][4], (unsigned long long)searched);
   }
   if (a.trace && lane == 0) atomicMax(&a.st->trace[trace_slot][5], global_timer_ns());
-  warp_sum_to_slot<NV, false>(acc, rsm);
-  double row, tot = 0;
-  if (!block_row_from_slots<NV>(rsm, row) || !grid_reduce_rows_tail<NV>(row, a.rs, lane, tot)) return;
-  if (lane < NV) a.rs.result[lane] = tot;
-  if (a.trace && lane == 0) a.st->trace[trace_slot][1] = global_timer_ns();
+  double row;
+  if (block_row_from_slots<NV>(rsm, row) && lane < NV) a.rs.partials[(size_t)blockIdx.x * NV + lane] = row;
 }
 
 // ---- kernel 2 of an iteration: fold + exchange + solve (one block) -----------------------------------------------------
-// The cached pass's block rows (a.rows of them) -> this GPU's totals (block_fold_rows: the whole block, in the fixed
-// order of the grid reduction; after the cold search kernel the totals are read from rs.result) -> all-reduce with the
+// The pass's block rows (a.rows of them) -> this GPU's totals (block_fold_rows: the whole block, in the fixed order of
+// the grid reduction) -> all-reduce with the
 // peer ranks over NVLink peer memory (reduce.cuh, bounded wait; every rank sums the rows in rank order ->
 // bit-identical totals) -> Kabsch / Gauss-Newton step, rotation(), compose, convergence test -> LoopState for the next
 // iteration's kernels. Everything after the fold runs in warp 0.
@@ -531,22 +549,18 @@ __global__ void __launch_bounds__(kBlock, 1) icp_finish_kernel(const __grid_cons
   __shared__ double sbuf[kCombinedValues + 8];
   static_assert(NV + 2 <= kExchangeVals, "row of the fused exchange");
   const unsigned int lane = threadIdx.x;
-  // griddepcontrol.wait returns once the whole grid before (cached pass or cold search kernel) has completed and its
+  // griddepcontrol.wait returns once the whole grid before (cached pass or cold pass) has completed and its
   // rows are visible; it also orders this kernel after the state of the previous iteration
   pdl_wait();
   pdl_launch_dependents();  // the next iteration's cached pass may start streaming
   if (threadIdx.x == 0) load_block_ctx(a, cx);
   __syncthreads();
   if (cx.done) return;
-  if (a.rows != 0) {
-    block_fold_rows<NV>(a.rs.partials, a.rows, sbuf);
-  } else if (threadIdx.x < NV) {
-    sbuf[threadIdx.x] = __ldcg(a.rs.result + threadIdx.x);
-  }
+  block_fold_rows<NV>(a.rs.partials, a.rows, sbuf);
   if (threadIdx.x >= 32) return;
   __syncwarp();
   const int trace_slot = a.trace ? (__ldcg(&a.st->iters) & 63) : 0;
-  if (a.trace && lane == 0 && a.rows != 0) a.st->trace[trace_slot][1] = global_timer_ns();
+  if (a.trace && lane == 0) a.st->trace[trace_slot][1] = global_timer_ns();
   // lanes < NV: the moments; lane NV: queries this rank searched in this iteration; lane NV + 1: its source points
   // (both ride along so that every rank sees the same global search share: the hand-over decision of the host)
   double tot = (lane < NV) ? sbuf[lane] : 0.0;
@@ -590,12 +604,12 @@ constexpr int kBridgeBatch = 2;  // enqueued behind the first batch: covers the 
 constexpr double kGiveUpShare = 0.15;
 
 // Enqueues the kernels of ICP iteration `it` of this call, with programmatic stream serialization (see pdl_wait
-// above): the search kernel in the cold first iteration (nothing cached yet), else the cached pass with its search of
-// the flagged queries; then the finish kernel.
+// above): the cold pass in the first iteration (nothing cached yet), else the cached pass with its search of the
+// flagged queries; then the finish kernel.
 template <int MODE>
 static int enqueue_iteration(cb_context* ctx, const LoopArgs& args, int it, int blocks_cold, int blocks_cached) {
   LoopArgs a = args;
-  a.rows = (uint32_t)(it == 0 ? 0 : blocks_cached);  // each block of the cached pass writes one row
+  a.rows = (uint32_t)(it == 0 ? blocks_cold : blocks_cached);  // each block of either pass writes one row
   if (it == 0)
     CB_TRY(launch_pdl(ctx, icp_search_kernel<MODE>, blocks_cold, kBlock, 0, a));
   else
@@ -649,14 +663,13 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   a.st = icp->d_state;
   static const bool trace = getenv("CB_LOOP_TRACE") != nullptr;
   a.trace = trace ? 1 : 0;
-  // cold iteration (first launch: nothing cached): search kernel, one 256-query chunk per block; warm iterations:
-  // the persistent cached pass (pipe_qpt x kBlock queries per tile), which also searches the queries it flags
-  const int blocks_cold = std::max(1, (int)((ns + kBlock - 1) / kBlock));
-  // once per device (function attributes belong to the device the context is on, not to the process): the pipeline's
-  // dynamic shared memory, the whole shared-memory carveout, and how many blocks
-  // of the cached pass are resident per SM
+  // cold iteration (first launch: nothing cached): the persistent cold pass (32-query chunks per warp); warm
+  // iterations: the persistent cached pass (pipe_qpt x kBlock queries per tile), which also searches the queries it flags
+  // once per device (function attributes belong to the device the context is on, not to the process): the pipelines'
+  // dynamic shared memory, the whole shared-memory carveout, and how many blocks of each pass are resident per SM
+  // ([0] / [1]: cached pass p2p / combined, [2] / [3]: cold pass)
   static bool attr_set_dev[64] = {};
-  static int resident_dev[64][2] = {};
+  static int resident_dev[64][4] = {};
   bool& attr_set = attr_set_dev[ctx->device & 63];
   int* resident = resident_dev[ctx->device & 63];
   if (!attr_set) {
@@ -672,13 +685,16 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
                                                           sizeof(PipeSmem<false>)));
     CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident[1], icp_cached_pipe_kernel<kModeCombined>, kBlock,
                                                           sizeof(PipeSmem<true>)));
+    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident[2], icp_search_kernel<kModeP2PCentered>, kBlock, 0));
+    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident[3], icp_search_kernel<kModeCombined>, kBlock, 0));
     attr_set = true;
   }
-  // persistent cached pass: a whole number of resident blocks per SM (never more blocks than tiles)
+  // persistent passes: a whole number of resident blocks per SM (never more blocks than tiles / chunks need)
   const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
   const int per_sm = std::max(1, resident[p2p ? 0 : 1]);
   const size_t tile = (size_t)pipe_qpt(!p2p) * kBlock;
   const int blocks_cached = grid_for(ctx, ns, tile, per_sm);
+  const int blocks_cold = grid_for(ctx, ns, kBlock, std::max(1, resident[p2p ? 2 : 3]));
   // the cached pass's flagged-query lists: per warp, room for every query of its block's tiles (about n_src in all)
   const size_t per_warp = ((ns + tile - 1) / tile + blocks_cached - 1) / blocks_cached * (tile / (kBlock / 32));
   const size_t flagged_need = per_warp * (size_t)blocks_cached * (kBlock / 32);
@@ -691,7 +707,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   }
   a.flagged = icp->d_loop_flagged;
   a.flagged_per_warp = (uint32_t)per_warp;
-  CB_TRY(get_reduce_scratch(ctx, blocks_cold, kMaxValues, &a.rs));
+  CB_TRY(get_reduce_scratch(ctx, std::max(blocks_cold, blocks_cached), kMaxValues, &a.rs));
   Exchange ex;
   std::memset(&ex, 0, sizeof(ex));
   const bool fused = ctx->world > 1 && arm_exchange(ctx, &ex);  // tables + timeout; the pass number lives in LoopState
