@@ -23,7 +23,7 @@
 // after its last tile, on dense warps. All bounds are rounded conservatively (directed rounding + 2^-18 relative
 // margins, far above the 6-ulp error of the fp32 distance evaluation); an exact tie can never pass the strict test.
 // As ICP converges the per-iteration motion shrinks geometrically and almost every query takes the cached path:
-// the iteration becomes one streaming pass (16 B query + 8 B cache + one 16 B gather per source point).
+// the iteration becomes one streaming pass (12 B query + 8 B cache + one 12 B gather per source point).
 #include "cache_rule.hpp"
 #include "icp_accumulate.cuh"
 #include "icp_kernels.cuh"
@@ -48,6 +48,11 @@ struct LoopArgs {
   GridView dst;
   const float4* src_pts;  // cell-sorted query cloud; .w = original index bits
   const float4* src_nrm;  // same order, or nullptr (symmetric metric when set)
+  // cached pass: packed xyz (12 B per point, same order) of src_pts (padded to whole 32-query windows), of dst.pts and
+  // of dst.nrm (nullptr unless the plane term is on): the bytes it streams and gathers, without the unread .w
+  const float* src_xyz;
+  const float* dst_xyz;
+  const float* dst_nxyz;
   uint32_t n_src;
   float max_d2, w_pt, w_pl, tol;
   int wk_pt, wk_pl;    // cb_weight_kind of the correspondence weight evaluators (combined metric)
@@ -218,11 +223,12 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
 }
 
 // ---- kernel 1 of a warm iteration: the cached pass and the search of what it could not decide ---------------------
-// Elementwise over the source cloud: per query 16 B (point) + 8 B (cache) streamed and one 16 B gather of the cached
-// match (+ 16 B normal for the plane term). Queries that pass the exclusion test accumulate their pair at once. The
-// others are searched by the warp that flagged them, after its last tile: after each 32-query slot the warp's ballot
-// appends the flagged query indices, in ascending order, to the warp's list in global memory (a.flagged); once the
-// warp's copies have drained it searches the list lane-dense, 32 at a time (search_chunk_body: same slack rule, warm
+// Elementwise over the source cloud: per query 12 B (point) + 8 B (cache) streamed and one 12 B gather of the cached
+// match (+ 12 B normal for the plane term), all from packed xyz copies (LoopArgs::src_xyz, dst_xyz, dst_nxyz): the
+// float4 arrays' .w holds index bits this pass never reads. Queries that pass the exclusion test accumulate their pair
+// at once. The others are searched by the warp that flagged them, after its last tile: after each 32-query slot the
+// warp's ballot appends the flagged query indices, in ascending order, to the warp's list in global memory
+// (a.flagged); once the warp's copies have drained it searches the list lane-dense, 32 at a time (search_chunk_body: same slack rule, warm
 // seed and cache update as the cold search), in its own pipeline buffers, and the searching lane adds its pair to the
 // warp's sums. Only __syncwarp is involved, so a searching warp holds up no other warp of its block. A converged
 // iteration flags a few dozen of 10^6 queries: the search gets no shared memory of its own and no call site inside the
@@ -236,16 +242,21 @@ __device__ __forceinline__ void load_block_ctx(const LoopArgs& a, BlockCtx& cx) 
 // slots occupied, long-scoreboard stalls on top - each thread can only keep the loads in flight that it has registers
 // for. Here every thread runs a private pipeline of cp.async copies into shared memory (LDGSTS: no destination
 // register, no scoreboard slot), kDepthA tiles of stage A and kDepthB of stage B:
-//   stage A (tile k+kDepthA-1)  the streamed arrays: its queries' point (16 B), exclusion radius (4 B), cached match (4 B)
+//   stage A (tile k+kDepthA-1)  the streamed arrays: the warp's 32 query points as one contiguous 384-byte window of
+//                               packed xyz (24 lanes x 16 B), then per lane the exclusion radius (4 B) and cached match
+//                               (4 B)
 //   stage B (tile k+kDepthB-1)  the gathers, once A has landed: the matched destination point (+ normal for the plane
-//                               term)
-//   stage C (tile k)            evaluation from shared memory
-// Each thread only ever reads what it copied itself, so cp.async.wait_group is all the synchronisation there is -
-// no block barrier inside the tile loop. The buffers are laid out warp by warp (WarpPipe), so a warp whose copies have
-// drained owns one contiguous region, and its search buffer (WideSearchSmem) lives there.
+//                               term), 3 x 4 B each
+//   stage C (tile k)            evaluation from shared memory; a lane reads its point at stride 3 floats (no bank
+//                               conflict)
+// Stage B reads only what its own lane copied in stage A. The query points are the one thing a lane reads from other
+// lanes' copies: so a __syncwarp follows each cp.async.wait_group before stage C, and another one after stage C keeps
+// the next step's stage A from overwriting a window a lane is still reading. There is no block barrier inside the tile
+// loop. The buffers are laid out warp by warp (WarpPipe), so a warp whose copies have drained owns one contiguous
+// region, and its search buffer (WideSearchSmem) lives there.
 //   p2p: 256-query tiles (one query per thread), stage A 4 deep and stage B 3 deep: each gather is issued two tiles
-//        ahead of its evaluation. 36 KB of pipeline, 4 blocks per SM (64 registers).
-//   combined: 512-query tiles, stage A 3 deep and stage B 2 deep: 68 KB of pipeline, 2 blocks per SM (128 registers).
+//        ahead of its evaluation. 29 KB of pipeline, 4 blocks per SM (64 registers).
+//   combined: 512-query tiles, stage A 3 deep and stage B 2 deep: 54 KB of pipeline, 2 blocks per SM (128 registers).
 //        At 3 blocks (80 registers, 256-query tiles) the exclusion test and the 28 accumulators spilled on every query.
 // (DESIGN §4.2 has the measured alternatives.)
 __host__ __device__ constexpr int pipe_qpt(bool normals) { return normals ? 2 : 1; }
@@ -257,9 +268,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void cp_async_16_cg(void* dst_smem, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src) : "memory");
 }
-__device__ __forceinline__ void cp_async_16_ca(void* dst_smem, const void* src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src) : "memory");
-}
 __device__ __forceinline__ void cp_async_4(void* dst_smem, const void* src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst_smem)), "l"(src) : "memory");
 }
@@ -269,16 +277,21 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// One warp's pipeline buffers: entry k * 32 + lane belongs to the warp's k-th query of a tile on that lane.
+// a query's cached exclusion radius and match, side by side: one 8-byte shared load
+struct alignas(8) RadiusSeed {
+  float r;
+  int seed;
+};
+// One warp's pipeline buffers: entry e = k * 32 + lane belongs to the warp's k-th query of a tile on that lane; the
+// packed xyz arrays hold its coordinates at 3 e, 3 e + 1, 3 e + 2 (src[.][k * 96 ...] is one 16-byte aligned window).
 template <bool kNormals>
-struct WarpPipe {
+struct alignas(16) WarpPipe {
   static constexpr int kA = pipe_depth_a(kNormals), kB = pipe_depth_b(kNormals);
   static constexpr int kW = pipe_qpt(kNormals) * 32;  // the warp's queries per tile
-  float4 src[kA][kW];
-  float r[kA][kW];
-  int seed[kA][kW];
-  float4 pt[kB][kW];
-  float4 nr[kNormals ? kB : 1][kNormals ? kW : 1];
+  float src[kA][3 * kW];
+  RadiusSeed rs[kA][kW];
+  float pt[kB][3 * kW];
+  float nr[kNormals ? kB : 1][kNormals ? 3 * kW : 1];
 };
 template <bool kNormals>
 struct PipeSmem {
@@ -309,11 +322,13 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
     if (tile < ntiles) {
 #pragma unroll
       for (int k = 0; k < kQpt; k++) {
-        const uint32_t i = tile * kTile + k * kBlock + tid;
+        // the warp's window: queries w0 .. w0 + 31 (src_xyz is padded to whole windows)
+        const uint32_t w0 = tile * kTile + k * kBlock + warp * 32u, i = w0 + lane;
+        if (w0 < a.n_src && lane < 24u)
+          cp_async_16_cg(&wp.src[buf][k * 96 + 4 * lane], a.src_xyz + (size_t)w0 * 3u + 4u * lane);
         if (i < a.n_src) {
-          cp_async_16_cg(&wp.src[buf][k * 32 + lane], a.src_pts + i);
-          cp_async_4(&wp.r[buf][k * 32 + lane], a.cache_r + i);
-          cp_async_4(&wp.seed[buf][k * 32 + lane], a.cache_pos + i);
+          cp_async_4(&wp.rs[buf][k * 32 + lane].r, a.cache_r + i);
+          cp_async_4(&wp.rs[buf][k * 32 + lane].seed, a.cache_pos + i);
         }
       }
     }
@@ -326,10 +341,17 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
       for (int k = 0; k < kQpt; k++) {
         const uint32_t e = k * 32 + lane, i = tile * kTile + k * kBlock + tid;
         if (i < a.n_src) {
-          const int sd = wp.seed[abuf][e];
-          if (sd >= 0 && wp.r[abuf][e] > 0.f) {
-            cp_async_16_ca(&wp.pt[bbuf][e], a.dst.pts + sd);
-            if (kNormals && want_nrm) cp_async_16_ca(&wp.nr[bbuf][e], a.dst.nrm + sd);
+          const RadiusSeed cs = wp.rs[abuf][e];
+          if (cs.seed >= 0 && cs.r > 0.f) {
+            const int sd = cs.seed;
+            const float* p = a.dst_xyz + (size_t)sd * 3u;
+#pragma unroll
+            for (int c = 0; c < 3; c++) cp_async_4(&wp.pt[bbuf][3 * e + c], p + c);
+            if (kNormals && want_nrm) {
+              const float* nv = a.dst_nxyz + (size_t)sd * 3u;
+#pragma unroll
+              for (int c = 0; c < 3; c++) cp_async_4(&wp.nr[kNormals ? bbuf : 0][3 * e + c], nv + c);
+            }
           }
         }
       }
@@ -395,6 +417,7 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
     cp_async_wait<2 * (kLeadA - kLeadB)>();
     stage_b(tile + kLeadB * stride, abuf_b, bbuf_prev);
     cp_async_wait<2 * kLeadB>();
+    __syncwarp();  // the other lanes' copies of this tile's query windows have landed too
     const uint32_t base = tile * kTile;
 #pragma unroll
     for (int k = 0; k < kQpt; k++) {
@@ -402,20 +425,24 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
       const bool active = i < a.n_src;
       bool miss = active;
       if (active) {
-        const float rc = wp.r[abuf][e];
-        const int sd = wp.seed[abuf][e];
+        const RadiusSeed cs = wp.rs[abuf][e];
+        const float rc = cs.r;
+        const int sd = cs.seed;
         if (rc > 0.f) {
-          const float4 sc = wp.src[abuf][e];
+          const float* sc = &wp.src[abuf][3 * e];
           // the exclusion test (cache_rule.hpp): hit -> the cached match is this iteration's exact search result
           rule::Verdict v;
           float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
-          rule::cached_match_test(cx.T, cx.Tp, sc.x, sc.y, sc.z, rc, sd, a.max_d2, [&] { return wp.pt[bbuf][e]; }, p, v);
+          rule::cached_match_test(
+              cx.T, cx.Tp, sc[0], sc[1], sc[2], rc, sd, a.max_d2,
+              [&] { return make_float4(wp.pt[bbuf][3 * e], wp.pt[bbuf][3 * e + 1], wp.pt[bbuf][3 * e + 2], 0.f); }, p, v);
           miss = v.miss;
           if (!miss) a.cache_r[i] = v.r2;
           if (v.pair) {
+            const float* nv = &wp.nr[kNormals ? bbuf : 0][kNormals ? 3 * e : 0];
             accumulate_pair<MODE, true>(
                 acc, cx, a.has_pt != 0, a.has_pl != 0, p, v.qx, v.qy, v.qz, a.src_nrm != nullptr,
-                [&] { return kNormals ? wp.nr[kNormals ? bbuf : 0][kNormals ? e : 0] : make_float4(0.f, 0.f, 0.f, 0.f); },
+                [&] { return kNormals ? make_float4(nv[0], nv[1], nv[2], 0.f) : make_float4(0.f, 0.f, 0.f, 0.f); },
                 [&] { return __ldg(a.src_nrm + i); }, v.d2);
           }
         }
@@ -425,6 +452,7 @@ __global__ void __launch_bounds__(kBlock, pipe_min_blocks(MODE == kModeCombined)
       if (miss) list[flagged + __popc(mm & ((1u << lane) - 1u))] = i;
       flagged += __popc(mm);
     }
+    __syncwarp();  // every lane has read this tile's windows before the next step's stage A reuses the buffer
     abuf = abuf_next;
     bbuf = bbuf_next;
   }
@@ -590,6 +618,21 @@ __global__ void __launch_bounds__(kBlock, 1) icp_finish_kernel(const __grid_cons
   if (lane == 0) loop_solve<MODE>(&a, &cx, sbuf, late ? 1 : 0, seq);
 }
 
+// The cached pass's packed copies: out[3 i .. 3 i + 2] = in[i].xyz for i < n, zeros for n <= i < n_out.
+__global__ void pack_xyz_kernel(const float4* __restrict__ in, size_t n, size_t n_out, float* __restrict__ out) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_out; i += (size_t)gridDim.x * blockDim.x) {
+    const float4 p = i < n ? __ldg(in + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+    out[3 * i] = p.x;
+    out[3 * i + 1] = p.y;
+    out[3 * i + 2] = p.z;
+  }
+}
+
+int pack_xyz(cb_context* ctx, DeviceScope& mem, const float4* in, size_t n, size_t n_out, float** out) {
+  CB_TRY(mem.alloc(out, 3 * std::max<size_t>(n_out, 1)));
+  return launch(ctx, pack_xyz_kernel, grid_for(ctx, n_out, kBlock), kBlock, 0, in, n, n_out, *out);
+}
+
 }  // namespace
 
 // widening of a search beyond the nearest distance, in cell edges of the destination grid: first iteration
@@ -656,6 +699,14 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   a.bail = (prm->w_pl > 0.f) && !dst_has_normals;
   a.cache_pos = icp->d_nn_pos;
   a.cache_r = icp->d_nn_d2;
+  // the cached pass's packed copies, once per ICP object (the clouds' index arrays do not change after they are built)
+  if (!icp->d_loop_src_xyz) CB_TRY(pack_xyz(ctx, icp->mem, icp->src->d_pts, ns, (ns + 31) / 32 * 32, &icp->d_loop_src_xyz));
+  if (!icp->d_loop_dst_xyz) CB_TRY(pack_xyz(ctx, icp->mem, icp->dst->d_pts, icp->dst->n, icp->dst->n, &icp->d_loop_dst_xyz));
+  if (a.has_pl && !icp->d_loop_dst_nxyz)
+    CB_TRY(pack_xyz(ctx, icp->mem, icp->dst->d_nrm, icp->dst->n, icp->dst->n, &icp->d_loop_dst_nxyz));
+  a.src_xyz = icp->d_loop_src_xyz;
+  a.dst_xyz = icp->d_loop_dst_xyz;
+  a.dst_nxyz = a.has_pl ? icp->d_loop_dst_nxyz : nullptr;
   const float h = 1.0f / a.dst.inv_h;  // cell edge of the destination grid
   a.slack_first = kSlackFirst * h;
   a.slack_min = kSlackMin * h;

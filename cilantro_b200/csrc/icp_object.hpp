@@ -62,6 +62,12 @@ struct cb_icp {
   cudaEvent_t batch_ev[2] = {nullptr, nullptr};  // end of a batch + its state copy
   uint32_t* d_loop_flagged = nullptr;  // the cached pass's per-warp lists of flagged queries (icp_loop.cu)
   size_t loop_flagged_cap = 0;         // in entries
+  // packed xyz copies the cached pass streams and gathers (icp_loop.cu, built by the first device-loop estimate()):
+  // src->d_pts padded with zeros to a whole number of 32-point windows, dst->d_pts, and dst->d_nrm once the plane term
+  // is on
+  float* d_loop_src_xyz = nullptr;
+  float* d_loop_dst_xyz = nullptr;
+  float* d_loop_dst_nxyz = nullptr;
   cb_cloud* src_full = nullptr;      // world > 1, engine modes: the whole source cloud replicated on this rank (owned)
   bool loop_last = false;            // the last estimate() ran on the device loop
   uint64_t searched_last = 0;        // queries its last iteration searched again (CB_LOOP_TRACE / cb_icp_loop_cache)
