@@ -225,7 +225,7 @@ EXPORTED = [
     "cb_knn1_radius", "cb_knn_radius", "cb_radius_search", "cb_find_correspondences",
     "cb_icp_default_params", "cb_icp_create", "cb_icp_destroy", "cb_icp_estimate", "cb_icp_iteration_times",
     "cb_icp_correspondences", "cb_icp_residuals", "cb_icp_accumulate", "cb_icp_loop_cache", "cb_icp_set_features",
-    "cb_solve_kabsch_moments", "cb_solve_gauss_newton", "cb_solve_rotation", "cb_compose",
+    "cb_solve_kabsch_moments", "cb_solve_gauss_newton", "cb_solve_rotation", "cb_compose", "cb_solve_sym_eigen",
     "cb_kmeans_cluster", "cb_kmeans_assign", "cb_kmeans_seed_indices",
     "cb_vectors_create", "cb_vectors_create_from_device", "cb_vectors_destroy", "cb_vectors_size",
     "cb_kmeans_cluster_vectors", "cb_kmeans_assign_vectors",
@@ -237,6 +237,7 @@ EXPORTED = [
     "cb_sparse_warp_icp_estimate", "cb_sparse_warp_icp_solve", "cb_sparse_warp_icp_resample",
     "cb_sparse_warp_icp_residuals", "cb_sparse_warp_icp_correspondences",
     "cb_mean_cov", "cb_pca", "cb_transform_points",
+    "cb_vectors_mean_cov", "cb_vectors_pca", "cb_vectors_project", "cb_vectors_reconstruct",
 ]
 
 _lib = None
@@ -557,6 +558,13 @@ class Vectors(_Handle):
         self.h = h
         self.n, self.D = int(n), int(D)
         ctx._adopt(self)
+
+    @classmethod
+    def _wrap(cls, ctx, handle, n, D):
+        self = cls.__new__(cls)
+        self.ctx, self.h, self.n, self.D = ctx, handle, int(n), int(D)
+        ctx._adopt(self)
+        return self
 
 
 def cloud_pair(ctx, xyz_a, normals_a, xyz_b, normals_b, offset_a=0, offset_b=0):
@@ -1068,17 +1076,77 @@ class SparseWarpIcp(_WarpIcpBase):
         return out[:n]
 
 
-def mean_cov(ctx, pts: Cloud):
-    mean = np.empty(3, np.float32)
-    cov = np.empty((3, 3), np.float32)
-    ok = _check(lib().cb_mean_cov(ctx.h, pts.h, _p(mean), _p(cov)))
+def _subset_args(subset):
+    """(pointer, count) of a subset index list for the cb_vectors_* covariance calls; (NULL, 0) for the whole set."""
+    if subset is None:
+        return None, 0, None
+    idx = np.ascontiguousarray(subset, np.uint64).reshape(-1)
+    keep = idx if idx.size else np.zeros(1, np.uint64)  # a valid pointer for an empty list
+    return _p(keep), idx.size, keep
+
+
+def mean_cov(ctx, pts, subset=None, min_sample_size=2):
+    """Mean and covariance of a Cloud (cb_mean_cov) or of a Vectors set, whole or the rows listed in subset
+    (cb_vectors_mean_cov): (mean [D], cov [D, D], ok)."""
+    if not isinstance(pts, Vectors):
+        mean = np.empty(3, np.float32)
+        cov = np.empty((3, 3), np.float32)
+        ok = _check(lib().cb_mean_cov(ctx.h, pts.h, _p(mean), _p(cov)))
+        return mean, cov, bool(ok)
+    D = pts.D
+    mean = np.empty(D, np.float32)
+    cov = np.empty((D, D), np.float32)
+    sp, m, _keep = _subset_args(subset)
+    ok = _check(lib().cb_vectors_mean_cov(ctx.h, pts.h, sp, C.c_size_t(m), C.c_size_t(min_sample_size), _p(mean),
+                                          _p(cov)))
     return mean, cov, bool(ok)
 
 
-def pca(ctx, pts: Cloud):
-    mean = np.empty(3, np.float32)
-    cov = np.empty((3, 3), np.float32)
-    ev = np.empty(3, np.float32)
-    evec = np.empty((3, 3), np.float32)
-    ok = _check(lib().cb_pca(ctx.h, pts.h, _p(mean), _p(cov), _p(ev), _p(evec)))
+def pca(ctx, pts, subset=None, min_sample_size=2):
+    """PCA of a Cloud (cb_pca) or of a Vectors set (cb_vectors_pca): dict(ok, mean, cov, eigenvalues descending,
+    eigenvectors [D, D] with the eigenvectors as columns)."""
+    D = pts.D if isinstance(pts, Vectors) else 3
+    mean = np.empty(D, np.float32)
+    cov = np.empty((D, D), np.float32)
+    ev = np.empty(D, np.float32)
+    evec = np.empty((D, D), np.float32)
+    if isinstance(pts, Vectors):
+        sp, m, _keep = _subset_args(subset)
+        ok = _check(lib().cb_vectors_pca(ctx.h, pts.h, sp, C.c_size_t(m), C.c_size_t(min_sample_size), _p(mean),
+                                         _p(cov), _p(ev), _p(evec)))
+    else:
+        ok = _check(lib().cb_pca(ctx.h, pts.h, _p(mean), _p(cov), _p(ev), _p(evec)))
     return {"ok": bool(ok), "mean": mean, "cov": cov, "eigenvalues": ev, "eigenvectors": evec}
+
+
+def _pca_map(ctx, entry, x, mean, evecs, D, k, dout, to_device):
+    mean = np.ascontiguousarray(mean, np.float32).reshape(D)
+    E = np.ascontiguousarray(evecs, np.float32).reshape(D, D)
+    out = None if to_device else np.empty((x.n, dout), np.float32)
+    h = C.c_void_p()
+    _check(getattr(lib(), entry)(ctx.h, x.h, _p(mean), _p(E), C.c_int(k), _p(out), C.byref(h) if to_device else None))
+    return Vectors._wrap(ctx, h, x.n, dout) if to_device else out
+
+
+def pca_project(ctx, vectors, mean, evecs, k, to_device=False):
+    """cb_vectors_project: the n x k projection of a Vectors set onto the first k columns of evecs, as an ndarray or
+    (to_device) a new Vectors set."""
+    return _pca_map(ctx, "cb_vectors_project", vectors, mean, evecs, vectors.D, int(k), int(k), to_device)
+
+
+def pca_reconstruct(ctx, q, mean, evecs, to_device=False):
+    """cb_vectors_reconstruct: n x D rows from the n x k projections q (a Vectors set), as an ndarray or a new
+    Vectors set."""
+    D = np.asarray(mean).size
+    return _pca_map(ctx, "cb_vectors_reconstruct", q, mean, evecs, D, D, D, to_device)
+
+
+def solve_sym_eigen(A):
+    """cb_solve_sym_eigen (host only): (eigenvalues descending [D], eigenvectors [D, D] as columns); all NaN for a
+    non-finite A, CbError when the iteration does not converge."""
+    A = np.ascontiguousarray(A, np.float64)
+    D = A.shape[0]
+    ev = np.empty(D, np.float32)
+    E = np.empty((D, D), np.float32)
+    _check(lib().cb_solve_sym_eigen(_p(A), C.c_int(D), _p(ev), _p(E)))
+    return ev, E

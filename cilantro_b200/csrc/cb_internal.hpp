@@ -196,6 +196,20 @@ int kmeans_features_assign(cb_context* ctx, const float* raw, size_t n, int D, c
 // Per-cluster sums stay in shared memory while K x (D + 1) doubles fit in this many bytes (both assignment kernels).
 constexpr size_t kKMeansSmemSumsBytes = 184 * 1024;
 
+// Covariance and PCA over D-dimensional rows (pca_features.cu), D != 3, n >= 2: mean (D) and covariance (D x D) of the
+// n rows at raw (device), under the contract of DESIGN §4.18. Synchronises the stream.
+int features_mean_cov(cb_context* ctx, const float* raw, size_t n, int D, float* mean, float* cov);
+// rows[i] = src[idx[i]], i < m, D floats each (device arrays; the indices are checked by the caller)
+int vectors_gather(cb_context* ctx, const float* raw, int D, const uint64_t* d_idx, size_t m, float* rows);
+// out (n x dout) of in (n x din) through the basis E (device, row-major D x D): the weight of input a and output b is
+// E[a * sa + b * sb]. project: the fold of (in_a - mean_a) (PCA projection); else the fold of in_a plus mean_b
+// (reconstruction). The fold orders are DESIGN §4.18's.
+int features_map(cb_context* ctx, const float* in, size_t n, int din, int dout, const float* d_E, int sa, int sb,
+                 const float* d_mean, bool project, float* out);
+// Symmetric eigen-decomposition in fp64 on the host (sym_eigen.cpp), cb_solve_sym_eigen's rules: 1 = solved, 0 = a
+// non-finite entry, -1 = no convergence (both with all-NaN output).
+int sym_eigen(const double* A, int D, float* evals, float* evecs);
+
 template <class T>
 int DeviceScope::alloc(T** p, size_t count) {
   *p = nullptr;

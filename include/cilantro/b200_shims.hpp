@@ -18,6 +18,7 @@
 //   VectorSet<float, D>, ConstVectorSetMatrixMap<float, D>  core/data_containers.hpp:73-112 (D != 3: k-means only)
 //   RigidTransformRANSACEstimator3f<>                       model_estimation/ransac_transform_estimator.hpp:9-122
 //   PrincipalComponentAnalysis3f                            core/principal_component_analysis.hpp:8-89
+//   (PrincipalComponentAnalysis<float, D>, Covariance<float, D>: core/principal_component_analysis.hpp, core/covariance.hpp)
 //   NormalEstimation3f                                      core/normal_estimation.hpp:11-421
 //   Points[Normals][Colors]GridDownsampler3f                core/grid_downsampler.hpp:8-340
 //   PointCloud3f (points / normals / colors, size, hasNormals, transform, gridDownsample[d], index subsets, remove,
@@ -1372,6 +1373,41 @@ struct VectorsHandle {
   VectorsHandle& operator=(const VectorsHandle&) = delete;
   ~VectorsHandle() { cb_vectors_destroy(h); }
 };
+
+// Dense R x C float matrices of the D-dimensional covariance and PCA (core/covariance.hpp,
+// core/principal_component_analysis.hpp): the reference's Eigen::Matrix<float, R, C> where Eigen is available, else a
+// small column-major stand-in with the members those classes use (rows, cols, resize, data, operator()).
+template <long R, long C>
+class DenseMatrixF {
+public:
+  DenseMatrixF() : rows_(R > 0 ? R : 0), cols_(C > 0 ? C : 0), d_(rows_ * cols_) {}
+  DenseMatrixF(size_t r, size_t c) : rows_(r), cols_(c), d_(r * c) {}
+  size_t rows() const { return rows_; }
+  size_t cols() const { return cols_; }
+  size_t size() const { return d_.size(); }
+  void resize(size_t r, size_t c) {
+    rows_ = r;
+    cols_ = c;
+    d_.resize(r * c);
+  }
+  float* data() { return d_.data(); }
+  const float* data() const { return d_.data(); }
+  float& operator()(size_t r, size_t c) { return d_[rows_ * c + r]; }
+  float operator()(size_t r, size_t c) const { return d_[rows_ * c + r]; }
+  float& operator[](size_t i) { return d_[i]; }
+  float operator[](size_t i) const { return d_[i]; }
+
+private:
+  size_t rows_, cols_;
+  std::vector<float> d_;
+};
+#ifdef CILANTRO_B200_HAS_EIGEN
+template <long R, long C>
+using DenseF = Eigen::Matrix<float, (int)R, (int)C>;
+#else
+template <long R, long C>
+using DenseF = DenseMatrixF<R, C>;
+#endif
 }  // namespace b200
 
 // KMeans<float, D, DistAdaptor> (clustering/kmeans.hpp:9-59,197-219) for any D, Eigen::Dynamic included: the

@@ -2,7 +2,10 @@
 // CovarianceT (core/covariance.hpp:15-371), 3-D float instances. They hold the method's settings; the computation runs
 // on the device inside NormalEstimation<float, 3, CovarianceT> (core/normal_estimation.hpp here).
 #pragma once
+#include <cstdint>
+#include <iterator>
 #include <type_traits>
+#include <vector>
 
 #include "../b200_shims.hpp"
 
@@ -11,21 +14,65 @@ namespace cilantro {
 template <typename ScalarT, ptrdiff_t EigenDim>
 class Covariance;
 
-// Covariance<float, 3> (:15-182): the plain mean and covariance of a neighbourhood; fewer than
-// getMinValidSampleSize() points give NaN.
-template <>
-class Covariance<float, 3> {
+// Covariance<float, D> (:15-182) for any D, Eigen::Dynamic included: the mean and (n - 1)-normalised covariance of a
+// vector set, whole or the listed columns, on the device (cb_vectors_mean_cov, DESIGN §4.18; at D = 3 the bits of
+// cb_mean_cov). Fewer than getMinValidSampleSize() points give NaN and false. NormalEstimation<float, 3, ...> takes
+// Covariance<float, 3> as the holder of that setting and runs its own per-neighbourhood kernel.
+template <ptrdiff_t EigenDim>
+class Covariance<float, EigenDim> {
 public:
   using Scalar = float;
-  enum { Dimension = 3 };
+  enum { Dimension = EigenDim };
+  using VectorType = b200::DenseF<EigenDim, 1>;
+  using MatrixType = b200::DenseF<EigenDim, EigenDim>;
+
   size_t getMinValidSampleSize() const { return min_sample_size_; }
   Covariance& setMinValidSampleSize(size_t min_size) {
     min_sample_size_ = min_size;
     return *this;
   }
 
+  // whole set (:30-80)
+  bool operator()(const ConstVectorSetMatrixMap<float, EigenDim>& points, VectorType& mean, MatrixType& cov,
+                  bool /*parallel*/ = false) const {
+    return run(points, nullptr, mean, cov);
+  }
+  // the columns [begin, end) lists (:83-172); duplicates count twice
+  template <typename IteratorT, typename = typename std::iterator_traits<IteratorT>::iterator_category>
+  bool operator()(const ConstVectorSetMatrixMap<float, EigenDim>& points, IteratorT begin, IteratorT end,
+                  VectorType& mean, MatrixType& cov, bool /*parallel*/ = false) const {
+    std::vector<uint64_t> idx;
+    for (IteratorT it = begin; it != end; ++it) idx.push_back((uint64_t)*it);
+    return run(points, &idx, mean, cov);
+  }
+  // a container of column indices (:174-179)
+  template <typename ContainerT, typename = decltype(std::declval<const ContainerT&>().begin())>
+  bool operator()(const ConstVectorSetMatrixMap<float, EigenDim>& points, const ContainerT& subset, VectorType& mean,
+                  MatrixType& cov, bool parallel = false) const {
+    return (*this)(points, subset.begin(), subset.end(), mean, cov, parallel);
+  }
+
 protected:
+  // subset nullptr: the whole set
+  bool run(const ConstVectorSetMatrixMap<float, EigenDim>& points, const std::vector<uint64_t>* subset,
+           VectorType& mean, MatrixType& cov) const {
+    const size_t D = points.rows();
+    b200::VectorsHandle v(points.data(), points.cols(), D);
+    mean.resize(D, 1);
+    cov.resize(D, D);
+    const uint64_t none = 0;  // a non-null pointer for an empty subset
+    const uint64_t* sp = subset ? (subset->empty() ? &none : subset->data()) : nullptr;
+    const int rc = cb_vectors_mean_cov(b200::Context::get(), v.h, sp, subset ? subset->size() : 0, min_sample_size_,
+                                       mean.data(), cov.data());  // cov is symmetric: either storage order
+    b200::check(rc, "cb_vectors_mean_cov");
+    return rc == 1;
+  }
   size_t min_sample_size_ = 2;
+};
+
+template <ptrdiff_t EigenDim>
+class Covariance<double, EigenDim> {
+  static_assert(EigenDim != EigenDim, "cilantro_b200 provides float Covariance only (no double instances)");
 };
 
 template <typename ScalarT, ptrdiff_t EigenDim, typename CovarianceT = Covariance<ScalarT, EigenDim>,

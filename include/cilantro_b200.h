@@ -414,6 +414,12 @@ int cb_icp_set_features(cb_icp* icp, int kind, const float* dst_normals, const f
 /* Host-only O(1) solves (no device needed; exported so the N>1 logic is testable on CPU). */
 /* estimateTransformPointToPointMetric from moments — transform_estimation.hpp:25-47. Returns 1 if n>=3. */
 int cb_solve_kabsch_moments(const double* sums16, float* T12);
+/* Symmetric eigen-decomposition of the D x D row-major A in fp64 (Householder + implicit symmetric QR), the solve of
+ * PrincipalComponentAnalysis::compute_ (principal_component_analysis.hpp:76-84): evals descending, evecs row-major with
+ * unit eigenvector columns, each signed so that its largest-magnitude component is positive (lowest index on ties),
+ * then the last column negated if det < 0. Returns 1; 0 for a non-finite A (all-NaN output); CB_ERR_UNSUPPORTED
+ * (all-NaN output) when the QR iteration does not converge, which cb_vectors_pca reports the same way. */
+int cb_solve_sym_eigen(const double* A, int D, float* evals, float* evecs);
 /* One Gauss-Newton update of estimateTransformCombinedMetric — :346-357: T_out = Ra ta Ra T_in. */
 int cb_solve_gauss_newton(const double* sums28, const float* T_in12, float* T_out12, float* dtheta_norm);
 /* LinearTransform::rotation() — core/space_transformations.hpp:43-51 (3x3 row-major in/out). */
@@ -697,6 +703,32 @@ int cb_sparse_warp_icp_correspondences(cb_sparse_warp_icp* icp, uint64_t* index_
  * else fills NaN and returns 0 (covariance.hpp:35-38). */
 int cb_mean_cov(cb_context* ctx, const cb_cloud* pts, float* mean3, float* cov9);
 int cb_pca(cb_context* ctx, const cb_cloud* pts, float* mean3, float* cov9, float* evals3, float* evecs9);
+
+/* ---- covariance / PCA over D-dimensional vector sets -------------------------------------------
+ * Covariance<float, D>::operator()(points, mean, cov) and its subset / iterator overloads (core/covariance.hpp:30-179)
+ * for any D: subset NULL = every row, else the m listed rows (duplicates count twice; an index >= n is
+ * CB_ERR_INVALID). mean D floats, cov D x D row-major. fp64 accumulation about a pivot (DESIGN §4.18); at D = 3 the
+ * bits of cb_mean_cov. A non-finite value in dimension j makes row and column j of cov NaN. Fewer than
+ * min_sample_size rows: NaN mean and cov, returns 0. Otherwise returns 1; n = 1 gives mean = the row and a NaN cov,
+ * n = 0 a NaN mean and cov = -0 (whole set) or +0 (subset), the reference's expressions. One GPU: a context with
+ * several ranks returns CB_ERR_UNSUPPORTED. */
+int cb_vectors_mean_cov(cb_context* ctx, const cb_vectors* v, const uint64_t* subset, size_t m,
+                        size_t min_sample_size, float* mean, float* cov);
+/* PrincipalComponentAnalysis<float, D> constructors (core/principal_component_analysis.hpp:17-31,76-84): the above,
+ * then the eigen-decomposition of the fp32 covariance (cb_solve_sym_eigen; at D = 3 cb_pca's). evals D descending,
+ * evecs D x D row-major with the eigenvectors as columns. Returns as cb_vectors_mean_cov (0: all NaN). */
+int cb_vectors_pca(cb_context* ctx, const cb_vectors* v, const uint64_t* subset, size_t m, size_t min_sample_size,
+                   float* mean, float* cov, float* evals, float* evecs);
+/* PrincipalComponentAnalysis::project(points, k) / project<k> (principal_component_analysis.hpp:46-57) with
+ * cb_vectors_pca's mean and evecs (first k columns), 1 <= k <= D: out_j = fold over d = 0 .. D-1 of
+ * acc = acc + E[d][j] * (p_d - mean_d) from acc = 0, fp32 without FMA. n x k rows to out_host and / or a new vector
+ * set *out_device (either may be NULL, not both). */
+int cb_vectors_project(cb_context* ctx, const cb_vectors* v, const float* mean, const float* evecs, int k,
+                       float* out_host, cb_vectors** out_device);
+/* reconstruct(points) / reconstruct<k> (principal_component_analysis.hpp:59-68) of q (n x k, 1 <= k <= D) into D
+ * dimensions: out_r = (fold over j = 0 .. k-1 of acc = acc + E[r][j] * q_j from acc = 0) + mean_r, fp32 without FMA. */
+int cb_vectors_reconstruct(cb_context* ctx, const cb_vectors* q, const float* mean, const float* evecs, int D,
+                           float* out_host, cb_vectors** out_device);
 
 /* transformPoints(tform, in, out) — core/space_transformations.hpp:203-216 (host in, host out). */
 int cb_transform_points(cb_context* ctx, const float* T12, const float* xyz, size_t n, float* out);

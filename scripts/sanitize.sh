@@ -5,7 +5,7 @@
 # memcheck: out-of-bounds / misaligned global, shared and local accesses, leaks of device allocations.
 # racecheck: shared-memory hazards between threads of a block (the warp-pooled search queues, the per-warp
 #            neighbourhood staging of the robust normals, the barrier-free block reduction, the D-dimensional
-#            k-means tiles staged between two barriers).
+#            k-means tiles and the covariance / projection tiles staged between two barriers).
 # synccheck: divergent / invalid use of __syncthreads / __syncwarp / *_sync shuffles.
 set -u
 cd "$(dirname "$0")/.."

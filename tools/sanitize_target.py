@@ -14,6 +14,7 @@ from cilantro_b200 import capi, synth  # noqa: E402
 
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import kmeans_features_ref  # noqa: E402
+import pca_features_ref  # noqa: E402
 
 N = int(os.environ.get("SANITIZE_N", "6000"))
 
@@ -104,6 +105,18 @@ def main():
     c_rd, c_rs = capi.Cloud(ctx, rd), capi.Cloud(ctx, rs)
     capi.ransac_rigid(ctx, c_rd, c_rs, seed=5, max_iter=64, thresh=0.01)
     capi.pca(ctx, capi.Cloud(ctx, pts))
+    # D-dimensional covariance / PCA: every column-tile width, partial chunks and tiles, a subset gather, a NaN value;
+    # projection and reconstruction with partial row and output tiles
+    for D, n in ((6, 1001), (13, 777), (31, 300), (70, 515)):
+        rows = rng.standard_normal((n, D)).astype(np.float32)
+        rows[5, D - 1] = np.nan
+        v = capi.Vectors(ctx, rows)
+        capi.pca(ctx, v, subset=np.arange(n)[::3])
+        r = capi.pca(ctx, v)
+        q = capi.pca_project(ctx, v, r["mean"], r["eigenvectors"], D // 2 + 1, to_device=True)
+        capi.pca_reconstruct(ctx, q, r["mean"], r["eigenvectors"])
+        np.testing.assert_array_equal(capi.pca_project(ctx, v, r["mean"], r["eigenvectors"], D),
+                                      pca_features_ref.project(rows, r["mean"], r["eigenvectors"], D))
     # plane RANSAC: early exit with re-estimation, a full run of growing batches, tiny clouds, a NaN row
     ps = synth.plane_scene(N, seed=3)["points"]
     ps[7] = np.nan
