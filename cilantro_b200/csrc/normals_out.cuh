@@ -21,9 +21,9 @@ struct NormalOut {
 __device__ __forceinline__ void finish_point(const NormalOut& o, uint32_t qi, int oi, float px, float py, float pz,
                                              bool valid, const float (&cv)[6]) {
   const float nan = __int_as_float(0x7fc00000);
-  float w[3] = {nan, nan, nan}, nv[3] = {nan, nan, nan};
+  float w[3], nv[3] = {nan, nan, nan}, curv = nan;
   if (valid) {
-    sym3_smallest(cv, w, nv);
+    sym3_smallest(cv, w, nv, curv);
     if (o.use_ref) {
       // eigenvectors().col(0).dot(ref_normals.col(i)) < 0 -> flip (normal_estimation.hpp:351-355)
       const float4 r = o.nrm[qi];
@@ -48,7 +48,7 @@ __device__ __forceinline__ void finish_point(const NormalOut& o, uint32_t qi, in
   o.raw_nrm[3 * (size_t)oi] = nv[0];
   o.raw_nrm[3 * (size_t)oi + 1] = nv[1];
   o.raw_nrm[3 * (size_t)oi + 2] = nv[2];
-  if (o.curvature) o.curvature[oi] = valid ? w[0] / (w[0] + w[1] + w[2]) : nan;  // :389
+  if (o.curvature) o.curvature[oi] = curv;  // :389
   if (o.cov6) {
 #pragma unroll
     for (int c = 0; c < 6; c++) o.cov6[6 * (size_t)oi + c] = valid ? cv[c] : nan;

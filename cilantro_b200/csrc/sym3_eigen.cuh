@@ -27,19 +27,37 @@ __device__ __forceinline__ void jacobi_rotate(float& app, float& aqq, float& apq
   a = c * v2p - s * v2q; b = s * v2p + c * v2q; v2p = a; v2q = b;
 }
 
-__device__ __forceinline__ void sym3_smallest(const float (&cv)[6], float (&w)[3], float (&n)[3]) {
+// The smallest eigenpair and the curvature w0 / (w0 + w1 + w2) (normal_estimation.hpp:389) of cv.
+// Below a largest |entry| of 2^-126 every entry is subnormal or zero: 1 / scale overflows to +inf below 2^-128, and
+// the eigenvalues would be subnormal. Such a matrix is multiplied by 2^64 first (exact), solved as any other, and
+// only its eigenvalues are multiplied back by 2^-64. The curvature is taken before that step, so it keeps all its
+// bits: an exact power-of-two scaling of a normal-range matrix gets that matrix's normal and curvature bit for bit.
+// A NaN or infinite entry makes every output NaN (an infinite entry: as Eigen's solver, which divides by the
+// infinite scale); the zero matrix gives n = e_x, w = 0 and curv = NaN (0 / 0).
+__device__ __forceinline__ void sym3_smallest(const float (&cv)[6], float (&w)[3], float (&n)[3], float& curv) {
+  bool finite = true;
+#pragma unroll
+  for (int c = 0; c < 6; c++) finite = finite && fabsf(cv[c]) <= 3.402823466e38f;
+  if (!finite) {
+    w[0] = w[1] = w[2] = n[0] = n[1] = n[2] = curv = __int_as_float(0x7fc00000);
+    return;
+  }
   float scale = fmaxf(fmaxf(fabsf(cv[0]), fabsf(cv[1])), fmaxf(fabsf(cv[2]), fabsf(cv[3])));
   scale = fmaxf(scale, fmaxf(fabsf(cv[4]), fabsf(cv[5])));
-  if (!(scale > 0.f)) {  // zero matrix: eigenvectors = identity (and NaN input falls through as NaN below)
+  if (!(scale > 0.f)) {  // zero matrix: eigenvectors = identity
     w[0] = w[1] = w[2] = scale;
     n[0] = 1.f;
     n[1] = 0.f;
     n[2] = 0.f;
+    curv = w[0] / (w[0] + w[1] + w[2]);
     return;
   }
+  const bool tiny = scale < 0x1p-126f;
+  const float up = tiny ? 0x1p64f : 1.f;
+  scale *= up;
   const float inv = 1.f / scale;
-  float a00 = cv[0] * inv, a01 = cv[1] * inv, a02 = cv[2] * inv, a11 = cv[3] * inv, a12 = cv[4] * inv,
-        a22 = cv[5] * inv;
+  float a00 = cv[0] * up * inv, a01 = cv[1] * up * inv, a02 = cv[2] * up * inv, a11 = cv[3] * up * inv,
+        a12 = cv[4] * up * inv, a22 = cv[5] * up * inv;
   float v00 = 1.f, v01 = 0.f, v02 = 0.f, v10 = 0.f, v11 = 1.f, v12 = 0.f, v20 = 0.f, v21 = 0.f, v22 = 1.f;
 #pragma unroll 1
   for (int sweep = 0; sweep < 8; ++sweep) {
@@ -60,10 +78,24 @@ __device__ __forceinline__ void sym3_smallest(const float (&cv)[6], float (&w)[3
   w[0] = lo * scale;
   w[1] = mid * scale;
   w[2] = hi * scale;
+  // (w0 + w1) + w2 with one rounding per operation: left to FMA contraction, the sum would round differently in
+  // each caller's inlined copy
+  curv = w[0] / __fadd_rn(__fadd_rn(w[0], w[1]), w[2]);
+  if (tiny) {
+    w[0] *= 0x1p-64f;
+    w[1] *= 0x1p-64f;
+    w[2] *= 0x1p-64f;
+  }
   const float rn = rsqrtf(nx * nx + ny * ny + nz * nz);
   n[0] = nx * rn;
   n[1] = ny * rn;
   n[2] = nz * rn;
+}
+
+// The smallest eigenpair alone (w and n as above).
+__device__ __forceinline__ void sym3_smallest(const float (&cv)[6], float (&w)[3], float (&n)[3]) {
+  float curv;
+  sym3_smallest(cv, w, n, curv);
 }
 
 }  // namespace cb

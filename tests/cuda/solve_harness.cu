@@ -81,15 +81,15 @@ __global__ void solve6_kernel(const double* in, double* out, int n) {
 __global__ void sym3_kernel(const float* in, float* out, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  float cv[6], w[3], nv[3];
+  float cv[6], w[3], nv[3], curv;
   for (int k = 0; k < 6; k++) cv[k] = in[6 * (size_t)i + k];
-  cb::sym3_smallest(cv, w, nv);
+  cb::sym3_smallest(cv, w, nv, curv);
   float* o = out + 7 * (size_t)i;
   for (int k = 0; k < 3; k++) {
     o[k] = w[k];
     o[3 + k] = nv[k];
   }
-  o[6] = w[0] / (w[0] + w[1] + w[2]);  // normals.cu finish_point
+  o[6] = curv;
 }
 
 #define CHECK(call)                                                                 \

@@ -14,6 +14,7 @@ import pytest
 
 from cilantro_b200 import synth
 from conftest import frob
+from normals_ref import check_eigen, fmt
 
 pytestmark = pytest.mark.gpu
 
@@ -83,10 +84,15 @@ def _check(cb, ctx, orc, ref_pts, qry_pts, T=None, max_d2=FMAX, ks=(1, 16), r2=N
     return out
 
 
-def _check_normals_k(cb, ctx, orc, pts, k):
+def _check_normals_k(cb, ctx, orc, pts, k, eigen=False):
+    """Covariances bit for bit against the oracle; eigen: also every normal and curvature against float64 eigh of
+    its own covariance (normals_ref.check_eigen)."""
     got = cb.Cloud(ctx, pts).estimate_normals(k=k, view_point=[0.5, 0.5, 10.0], want_cov=True)
     want = orc.estimate_normals(pts, orc.BruteKnn(pts), k=k, view_point=[0.5, 0.5, 10.0])
     assert np.array_equal(_bits(got["cov6"]), _bits(want[2])), f"normals k={k}: covariances differ bitwise"
+    if eigen:
+        worst = check_eigen(got["cov6"], got["normals"], got["curvature"], f"normals k={k}")
+        print(f"[grid-edges] normals k={k} vs float64: {fmt(worst)}")
     return got
 
 
@@ -127,8 +133,11 @@ def test_power_of_two_scale_sweep(cb, ctx, orc):
         bnd = _check(cb, ctx, orc, ref, qry, T=T, max_d2=bound, ks=(), corr_d2=bound, ref=cl)
         ks = _check(cb, ctx, orc, ref, qry[sub], T=T, max_d2=FMAX, ks=K_BOUNDARIES, ref=cl,
                     r2=F32(min(0.02**2 * 4.0**e, FMAX)))
-        if e in (-40, 0, 40):
-            _check_normals_k(cb, ctx, orc, ref, 16)
+        if e in (-60, -40, 0, 40):  # at 2^-60 the covariances are ~1e-40: subnormal
+            nrm = _check_normals_k(cb, ctx, orc, ref, 16, eigen=True)
+            if e == -60:
+                big = np.abs(nrm["cov6"]).max(axis=1)
+                assert ((big > 0) & (big < FMIN)).any()
         if e == 0:
             base = dict(edge=info["cell_edge"], dims=info["dims"], out=out, bnd=bnd, ks=ks)
         elif -40 <= e <= 60:
