@@ -238,6 +238,7 @@ EXPORTED = [
     "cb_sparse_warp_icp_residuals", "cb_sparse_warp_icp_correspondences",
     "cb_mean_cov", "cb_pca", "cb_transform_points",
     "cb_vectors_mean_cov", "cb_vectors_pca", "cb_vectors_project", "cb_vectors_reconstruct",
+    "cb_vectors_mds",
 ]
 
 _lib = None
@@ -1150,3 +1151,38 @@ def solve_sym_eigen(A):
     E = np.empty((D, D), np.float32)
     _check(lib().cb_solve_sym_eigen(_p(A), C.c_int(D), _p(ev), _p(E)))
     return ev, E
+
+
+def mds_nev(n, max_dim, estimate_dim):
+    """The number of eigenpairs cb_vectors_mds computes: min(max_dim + 1, n - 1) with estimation, else max_dim."""
+    return min(max_dim + 1, n - 1) if estimate_dim else max_dim
+
+
+def mds(ctx, distances, max_dim, estimate_dim=False, squared=True, to_device=False):
+    """cb_vectors_mds: classical multidimensional scaling of an [n, n] distance matrix (an array or a Vectors set with
+    D = n). Returns dict(ok, eigenvalues [nev], dim, embedding): the embedding as an [n, dim] array or, to_device, a
+    new Vectors set."""
+    if isinstance(distances, Vectors):
+        dist, own = distances, None
+    else:
+        a = np.ascontiguousarray(distances, np.float32)
+        if a.ndim != 2:
+            raise ValueError("distances must be an [n, n] array")
+        dist = own = Vectors(ctx, a)
+    try:
+        n = dist.n
+        max_dim = int(max_dim)
+        ev = np.empty(max(1, mds_nev(n, max_dim, estimate_dim)), np.float32)
+        emb = None if to_device else np.empty(max(1, n * max_dim), np.float32)
+        nev = C.c_size_t()
+        dim = C.c_size_t()
+        h = C.c_void_p()
+        ok = _check(lib().cb_vectors_mds(ctx.h, dist.h, C.c_size_t(max_dim), C.c_int(int(bool(estimate_dim))),
+                                         C.c_int(int(bool(squared))), _p(ev), C.byref(nev), C.byref(dim),
+                                         None if to_device else _p(emb), C.byref(h) if to_device else None))
+    finally:
+        if own is not None:
+            own.close()
+    d = dim.value
+    out = Vectors._wrap(ctx, h, n, d) if to_device else emb[:n * d].reshape(n, d)
+    return {"ok": bool(ok), "eigenvalues": ev[:nev.value].copy(), "dim": d, "embedding": out}

@@ -209,6 +209,9 @@ int features_map(cb_context* ctx, const float* in, size_t n, int din, int dout, 
 // Symmetric eigen-decomposition in fp64 on the host (sym_eigen.cpp), cb_solve_sym_eigen's rules: 1 = solved, 0 = a
 // non-finite entry, -1 = no convergence (both with all-NaN output).
 int sym_eigen(const double* A, int D, float* evals, float* evecs);
+// The same solve with fp64 output and no sign rules: evals descending, the eigenvectors as unit columns of evecs
+// (row-major D x D). Multidimensional scaling (mds.cu) runs it on its projected matrices.
+int sym_eigen_f64(const double* A, int D, double* evals, double* evecs);
 
 template <class T>
 int DeviceScope::alloc(T** p, size_t count) {

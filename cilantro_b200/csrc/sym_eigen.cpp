@@ -164,10 +164,9 @@ int det_sign(std::vector<double>& M, int n) {
 
 namespace cb {
 
-// Eigenvalues descending; eigenvectors as unit columns of evecs (row-major D x D), each signed so that its
-// largest-magnitude component is positive (the lowest index on ties), then the last column negated when det < 0.
+// Eigenvalues descending, eigenvectors as unit columns of evecs (row-major D x D), all fp64 and without the sign rules.
 // Returns 1; 0 for a non-finite entry and -1 when the QR iteration did not converge, both with all-NaN output.
-int sym_eigen(const double* A, int D, float* evals, float* evecs) {
+int sym_eigen_f64(const double* A, int D, double* evals, double* evecs) {
   const size_t DD = (size_t)D * D;
   double amax = 0.0;
   bool finite = true;
@@ -175,7 +174,7 @@ int sym_eigen(const double* A, int D, float* evals, float* evecs) {
     finite = finite && std::isfinite(A[i]);
     amax = std::max(amax, std::fabs(A[i]));
   }
-  const float nan = std::numeric_limits<float>::quiet_NaN();
+  const double nan = std::numeric_limits<double>::quiet_NaN();
   auto fail = [&](int rc) {
     std::fill(evals, evals + D, nan);
     std::fill(evecs, evecs + DD, nan);
@@ -195,19 +194,36 @@ int sym_eigen(const double* A, int D, float* evals, float* evecs) {
   std::vector<int> order((size_t)D);
   std::iota(order.begin(), order.end(), 0);
   std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return d[x] > d[y]; });
-  std::vector<double> E(DD);
   for (int j = 0; j < D; j++) {
     const double* v = &zt[(size_t)order[j] * D];
+    for (int i = 0; i < D; i++) evecs[(size_t)i * D + j] = v[i];
+    evals[j] = d[order[j]] * scale;
+  }
+  return 1;
+}
+
+// sym_eigen_f64, then each eigenvector signed so that its largest-magnitude component is positive (the lowest index on
+// ties), the last column negated when det < 0, and everything rounded to fp32.
+int sym_eigen(const double* A, int D, float* evals, float* evecs) {
+  const size_t DD = (size_t)D * D;
+  std::vector<double> d((size_t)D), E(DD);
+  const int rc = sym_eigen_f64(A, D, d.data(), E.data());
+  if (rc != 1) {
+    std::fill(evals, evals + D, std::numeric_limits<float>::quiet_NaN());
+    std::fill(evecs, evecs + DD, std::numeric_limits<float>::quiet_NaN());
+    return rc;
+  }
+  for (int j = 0; j < D; j++) {
     int big = 0;
     for (int i = 1; i < D; i++)
-      if (std::fabs(v[i]) > std::fabs(v[big])) big = i;
-    const double sgn = v[big] < 0.0 ? -1.0 : 1.0;
-    for (int i = 0; i < D; i++) E[(size_t)i * D + j] = sgn * v[i];
+      if (std::fabs(E[(size_t)i * D + j]) > std::fabs(E[(size_t)big * D + j])) big = i;
+    if (E[(size_t)big * D + j] < 0.0)
+      for (int i = 0; i < D; i++) E[(size_t)i * D + j] = -E[(size_t)i * D + j];
   }
   std::vector<double> M(E);
   if (det_sign(M, D) < 0)
     for (int i = 0; i < D; i++) E[(size_t)i * D + D - 1] = -E[(size_t)i * D + D - 1];
-  for (int j = 0; j < D; j++) evals[j] = (float)(d[order[j]] * scale);
+  for (int j = 0; j < D; j++) evals[j] = (float)d[j];
   for (size_t i = 0; i < DD; i++) evecs[i] = (float)E[i];
   return 1;
 }

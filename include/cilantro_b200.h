@@ -730,6 +730,24 @@ int cb_vectors_project(cb_context* ctx, const cb_vectors* v, const float* mean, 
 int cb_vectors_reconstruct(cb_context* ctx, const cb_vectors* q, const float* mean, const float* evecs, int D,
                            float* out_host, cb_vectors** out_device);
 
+/* ---- multidimensional scaling ------------------------------------------------------------------
+ * computeDistancePreservingSpectralEmbedding / MultidimensionalScaling<float, D>
+ * (utilities/multidimensional_scaling.hpp:35-83, 86-121) on an n x n fp32 distance matrix held as a cb_vectors with
+ * D = n (row i = row i of the matrix). Entries are squared once in fp32 unless distances_are_squared. B is the symmetric
+ * matrix whose entries for i >= j are -1/2 (E_ij - r_i - c_j + g) (row means r, column means c, grand mean g, fp64): the
+ * lower triangle of -1/2 J E J, the triangle the reference's eigen-solver reads. nev = estimate_dim ?
+ * min(max_dim + 1, n - 1) : max_dim eigenpairs of largest |lambda| (descending |lambda|, the positive value first at
+ * equal magnitude) are found with fp64 products on the device; then negative eigenvalues are clamped to 0, the dimension
+ * is max_dim or, with estimate_dim, estimateEmbeddingDimensionEigengap (:9-31) of the clamped values, and each
+ * eigenvector is signed so that its largest-magnitude component is positive (lowest index on ties).
+ * eigenvalues: nev floats (*nev is set); *dim is set; the embedding diag(sqrt(lambda)) V^T, dim x n in the reference, is
+ * written as n x dim rows to embedded_host (n x max_dim floats of room) and / or a new vector set *embedded_device
+ * (either may be NULL). nev outside [1, n - 1], estimate_dim with max_dim >= n, or a non-square set (D != n) is
+ * CB_ERR_INVALID; a context with several ranks is CB_ERR_UNSUPPORTED. A non-finite (squared) entry returns 0 with NaN
+ * outputs (dim as without estimation); no convergence within the restart cap returns CB_ERR_UNSUPPORTED. Returns 1. */
+int cb_vectors_mds(cb_context* ctx, const cb_vectors* dist, size_t max_dim, int estimate_dim, int distances_are_squared,
+                   float* eigenvalues, size_t* nev, size_t* dim, float* embedded_host, cb_vectors** embedded_device);
+
 /* transformPoints(tform, in, out) — core/space_transformations.hpp:203-216 (host in, host out). */
 int cb_transform_points(cb_context* ctx, const float* T12, const float* xyz, size_t n, float* out);
 
