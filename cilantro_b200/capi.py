@@ -239,6 +239,7 @@ EXPORTED = [
     "cb_mean_cov", "cb_pca", "cb_transform_points",
     "cb_vectors_mean_cov", "cb_vectors_pca", "cb_vectors_project", "cb_vectors_reconstruct",
     "cb_vectors_mds",
+    "cb_depth_image_to_points", "cb_points_to_depth_image", "cb_points_to_index_map",
 ]
 
 _lib = None
@@ -1186,3 +1187,115 @@ def mds(ctx, distances, max_dim, estimate_dim=False, squared=True, to_device=Fal
     d = dim.value
     out = Vectors._wrap(ctx, h, n, d) if to_device else emb[:n * d].reshape(n, d)
     return {"ok": bool(ok), "eigenvalues": ev[:nev.value].copy(), "dim": d, "embedding": out}
+
+
+class DepthConverter(C.Structure):
+    """cb_depth_converter: DepthValueConverter<RawDepth, float>(scale) or, with max_depth, TruncatedDepthValueConverter
+    (scale, max_depth); RawDepth is np.uint16 or np.float32."""
+
+    _fields_ = [("raw_type", C.c_int32), ("truncated", C.c_int32), ("scale", C.c_float), ("max_depth", C.c_float)]
+
+    def __init__(self, dtype=np.uint16, scale=1.0, max_depth=None):
+        dt = np.dtype(dtype)
+        if dt not in (np.dtype(np.uint16), np.dtype(np.float32)):
+            raise ValueError(f"raw depth must be uint16 or float32, not {dt}")
+        super().__init__(0 if dt == np.uint16 else 1, int(max_depth is not None), float(scale),
+                         float(max_depth) if max_depth is not None else 0.0)
+        self.dtype = dt
+
+
+def _image_arg(img, dtype, shape):
+    """(pointer, keep-alive) of an image given as a host array or a CUDA array (__cuda_array_interface__, e.g. a torch
+    CUDA tensor), which is passed as a device pointer after the stream the interface names has been synchronised."""
+    cai = getattr(img, "__cuda_array_interface__", None)
+    if cai is not None:
+        if np.dtype(cai["typestr"]) != dtype or tuple(cai["shape"]) != tuple(shape) or cai.get("strides") not in (None,):
+            raise ValueError(f"device image must be a contiguous {dtype} array of shape {shape}")
+        stream = cai.get("stream")
+        if stream is not None:  # the producer's stream, to be waited for (CUDA array interface v3); 1 / 2 = default
+            import torch
+
+            if stream in (1, 2):
+                torch.cuda.synchronize()
+            else:
+                torch.cuda.ExternalStream(stream).synchronize()
+        return C.c_void_p(cai["data"][0]), img
+    a = np.ascontiguousarray(img)
+    if a.dtype != dtype or a.shape != tuple(shape):
+        raise ValueError(f"image must be a {dtype} array of shape {shape}, got {a.dtype} {a.shape}")
+    return _p(a), a
+
+
+def _intrinsics(K):
+    return np.ascontiguousarray(K, np.float32).reshape(9)
+
+
+def _extrinsics(T):
+    return None if T is None else _T(T).reshape(12)
+
+
+def depth_image_to_points(ctx, depth, K, converter=None, rgb=None, extrinsics=None, normals=False, keep_invalid=False,
+                          to_device=False):
+    """cb_depth_image_to_points: depthImageToPoints / depthImageToPointsNormals / RGBDImagesToPointsColors /
+    RGBDImagesToPointsNormalsColors. depth: [h, w] uint16 or float32 (the converter's raw type), rgb: [h, w, 3] uint8;
+    each a host array or a CUDA array. Returns dict(points, normals, colors, count) of host arrays (None where not
+    asked for) or, to_device, dict(cloud, colors, count) with a device Cloud of the points (and normals)."""
+    conv = converter if converter is not None else DepthConverter()
+    shape = getattr(depth, "shape", None)
+    if shape is None or len(shape) != 2:
+        raise ValueError("depth must be an [h, w] image")
+    h, w = int(shape[0]), int(shape[1])
+    dp, keep_d = _image_arg(depth, conv.dtype, (h, w))
+    rp, keep_r = (None, None) if rgb is None else _image_arg(rgb, np.dtype(np.uint8), (h, w, 3))
+    Kf, Tf = _intrinsics(K), _extrinsics(extrinsics)
+    npix = w * h
+    pts = None if to_device else np.empty((max(npix, 1), 3), np.float32)
+    nrm = np.empty((max(npix, 1), 3), np.float32) if (normals and not to_device) else None
+    col = np.empty((max(npix, 1), 3), np.float32) if rgb is not None else None
+    cnt = C.c_size_t()
+    hdl = C.c_void_p()
+    _check(lib().cb_depth_image_to_points(ctx.h, dp, rp, C.c_size_t(w), C.c_size_t(h), C.byref(conv), _p(Kf), _p(Tf),
+                                          C.c_int(int(bool(normals))), C.c_int(int(bool(keep_invalid))), _p(pts),
+                                          _p(nrm), _p(col), C.byref(cnt), C.byref(hdl) if to_device else None))
+    del keep_d, keep_r
+    m = cnt.value
+    col = None if col is None else col[:m].copy()
+    if to_device:
+        return {"cloud": Cloud._wrap(ctx, hdl), "colors": col, "count": m}
+    return {"points": pts[:m].copy(), "normals": None if nrm is None else nrm[:m].copy(), "colors": col, "count": m}
+
+
+def _points_arg(points):
+    if isinstance(points, Cloud):
+        return None, points.h, points.n, None
+    xyz = _f32(np.asarray(points, np.float32).reshape(-1, 3))
+    return _p(xyz), None, xyz.shape[0], xyz
+
+
+def points_to_depth_image(ctx, points, K, w, h, converter=None, colors=None, extrinsics=None):
+    """cb_points_to_depth_image: pointsToDepthImage or, with colors, pointsColorsToRGBDImages. points: [n, 3] host
+    array or a Cloud. Returns the [h, w] depth image of the converter's raw type, or (depth, [h, w, 3] uint8 rgb)."""
+    conv = converter if converter is not None else DepthConverter()
+    xp, ch, n, keep = _points_arg(points)
+    col = None if colors is None else _f32(np.asarray(colors, np.float32).reshape(-1, 3))
+    if col is not None and col.shape[0] != n:
+        raise ValueError("one colour per point")
+    depth = np.empty((h, w), conv.dtype)
+    rgb = np.empty((h, w, 3), np.uint8) if col is not None else None
+    Kf, Tf = _intrinsics(K), _extrinsics(extrinsics)
+    _check(lib().cb_points_to_depth_image(ctx.h, xp, ch, C.c_size_t(n), _p(col), _p(Kf), _p(Tf), C.byref(conv),
+                                          C.c_size_t(w), C.c_size_t(h), _p(depth), _p(rgb)))
+    del keep
+    return depth if rgb is None else (depth, rgb)
+
+
+def points_to_index_map(ctx, points, K, w, h, extrinsics=None):
+    """cb_points_to_index_map: pointsToIndexMap with IndexT = uint64; empty pixels hold 2^64 - 1. points: [n, 3]
+    host array or a Cloud. Returns the [h, w] uint64 index map."""
+    xp, ch, n, keep = _points_arg(points)
+    out = np.empty((h, w), np.uint64)
+    Kf, Tf = _intrinsics(K), _extrinsics(extrinsics)
+    _check(lib().cb_points_to_index_map(ctx.h, xp, ch, C.c_size_t(n), _p(Kf), _p(Tf), C.c_size_t(w), C.c_size_t(h),
+                                        _p(out)))
+    del keep
+    return out

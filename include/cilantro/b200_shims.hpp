@@ -1909,6 +1909,49 @@ struct PointCloud3f {
       k++;
     }
   }
+  // A depth or RGB-D frame (utilities/point_cloud.hpp:83-116, 463-500) through the drop-ins of
+  // core/image_point_cloud_conversions.hpp, which must be included where these are used. IntrinsicsT is anything
+  // b200::Intrinsics3f converts from.
+  template <class DepthConverterT, class IntrinsicsT, class = typename DepthConverterT::RawDepth>
+  PointCloud3f(const typename DepthConverterT::RawDepth* depth_data, const DepthConverterT& depth_converter,
+               size_t image_w, size_t image_h, const IntrinsicsT& intrinsics, bool keep_invalid = false,
+               bool compute_normals = false) {
+    fromDepthImage(depth_data, depth_converter, image_w, image_h, intrinsics, keep_invalid, compute_normals);
+  }
+  template <class DepthConverterT, class IntrinsicsT, class = typename DepthConverterT::RawDepth>
+  PointCloud3f(const unsigned char* rgb_data, const typename DepthConverterT::RawDepth* depth_data,
+               const DepthConverterT& depth_converter, size_t image_w, size_t image_h, const IntrinsicsT& intrinsics,
+               bool keep_invalid = false, bool compute_normals = false) {
+    fromRGBDImages(rgb_data, depth_data, depth_converter, image_w, image_h, intrinsics, keep_invalid, compute_normals);
+  }
+  template <class DepthConverterT, class IntrinsicsT, class = typename DepthConverterT::RawDepth>
+  PointCloud3f& fromDepthImage(const typename DepthConverterT::RawDepth* depth_data,
+                               const DepthConverterT& depth_converter, size_t image_w, size_t image_h,
+                               const IntrinsicsT& intrinsics, bool keep_invalid = false, bool compute_normals = false) {
+    colors.resize(3, 0);
+    if (compute_normals) {
+      depthImageToPointsNormals(depth_data, depth_converter, image_w, image_h, intrinsics, points, normals,
+                                keep_invalid);
+    } else {
+      normals.resize(3, 0);
+      depthImageToPoints(depth_data, depth_converter, image_w, image_h, intrinsics, points, keep_invalid);
+    }
+    return *this;
+  }
+  template <class DepthConverterT, class IntrinsicsT, class = typename DepthConverterT::RawDepth>
+  PointCloud3f& fromRGBDImages(const unsigned char* rgb_data, const typename DepthConverterT::RawDepth* depth_data,
+                               const DepthConverterT& depth_converter, size_t image_w, size_t image_h,
+                               const IntrinsicsT& intrinsics, bool keep_invalid = false, bool compute_normals = false) {
+    if (compute_normals) {
+      RGBDImagesToPointsNormalsColors(rgb_data, depth_data, depth_converter, image_w, image_h, intrinsics, points,
+                                      normals, colors, keep_invalid);
+    } else {
+      normals.resize(3, 0);
+      RGBDImagesToPointsColors(rgb_data, depth_data, depth_converter, image_w, image_h, intrinsics, points, colors,
+                               keep_invalid);
+    }
+    return *this;
+  }
   // remove(indices) (utilities/point_cloud.hpp:154-199): each removed point takes the place of the last kept one, so
   // the order of the survivors is the reference's, not the original order
   template <typename IndexT>

@@ -748,6 +748,53 @@ int cb_vectors_reconstruct(cb_context* ctx, const cb_vectors* q, const float* me
 int cb_vectors_mds(cb_context* ctx, const cb_vectors* dist, size_t max_dim, int estimate_dim, int distances_are_squared,
                    float* eigenvalues, size_t* nev, size_t* dim, float* embedded_host, cb_vectors** embedded_device);
 
+/* ---- depth images <-> clouds -------------------------------------------------------------------------------------
+ * core/image_point_cloud_conversions.hpp with MetricDepth = float, under the contract of DESIGN §4.20. A converter is
+ * DepthValueConverter<RawDepth, float>(scale) (:7-24) or, truncated, TruncatedDepthValueConverter(scale, max_depth)
+ * (:26-51): metric = (1.0f / scale) * float(raw), truncated to 0 at or above max_depth. scale must be finite and
+ * nonzero. Intrinsics K are float32[9], row-major, any invertible 3 x 3; extrinsics are float32[12] [R | t] taken as a
+ * rigid transform, or NULL. Images are row-major, pixel k = y * w + x; rgb is 3 bytes per pixel. w * h >= 2^32 pixels
+ * or n >= 2^32 points is CB_ERR_UNSUPPORTED. One GPU. */
+typedef enum cb_raw_depth { CB_DEPTH_U16 = 0 /* unsigned short */, CB_DEPTH_F32 = 1 /* float */ } cb_raw_depth;
+typedef struct cb_depth_converter {
+  int32_t raw_type;  /* cb_raw_depth */
+  int32_t truncated; /* 0: DepthValueConverter, 1: TruncatedDepthValueConverter */
+  float scale;       /* the converters' mult */
+  float max_depth;   /* truncated only */
+} cb_depth_converter;
+
+/* depthImageToPoints (:53-147), depthImageToPointsNormals (:149-344), RGBDImagesToPointsColors (:346-473) and
+ * RGBDImagesToPointsNormalsColors (:475-695), each with and without extrinsics, and PointCloud's image constructors /
+ * fromDepthImage / fromRGBDImages (utilities/point_cloud.hpp:83-116, 463-500). depth (w * h raw values) and rgb (NULL,
+ * or 3 w h bytes) may each be host memory or device memory of the context's device (another device's memory is
+ * CB_ERR_INVALID). A device image is read on the context's stream without waiting for any other stream: the work that
+ * wrote it must have completed (e.g. its stream synchronised) before the call. want_normals selects the ...Normals variants. keep_invalid: all
+ * w * h pixels in pixel order (invalid ones as computed, normals NaN where there is none); else the kept pixels in
+ * ascending pixel order: p.z > 0, or with normals a non-NaN normal. *count is set. points / normals / colors (each may
+ * be NULL; colors needs rgb, normals needs want_normals) are host arrays with room for 3 w h floats;
+ * *out_device (NULL = none) receives a new cloud of the points (and normals) that cb_cloud_grid_downsample,
+ * cb_cloud_estimate_normals and cb_icp_create take. Launches per call: 1 with keep_invalid, else 5. */
+int cb_depth_image_to_points(cb_context* ctx, const void* depth, const unsigned char* rgb, size_t w, size_t h,
+                             const cb_depth_converter* conv, const float* K, const float* extrinsics, int want_normals,
+                             int keep_invalid, float* points, float* normals, float* colors, size_t* count,
+                             cb_cloud** out_device);
+
+/* pointsToDepthImage (:697-772) and, with colors, pointsColorsToRGBDImages (:774-863), with and without extrinsics.
+ * The points are n packed xyz on the host (xyz) or a cloud (cloud, n ignored); exactly one of them. colors: NULL or
+ * 3 n host floats, given together with rgb. Writes w * h raw values to depth (host) and 3 w h bytes to rgb (host). Per
+ * pixel the smallest raw depth wins, the lowest point index on ties, and the colour is the winner's; a raw depth that
+ * does not fit an unsigned short is skipped, a colour byte saturates (NaN -> 0). Launches per call: 2. */
+int cb_points_to_depth_image(cb_context* ctx, const float* xyz, const cb_cloud* cloud, size_t n, const float* colors,
+                             const float* K, const float* extrinsics, const cb_depth_converter* conv, size_t w,
+                             size_t h, void* depth, unsigned char* rgb);
+
+/* pointsToIndexMap (:865-934), with and without extrinsics, IndexT = uint64_t: per pixel the index of the point of
+ * smallest camera-frame z, the lowest index on ties, plus the cloud's index_offset when the points are a cloud;
+ * UINT64_MAX where no point projects. Points as in
+ * cb_points_to_depth_image. Launches per call: 2. */
+int cb_points_to_index_map(cb_context* ctx, const float* xyz, const cb_cloud* cloud, size_t n, const float* K,
+                           const float* extrinsics, size_t w, size_t h, uint64_t* index_map);
+
 /* transformPoints(tform, in, out) — core/space_transformations.hpp:203-216 (host in, host out). */
 int cb_transform_points(cb_context* ctx, const float* T12, const float* xyz, size_t n, float* out);
 

@@ -14,6 +14,7 @@ from cilantro_b200 import capi, synth  # noqa: E402
 
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import kmeans_features_ref  # noqa: E402
+import depth_images_ref  # noqa: E402
 import pca_features_ref  # noqa: E402
 
 N = int(os.environ.get("SANITIZE_N", "6000"))
@@ -158,6 +159,20 @@ def main():
     sicp.solve(f, s, T_dense_src=got["T_dense"], max_gn_iter=1, max_cg_iter=20, ctrl_sigma=0.0125)
     sicp.resample(got["T"], ctrl_sigma=0.0125)
     sicp.residuals(got["T_dense"])
+    # depth images: every back-projection pass (tile halo at the image edges, count / scan / write) and the z-buffer
+    dimg = depth_images_ref.frame("holed", 45, 19, np.uint16)
+    rgb = depth_images_ref.rgb_frame(45, 19)
+    conv = capi.DepthConverter(np.uint16, 1000.0)
+    for keep in (False, True):
+        got = capi.depth_image_to_points(ctx, dimg, depth_images_ref.K_GENERAL, conv, rgb=rgb, normals=True,
+                                         keep_invalid=keep)
+        want = depth_images_ref.depth_to_points(dimg, depth_images_ref.K_GENERAL, 1000.0, None, rgb, None, True, keep)
+        assert np.array_equal(got["points"], want[0], equal_nan=True), "depth image points"
+    pts = got["points"]
+    d, _ = capi.points_to_depth_image(ctx, pts, depth_images_ref.K_GENERAL, 45, 19, conv, colors=np.ones_like(pts))
+    want = depth_images_ref.points_to_depth_image(pts, depth_images_ref.K_GENERAL, 45, 19, scale=1000.0)
+    assert np.array_equal(d, want), "z-buffer"
+    capi.points_to_index_map(ctx, pts, depth_images_ref.K_GENERAL, 45, 19)
     ctx.close()
     print("sanitize target: all checks passed")
 
