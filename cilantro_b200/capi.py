@@ -225,6 +225,7 @@ EXPORTED = [
     "cb_knn1_radius", "cb_knn_radius", "cb_radius_search", "cb_find_correspondences",
     "cb_icp_default_params", "cb_icp_create", "cb_icp_destroy", "cb_icp_estimate", "cb_icp_iteration_times",
     "cb_icp_correspondences", "cb_icp_residuals", "cb_icp_accumulate", "cb_icp_loop_cache", "cb_icp_set_features",
+    "cb_icp_set_projection",
     "cb_solve_kabsch_moments", "cb_solve_gauss_newton", "cb_solve_rotation", "cb_compose", "cb_solve_sym_eigen",
     "cb_kmeans_cluster", "cb_kmeans_assign", "cb_kmeans_seed_indices",
     "cb_vectors_create", "cb_vectors_create_from_device", "cb_vectors_destroy", "cb_vectors_size",
@@ -756,6 +757,14 @@ class Icp(_Handle):
         sn, sc = arr(src_normals, self.src.n), arr(src_colors, self.src.n)
         _check(lib().cb_icp_set_features(self.h, C.c_int(FEATURE_KINDS[kind]), _p(dn), _p(dc), _p(sn), _p(sc),
                                          C.c_float(normal_weight), C.c_float(color_weight)))
+
+    def set_projection(self, K, w, h, extrinsics=None):
+        """cb_icp_set_projection: match each source point to the destination point its pixel shows in a w x h image
+        with intrinsics K (3 x 3) seen from the camera pose `extrinsics` ([R | t], 3 x 4; None = identity), as
+        CorrespondenceSearchProjective does. K = None detaches the projection (the kd-tree search again)."""
+        Kp = None if K is None else np.ascontiguousarray(np.asarray(K, np.float32).reshape(3, 3))
+        E = None if extrinsics is None else _T(extrinsics)
+        _check(lib().cb_icp_set_projection(self.h, _p(Kp), C.c_size_t(int(w)), C.c_size_t(int(h)), _p(E)))
 
 
 def solve_kabsch_moments(sums16):

@@ -771,6 +771,22 @@ static bool icp_engine(const cb_icp* icp, const cb_icp_params* prm) {
   return engine_mode(prm) || icp->feat.kind != CB_FEATURES_POINT;
 }
 
+// With a projection attached (cb_icp_set_projection) the kd-tree-only options have no meaning.
+static int check_projective(const cb_icp* icp, const cb_icp_params* prm) {
+  if (!icp->proj.on) return CB_OK;
+  CB_CHECK(prm->search_dir == CB_SECOND_TO_FIRST && !prm->require_reciprocal && !prm->one_to_one &&
+               icp->feat.kind == CB_FEATURES_POINT,
+           CB_ERR_INVALID, "projective search: search_dir, require_reciprocal, one_to_one and features are kd-tree options");
+  return CB_OK;
+}
+
+// The projective search's per-query result under a->T into a->nn_pos / a->nn_d2 (filled with store = true), for the
+// passes that accumulate without a search.
+static int projective_pass_input(cb_icp* icp, const IcpArgs& a) {
+  return launch_projective_search(icp->ctx, icp->proj, icp->src->d_pts, (uint32_t)icp->src->n, icp->dst->d_pts, a.T,
+                                  a.max_d2, a.nn_pos, a.nn_d2, nullptr, nullptr);
+}
+
 // One estimator call of updateEstimate(): returns tform_iter (already un-centred), and the
 // correspondence count of the search pass. k0/k1 (nullable) are recorded around the search kernel.
 
@@ -785,11 +801,12 @@ static int icp_update(cb_icp* icp, const cb_icp_params* prm, const float* T, flo
     // updateCorrespondences(): the explicit list (icp_engine.cu); the passes below accumulate over it
     if (k0) CB_CUDA(cudaEventRecord(k0, ctx->stream));
     CB_TRY(ensure_src_full(icp));
-    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, esrc(icp), prm, T, &icp->pairs, &icp->feat));
+    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, esrc(icp), prm, T, &icp->pairs, &icp->feat, &icp->proj));
     if (k1) CB_CUDA(cudaEventRecord(k1, ctx->stream));
   }
+  const bool proj = icp->proj.on && !engine;
   if (prm->metric == CB_ICP_POINT_TO_POINT) {
-    CB_TRY(icp_fill_args(icp, prm, T, nullptr, false, &a));
+    CB_TRY(icp_fill_args(icp, prm, T, nullptr, proj, &a));
     if (engine) {
       // moments about the pivots (dst mean, T * src mean): no cancellation for clouds far from the origin
       CB_TRY(launch_pairs_pass(ctx, a, icp->pairs, icp->dst, esrc(icp), kModeP2PCentered, false, false));
@@ -801,7 +818,8 @@ static int icp_update(cb_icp* icp, const cb_icp_params* prm, const float* T, flo
       return CB_OK;
     }
     if (k0) CB_CUDA(cudaEventRecord(k0, ctx->stream));
-    CB_TRY(launch_icp_pass(ctx, a, kModeP2PCentered, true, false, false));
+    if (proj) CB_TRY(projective_pass_input(icp, a));
+    CB_TRY(launch_icp_pass(ctx, a, kModeP2PCentered, !proj, false, false));
     if (k1) CB_CUDA(cudaEventRecord(k1, ctx->stream));
     CB_TRY(icp_fetch(ctx, kP2PValues, sums));
     kabsch_from_pivoted_moments(sums, a.dm, a.sm, Titer);
@@ -820,7 +838,8 @@ static int icp_update(cb_icp* icp, const cb_icp_params* prm, const float* T, flo
   const bool bail_no_normals = w_pl_on && !dst_has_normals;
   const int max_opt = std::max(prm->max_opt_iter, 0);
   for (int it = 0; it < std::max(max_opt, 1); ++it) {
-    CB_TRY(icp_fill_args(icp, prm, T, Tin, max_opt > 1 && !engine, &a));  // (stores d2 too: the RBF weights of inner passes read it)
+    // (stores d2 too: the RBF weights of inner passes read it; the projective search writes its result there)
+    CB_TRY(icp_fill_args(icp, prm, T, Tin, (max_opt > 1 || proj) && !engine, &a));
     const bool search = (it == 0);
     if (engine) {
       CB_TRY(launch_pairs_pass(ctx, a, icp->pairs, icp->dst, esrc(icp), kModeCombined, w_pt_on,
@@ -828,7 +847,8 @@ static int icp_update(cb_icp* icp, const cb_icp_params* prm, const float* T, flo
     } else {
       // the first pass always runs (it is also the correspondence search of this ICP iteration)
       if (search && k0) CB_CUDA(cudaEventRecord(k0, ctx->stream));
-      CB_TRY(launch_icp_pass(ctx, a, kModeCombined, search, w_pt_on, w_pl_on && dst_has_normals));
+      if (search && proj) CB_TRY(projective_pass_input(icp, a));
+      CB_TRY(launch_icp_pass(ctx, a, kModeCombined, search && !proj, w_pt_on, w_pl_on && dst_has_normals));
       if (search && k1) CB_CUDA(cudaEventRecord(k1, ctx->stream));
     }
     CB_TRY(icp_fetch(ctx, kCombinedValues, sums, /*allreduce=*/!(engine && ctx->world > 1)));
@@ -859,6 +879,7 @@ static int icp_update(cb_icp* icp, const cb_icp_params* prm, const float* T, flo
 int cb_icp_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res) {
   CB_CHECK(icp && prm && res, CB_ERR_INVALID, "null argument");
   CB_CHECK(prm->metric == CB_ICP_POINT_TO_POINT || prm->metric == CB_ICP_COMBINED, CB_ERR_INVALID, "bad metric");
+  CB_TRY(check_projective(icp, prm));
   cb_context* ctx = icp->ctx;
   CB_CUDA(cudaSetDevice(ctx->device));
   int hand_over = 0;
@@ -977,16 +998,18 @@ int cb_icp_accumulate(cb_icp* icp, const cb_icp_params* prm, const float* T12, d
   CB_CHECK(icp && prm && T12 && sums, CB_ERR_INVALID, "null argument");
   cb_context* ctx = icp->ctx;
   CB_CUDA(cudaSetDevice(ctx->device));
+  CB_TRY(check_projective(icp, prm));
   IcpArgs a;
   double tmp[kMaxValues];
   int nv;
-  if (icp->feat.kind != CB_FEATURES_POINT) {
-    // the feature search's correspondence list (icp_engine.cu), accumulated like the list path's passes
+  if (icp->feat.kind != CB_FEATURES_POINT || (icp->proj.on && engine_mode(prm))) {
+    // the feature search's or the fraction-filtered projective correspondence list (icp_engine.cu), accumulated like
+    // the list path's passes
     const bool p2p = prm->metric == CB_ICP_POINT_TO_POINT;
     nv = p2p ? kP2PValues : kCombinedValues;
     CB_CHECK(p2p || !(prm->w_pl > 0.f) || icp->dst->d_nrm, CB_ERR_INVALID, "dst has no normals");
     CB_CHECK(cap >= nv, CB_ERR_INVALID, "sums buffer too small");
-    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, icp->src, prm, T12, &icp->pairs, &icp->feat));
+    CB_TRY(engine_find_pairs(ctx, icp->mem, icp->dst, icp->src, prm, T12, &icp->pairs, &icp->feat, &icp->proj));
     CB_TRY(icp_fill_args(icp, prm, T12, nullptr, false, &a));
     CB_TRY(launch_pairs_pass(ctx, a, icp->pairs, icp->dst, icp->src, p2p ? kModeP2P : kModeCombined,
                              !p2p && prm->w_pt > 0.f, !p2p && prm->w_pl > 0.f));
@@ -998,13 +1021,16 @@ int cb_icp_accumulate(cb_icp* icp, const cb_icp_params* prm, const float* T12, d
   }
   CB_TRY(icp_fill_args(icp, prm, T12, nullptr, true, &a));
   icp->engine_last = false;  // cb_icp_correspondences reads this pass's per-query result
+  const bool proj = icp->proj.on;
   if (prm->metric == CB_ICP_POINT_TO_POINT) {
     nv = kP2PValues;
-    CB_TRY(launch_icp_pass(ctx, a, kModeP2P, true, false, false));
+    if (proj) CB_TRY(projective_pass_input(icp, a));
+    CB_TRY(launch_icp_pass(ctx, a, kModeP2P, !proj, false, false));
   } else {
     nv = kCombinedValues;
     CB_CHECK(!(prm->w_pl > 0.f) || icp->dst->d_nrm, CB_ERR_INVALID, "dst has no normals");
-    CB_TRY(launch_icp_pass(ctx, a, kModeCombined, true, prm->w_pt > 0.f, prm->w_pl > 0.f));
+    if (proj) CB_TRY(projective_pass_input(icp, a));
+    CB_TRY(launch_icp_pass(ctx, a, kModeCombined, !proj, prm->w_pt > 0.f, prm->w_pl > 0.f));
   }
   CB_CHECK(cap >= nv, CB_ERR_INVALID, "sums buffer too small");
   CB_TRY(icp_fetch(ctx, nv, tmp));
@@ -1036,6 +1062,12 @@ int cb_icp_correspondences(cb_icp* icp, uint64_t* index_first, uint64_t* index_s
     return CB_OK;
   }
   if (ns == 0) return CB_OK;
+  if (!icp->nn_stored && icp->proj.on) {  // the device loop's projective run: re-run its last search
+    CB_TRY(launch_projective_search(ctx, icp->proj, icp->src->d_pts, (uint32_t)ns, icp->dst->d_pts,
+                                    to_rigid(icp->T_search), icp->max_d2_search, icp->d_nn_pos, icp->d_nn_d2, nullptr,
+                                    nullptr));
+    icp->nn_stored = true;
+  }
   if (!icp->nn_stored) {  // re-run the last search, this time keeping the per-query result
     IcpArgs a{};
     a.dst = grid_view(icp->dst);

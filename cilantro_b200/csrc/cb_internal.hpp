@@ -304,12 +304,15 @@ struct FeatureSet {
   float4* dst_sorted = nullptr;  // the same in the destination grid's cell order
   float4* src_raw = nullptr;     // source tails, original order, untransformed
 };
+struct ProjectiveMap;
 // findCorrespondences(tform) of CorrespondenceSearchKDTree (correspondence_search_kd_tree.hpp:107-229) for
 // the current estimate T: searches, union / intersection, fraction and one-to-one filters. Replaces *pairs, whose
 // buffers belong to `owner`. feat (nullable, or kind CB_FEATURES_POINT): search on the xyz distance; otherwise on the
-// feature distance (feature_search.cu), which is then the pairs' value.
+// feature distance (feature_search.cu), which is then the pairs' value. proj (nullable, or not on): with a projection
+// attached the SECOND_TO_FIRST result is the projective search's (CorrespondenceSearchProjective, DESIGN §4.21).
 int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const cb_cloud* src,
-                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs, const FeatureSet* feat = nullptr);
+                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs, const FeatureSet* feat = nullptr,
+                      const ProjectiveMap* proj = nullptr);
 
 // nccl_dyn.cpp
 int nccl_unique_id(void* out128);

@@ -15,6 +15,7 @@
 // smallest key, lowest index on ties, the colour of the winner.
 #include "cb_internal.hpp"
 #include "launch.cuh"
+#include "projection.hpp"
 #include <cmath>
 #include <cstring>
 
@@ -176,32 +177,18 @@ enum RenderMode { kDepthU16 = 0, kDepthF32 = 1, kIndexMap = 2 };
 struct Render {
   const float* pts;
   uint32_t n;
-  uint32_t w, h;
   int mode;  // RenderMode
   int truncated;
   float scale, max_depth;
-  float K0[3], K1[3];  // rows 0 and 1 of the intrinsics
-  int extr;            // camera frame = L p + tr (extrinsics.inverse())
-  float L[9], tr[3];
+  Projection prj;  // intrinsics, extrinsics.inverse(), image size (projection.hpp)
   unsigned long long* keys;  // w * h, kEmpty on entry
 };
 
 __global__ void __launch_bounds__(256) render_keys_kernel(const Render P) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < P.n; i += (size_t)gridDim.x * blockDim.x) {
-    float q0 = P.pts[3 * i], q1 = P.pts[3 * i + 1], q2 = P.pts[3 * i + 2];
-    if (P.extr) {
-      const float c0 = __fadd_rn(dot3(P.L, q0, q1, q2), P.tr[0]), c1 = __fadd_rn(dot3(P.L + 3, q0, q1, q2), P.tr[1]),
-                  c2 = __fadd_rn(dot3(P.L + 6, q0, q1, q2), P.tr[2]);
-      q0 = c0;
-      q1 = c1;
-      q2 = c2;
-    }
-    if (!(q2 > 0.0f)) continue;  // z <= 0; a NaN z projects to NaN and is skipped below in any case
-    const float inv_z = __fdiv_rn(1.0f, q2);
-    const float fx = __fmul_rn(inv_z, dot3(P.K0, q0, q1, q2)), fy = __fmul_rn(inv_z, dot3(P.K1, q0, q1, q2));
-    if (!isfinite(fx) || !isfinite(fy)) continue;
-    const float rx = roundf(fx), ry = roundf(fy);  // llround: half away from zero
-    if (!(rx >= 0.0f && ry >= 0.0f) || (double)rx >= (double)P.w || (double)ry >= (double)P.h) continue;
+    uint32_t px, py;
+    float q2;
+    if (!project_pixel(P.prj, P.pts[3 * i], P.pts[3 * i + 1], P.pts[3 * i + 2], px, py, q2)) continue;
     uint32_t key;
     if (P.mode == kIndexMap) {
       key = __float_as_uint(q2);
@@ -217,7 +204,7 @@ __global__ void __launch_bounds__(256) render_keys_kernel(const Render P) {
       }
       if (key == 0) continue;  // a raw depth of 0 never writes
     }
-    atomicMin(&P.keys[(size_t)(uint32_t)ry * P.w + (uint32_t)rx], ((unsigned long long)key << 32) | i);
+    atomicMin(&P.keys[(size_t)py * P.prj.w + px], ((unsigned long long)key << 32) | i);
   }
 }
 
@@ -401,6 +388,12 @@ int depth_to_points(cb_context* ctx, const void* depth, const unsigned char* rgb
   return CB_OK;
 }
 
+// keys (w * h) = the z-buffer of P.pts: (key << 32 | index) of each pixel's winner, kEmpty where no point lands
+int zbuffer(cb_context* ctx, const Render& P) {
+  CB_CUDA(cudaMemsetAsync(P.keys, 0xff, (size_t)P.prj.w * P.prj.h * sizeof(unsigned long long), ctx->stream));
+  return launch(ctx, render_keys_kernel, grid_for(ctx, P.n, 256), 256, 0, P);
+}
+
 int render(cb_context* ctx, const float* xyz, const cb_cloud* cloud, size_t n, const float* colors, const float* K,
            const float* extr, int mode, const cb_depth_converter* conv, size_t w, size_t h, void* depth, uint8_t* rgb,
            uint64_t* index_map) {
@@ -417,25 +410,13 @@ int render(cb_context* ctx, const float* xyz, const cb_cloud* cloud, size_t n, c
   Render P;
   std::memset(&P, 0, sizeof(P));
   P.n = (uint32_t)n;
-  P.w = (uint32_t)w;
-  P.h = (uint32_t)h;
   P.mode = mode;
   if (conv) {
     P.truncated = conv->truncated ? 1 : 0;
     P.scale = conv->scale;
     P.max_depth = conv->max_depth;
   }
-  for (int j = 0; j < 3; j++) {
-    P.K0[j] = K[j];
-    P.K1[j] = K[3 + j];
-  }
-  if (extr) {
-    // extrinsics.inverse() of an isometry: linear R^T, translation -(R^T t)
-    P.extr = 1;
-    for (int i = 0; i < 3; i++)
-      for (int j = 0; j < 3; j++) P.L[3 * i + j] = extr[4 * j + i];
-    for (int i = 0; i < 3; i++) P.tr[i] = -rdot(P.L[3 * i], P.L[3 * i + 1], P.L[3 * i + 2], extr[3], extr[7], extr[11]);
-  }
+  P.prj = make_projection(K, extr, (uint32_t)w, (uint32_t)h);
   if (cloud) {
     P.pts = cloud->d_raw;
   } else if (n) {
@@ -450,8 +431,7 @@ int render(cb_context* ctx, const float* xyz, const cb_cloud* cloud, size_t n, c
     if (n) CB_CUDA(cudaMemcpyAsync(d_col, colors, 3 * n * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
   }
   CB_TRY(scope.alloc(&P.keys, npix));
-  CB_CUDA(cudaMemsetAsync(P.keys, 0xff, npix * sizeof(unsigned long long), ctx->stream));
-  CB_TRY(launch(ctx, render_keys_kernel, grid_for(ctx, n, 256), 256, 0, P));
+  CB_TRY(zbuffer(ctx, P));
   void* d_depth = nullptr;
   uint8_t* d_rgb = nullptr;
   const size_t depth_bytes = npix * (mode == kDepthU16 ? sizeof(uint16_t) : sizeof(float));
@@ -473,6 +453,19 @@ int render(cb_context* ctx, const float* xyz, const cb_cloud* cloud, size_t n, c
 }
 
 }  // namespace
+
+namespace cb {
+int index_map_keys(cb_context* ctx, const float* d_pts, size_t n, const Projection& prj, unsigned long long* keys) {
+  Render P;
+  std::memset(&P, 0, sizeof(P));
+  P.pts = d_pts;
+  P.n = (uint32_t)n;
+  P.mode = kIndexMap;
+  P.prj = prj;
+  P.keys = keys;
+  return zbuffer(ctx, P);
+}
+}  // namespace cb
 
 int cb_depth_image_to_points(cb_context* ctx, const void* depth, const unsigned char* rgb, size_t w, size_t h,
                              const cb_depth_converter* conv, const float* K, const float* extrinsics, int want_normals,

@@ -23,6 +23,7 @@
 #include "feature_search.cuh"
 #include "icp_accumulate.cuh"
 #include "icp_kernels.cuh"
+#include "icp_object.hpp"
 #include "launch.cuh"
 #include "reduce.cuh"
 #include <algorithm>
@@ -230,7 +231,8 @@ int launch_pairs_pass(cb_context* ctx, const IcpArgs& a, const EnginePairs& pair
 }
 
 int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const cb_cloud* src,
-                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs, const FeatureSet* feat) {
+                      const cb_icp_params* prm, const float* T12, EnginePairs* pairs, const FeatureSet* feat,
+                      const ProjectiveMap* proj) {
   // (with several ranks the caller passes the whole source cloud, replicated: capi_core.cu, ensure_src_full)
   CB_CHECK(prm->search_dir >= CB_SECOND_TO_FIRST && prm->search_dir <= CB_BOTH, CB_ERR_INVALID, "bad search_dir");
   CB_TRY(owner.free(pairs->first));
@@ -246,7 +248,13 @@ int engine_find_pairs(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, 
   Dev dev(ctx);
   int *s2f_idx = nullptr, *f2s_idx = nullptr;
   float *s2f_d2 = nullptr, *f2s_d2 = nullptr;
-  if (want_s2f && features) {
+  if (want_s2f && proj && proj->on) {
+    // find_correspondences_ of CorrespondenceSearchProjective: one pixel per query (projective_search.cu)
+    CB_TRY(dev.alloc(&s2f_idx, n_src));
+    CB_TRY(dev.alloc(&s2f_d2, n_src));
+    CB_TRY(launch_projective_search(ctx, *proj, src->d_pts, n_src, dst->d_pts, rigid_of(T12), prm->max_d2, nullptr,
+                                    nullptr, s2f_idx, s2f_d2));
+  } else if (want_s2f && features) {
     // queries = transformFeatures(T) of the source features, tree = the destination features
     CB_TRY(dev.alloc(&s2f_idx, n_src));
     CB_TRY(dev.alloc(&s2f_d2, n_src));

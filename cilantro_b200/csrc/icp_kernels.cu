@@ -202,8 +202,8 @@ int launch_icp_pass(cb_context* ctx, const IcpArgs& a, int mode, bool search, bo
     kernel = icp_pass_kernel<kModeKnn, true>;
   else if (mode == kModeP2P)
     kernel = search ? icp_pass_kernel<kModeP2P, true> : icp_pass_kernel<kModeP2P, false>;
-  else if (mode == kModeP2PCentered)  // Kabsch moments about the pivots a.dm / a.sm (the ICP loop, a search pass)
-    kernel = icp_pass_kernel<kModeP2PCentered, true>;
+  else if (mode == kModeP2PCentered)  // Kabsch moments about the pivots a.dm / a.sm (the ICP loop)
+    kernel = search ? icp_pass_kernel<kModeP2PCentered, true> : icp_pass_kernel<kModeP2PCentered, false>;
   // only the combined metric reads has_pt / has_pl
   return launch(ctx, kernel, blocks, kBlock, 0, args, has_pt, has_pl);
 }

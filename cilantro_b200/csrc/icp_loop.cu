@@ -24,6 +24,9 @@
 // margins, far above the 6-ulp error of the fp32 distance evaluation); an exact tie can never pass the strict test.
 // As ICP converges the per-iteration motion shrinks geometrically and almost every query takes the cached path:
 // the iteration becomes one streaming pass (12 B query + 8 B cache + one 12 B gather per source point).
+//
+// With a projection attached (cb_icp_set_projection, DESIGN §4.21) the first kernel is icp_projective_kernel instead:
+// every source point looks up the one destination point its pixel shows, with no cache and no search.
 #include "cache_rule.hpp"
 #include "icp_accumulate.cuh"
 #include "icp_kernels.cuh"
@@ -70,6 +73,9 @@ struct LoopArgs {
   ReduceScratch rs;
   uint32_t rows;  // block rows of the pass in rs.partials (its grid size)
   int trace;      // CB_LOOP_TRACE: fill LoopState::trace
+  // projective search (icp_projective_kernel): the index map (sorted dst positions, -1 empty) and its projection
+  const int* proj_map;
+  Projection prj;
 };
 
 // per-block copy of the loop state; also the `Args` of accumulate_pair (T, dm, sm, w_pt, w_pl)
@@ -564,6 +570,65 @@ __global__ void __launch_bounds__(kBlock, cold_min_blocks(MODE == kModeCombined)
   if (block_row_from_slots<NV>(rsm, row) && lane < NV) a.rs.partials[(size_t)blockIdx.x * NV + lane] = row;
 }
 
+// ---- kernel 1 of a projective iteration: project, look up, accumulate ------------------------------------------------
+// find_correspondences_ of CorrespondenceSearchProjective (DESIGN §4.21) fused with the accumulation. PERSISTENT and
+// grid-stride over the cell-sorted source, so the assignment and the summation order are fixed: per query the packed
+// point (12 B), one map read (4 B), and for a pixel that shows a destination point its packed coordinates (12 B) and,
+// with the plane term, its normal (12 B); the symmetric metric adds the source normal. Nothing is cached, nothing is
+// searched: searched_cur stays 0, so the loop never hands the run over.
+// Register budget (__launch_bounds__ caps): p2p at most 64 registers for 4 blocks per SM (it uses 64); combined at most 128
+// for 2 blocks per SM (it uses 108; at the 80-register cap of 3 blocks its 28 accumulators spilled).
+__host__ __device__ constexpr int proj_min_blocks(bool combined) { return combined ? 2 : 4; }
+
+template <int MODE>
+__global__ void __launch_bounds__(kBlock, proj_min_blocks(MODE == kModeCombined))
+    icp_projective_kernel(const __grid_constant__ LoopArgs a) {
+  constexpr int NV = (MODE == kModeP2PCentered) ? kP2PValues : kCombinedValues;
+  __shared__ BlockCtx cx;
+  __shared__ AsyncReduceSmem<NV> rsm;
+  const unsigned int tid = threadIdx.x, lane = tid & 31u;
+  pdl_wait();               // the state of the previous finish kernel
+  pdl_launch_dependents();  // the finish kernel may be scheduled now and wait for this grid to drain
+  if (tid == 0) {
+    rsm.arrived = 0u;
+    load_block_ctx(a, cx);
+  }
+  __syncthreads();
+  if (cx.done) return;  // converged (or failed) in an earlier launch of this batch
+  // (the fold adds value by value into zeroed slots: the transposing butterfly of warp_sum_to_slot<16, false> would
+  // keep acc[] in local memory)
+  if (lane < NV) rsm.slot[tid >> 5][lane] = 0.0;
+  __syncwarp();  // the zeroed slots are visible to lane 0's read-modify-write in warp_sum_to_slot
+  double acc[NV];
+#pragma unroll
+  for (int v = 0; v < NV; v++) acc[v] = 0.0;
+#pragma unroll 1
+  for (uint32_t i = blockIdx.x * kBlock + tid; i < a.n_src; i += gridDim.x * kBlock) {
+    const float* s = a.src_xyz + (size_t)i * 3u;
+    float qx, qy, qz;
+    rule::transform_point(cx.T, __ldg(s), __ldg(s + 1), __ldg(s + 2), qx, qy, qz);
+    uint32_t px, py;
+    float cz;
+    if (!project_pixel(a.prj, qx, qy, qz, px, py, cz)) continue;
+    const int pos = __ldg(a.proj_map + (size_t)py * a.prj.w + px);
+    if (pos < 0) continue;
+    const float* p = a.dst_xyz + (size_t)pos * 3u;
+    const float4 dp = make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), 0.f);
+    const float d2 = rule::contract_d2(qx, qy, qz, dp.x, dp.y, dp.z);
+    if (!(d2 < a.max_d2)) continue;
+    accumulate_pair<MODE, true>(
+        acc, cx, a.has_pt != 0, a.has_pl != 0, dp, qx, qy, qz, a.src_nrm != nullptr,
+        [&] {
+          const float* n = a.dst_nxyz + (size_t)pos * 3u;
+          return make_float4(__ldg(n), __ldg(n + 1), __ldg(n + 2), 0.f);
+        },
+        [&] { return __ldg(a.src_nrm + i); }, d2);
+  }
+  warp_sum_to_slot<NV, true>(acc, rsm);
+  double row;
+  if (block_row_from_slots<NV>(rsm, row) && lane < NV) a.rs.partials[(size_t)blockIdx.x * NV + lane] = row;
+}
+
 // ---- kernel 2 of an iteration: fold + exchange + solve (one block) -----------------------------------------------------
 // The pass's block rows (a.rows of them) -> this GPU's totals (block_fold_rows: the whole block, in the fixed order of
 // the grid reduction) -> all-reduce with the
@@ -648,12 +713,16 @@ constexpr double kGiveUpShare = 0.15;
 
 // Enqueues the kernels of ICP iteration `it` of this call, with programmatic stream serialization (see pdl_wait
 // above): the cold pass in the first iteration (nothing cached yet), else the cached pass with its search of the
-// flagged queries; then the finish kernel.
+// flagged queries; with a projection the projective pass in every iteration; then the finish kernel.
 template <int MODE>
-static int enqueue_iteration(cb_context* ctx, const LoopArgs& args, int it, int blocks_cold, int blocks_cached) {
+static int enqueue_iteration(cb_context* ctx, const LoopArgs& args, int it, int blocks_cold, int blocks_cached,
+                             int blocks_proj) {
   LoopArgs a = args;
-  a.rows = (uint32_t)(it == 0 ? blocks_cold : blocks_cached);  // each block of either pass writes one row
-  if (it == 0)
+  // each block of any pass writes one row
+  a.rows = (uint32_t)(a.proj_map ? blocks_proj : it == 0 ? blocks_cold : blocks_cached);
+  if (a.proj_map)
+    CB_TRY(launch_pdl(ctx, icp_projective_kernel<MODE>, blocks_proj, kBlock, 0, a));
+  else if (it == 0)
     CB_TRY(launch_pdl(ctx, icp_search_kernel<MODE>, blocks_cold, kBlock, 0, a));
   else
     CB_TRY(launch_pdl(ctx, icp_cached_pipe_kernel<MODE>, blocks_cached, kBlock, sizeof(PipeSmem<MODE == kModeCombined>),
@@ -749,7 +818,12 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   // the cached pass's flagged-query lists: per warp, room for every query of its block's tiles (about n_src in all)
   const size_t per_warp = ((ns + tile - 1) / tile + blocks_cached - 1) / blocks_cached * (tile / (kBlock / 32));
   const size_t flagged_need = per_warp * (size_t)blocks_cached * (kBlock / 32);
-  if (icp->loop_flagged_cap < flagged_need) {
+  const bool projective = icp->proj.on;
+  const int blocks_proj = grid_for(ctx, ns, kBlock, proj_min_blocks(!p2p));
+  if (projective) {
+    a.proj_map = icp->proj.d_map;
+    a.prj = icp->proj.prj;
+  } else if (icp->loop_flagged_cap < flagged_need) {
     if (icp->d_loop_flagged) CB_TRY(icp->mem.free(icp->d_loop_flagged));
     icp->d_loop_flagged = nullptr;
     icp->loop_flagged_cap = 0;
@@ -758,7 +832,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   }
   a.flagged = icp->d_loop_flagged;
   a.flagged_per_warp = (uint32_t)per_warp;
-  CB_TRY(get_reduce_scratch(ctx, std::max(blocks_cold, blocks_cached), kMaxValues, &a.rs));
+  CB_TRY(get_reduce_scratch(ctx, std::max(std::max(blocks_cold, blocks_cached), blocks_proj), kMaxValues, &a.rs));
   Exchange ex;
   std::memset(&ex, 0, sizeof(ex));
   const bool fused = ctx->world > 1 && arm_exchange(ctx, &ex);  // tables + timeout; the pass number lives in LoopState
@@ -792,9 +866,9 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
       if (prm->flush_l2) CB_TRY(cb_context_flush_l2(ctx));
       if (timing) CB_CUDA(cudaEventRecord(icp->events[2 * (issued + k)], ctx->stream));
       if (p2p)
-        CB_TRY(enqueue_iteration<kModeP2PCentered>(ctx, a, issued + k, blocks_cold, blocks_cached));
+        CB_TRY(enqueue_iteration<kModeP2PCentered>(ctx, a, issued + k, blocks_cold, blocks_cached, blocks_proj));
       else
-        CB_TRY(enqueue_iteration<kModeCombined>(ctx, a, issued + k, blocks_cold, blocks_cached));
+        CB_TRY(enqueue_iteration<kModeCombined>(ctx, a, issued + k, blocks_cold, blocks_cached, blocks_proj));
       if (timing) CB_CUDA(cudaEventRecord(icp->events[2 * (issued + k) + 1], ctx->stream));
     }
     issued += n;
@@ -853,7 +927,7 @@ int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res,
   icp->nn_stored = false;  // d_nn_pos / d_nn_d2 hold the cache, not a per-query result list
   icp->warm_ok = false;
   icp->engine_last = false;
-  icp->loop_last = true;
+  icp->loop_last = !projective;  // (cb_icp_loop_cache inspects the kd-tree search's cache)
   icp->searched_last = hs->searched_last;
   std::memcpy(icp->T_search, hs->T_prev, sizeof(icp->T_search));
   icp->max_d2_search = prm->max_d2;

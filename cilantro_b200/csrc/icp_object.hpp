@@ -2,6 +2,8 @@
 // device-resident loop (icp_loop.cu).
 #pragma once
 #include "cb_internal.hpp"
+#include "nn_search.cuh"
+#include "projection.hpp"
 #include <vector>
 
 namespace cb {
@@ -30,6 +32,13 @@ struct LoopState {
   // peers' rows summed / state written, the number of queries that needed a search, %globaltimer when the last warp
   // of the grid reached the reduction (its tiles and searches done)
   unsigned long long trace[64][6];
+};
+
+// The projective correspondence search attached by cb_icp_set_projection (projective_search.cu, DESIGN §4.21).
+struct ProjectiveMap {
+  bool on = false;
+  Projection prj;
+  int* d_map = nullptr;  // w * h: sorted position of the destination point each pixel shows, -1 empty (owned by cb_icp)
 };
 
 }  // namespace cb
@@ -69,7 +78,8 @@ struct cb_icp {
   float* d_loop_dst_xyz = nullptr;
   float* d_loop_dst_nxyz = nullptr;
   cb_cloud* src_full = nullptr;      // world > 1, engine modes: the whole source cloud replicated on this rank (owned)
-  bool loop_last = false;            // the last estimate() ran on the device loop
+  bool loop_last = false;            // the last estimate() ran on the device loop's kd-tree search
+  cb::ProjectiveMap proj;            // cb_icp_set_projection: the search is projective while proj.on
   uint64_t searched_last = 0;        // queries its last iteration searched again (CB_LOOP_TRACE / cb_icp_loop_cache)
 };
 
@@ -81,4 +91,14 @@ namespace cb {
 // host-driven loop, whose plain search is cheaper per searched query.
 int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res, int* hand_over);
 unsigned long long exchange_timeout_ns();
+
+// Projective correspondence search (projective_search.cu). Per source point of the cell-sorted cloud src_pts, under T:
+// nn_pos / nn_d2 by sorted position (the destination's sorted position, -1 none), out_idx / out_d2 by original index
+// (the destination's original index, -1 none); every output is nullable.
+int launch_projective_search(cb_context* ctx, const ProjectiveMap& pm, const float4* src_pts, uint32_t n_src,
+                             const float4* dst_pts, const Rigid& T, float max_d2, int* nn_pos, float* nn_d2,
+                             int* out_idx, float* out_d2);
+// The z-buffer of the index map (depth_images.cu): keys (w * h) = (bits of camera z << 32 | index) of each pixel's
+// winner among the n packed points at d_pts, ~0 where none lands.
+int index_map_keys(cb_context* ctx, const float* d_pts, size_t n, const Projection& prj, unsigned long long* keys);
 }  // namespace cb

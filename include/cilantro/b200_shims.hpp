@@ -905,6 +905,15 @@ public:
   // after the ICP's estimate(), as the reference's engine holds them
   const SearchResult& getCorrespondences() const { return feat_corr_; }
   void b200_set_correspondences(const SearchResult& c) { feat_corr_ = c; }
+  // EngineRigidICP3f::estimate(): the features go to the ICP object (every call: the adaptors may have changed)
+  void b200_attach(cb_icp* icp, size_t n_dst, size_t n_src, uint64_t&) {
+    if (dst_.b200_size() != n_dst || src_.b200_size() != n_src)
+      throw std::invalid_argument("cilantro_b200: the feature adaptors' sizes differ from the ICP's point sets");
+    b200::check(cb_icp_set_features(icp, dst_.b200_kind(), dst_.b200_normals(), dst_.b200_colors(), src_.b200_normals(),
+                                    src_.b200_colors(), dst_.b200_normal_weight(), dst_.b200_color_weight()),
+                "cb_icp_set_features");
+  }
+  const CorrespondenceSearchEngineB200& b200_settings() const { return *this; }
 
 private:
   SearchFeatureAdaptorT& dst_;
@@ -914,8 +923,8 @@ private:
 };
 
 namespace b200 {
-// The engine-templated ICP classes: the reference's constructor order, the engine's settings and features read at every
-// estimate().
+// The engine-templated ICP classes: the reference's constructor order, the engine's settings and its search space
+// (feature adaptors, or a projection) handed to the ICP object at every estimate() (Engine::b200_attach).
 template <class Engine, class Base>
 class EngineRigidICP3f : public Base {
 public:
@@ -924,14 +933,8 @@ public:
   Engine& correspondenceSearchEngine() { return engine_; }
   const Engine& correspondenceSearchEngine() const { return engine_; }
   EngineRigidICP3f& estimate() {
-    auto& dst = engine_.b200_dst_features();
-    auto& src = engine_.b200_src_features();
-    if (dst.b200_size() != n_dst_ || src.b200_size() != n_src_)
-      throw std::invalid_argument("cilantro_b200: the feature adaptors' sizes differ from the ICP's point sets");
-    check(cb_icp_set_features(this->b200_icp(), dst.b200_kind(), dst.b200_normals(), dst.b200_colors(),
-                              src.b200_normals(), src.b200_colors(), dst.b200_normal_weight(), dst.b200_color_weight()),
-          "cb_icp_set_features");
-    Base::correspondenceSearchEngine() = static_cast<const CorrespondenceSearchEngineB200&>(engine_);
+    engine_.b200_attach(this->b200_icp(), n_dst_, n_src_, attached_);
+    Base::correspondenceSearchEngine() = engine_.b200_settings();
     Base::estimate();
     return *this;
   }
@@ -947,6 +950,7 @@ public:
 
 private:
   Engine& engine_;
+  uint64_t attached_ = 0;  // the engine's state this ICP object last took (a projective engine's generation)
 
 protected:
   size_t n_dst_ = 0, n_src_ = 0;

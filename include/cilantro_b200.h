@@ -411,6 +411,23 @@ typedef enum cb_feature_kind {
 int cb_icp_set_features(cb_icp* icp, int kind, const float* dst_normals, const float* dst_colors,
                         const float* src_normals, const float* src_colors, float normal_weight, float color_weight);
 
+/* Projective correspondence search: CorrespondenceSearchProjective<float> as SimpleCombinedMetricRigidProjectiveICP3f
+ * and the ICPs over that engine take it (correspondence_search/correspondence_search_projective.hpp:156-209). K9 is the
+ * row-major 3 x 3 intrinsic matrix, w x h the image, E12 the row-major 3 x 4 camera pose [R | t] (NULL = identity).
+ * This call builds the index map over the destination cloud (pointsToIndexMap's rule: smallest camera z, lowest index
+ * on ties, non-finite points skipped) and keeps it on the device, 4 B per pixel, until the next call or
+ * cb_icp_destroy. From then on every source point q = T s is matched to the destination point its pixel
+ * (llround of the projection through E^-1 and K) shows, kept iff its squared distance is < max_d2; the list is in
+ * ascending source index and a destination point may be matched many times (DESIGN §4.21). cb_icp_estimate,
+ * cb_icp_accumulate and cb_icp_correspondences honour it, with inlier_fraction < 1 applied as
+ * filterCorrespondencesFraction; cb_icp_residuals stays the kd-tree search, as the reference's computeResiduals;
+ * cb_icp_loop_cache returns CB_ERR_INVALID after a projective run. K9 = NULL detaches the projection and restores the
+ * kd-tree paths. w or h = 0: no correspondences. CB_ERR_INVALID: non-finite K9 or E12, w h >= 2^32, and at
+ * cb_icp_estimate / cb_icp_accumulate a search_dir other than CB_SECOND_TO_FIRST, require_reciprocal, one_to_one or
+ * features attached. Several ranks: CB_ERR_UNSUPPORTED. On an error the projection attached before the call (or none)
+ * stays in force. Launches: 3 (2 for an empty destination cloud). */
+int cb_icp_set_projection(cb_icp* icp, const float* K9, size_t w, size_t h, const float* E12);
+
 /* Host-only O(1) solves (no device needed; exported so the N>1 logic is testable on CPU). */
 /* estimateTransformPointToPointMetric from moments — transform_estimation.hpp:25-47. Returns 1 if n>=3. */
 int cb_solve_kabsch_moments(const double* sums16, float* T12);

@@ -173,6 +173,14 @@ def main():
     want = depth_images_ref.points_to_depth_image(pts, depth_images_ref.K_GENERAL, 45, 19, scale=1000.0)
     assert np.array_equal(d, want), "z-buffer"
     capi.points_to_index_map(ctx, pts, depth_images_ref.K_GENERAL, 45, 19)
+    # projective ICP: the index map build, the per-query search (host loop, list path) and the device loop's pass
+    moved = (pts + np.float32(0.002)).astype(np.float32)
+    picp = capi.Icp(ctx, capi.Cloud(ctx, pts, got["normals"]), capi.Cloud(ctx, moved))
+    picp.set_projection(depth_images_ref.K_GENERAL, 45, 19)
+    for kw in (dict(metric="p2p"), dict(metric="combined", w_pt=0.1), dict(metric="combined", host_loop=True),
+               dict(metric="p2p", inlier_fraction=0.5)):
+        picp.estimate(max_iter=3, max_d2=np.float32(0.01), **kw)
+    picp.correspondences()
     ctx.close()
     print("sanitize target: all checks passed")
 
