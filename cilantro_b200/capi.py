@@ -233,10 +233,10 @@ EXPORTED = [
     "cb_ransac_score", "cb_ransac_residuals", "cb_ransac_rigid",
     "cb_plane_score", "cb_plane_residuals", "cb_ransac_plane",
     "cb_warp_default_params", "cb_warp_icp_create", "cb_warp_icp_destroy", "cb_warp_icp_estimate", "cb_warp_icp_solve",
-    "cb_warp_icp_residuals", "cb_warp_icp_correspondences",
+    "cb_warp_icp_residuals", "cb_warp_icp_correspondences", "cb_warp_icp_set_projection",
     "cb_sparse_warp_default_params", "cb_sparse_warp_icp_create", "cb_sparse_warp_icp_destroy",
     "cb_sparse_warp_icp_estimate", "cb_sparse_warp_icp_solve", "cb_sparse_warp_icp_resample",
-    "cb_sparse_warp_icp_residuals", "cb_sparse_warp_icp_correspondences",
+    "cb_sparse_warp_icp_residuals", "cb_sparse_warp_icp_correspondences", "cb_sparse_warp_icp_set_projection",
     "cb_mean_cov", "cb_pca", "cb_transform_points",
     "cb_vectors_mean_cov", "cb_vectors_pca", "cb_vectors_project", "cb_vectors_reconstruct",
     "cb_vectors_mds",
@@ -952,9 +952,10 @@ def _t_set(T, n):
 
 
 class _WarpIcpBase(_Handle):
-    """What WarpIcp and SparseWarpIcp share: the last estimate's correspondences and solve() on given ones."""
+    """What WarpIcp and SparseWarpIcp share: the last estimate's correspondences, solve() on given ones and the
+    projective search."""
 
-    _entries = None  # the names of the object's cb_*_solve and cb_*_correspondences entries
+    _entries = None  # the names of the object's cb_*_solve, cb_*_correspondences and cb_*_set_projection entries
 
     def _solve(self, prm, first, second, T_src, m):
         # m unknown blocks; T_src holds one transform per source point
@@ -979,12 +980,20 @@ class _WarpIcpBase(_Handle):
         c = cnt.value
         return i1[:c].astype(np.int64), i2[:c].astype(np.int64), v[:c]
 
+    def set_projection(self, K, w, h, extrinsics=None):
+        """cb_*warp_icp_set_projection: match each warped point to the destination point its pixel shows in a w x h
+        image with intrinsics K (3 x 3) seen from the camera pose `extrinsics` ([R | t], 3 x 4; None = identity), as
+        the Projective warp-field ICPs do. K = None detaches the projection (the grid search again)."""
+        Kp = None if K is None else np.ascontiguousarray(np.asarray(K, np.float32).reshape(3, 3))
+        E = None if extrinsics is None else _T(extrinsics)
+        _check(getattr(lib(), self._entries[2])(self.h, _p(Kp), C.c_size_t(int(w)), C.c_size_t(int(h)), _p(E)))
+
 
 class WarpIcp(_WarpIcpBase):
     """cb_warp_icp_*: SimpleCombinedMetricDenseRigidWarpFieldICP3f. Transforms are (n_src, 3, 4) float32."""
 
     _destroy = "cb_warp_icp_destroy"
-    _entries = ("cb_warp_icp_solve", "cb_warp_icp_correspondences")
+    _entries = ("cb_warp_icp_solve", "cb_warp_icp_correspondences", "cb_warp_icp_set_projection")
 
     def __init__(self, ctx, dst: Cloud, src: Cloud, reg_offsets, reg_index, reg_value):
         self.ctx, self.dst, self.src = ctx, dst, src
@@ -1035,7 +1044,8 @@ class SparseWarpIcp(_WarpIcpBase):
     and dense transforms (n_src, 3, 4) float32."""
 
     _destroy = "cb_sparse_warp_icp_destroy"
-    _entries = ("cb_sparse_warp_icp_solve", "cb_sparse_warp_icp_correspondences")
+    _entries = ("cb_sparse_warp_icp_solve", "cb_sparse_warp_icp_correspondences",
+                "cb_sparse_warp_icp_set_projection")
 
     def __init__(self, ctx, dst: Cloud, src: Cloud, ctrl, n_ctrl, reg):
         self.ctx, self.dst, self.src, self.n_ctrl = ctx, dst, src, int(n_ctrl)

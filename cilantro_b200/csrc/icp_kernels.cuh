@@ -2,6 +2,7 @@
 #pragma once
 #include "cb_internal.hpp"
 #include "nn_search.cuh"
+#include "projection.hpp"
 
 namespace cb {
 
@@ -60,5 +61,17 @@ int launch_transform_points(cb_context* ctx, const Rigid& T, const float* d_in, 
 // out_val[orig(p)] = nn_d2[p] (nullable) - the getters' translation from sorted positions to caller indices.
 int launch_translate_matches(cb_context* ctx, const int* nn_pos, const float* nn_d2, const float4* src_pts,
                              const float4* dst_pts, uint32_t n_src, int* out_first, float* out_val);
+
+// Projective correspondence search (projective_search.cu). Per source point of the cloud src_pts (.w = original index
+// bits), under T: nn_pos / nn_d2 by position in src_pts (the destination's sorted position, -1 none), out_idx / out_d2
+// by original index (the destination's original index, -1 none); every output is nullable.
+int launch_projective_search(cb_context* ctx, const ProjectiveMap& pm, const float4* src_pts, uint32_t n_src,
+                             const float4* dst_pts, const Rigid& T, float max_d2, int* nn_pos, float* nn_d2,
+                             int* out_idx, float* out_d2);
+// The index map of the projection (K9 row-major 3 x 3, E12 row-major [R | t] or nullptr, w x h pixels) over the indexed
+// cloud dst, into *out (on, its d_map owned by `owner`). Non-finite K or E, or w * h >= 2^32, give CB_ERR_INVALID; on
+// any error *out is untouched and nothing stays allocated. Synchronises the stream.
+int build_projective_map(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const float* K9, size_t w, size_t h,
+                         const float* E12, ProjectiveMap* out);
 
 }  // namespace cb

@@ -34,13 +34,6 @@ struct LoopState {
   unsigned long long trace[64][6];
 };
 
-// The projective correspondence search attached by cb_icp_set_projection (projective_search.cu, DESIGN §4.21).
-struct ProjectiveMap {
-  bool on = false;
-  Projection prj;
-  int* d_map = nullptr;  // w * h: sorted position of the destination point each pixel shows, -1 empty (owned by cb_icp)
-};
-
 }  // namespace cb
 
 struct cb_icp {
@@ -92,12 +85,6 @@ namespace cb {
 int icp_loop_estimate(cb_icp* icp, const cb_icp_params* prm, cb_icp_result* res, int* hand_over);
 unsigned long long exchange_timeout_ns();
 
-// Projective correspondence search (projective_search.cu). Per source point of the cell-sorted cloud src_pts, under T:
-// nn_pos / nn_d2 by sorted position (the destination's sorted position, -1 none), out_idx / out_d2 by original index
-// (the destination's original index, -1 none); every output is nullable.
-int launch_projective_search(cb_context* ctx, const ProjectiveMap& pm, const float4* src_pts, uint32_t n_src,
-                             const float4* dst_pts, const Rigid& T, float max_d2, int* nn_pos, float* nn_d2,
-                             int* out_idx, float* out_d2);
 // The z-buffer of the index map (depth_images.cu): keys (w * h) = (bits of camera z << 32 | index) of each pixel's
 // winner among the n packed points at d_pts, ~0 where none lands.
 int index_map_keys(cb_context* ctx, const float* d_pts, size_t n, const Projection& prj, unsigned long long* keys);

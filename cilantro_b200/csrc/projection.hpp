@@ -17,6 +17,15 @@ struct Projection {
   uint32_t w, h;
 };
 
+// A projective correspondence search attached to an ICP object (cb_icp_set_projection, cb_warp_icp_set_projection,
+// cb_sparse_warp_icp_set_projection; built by build_projective_map in projective_search.cu, DESIGN §4.21, §4.22).
+struct ProjectiveMap {
+  bool on = false;
+  Projection prj;
+  int* d_map = nullptr;  // w * h: sorted position of the destination point each pixel shows, -1 empty (owned by the
+                         // object)
+};
+
 namespace rule {
 #if defined(__CUDA_ARCH__)
 CB_RULE_HD float div_rn(float a, float b) { return __fdiv_rn(a, b); }

@@ -1,14 +1,16 @@
 // Projective correspondence search of rigid ICP (CorrespondenceSearchProjective, correspondence_search/
 // correspondence_search_projective.hpp:156-209) under the contract of DESIGN §4.21 (product code, sm_90a).
 //
-// cb_icp_set_projection builds the index map over the destination cloud ONCE: the z-buffer of pointsToIndexMap
+// build_projective_map builds the index map over the destination cloud ONCE per attach (cb_icp_set_projection and the
+// warp-field objects' set_projection, warp_field_common.cuh): the z-buffer of pointsToIndexMap
 // (depth_images.cu, index_map_keys: smallest camera z, lowest original index on ties, non-finite points skipped), then
 // one pass turns each pixel's winner into its position in the destination's cell-sorted arrays (4 B per pixel, -1
 // empty), so that the passes gather from the same arrays as the kd-tree paths. Per source point the search is O(1):
 // q = T s (rule::transform_point), the pixel q lands in (project_pixel, projection.hpp), one map read and the contract
 // distance to that one destination point, kept iff d2 < max_d2.
 //   launch_projective_search  per-query result: the host-driven loop's passes (icp_pass_kernel without search) and
-//                             the list path of icp_engine.cu read it
+//                             the list path of icp_engine.cu read it; the warp-field ICPs run it on their warped
+//                             points with the identity (warp_search, DESIGN §4.22)
 //   icp_projective_kernel     the device-resident loop's pass (icp_loop.cu)
 #include "icp_kernels.cuh"
 #include "icp_object.hpp"
@@ -84,39 +86,17 @@ int launch_projective_search(cb_context* ctx, const ProjectiveMap& pm, const flo
                 (const int*)pm.d_map, src_pts, n_src, dst_pts, T, max_d2, nn_pos, nn_d2, out_idx, out_d2);
 }
 
-}  // namespace cb
-
-using namespace cb;
-
-int cb_icp_set_projection(cb_icp* icp, const float* K9, size_t w, size_t h, const float* E12) {
-  CB_CHECK(icp, CB_ERR_INVALID, "null argument");
-  cb_context* ctx = icp->ctx;
-  CB_CHECK(ctx->world == 1, CB_ERR_UNSUPPORTED, "projective correspondence search with several ranks");
-  if (K9) {
-    CB_CHECK(all_finite(K9, 9), CB_ERR_INVALID, "intrinsics are not finite");
-    CB_CHECK(!E12 || all_finite(E12, 12), CB_ERR_INVALID, "extrinsics are not finite");
-    CB_CHECK(w < (1ull << 32) && h < (1ull << 32) && (unsigned __int128)w * h < ((unsigned __int128)1 << 32),
-             CB_ERR_INVALID, "images of >= 2^32 pixels are not supported");
-  }
-  CB_CUDA(cudaSetDevice(ctx->device));
-  // the object's search changes: nothing it found before describes the new one
-  auto replace = [&](const ProjectiveMap& next) -> int {
-    CB_TRY(icp->mem.free(icp->proj.d_map));
-    icp->proj = next;
-    icp->nn_valid = false;
-    icp->nn_stored = false;
-    icp->warm_ok = false;
-    icp->engine_last = false;
-    icp->loop_last = false;
-    return CB_OK;
-  };
-  if (!K9) return replace(ProjectiveMap());  // detached: the kd-tree paths
-  // the new map is built beside the attached one, which stays in force when the build fails
+int build_projective_map(cb_context* ctx, DeviceScope& owner, const cb_cloud* dst, const float* K9, size_t w, size_t h,
+                         const float* E12, ProjectiveMap* out) {
+  CB_CHECK(all_finite(K9, 9), CB_ERR_INVALID, "intrinsics are not finite");
+  CB_CHECK(!E12 || all_finite(E12, 12), CB_ERR_INVALID, "extrinsics are not finite");
+  CB_CHECK(w < (1ull << 32) && h < (1ull << 32) && (unsigned __int128)w * h < ((unsigned __int128)1 << 32),
+           CB_ERR_INVALID, "images of >= 2^32 pixels are not supported");
   ProjectiveMap pm;
   pm.on = true;
   pm.prj = make_projection(K9, E12, (uint32_t)w, (uint32_t)h);
-  const size_t npix = w * h, nd = icp->dst->n;
-  CB_TRY(icp->mem.alloc(&pm.d_map, npix));
+  const size_t npix = w * h, nd = dst->n;
+  CB_TRY(owner.alloc(&pm.d_map, npix));
   auto build = [&]() -> int {
     if (npix == 0) return CB_OK;  // no pixel: no correspondences
     DeviceScope scope(ctx);
@@ -124,9 +104,9 @@ int cb_icp_set_projection(cb_icp* icp, const float* K9, size_t w, size_t h, cons
     uint32_t* inv = nullptr;
     CB_TRY(scope.alloc(&keys, npix));
     CB_TRY(scope.alloc(&inv, nd));
-    CB_TRY(index_map_keys(ctx, icp->dst->d_raw, nd, pm.prj, keys));
+    CB_TRY(index_map_keys(ctx, dst->d_raw, nd, pm.prj, keys));
     if (nd)
-      CB_TRY(launch(ctx, inverse_order_kernel, grid_for(ctx, nd, kThreads), kThreads, 0, (const float4*)icp->dst->d_pts,
+      CB_TRY(launch(ctx, inverse_order_kernel, grid_for(ctx, nd, kThreads), kThreads, 0, (const float4*)dst->d_pts,
                     (uint32_t)nd, inv));
     CB_TRY(launch(ctx, index_map_positions_kernel, grid_for(ctx, npix, kThreads), kThreads, 0,
                   (const unsigned long long*)keys, npix, (const uint32_t*)inv, pm.d_map));
@@ -135,8 +115,32 @@ int cb_icp_set_projection(cb_icp* icp, const float* K9, size_t w, size_t h, cons
   };
   const int rc = build();
   if (rc != CB_OK) {
-    icp->mem.free(pm.d_map);
+    owner.free(pm.d_map);
     return rc;
   }
-  return replace(pm);
+  *out = pm;
+  return CB_OK;
+}
+
+}  // namespace cb
+
+using namespace cb;
+
+int cb_icp_set_projection(cb_icp* icp, const float* K9, size_t w, size_t h, const float* E12) {
+  CB_CHECK(icp, CB_ERR_INVALID, "null argument");
+  cb_context* ctx = icp->ctx;
+  CB_CHECK(ctx->world == 1, CB_ERR_UNSUPPORTED, "projective correspondence search with several ranks");
+  CB_CUDA(cudaSetDevice(ctx->device));
+  // the new map is built beside the attached one, which stays in force when the build fails
+  ProjectiveMap next;  // K9 == NULL: detached, the kd-tree paths
+  if (K9) CB_TRY(build_projective_map(ctx, icp->mem, icp->dst, K9, w, h, E12, &next));
+  // the object's search changes: nothing it found before describes the new one
+  CB_TRY(icp->mem.free(icp->proj.d_map));
+  icp->proj = next;
+  icp->nn_valid = false;
+  icp->nn_stored = false;
+  icp->warm_ok = false;
+  icp->engine_last = false;
+  icp->loop_last = false;
+  return CB_OK;
 }

@@ -14,7 +14,8 @@
 //   * sparse_cg_kernel: one cooperative launch per Gauss-Newton step running the whole CG; its matvec is
 //     P_i = sum_k w_ik p_{n_ik}, y_i = B_i P_i (per point), a grid sync, then q_j = sum w_ij y_i + arcs (per node).
 // The node->(point, slot) incidence is built once, by the stable radix sort keyed by node, so every gather runs in a
-// fixed order. Per ICP iteration: the grid 1-NN of the dense path on the warped points, the Gauss-Newton steps,
+// fixed order. Per ICP iteration: the search of the dense path on the warped points (grid 1-NN, or projective with a
+// projection attached), the Gauss-Newton steps,
 // warp_compose_kernel over the nodes (preApply with projection, the last_delta max) and sparse_resample_kernel (node
 // transforms -> per-point transforms -> warped points for the next search).
 //
@@ -655,6 +656,11 @@ int cb_sparse_warp_icp_residuals(cb_sparse_warp_icp* w, const cb_sparse_warp_par
 int cb_sparse_warp_icp_correspondences(cb_sparse_warp_icp* w, uint64_t* index_first, uint64_t* index_second,
                                        float* value, size_t* count) {
   return warp_correspondences(w, index_first, index_second, value, count);
+}
+
+int cb_sparse_warp_icp_set_projection(cb_sparse_warp_icp* w, const float* K9, size_t width, size_t height,
+                                      const float* E12) {
+  return warp_set_projection(w, K9, width, height, E12);
 }
 
 }  // extern "C"

@@ -13,7 +13,8 @@
 // arcs it is the lower end of), then warp_cg_kernel, one cooperative launch that runs the whole CG loop with grid
 // syncs between the matvec, the dot products and the vector updates, and adds the solution to the unknowns. The host
 // reads one small record per step (the exact max of |delta_i|^2, the CG iteration count). Per ICP iteration the
-// search is the grid 1-NN of the ICP pass kernel on the warped points, and warp_compose_kernel turns the unknowns into
+// search is the grid 1-NN of the ICP pass kernel on the warped points (or, with a projection attached, the projective
+// search of rigid ICP, DESIGN §4.22), and warp_compose_kernel turns the unknowns into
 // transforms, applies them and warps the points for the next search.
 //
 // Arithmetic: vectors, blocks and the assembly are fp32 like the reference's scalar type, every operation rounded on
@@ -316,6 +317,10 @@ int cb_warp_icp_residuals(cb_warp_icp* w, const cb_warp_params* p, const float* 
 int cb_warp_icp_correspondences(cb_warp_icp* w, uint64_t* index_first, uint64_t* index_second, float* value,
                                 size_t* count) {
   return warp_correspondences(w, index_first, index_second, value, count);
+}
+
+int cb_warp_icp_set_projection(cb_warp_icp* w, const float* K9, size_t width, size_t height, const float* E12) {
+  return warp_set_projection(w, K9, width, height, E12);
 }
 
 }  // extern "C"

@@ -515,6 +515,7 @@ struct WarpCore {
   WarpStats* h_stats = nullptr;  // pinned
   int cg_grid = 0;
   bool have_corr = false;
+  ProjectiveMap proj;  // set_projection: warp_search is projective while proj.on (DESIGN §4.22)
 };
 
 int check_params(const WarpCore* w, const cb_warp_params* p) {
@@ -657,9 +658,14 @@ int upload_arc_incidence(WarpCore* w, const std::vector<uint32_t>& lo, const std
   return CB_OK;
 }
 
-// The grid 1-NN of the ICP pass kernel on the warped points: nn[i] = destination index within max_d2, or -1.
+// updateCorrespondences on the warped points: nn[i] = destination index within max_d2, or -1. With a projection
+// attached, the projective search of rigid ICP (projective_search.cu) on the warped points under the identity; else
+// the grid 1-NN of the ICP pass kernel.
 int warp_search(const WarpCore* w, float max_d2) {
   if (w->n == 0) return CB_OK;
+  if (w->proj.on)
+    return launch_projective_search(w->ctx, w->proj, w->d_warped, w->n, w->dst->d_pts, rigid_from_t12(nullptr), max_d2,
+                                    nullptr, nullptr, w->d_nn, w->d_nn_d2);
   IcpArgs a{};
   a.dst = grid_view(w->dst);
   a.src_pts = w->d_warped;
@@ -670,6 +676,19 @@ int warp_search(const WarpCore* w, float max_d2) {
   a.out_idx = w->d_nn;
   a.out_d2 = w->d_nn_d2;
   return launch_icp_pass(w->ctx, a, kModeKnn, true, false, false);
+}
+
+// cb_warp_icp_set_projection / cb_sparse_warp_icp_set_projection: K9 attaches the projective search (the index map
+// over the destination is built here, once), NULL detaches it. On any error the attached search stays in force.
+int warp_set_projection(WarpCore* w, const float* K9, size_t width, size_t height, const float* E12) {
+  CB_CHECK(w, CB_ERR_INVALID, "null argument");
+  CB_CUDA(cudaSetDevice(w->ctx->device));
+  ProjectiveMap next;  // K9 == NULL: detached, the grid search
+  if (K9) CB_TRY(build_projective_map(w->ctx, w->mem, w->dst, K9, width, height, E12, &next));
+  CB_TRY(w->mem.free(w->proj.d_map));
+  w->proj = next;
+  w->have_corr = false;  // the last list came from the other search
+  return CB_OK;
 }
 
 // computeResiduals() of both warp-field ICP classes on the warped points (see cb_warp_icp_residuals).

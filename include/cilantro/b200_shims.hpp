@@ -1033,11 +1033,27 @@ inline void transformPoints(const TransformSet<RigidTransform3f>& tforms, const 
 }
 
 namespace b200 {
+// The correspondence engine a warp-field ICP drop-in owns, built from its point sets before the rest of the object (the
+// order of the reference's Simple*WarpFieldICPWrapper). This one is the kd-tree engine: settings only, nothing to
+// attach. The projective engine's is in correspondence_search/correspondence_search_projective.hpp.
+template <class Engine>
+struct WarpEngine {
+  WarpEngine(const ConstVectorSetMatrixMap3f&, const ConstVectorSetMatrixMap3f&) {}
+  const CorrespondenceSearchEngineB200& settings() const { return engine; }
+  // estimate(): hands the engine's search space to the object through its set_projection entry
+  template <class Entry, class Handle>
+  void attach(Entry, Handle*, const char*) {}
+  // getCorrespondences(): the last estimate's list, for the engine's own getter
+  void publish(const CorrespondenceSet<float, size_t>&) {}
+  Engine engine;
+};
+
 // The surface both warp-field ICP drop-ins share: IterativeClosestPointBase (registration/icp_base.hpp:40-106) and
 // CombinedMetric*WarpFieldICP over their cb_warp_params, the correspondence engine and evaluators, the dst/src cloud
 // pair and the last estimate's correspondences. Setters return Derived, so calls chain as in the reference. Result is
-// the C result record (iterations, last_delta, cg_iterations); the transforms are one per unknown block.
-template <class Derived, class Result>
+// the C result record (iterations, last_delta, cg_iterations); the transforms are one per unknown block. Engine: the
+// kd-tree engine's settings (CorrespondenceSearchEngineB200) or CorrespondenceSearchProjective<float>.
+template <class Derived, class Result, class Engine = CorrespondenceSearchEngineB200>
 class WarpFieldICP {
 public:
   using Transform = TransformSet<RigidTransform3f>;
@@ -1048,7 +1064,7 @@ public:
   WarpFieldICP(const WarpFieldICP&) = delete;
   WarpFieldICP& operator=(const WarpFieldICP&) = delete;
 
-  CorrespondenceSearchEngineB200& correspondenceSearchEngine() { return engine_; }
+  Engine& correspondenceSearchEngine() { return engine_.engine; }
   PointToPointCorrespondenceWeightEvaluator& pointToPointCorrespondenceWeightEvaluator() { return pt_eval_; }
   PointToPlaneCorrespondenceWeightEvaluator& pointToPlaneCorrespondenceWeightEvaluator() { return pl_eval_; }
   RegularizationWeightEvaluator& regularizationWeightEvaluator() { return reg_eval_; }
@@ -1128,7 +1144,7 @@ protected:
   // p: the derived class's cb_warp_params (filled by it); n_blocks: the transforms' count
   WarpFieldICP(cb_warp_params& p, const ConstVectorSetMatrixMap3f& dst_p, const ConstVectorSetMatrixMap3f& dst_n,
                const ConstVectorSetMatrixMap3f& src_p, size_t n_blocks)
-      : n_src_(src_p.cols()), p_(p) {
+      : engine_(dst_p, src_p), n_src_(src_p.cols()), p_(p) {
     const float* dn = (dst_n.cols() == dst_p.cols() && dst_p.cols() > 0) ? dst_n.data() : nullptr;
     check(cb_cloud_create_pair(Context::get(), dst_p.data(), dn, dst_p.cols(), 0, src_p.data(), nullptr,
                                src_p.cols(), 0, &dst_.h, &src_.h),
@@ -1160,7 +1176,7 @@ protected:
   void fill() {
     cb_icp_params e;
     cb_icp_default_params(&e);
-    engine_.fill(e);
+    engine_.settings().fill(e);
     p_.max_d2 = e.max_d2;
     p_.search_dir = e.search_dir;
     p_.inlier_fraction = e.inlier_fraction;
@@ -1182,159 +1198,167 @@ protected:
       corr_.resize(cnt);
       for (size_t i = 0; i < cnt; i++) corr_[i] = {(size_t)a[i], (size_t)b[i], v[i]};
       corr_fresh_ = true;
+      engine_.publish(corr_);
     }
     return corr_;
   }
 
+  WarpEngine<Engine> engine_;  // first: built before the clouds, as the reference builds its engine before the ICP
   size_t n_src_;
   CloudHandle dst_, src_;
   cb_warp_params& p_;
   Result res_;
   Transform transform_init_, transform_;
-  CorrespondenceSearchEngineB200 engine_;
   PointToPointCorrespondenceWeightEvaluator pt_eval_;
   PointToPlaneCorrespondenceWeightEvaluator pl_eval_;
   RegularizationWeightEvaluator reg_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
   CorrespondenceSet<float, size_t> corr_;
   bool corr_fresh_ = false;
 };
-}  // namespace b200
 
-// ---- SimpleCombinedMetricDenseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:99-144, 284-285) ----------
 // CombinedMetricDenseWarpFieldICP<RigidTransform<float,3>> (icp_warp_field_combined_metric_dense.hpp) with the Simple
 // instance's evaluators (unity data-term weights, RBFKernelWeightEvaluator<float, float, true> regularisation weights)
-// on cb_warp_icp_* (DESIGN §4.13). The correspondence engine takes the default settings only; another search
-// direction, reciprocity, one-to-one or fraction makes estimate() throw (CB_ERR_UNSUPPORTED).
-class SimpleCombinedMetricDenseRigidWarpFieldICP3f
-    : public b200::WarpFieldICP<SimpleCombinedMetricDenseRigidWarpFieldICP3f, cb_warp_result> {
+// on cb_warp_icp_* (DESIGN §4.13) over the correspondence engine Engine. The engine takes the default settings only;
+// another search direction, reciprocity, one-to-one or fraction makes estimate() throw (CB_ERR_UNSUPPORTED).
+template <class Derived, class Engine = CorrespondenceSearchEngineB200>
+class DenseRigidWarpFieldICP3f : public WarpFieldICP<Derived, cb_warp_result, Engine> {
+  using Base = WarpFieldICP<Derived, cb_warp_result, Engine>;
+
 public:
-  using WarpFieldICP::estimate;
+  using Base::estimate;
 
   // regularization_neighborhoods: one list per neighbourhood, N[0] the centre (what KDTree3f<>::search returns)
   template <typename IndexT>
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f(const ConstVectorSetMatrixMap3f& dst_p,
-                                               const ConstVectorSetMatrixMap3f& dst_n,
-                                               const ConstVectorSetMatrixMap3f& src_p,
-                                               const std::vector<NeighborSet<float, IndexT>>& regularization_neighborhoods)
-      : WarpFieldICP(prm_, dst_p, dst_n, src_p, src_p.cols()) {
+  DenseRigidWarpFieldICP3f(const ConstVectorSetMatrixMap3f& dst_p, const ConstVectorSetMatrixMap3f& dst_n,
+                           const ConstVectorSetMatrixMap3f& src_p,
+                           const std::vector<NeighborSet<float, IndexT>>& regularization_neighborhoods)
+      : Base(prm_, dst_p, dst_n, src_p, src_p.cols()) {
     std::vector<uint64_t> off;
     std::vector<int64_t> idx;
     std::vector<float> val;
-    csr(regularization_neighborhoods, off, idx, val);
-    b200::check(cb_warp_icp_create(b200::Context::get(), dst_.h, src_.h, off.data(), idx.data(), val.data(),
-                                   regularization_neighborhoods.size(), &icp_),
-                "cb_warp_icp_create");
+    Base::csr(regularization_neighborhoods, off, idx, val);
+    check(cb_warp_icp_create(Context::get(), this->dst_.h, this->src_.h, off.data(), idx.data(), val.data(),
+                             regularization_neighborhoods.size(), &icp_),
+          "cb_warp_icp_create");
     cb_warp_default_params(&prm_);
   }
-  ~SimpleCombinedMetricDenseRigidWarpFieldICP3f() {
+  ~DenseRigidWarpFieldICP3f() {
     if (icp_) cb_warp_icp_destroy(icp_);
   }
 
-  SimpleCombinedMetricDenseRigidWarpFieldICP3f& estimate() {
-    if (transform_init_.size() != n_src_) throw std::runtime_error("initial transform: one transform per source point expected");
-    fill();
-    std::vector<float> T_in(12 * n_src_), T_out(12 * n_src_);
-    for (size_t i = 0; i < n_src_; i++) std::memcpy(&T_in[12 * i], transform_init_[i].data(), 12 * sizeof(float));
-    b200::check(cb_warp_icp_estimate(icp_, &prm_, T_in.data(), T_out.data(), &res_), "cb_warp_icp_estimate");
-    transform_.resize(n_src_);
-    for (size_t i = 0; i < n_src_; i++) transform_[i] = RigidTransform3f(&T_out[12 * i]);
-    corr_fresh_ = false;
-    return *this;
+  Derived& estimate() {
+    const size_t n = this->n_src_;
+    if (this->transform_init_.size() != n) throw std::runtime_error("initial transform: one transform per source point expected");
+    this->engine_.attach(cb_warp_icp_set_projection, icp_, "cb_warp_icp_set_projection");
+    this->fill();
+    std::vector<float> T_in(12 * n), T_out(12 * n);
+    for (size_t i = 0; i < n; i++) std::memcpy(&T_in[12 * i], this->transform_init_[i].data(), 12 * sizeof(float));
+    check(cb_warp_icp_estimate(icp_, &prm_, T_in.data(), T_out.data(), &this->res_), "cb_warp_icp_estimate");
+    this->transform_.resize(n);
+    for (size_t i = 0; i < n; i++) this->transform_[i] = RigidTransform3f(&T_out[12 * i]);
+    this->corr_fresh_ = false;
+    return this->self();
   }
 
   // getResiduals() -> computeResiduals() (icp_warp_field_combined_metric_dense.hpp:216-236): 1 x N_src
   std::vector<float> getResiduals() {
-    fill();
-    std::vector<float> T(12 * n_src_), r(n_src_);
-    for (size_t i = 0; i < n_src_ && i < transform_.size(); i++) std::memcpy(&T[12 * i], transform_[i].data(), 12 * sizeof(float));
-    b200::check(cb_warp_icp_residuals(icp_, &prm_, T.data(), r.data()), "cb_warp_icp_residuals");
+    this->fill();
+    const size_t n = this->n_src_;
+    std::vector<float> T(12 * n), r(n);
+    for (size_t i = 0; i < n && i < this->transform_.size(); i++)
+      std::memcpy(&T[12 * i], this->transform_[i].data(), 12 * sizeof(float));
+    check(cb_warp_icp_residuals(icp_, &prm_, T.data(), r.data()), "cb_warp_icp_residuals");
     return r;
   }
 
   const CorrespondenceSet<float, size_t>& getCorrespondences() {
-    return correspondences(cb_warp_icp_correspondences, icp_, "cb_warp_icp_correspondences");
+    return this->correspondences(cb_warp_icp_correspondences, icp_, "cb_warp_icp_correspondences");
   }
 
-  double getLastEstimateDeviceMilliseconds() const { return res_.gpu_ms_search + res_.gpu_ms_solve; }
+  double getLastEstimateDeviceMilliseconds() const { return this->res_.gpu_ms_search + this->res_.gpu_ms_solve; }
 
 private:
   cb_warp_icp* icp_ = nullptr;
   cb_warp_params prm_;
 };
 
-// ---- SimpleCombinedMetricSparseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:146-199, 313-314) ---------
 // CombinedMetricSparseWarpFieldICP<RigidTransform<float,3>> (icp_warp_field_combined_metric_sparse.hpp) with the Simple
 // instance's evaluators (unity data-term weights, RBFKernelWeightEvaluator<float, float, true> control and
-// regularisation weights) on cb_sparse_warp_icp_* (DESIGN §4.14). getTransform() holds one transform per control
-// node, getDenseWarpField() one per source point. The correspondence engine takes the default settings only.
-class SimpleCombinedMetricSparseRigidWarpFieldICP3f
-    : public b200::WarpFieldICP<SimpleCombinedMetricSparseRigidWarpFieldICP3f, cb_sparse_warp_result> {
+// regularisation weights) on cb_sparse_warp_icp_* (DESIGN §4.14) over the correspondence engine Engine. getTransform()
+// holds one transform per control node, getDenseWarpField() one per source point. The engine takes the default
+// settings only.
+template <class Derived, class Engine = CorrespondenceSearchEngineB200>
+class SparseRigidWarpFieldICP3f : public WarpFieldICP<Derived, cb_sparse_warp_result, Engine> {
+  using Base = WarpFieldICP<Derived, cb_sparse_warp_result, Engine>;
+
 public:
+  using Transform = typename Base::Transform;
   using ControlWeightEvaluator = RBFKernelWeightEvaluator<float, float, true>;
-  using WarpFieldICP::estimate;
+  using Base::estimate;
 
   // src_to_control_nn: one list of (node, squared distance) per source point; regularization_nn: one list per node
   // neighbourhood, N[0] the centre (what KDTree<float, 3>::search over the nodes returns)
   template <typename IndexT, typename RegIndexT>
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f(const ConstVectorSetMatrixMap3f& dst_p,
-                                                const ConstVectorSetMatrixMap3f& dst_n,
-                                                const ConstVectorSetMatrixMap3f& src_p,
-                                                const std::vector<NeighborSet<float, IndexT>>& src_to_control_nn,
-                                                size_t num_control_nodes,
-                                                const std::vector<NeighborSet<float, RegIndexT>>& regularization_nn)
-      : WarpFieldICP(prm_.base, dst_p, dst_n, src_p, num_control_nodes), n_ctrl_(num_control_nodes) {
+  SparseRigidWarpFieldICP3f(const ConstVectorSetMatrixMap3f& dst_p, const ConstVectorSetMatrixMap3f& dst_n,
+                            const ConstVectorSetMatrixMap3f& src_p,
+                            const std::vector<NeighborSet<float, IndexT>>& src_to_control_nn, size_t num_control_nodes,
+                            const std::vector<NeighborSet<float, RegIndexT>>& regularization_nn)
+      : Base(prm_.base, dst_p, dst_n, src_p, num_control_nodes), n_ctrl_(num_control_nodes) {
     std::vector<uint64_t> coff, roff;
     std::vector<int64_t> cidx, ridx;
     std::vector<float> cval, rval;
-    csr(src_to_control_nn, coff, cidx, cval);
-    csr(regularization_nn, roff, ridx, rval);
-    b200::check(cb_sparse_warp_icp_create(b200::Context::get(), dst_.h, src_.h, coff.data(), cidx.data(), cval.data(),
-                                          src_to_control_nn.size(), n_ctrl_, roff.data(), ridx.data(), rval.data(),
-                                          regularization_nn.size(), &icp_),
-                "cb_sparse_warp_icp_create");
+    Base::csr(src_to_control_nn, coff, cidx, cval);
+    Base::csr(regularization_nn, roff, ridx, rval);
+    check(cb_sparse_warp_icp_create(Context::get(), this->dst_.h, this->src_.h, coff.data(), cidx.data(), cval.data(),
+                                    src_to_control_nn.size(), n_ctrl_, roff.data(), ridx.data(), rval.data(),
+                                    regularization_nn.size(), &icp_),
+          "cb_sparse_warp_icp_create");
     cb_sparse_warp_default_params(&prm_);
-    transform_dense_.assign(n_src_, RigidTransform3f());
+    transform_dense_.assign(this->n_src_, RigidTransform3f());
   }
-  ~SimpleCombinedMetricSparseRigidWarpFieldICP3f() {
+  ~SparseRigidWarpFieldICP3f() {
     if (icp_) cb_sparse_warp_icp_destroy(icp_);
   }
 
   ControlWeightEvaluator& controlWeightEvaluator() { return ctrl_eval_; }
   const Transform& getDenseWarpField() const { return transform_dense_; }
 
-  SimpleCombinedMetricSparseRigidWarpFieldICP3f& estimate() {
-    if (transform_init_.size() != n_ctrl_) throw std::runtime_error("initial transform: one transform per control node expected");
+  Derived& estimate() {
+    const size_t n = this->n_src_;
+    if (this->transform_init_.size() != n_ctrl_) throw std::runtime_error("initial transform: one transform per control node expected");
+    this->engine_.attach(cb_sparse_warp_icp_set_projection, icp_, "cb_sparse_warp_icp_set_projection");
     fill();
-    std::vector<float> T_in(12 * n_ctrl_), T_out(12 * n_ctrl_), T_dense(12 * n_src_);
-    for (size_t j = 0; j < n_ctrl_; j++) std::memcpy(&T_in[12 * j], transform_init_[j].data(), 12 * sizeof(float));
-    b200::check(cb_sparse_warp_icp_estimate(icp_, &prm_, T_in.data(), T_out.data(), T_dense.data(), &res_),
-                "cb_sparse_warp_icp_estimate");
-    for (size_t j = 0; j < n_ctrl_; j++) transform_[j] = RigidTransform3f(&T_out[12 * j]);
-    for (size_t i = 0; i < n_src_; i++) transform_dense_[i] = RigidTransform3f(&T_dense[12 * i]);
-    corr_fresh_ = false;
-    return *this;
+    std::vector<float> T_in(12 * n_ctrl_), T_out(12 * n_ctrl_), T_dense(12 * n);
+    for (size_t j = 0; j < n_ctrl_; j++) std::memcpy(&T_in[12 * j], this->transform_init_[j].data(), 12 * sizeof(float));
+    check(cb_sparse_warp_icp_estimate(icp_, &prm_, T_in.data(), T_out.data(), T_dense.data(), &this->res_),
+          "cb_sparse_warp_icp_estimate");
+    for (size_t j = 0; j < n_ctrl_; j++) this->transform_[j] = RigidTransform3f(&T_out[12 * j]);
+    for (size_t i = 0; i < n; i++) transform_dense_[i] = RigidTransform3f(&T_dense[12 * i]);
+    this->corr_fresh_ = false;
+    return this->self();
   }
 
   // getResiduals() -> computeResiduals() (icp_warp_field_combined_metric_sparse.hpp:243-263) on the dense field
   std::vector<float> getResiduals() {
     fill();
-    std::vector<float> T(12 * n_src_), r(n_src_);
-    for (size_t i = 0; i < n_src_; i++) std::memcpy(&T[12 * i], transform_dense_[i].data(), 12 * sizeof(float));
-    b200::check(cb_sparse_warp_icp_residuals(icp_, &prm_, T.data(), r.data()), "cb_sparse_warp_icp_residuals");
+    const size_t n = this->n_src_;
+    std::vector<float> T(12 * n), r(n);
+    for (size_t i = 0; i < n; i++) std::memcpy(&T[12 * i], transform_dense_[i].data(), 12 * sizeof(float));
+    check(cb_sparse_warp_icp_residuals(icp_, &prm_, T.data(), r.data()), "cb_sparse_warp_icp_residuals");
     return r;
   }
 
   const CorrespondenceSet<float, size_t>& getCorrespondences() {
-    return correspondences(cb_sparse_warp_icp_correspondences, icp_, "cb_sparse_warp_icp_correspondences");
+    return this->correspondences(cb_sparse_warp_icp_correspondences, icp_, "cb_sparse_warp_icp_correspondences");
   }
 
   double getLastEstimateDeviceMilliseconds() const {
-    return res_.gpu_ms_search + res_.gpu_ms_resample + res_.gpu_ms_assemble + res_.gpu_ms_cg;
+    return this->res_.gpu_ms_search + this->res_.gpu_ms_resample + this->res_.gpu_ms_assemble + this->res_.gpu_ms_cg;
   }
 
 private:
   void fill() {
-    WarpFieldICP::fill();
+    Base::fill();
     prm_.ctrl_coeff = ctrl_eval_.b200_coeff();
   }
   size_t n_ctrl_;
@@ -1342,6 +1366,23 @@ private:
   cb_sparse_warp_params prm_;
   Transform transform_dense_;
   ControlWeightEvaluator ctrl_eval_;  // sigma 1 (common_pair_evaluators.hpp:51)
+};
+}  // namespace b200
+
+// ---- SimpleCombinedMetricDenseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:99-144, 284-285) ----------
+// The dense warp field over the kd-tree engine.
+class SimpleCombinedMetricDenseRigidWarpFieldICP3f
+    : public b200::DenseRigidWarpFieldICP3f<SimpleCombinedMetricDenseRigidWarpFieldICP3f> {
+public:
+  using DenseRigidWarpFieldICP3f::DenseRigidWarpFieldICP3f;
+};
+
+// ---- SimpleCombinedMetricSparseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:146-199, 313-314) ---------
+// The sparse warp field over the kd-tree engine.
+class SimpleCombinedMetricSparseRigidWarpFieldICP3f
+    : public b200::SparseRigidWarpFieldICP3f<SimpleCombinedMetricSparseRigidWarpFieldICP3f> {
+public:
+  using SparseRigidWarpFieldICP3f::SparseRigidWarpFieldICP3f;
 };
 
 // ---- KMeans<float, D> / KMeans2f<> / KMeans3f<> / KMeansXf<> ---------------------------------------------

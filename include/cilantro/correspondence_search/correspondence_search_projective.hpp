@@ -1,8 +1,10 @@
 // Same include path as cilantro's correspondence_search/correspondence_search_projective.hpp: the projective
-// correspondence search as the engine of rigid ICP, and SimpleCombinedMetricRigidProjectiveICP3f
-// (registration/icp_common_instances.hpp:223-270). The search itself runs on the device: estimate() hands the projection
-// to the ICP object (cb_icp_set_projection, DESIGN §4.21), which keeps the index map over the destination on the device
-// and rebuilds it only when a projection setter changed. Only the float instance with PointFeaturesAdaptor3f and
+// correspondence search as the engine of rigid ICP and of the warp-field ICPs, SimpleCombinedMetricRigidProjectiveICP3f
+// (registration/icp_common_instances.hpp:223-270), SimpleCombinedMetricDenseRigidWarpFieldProjectiveICP3f and
+// SimpleCombinedMetricSparseRigidWarpFieldProjectiveICP3f (:233-245, 298-299, 327-328). The search itself runs on the
+// device: estimate() hands the projection to the ICP object (cb_icp_set_projection, cb_warp_icp_set_projection,
+// cb_sparse_warp_icp_set_projection; DESIGN §4.21, §4.22), which keeps the index map over the destination on the
+// device and rebuilds it only when a projection setter changed. Only the float instance with PointFeaturesAdaptor3f and
 // DistanceEvaluator exists; any other ScalarT, evaluation adaptor or evaluator is a compile-time error. Intrinsics are a
 // b200::Intrinsics3f (row-major 3 x 3), converted implicitly from an Eigen::Matrix<float, 3, 3> where Eigen is available.
 #pragma once
@@ -77,13 +79,20 @@ public:
     return *this;
   }
 
-  // b200::EngineRigidICP3f::estimate(): (re)attaches the projection when the ICP object has not taken this state yet
+  // estimate() of an ICP object over this engine: (re)attaches the projection through the object's set_projection
+  // entry when the object has not taken this state yet (attached: the generation it last took)
+  template <class Handle>
+  void b200_attach(int (*entry)(Handle*, const float*, size_t, size_t, const float*), Handle* icp, uint64_t& attached,
+                   const char* what) {
+    if (attached == gen_) return;
+    b200::check(entry(icp, K_.m, w_, h_, E_.data()), what);
+    attached = gen_;
+  }
+  // b200::EngineRigidICP3f::estimate()
   void b200_attach(cb_icp* icp, size_t n_dst, size_t n_src, uint64_t& attached) {
     if (dst_.b200_size() != n_dst || src_.b200_size() != n_src)
       throw std::invalid_argument("cilantro_b200: the engine's point adaptors' sizes differ from the ICP's point sets");
-    if (attached == gen_) return;
-    b200::check(cb_icp_set_projection(icp, K_.m, w_, h_, E_.data()), "cb_icp_set_projection");
-    attached = gen_;
+    b200_attach(cb_icp_set_projection, icp, attached, "cb_icp_set_projection");
   }
   const CorrespondenceSearchEngineB200& b200_settings() const { return settings_; }
   void b200_set_correspondences(const SearchResult& c) { corr_ = c; }
@@ -111,6 +120,24 @@ struct ProjectiveICPEntities3f {
   CorrespondenceSearchProjective<float> corr_search_;
   UnityWeightEvaluator<float, float> point_corr_weight_eval_, plane_corr_weight_eval_;
 };
+
+// The projective engine of a warp-field ICP drop-in, with the adaptors and the evaluator it is built on (see the
+// kd-tree engine's WarpEngine in b200_shims.hpp)
+template <>
+struct WarpEngine<CorrespondenceSearchProjective<float>> {
+  WarpEngine(const ConstVectorSetMatrixMap3f& dst, const ConstVectorSetMatrixMap3f& src)
+      : dst_feat(dst), src_feat(src), engine(dst_feat, src_feat, dist_eval) {}
+  const CorrespondenceSearchEngineB200& settings() const { return engine.b200_settings(); }
+  template <class Handle>
+  void attach(int (*entry)(Handle*, const float*, size_t, size_t, const float*), Handle* icp, const char* what) {
+    engine.b200_attach(entry, icp, attached, what);
+  }
+  void publish(const CorrespondenceSet<float, size_t>& c) { engine.b200_set_correspondences(c); }
+  PointFeaturesAdaptor3f dst_feat, src_feat;
+  DistanceEvaluator<float, float> dist_eval;
+  CorrespondenceSearchProjective<float> engine;
+  uint64_t attached = 0;  // the engine's generation the ICP object last took
+};
 }  // namespace b200
 
 // SimpleCombinedMetricRigidProjectiveICP3f (icp_common_instances.hpp:223-225, :269-270): the combined metric over the
@@ -132,6 +159,24 @@ public:
       : b200::ProjectiveICPEntities3f(dst_points, src_points),
         Base(dst_points, dst_normals, src_points, src_normals, corr_search_, point_corr_weight_eval_,
              plane_corr_weight_eval_) {}
+};
+
+// SimpleCombinedMetricDenseRigidWarpFieldProjectiveICP3f (icp_common_instances.hpp:233-235, :298-299): the dense warp
+// field over the projective search of the warped points, with the constructor of its kd-tree sibling
+class SimpleCombinedMetricDenseRigidWarpFieldProjectiveICP3f
+    : public b200::DenseRigidWarpFieldICP3f<SimpleCombinedMetricDenseRigidWarpFieldProjectiveICP3f,
+                                            CorrespondenceSearchProjective<float>> {
+public:
+  using DenseRigidWarpFieldICP3f::DenseRigidWarpFieldICP3f;
+};
+
+// SimpleCombinedMetricSparseRigidWarpFieldProjectiveICP3f (icp_common_instances.hpp:243-245, :327-328): the sparse warp
+// field over the projective search of the points warped by the dense field, with the constructor of its kd-tree sibling
+class SimpleCombinedMetricSparseRigidWarpFieldProjectiveICP3f
+    : public b200::SparseRigidWarpFieldICP3f<SimpleCombinedMetricSparseRigidWarpFieldProjectiveICP3f,
+                                             CorrespondenceSearchProjective<float>> {
+public:
+  using SparseRigidWarpFieldICP3f::SparseRigidWarpFieldICP3f;
 };
 
 }  // namespace cilantro

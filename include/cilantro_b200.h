@@ -638,6 +638,18 @@ int cb_warp_icp_residuals(cb_warp_icp* icp, const cb_warp_params* prm, const flo
 /* getCorrespondences() after the last iteration of the last estimate(), ascending source index; arrays hold n_src. */
 int cb_warp_icp_correspondences(cb_warp_icp* icp, uint64_t* index_first, uint64_t* index_second, float* value,
                                 size_t* count);
+/* Projective correspondence search for the dense warp field: SimpleCombinedMetricDenseRigidWarpFieldProjectiveICP3f
+ * (registration/icp_common_instances.hpp:233-245, 298-299), whose updateCorrespondences() calls the projective engine's
+ * findCorrespondences(transform_) (correspondence_search/correspondence_search_projective.hpp:68-75, 156-209). K9, w, h
+ * and E12 as in cb_icp_set_projection, whose index map this call builds over the destination cloud and keeps on the
+ * device until the next call or cb_warp_icp_destroy. From then on cb_warp_icp_estimate matches every warped point
+ * T_i s_i to the destination point its pixel shows, kept iff its squared distance is < max_d2: the contract of
+ * DESIGN §4.21 on the warped points (DESIGN §4.22). cb_warp_icp_residuals stays the kd-tree search, as the reference's
+ * computeResiduals. K9 = NULL detaches the projection and restores the grid search. w or h = 0: no correspondences (the
+ * estimate returns identities with last_delta = 0). Non-finite K9 or E12, w h >= 2^32: CB_ERR_INVALID. On an error
+ * the projection attached before the call (or none) stays in force; a successful call makes cb_warp_icp_correspondences
+ * return CB_ERR_INVALID until the next estimate. Launches: 3 (2 for an empty destination cloud). */
+int cb_warp_icp_set_projection(cb_warp_icp* icp, const float* K9, size_t w, size_t h, const float* E12);
 
 /* ---- non-rigid ICP: sparse rigid warp field on control nodes ------------------------------------
  * cb_sparse_warp_icp_* replaces SimpleCombinedMetricSparseRigidWarpFieldICP3f (registration/icp_common_instances.hpp:
@@ -712,6 +724,11 @@ int cb_sparse_warp_icp_residuals(cb_sparse_warp_icp* icp, const cb_sparse_warp_p
 /* getCorrespondences() after the last iteration of the last estimate(), ascending source index; arrays hold n_src. */
 int cb_sparse_warp_icp_correspondences(cb_sparse_warp_icp* icp, uint64_t* index_first, uint64_t* index_second,
                                        float* value, size_t* count);
+/* Projective correspondence search for the sparse warp field: SimpleCombinedMetricSparseRigidWarpFieldProjectiveICP3f
+ * (registration/icp_common_instances.hpp:233-245, 327-328), whose updateCorrespondences() calls the projective engine's
+ * findCorrespondences(transform_dense_) (icp_warp_field_combined_metric_sparse.hpp:208-209). The rules of
+ * cb_warp_icp_set_projection, on the points warped by the resampled dense field. */
+int cb_sparse_warp_icp_set_projection(cb_sparse_warp_icp* icp, const float* K9, size_t w, size_t h, const float* E12);
 
 /* ---- covariance / PCA ------------------------------------------------------------------------
  * Replaces Covariance<float,3>::operator() (core/covariance.hpp:31-80) and

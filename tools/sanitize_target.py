@@ -181,6 +181,17 @@ def main():
                dict(metric="p2p", inlier_fraction=0.5)):
         picp.estimate(max_iter=3, max_d2=np.float32(0.01), **kw)
     picp.correspondences()
+    # projective warp-field ICPs: attach, estimate, re-attach, detach and estimate on the grid search
+    pd, pm = capi.Cloud(ctx, pts, got["normals"]), capi.Cloud(ctx, moved)
+    pnodes = pm.grid_downsample(0.05)
+    for obj in (capi.WarpIcp(ctx, pd, pm, *capi.neighborhood_csr(*capi.knn_radius(ctx, pm, pm, 8))),
+                capi.SparseWarpIcp(ctx, pd, pm, capi.neighborhood_csr(*capi.knn_radius(ctx, pnodes, pm, 4)), pnodes.n,
+                                   capi.neighborhood_csr(*capi.knn_radius(ctx, pnodes, pnodes, 8)))):
+        for K9, pw in ((depth_images_ref.K_GENERAL, 45), (depth_images_ref.K_GENERAL, 40), (None, 0)):
+            obj.set_projection(K9, pw, 19 if K9 is not None else 0)
+            obj.estimate(stiffness=200.0, huber=1e-2, max_iter=3, max_d2=np.float32(0.01), max_gn_iter=1,
+                         max_cg_iter=30)
+            obj.correspondences()
     ctx.close()
     print("sanitize target: all checks passed")
 
