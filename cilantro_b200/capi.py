@@ -852,27 +852,32 @@ def ransac_residuals(ctx, dst: Cloud, src: Cloud, T, thresh):
     return res, inl[:cnt.value].astype(np.int64)
 
 
-def ransac_rigid(ctx, dst: Cloud, src: Cloud, seed, max_iter=100, thresh=0.01, inlier_count_thresh=None,
-                 re_estimate=True):
-    n = dst.n
+def _ransac(fn, ctx, clouds, seed, max_iter, thresh, inlier_count_thresh, re_estimate, res):
+    """One cb_ransac_rigid / cb_ransac_plane call: the fields of its result struct res (arrays as float32, times as
+    float, counts as int), the inlier list and the n residuals. The default target is the reference's n/2 + n%2."""
+    n = clouds[0].n
     if inlier_count_thresh is None:
         inlier_count_thresh = n // 2 + n % 2
-    res = RansacResult()
-    inl = np.empty(n, np.uint64)
-    resid = np.empty(n, np.float32)
-    _check(lib().cb_ransac_rigid(ctx.h, dst.h, src.h, C.c_uint32(seed), C.c_size_t(inlier_count_thresh),
-                                 C.c_size_t(max_iter), C.c_float(thresh), C.c_int(int(re_estimate)), C.byref(res),
-                                 _p(inl), _p(resid)))
-    return {
-        "T": np.array(list(res.T), np.float32).reshape(3, 4),
-        "iterations": int(res.iterations),
-        "num_inliers": int(res.num_inliers),
-        "best_iteration": int(res.best_iteration),
-        "inliers": inl[: res.num_inliers].astype(np.int64),
-        "residuals": resid,
-        "gpu_ms_total": float(res.gpu_ms_total),
-        "kernel_launches": int(res.kernel_launches),
-    }
+    inl = np.empty(max(n, 1), np.uint64)
+    resid = np.empty(max(n, 1), np.float32)
+    _check(fn(ctx.h, *(c.h for c in clouds), C.c_uint32(seed), C.c_size_t(inlier_count_thresh), C.c_size_t(max_iter),
+              C.c_float(thresh), C.c_int(int(re_estimate)), C.byref(res), _p(inl), _p(resid)))
+    out = {}
+    for key, typ in res._fields_:
+        v = getattr(res, key)
+        out[key] = (np.array(list(v), np.float32) if issubclass(typ, C.Array)
+                    else float(v) if typ is C.c_double else int(v))
+    out["inliers"] = inl[:res.num_inliers].astype(np.int64)
+    out["residuals"] = resid[:n].copy()
+    return out
+
+
+def ransac_rigid(ctx, dst: Cloud, src: Cloud, seed, max_iter=100, thresh=0.01, inlier_count_thresh=None,
+                 re_estimate=True):
+    out = _ransac(lib().cb_ransac_rigid, ctx, (dst, src), seed, max_iter, thresh, inlier_count_thresh, re_estimate,
+                  RansacResult())
+    out["T"] = out["T"].reshape(3, 4)
+    return out
 
 
 def plane_score(ctx, cloud: Cloud, planes, thresh):
@@ -896,23 +901,8 @@ def plane_residuals(ctx, cloud: Cloud, plane, thresh):
 def ransac_plane(ctx, cloud: Cloud, seed, max_iter=100, thresh=0.1, inlier_count_thresh=None, re_estimate=True):
     """cb_ransac_plane (PlaneRANSACEstimator3f::estimate with the seed injected). Defaults are the reference's
     (ransac_hyperplane_estimator.hpp:18): target n/2 + n%2, 100 iterations, threshold 0.1, re-estimation on."""
-    n = cloud.n
-    if inlier_count_thresh is None:
-        inlier_count_thresh = n // 2 + n % 2
-    res = RansacPlaneResult()
-    inl = np.empty(max(n, 1), np.uint64)
-    resid = np.empty(max(n, 1), np.float32)
-    _check(lib().cb_ransac_plane(ctx.h, cloud.h, C.c_uint32(seed), C.c_size_t(inlier_count_thresh),
-                                 C.c_size_t(max_iter), C.c_float(thresh), C.c_int(int(re_estimate)), C.byref(res),
-                                 _p(inl), _p(resid)))
-    out = {k: int(getattr(res, k)) for k in ("iterations", "best_iteration", "num_inliers", "kernel_launches")}
-    out.update({k: float(getattr(res, k)) for k in ("gpu_ms_total", "gpu_ms_fit", "gpu_ms_score", "gpu_ms_reestimate",
-                                                    "gpu_ms_final")})
-    out["plane"] = np.array(list(res.plane), np.float32)
-    out["hyp_plane"] = np.array(list(res.hyp_plane), np.float32)
-    out["inliers"] = inl[:res.num_inliers].astype(np.int64)
-    out["residuals"] = resid[:n].copy()
-    return out
+    return _ransac(lib().cb_ransac_plane, ctx, (cloud,), seed, max_iter, thresh, inlier_count_thresh, re_estimate,
+                   RansacPlaneResult())
 
 
 def warp_params(w_pt=0.0, w_pl=1.0, stiffness=1.0, huber=1e-4, max_gn_iter=10, gn_tol=1e-5, max_cg_iter=1000,

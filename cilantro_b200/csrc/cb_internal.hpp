@@ -254,6 +254,12 @@ int ensure_index(cb_cloud* c);
 int points_bbox(cb_context* ctx, const float* d_raw, size_t n, float mn[3], float mx[3]);
 // d_data has n + 1 entries; on return d_data[i] = sum_{j<i} in[j], d_data[n] = total (grid_index.cu).
 int exclusive_scan_u32(cb_context* ctx, uint32_t* d_data, size_t n, uint32_t total);
+// The inlier list of one RANSAC model (ransac.cu), after its residual kernel wrote d_flags[i] = residual_i <= thresh
+// and d_flags[n] = 0 (n + 2 entries) and, when residuals is non-null, the residuals into d_res. Scans the flags and
+// downloads the count into *num_inliers, the residuals, and the ascending inlier indices plus index_offset into
+// inliers, each when non-null; synchronises the stream. n < 2^32 - 1 (a 32-bit scan).
+int ransac_inliers(cb_context* ctx, uint32_t* d_flags, const float* d_res, size_t n, uint64_t index_offset,
+                   float* residuals, uint64_t* inliers, size_t* num_inliers);
 // Stable LSD radix sort of (key, value) pairs on the low `bits` bits of the keys (radix_sort.cu). The
 // result is left in d_keys / d_vals; d_keys_tmp / d_vals_tmp are same-sized scratch.
 int radix_sort_pairs_u64(cb_context* ctx, uint64_t* d_keys, uint32_t* d_vals, uint64_t* d_keys_tmp,

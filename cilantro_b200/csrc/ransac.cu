@@ -18,7 +18,8 @@
 #include "nn_search.cuh"
 #include "reduce.cuh"
 #include "host_solve.hpp"
-#include "ransac_sampler.hpp"
+#include "ransac_loop.hpp"
+#include "stats_kernels.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -85,15 +86,30 @@ __global__ void __launch_bounds__(kBlock) ransac_score_kernel(const float* __res
     if (s_cnt[h]) atomicAdd(counts + h, s_cnt[h]);
 }
 
-// residuals of one model, with the real (correctly rounded) square root
+// residuals (may be null) of one model, with the real (correctly rounded) square root, and its inlier flags;
+// flags[n] = 0 (the scan turns it into the count)
 __global__ void ransac_residual_kernel(const float* __restrict__ dst, const float* __restrict__ src, size_t n,
-                                       const Rigid T, float* __restrict__ out) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+                                       const Rigid T, float thresh, float* __restrict__ res,
+                                       uint32_t* __restrict__ flags) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i <= n; i += (size_t)gridDim.x * blockDim.x) {
+    if (i == n) {
+      flags[n] = 0u;
+      continue;
+    }
     float qx, qy, qz;
     rule::transform_point(T, src[3 * i], src[3 * i + 1], src[3 * i + 2], qx, qy, qz);
     const float e0 = __fsub_rn(qx, dst[3 * i]), e1 = __fsub_rn(qy, dst[3 * i + 1]), e2 = __fsub_rn(qz, dst[3 * i + 2]);
-    out[i] = __fsqrt_rn(sum3(__fmul_rn(e0, e0), __fmul_rn(e1, e1), __fmul_rn(e2, e2)));
+    const float r = __fsqrt_rn(sum3(__fmul_rn(e0, e0), __fmul_rn(e1, e1), __fmul_rn(e2, e2)));
+    if (res) res[i] = r;
+    flags[i] = r <= thresh ? 1u : 0u;  // ransac_base.hpp:99
   }
+}
+
+// stable compaction: after the exclusive scan, point i is an inlier iff scan[i + 1] > scan[i]
+__global__ void inlier_scatter_kernel(const uint32_t* __restrict__ scan, size_t n, uint64_t index_offset,
+                                      uint64_t* __restrict__ out) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    if (scan[i + 1] > scan[i]) out[scan[i]] = i + index_offset;
 }
 
 // Kabsch moments over the inliers of model T (re-estimation step, ransac_base.hpp:118-120):
@@ -190,22 +206,78 @@ int score_batch(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const
   return CB_OK;
 }
 
-Rigid rigid_of(const float* T12) {
-  Rigid r;
-  for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) r.r[i * 3 + j] = T12[i * 4 + j];
-    r.t[i] = T12[i * 4 + 3];
-  }
-  return r;
-}
+constexpr size_t kLoopBatch = 1024;  // hypotheses generated and scored per round trip of cb_ransac_rigid
 
-int residuals_device(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, const float* T12, float* d_out) {
-  if (dst->n == 0) return CB_OK;
-  return launch(ctx, ransac_residual_kernel, grid_for(ctx, dst->n, 256), 256, 0, dst->d_raw, src->d_raw, dst->n,
-                rigid_of(T12), d_out);
-}
+// The rigid model of ransac_loop: each sample's pairs are gathered on the device and fitted by Kabsch on the host
+// (ransac_transform_estimator.hpp:72-82), then the batch is scored on the device.
+struct RigidHypotheses {
+  cb_context* ctx;
+  const cb_cloud *dst, *src;
+  float x_max;
+  float* d_T;
+  uint32_t* d_counts;
+  uint32_t* d_idx;
+  float* d_pairs;
+  std::vector<float> h_pairs = std::vector<float>(kLoopBatch * 18), h_T = std::vector<float>(kLoopBatch * 12);
+  float best_T[12];
+
+  int fit(const uint32_t* idx, size_t nb, size_t sample_size) {
+    if (sample_size > 0) {
+      CB_CUDA(cudaMemcpyAsync(d_idx, idx, nb * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+      CB_TRY(launch(ctx, gather_pairs_kernel, (int)((nb * 3 + 255) / 256), 256, 0, dst->d_raw, src->d_raw, d_idx,
+                    nb * 3, d_pairs));
+      CB_CUDA(cudaMemcpyAsync(h_pairs.data(), d_pairs, nb * 18 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+      CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    for (size_t b = 0; b < nb; b++) {
+      double m[16] = {0};
+      for (size_t i = 0; i < sample_size; i++) {
+        const float* p = &h_pairs[(b * 3 + i) * 6];
+        m[0] += 1.0;
+        for (int r = 0; r < 3; r++) {
+          m[1 + r] += p[r];
+          m[4 + r] += p[3 + r];
+          for (int c = 0; c < 3; c++) m[7 + r * 3 + c] += (double)p[r] * (double)p[3 + c];
+        }
+      }
+      kabsch_from_moments(m, &h_T[b * 12]);
+    }
+    CB_CUDA(cudaMemcpyAsync(d_T, h_T.data(), nb * 12 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    return CB_OK;
+  }
+  int score(size_t nb, uint32_t* counts) {
+    CB_TRY(score_batch(ctx, dst, src, d_T, (int)nb, x_max, d_counts));
+    CB_CUDA(cudaMemcpyAsync(counts, d_counts, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    return CB_OK;
+  }
+  void keep(size_t b) { std::memcpy(best_T, &h_T[b * 12], sizeof(best_T)); }
+};
 
 }  // namespace
+
+int cb::ransac_inliers(cb_context* ctx, uint32_t* d_flags, const float* d_res, size_t n, uint64_t index_offset,
+                       float* residuals, uint64_t* inliers, size_t* num_inliers) {
+  size_t k = 0;
+  if (n > 0) {
+    CB_TRY(exclusive_scan_u32(ctx, d_flags, n + 1, 0u));
+    uint32_t cnt = 0;
+    CB_CUDA(cudaMemcpyAsync(&cnt, d_flags + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    if (residuals) CB_CUDA(cudaMemcpyAsync(residuals, d_res, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    k = cnt;
+    if (inliers && k > 0) {
+      DeviceScope scope(ctx);
+      uint64_t* d_inl = nullptr;
+      CB_TRY(scope.alloc(&d_inl, k));
+      CB_TRY(launch(ctx, inlier_scatter_kernel, grid_for(ctx, n + 1, 256), 256, 0, d_flags, n, index_offset, d_inl));
+      CB_CUDA(cudaMemcpyAsync(inliers, d_inl, k * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+      CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+  }
+  if (num_inliers) *num_inliers = k;
+  return CB_OK;
+}
 
 extern "C" {
 
@@ -235,25 +307,15 @@ int cb_ransac_residuals(cb_context* ctx, const cb_cloud* dst, const cb_cloud* sr
   CB_TRY(check_pair(ctx, dst, src));
   CB_CHECK(T12, CB_ERR_INVALID, "null argument");
   const size_t n = dst->n;
-  std::vector<float> h(n);
-  if (n) {
-    DeviceScope scope(ctx);
-    float* d_out = nullptr;
-    CB_TRY(scope.alloc(&d_out, n));
-    CB_TRY(residuals_device(ctx, dst, src, T12, d_out));
-    CB_CUDA(cudaMemcpyAsync(h.data(), d_out, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
-  }
-  size_t k = 0;
-  for (size_t i = 0; i < n; i++) {
-    if (residuals) residuals[i] = h[i];
-    if (h[i] <= thresh) {  // ransac_base.hpp:99
-      if (inliers) inliers[k] = (uint64_t)i + dst->index_offset;
-      ++k;
-    }
-  }
-  if (num_inliers) *num_inliers = k;
-  return CB_OK;
+  DeviceScope scope(ctx);
+  uint32_t* d_flags = nullptr;
+  float* d_res = nullptr;
+  CB_TRY(scope.alloc(&d_flags, n + 2));
+  if (residuals) CB_TRY(scope.alloc(&d_res, n));
+  if (n)  // n + 1 items: the kernel also writes flags[n]
+    CB_TRY(launch(ctx, ransac_residual_kernel, grid_for(ctx, n + 1, 256), 256, 0, dst->d_raw, src->d_raw, n,
+                  rigid_from_t12(T12), thresh, d_res, d_flags));
+  return ransac_inliers(ctx, d_flags, d_res, n, dst->index_offset, residuals, inliers, num_inliers);
 }
 
 int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, uint32_t seed,
@@ -264,103 +326,41 @@ int cb_ransac_rigid(cb_context* ctx, const cb_cloud* dst, const cb_cloud* src, u
   CB_CHECK(ctx->world == 1, CB_ERR_UNSUPPORTED, "cb_ransac_rigid runs per process; shard hypotheses with cb_ransac_score");
   const uint64_t launches0 = ctx->launches;
   const size_t n = dst->n;
-  size_t sample_size = 3;  // MinSampleSize for a rigid 3-D transform (ransac_transform_estimator.hpp:21-23)
-  if (n < sample_size) sample_size = n;                   // ransac_base.hpp:67
-  if (inlier_count_thresh > n) inlier_count_thresh = n;   // :68
-  const float x_max = sqrt_threshold(thresh);
-
-  RansacSampler sampler(n, seed);  // :72-73 with the seed injected
-
-  float best_T[12];
-  t34_identity(best_T);
-  size_t best_count = 0, best_it = 0, it = 0;
-  bool have_best = false, done = false;
-
-  const size_t B = 1024;  // hypotheses generated and scored per round trip
+  RansacSampler sampler(n, seed);
+  RigidHypotheses h{ctx, dst, src, sqrt_threshold(thresh)};
+  t34_identity(h.best_T);
   DeviceScope scope(ctx);
-  float* d_T = nullptr;
-  uint32_t* d_counts = nullptr;
-  uint32_t* d_idx = nullptr;
-  float* d_pairs = nullptr;
-  CB_TRY(scope.alloc(&d_T, B * 12));
-  CB_TRY(scope.alloc(&d_counts, B));
-  CB_TRY(scope.alloc(&d_idx, B * 3));
-  CB_TRY(scope.alloc(&d_pairs, B * 3 * 6));
-  std::vector<uint32_t> h_idx(B * 3), h_counts(B);
-  std::vector<float> h_pairs(B * 18), h_T(B * 12);
+  CB_TRY(scope.alloc(&h.d_T, kLoopBatch * 12));
+  CB_TRY(scope.alloc(&h.d_counts, kLoopBatch));
+  CB_TRY(scope.alloc(&h.d_idx, kLoopBatch * 3));
+  CB_TRY(scope.alloc(&h.d_pairs, kLoopBatch * 3 * 6));
   ScopedEvents ev;
   CB_TRY(ev.create());
   CB_CUDA(cudaEventRecord(ev.e0, ctx->stream));
-  while (!done && it < max_iter) {
-    const size_t nb = std::min(B, max_iter - it);
-    // sample (:83-91): partial Fisher-Yates on a permutation that persists across hypotheses
-    for (size_t b = 0; b < nb; b++) sampler.next(sample_size, &h_idx[b * 3]);
-    // estimateModel(sample) (:94, ransac_transform_estimator.hpp:72-82): Kabsch on the sample
-    if (sample_size > 0) {
-      CB_CUDA(cudaMemcpyAsync(d_idx, h_idx.data(), nb * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-      CB_TRY(launch(ctx, gather_pairs_kernel, (int)((nb * 3 + 255) / 256), 256, 0, dst->d_raw, src->d_raw, d_idx,
-                    nb * 3, d_pairs));
-      CB_CUDA(cudaMemcpyAsync(h_pairs.data(), d_pairs, nb * 18 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-      CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-    for (size_t b = 0; b < nb; b++) {
-      double m[16] = {0};
-      for (size_t i = 0; i < sample_size; i++) {
-        const float* p = &h_pairs[(b * 3 + i) * 6];
-        m[0] += 1.0;
-        for (int r = 0; r < 3; r++) {
-          m[1 + r] += p[r];
-          m[4 + r] += p[3 + r];
-          for (int c = 0; c < 3; c++) m[7 + r * 3 + c] += (double)p[r] * (double)p[3 + c];
-        }
-      }
-      kabsch_from_moments(m, &h_T[b * 12]);
-    }
-    CB_CUDA(cudaMemcpyAsync(d_T, h_T.data(), nb * 12 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    CB_TRY(score_batch(ctx, dst, src, d_T, (int)nb, x_max, d_counts));
-    CB_CUDA(cudaMemcpyAsync(h_counts.data(), d_counts, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    // sequential semantics over the batch (:103-114)
-    for (size_t b = 0; b < nb; b++) {
-      it++;
-      const size_t cnt = h_counts[b];
-      if (cnt < sample_size) continue;       // :104
-      if (cnt > best_count) {                // :107 (model_inliers_ starts empty, so size 0)
-        best_count = cnt;
-        std::memcpy(best_T, &h_T[b * 12], sizeof(best_T));
-        best_it = it - 1;
-        have_best = true;
-      }
-      if (best_count >= inlier_count_thresh) {  // :114
-        done = true;
-        break;
-      }
-    }
-  }
+  RansacRun run;
+  CB_TRY(ransac_loop(sampler, inlier_count_thresh, max_iter, kLoopBatch, kLoopBatch, h, &run));
   // no hypothesis ever reached sample_size inliers: model_inliers_ is empty, so the re-estimation
   // is a Kabsch over zero pairs = identity (transform_estimation.hpp:20-23)
-  if (re_estimate && have_best) {  // :118-128
+  if (re_estimate && run.have_best) {  // :118-128
     const int blocks = grid_for(ctx, n, kReduceBlock, 4);
     ReduceScratch rs;
     CB_TRY(get_reduce_scratch(ctx, blocks, 16, &rs));
-    CB_TRY(launch(ctx, inlier_moments_kernel, blocks, kReduceBlock, 0, dst->d_raw, src->d_raw, n, rigid_of(best_T),
-                  x_max, rs));
+    CB_TRY(launch(ctx, inlier_moments_kernel, blocks, kReduceBlock, 0, dst->d_raw, src->d_raw, n,
+                  rigid_from_t12(h.best_T), h.x_max, rs));
     double m[16];
-    CB_CUDA(cudaMemcpyAsync(ctx->h_result, ctx->d_result, sizeof(m), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    std::memcpy(m, ctx->h_result, sizeof(m));
-    kabsch_from_moments(m, best_T);
+    CB_TRY(fetch_result(ctx, 16, false, m));
+    kabsch_from_moments(m, h.best_T);
   }
-  size_t n_inl = best_count;
+  size_t n_inl = run.best_count;
   CB_CUDA(cudaEventRecord(ev.e1, ctx->stream));
-  CB_TRY(cb_ransac_residuals(ctx, dst, src, best_T, thresh, residuals, inliers, &n_inl));
+  CB_TRY(cb_ransac_residuals(ctx, dst, src, h.best_T, thresh, residuals, inliers, &n_inl));
   CB_CUDA(cudaEventSynchronize(ev.e1));  // (cb_ransac_residuals does not synchronise an empty cloud)
   float ms = 0.f;
   CB_CUDA(cudaEventElapsedTime(&ms, ev.e0, ev.e1));
-  std::memcpy(res->T, best_T, sizeof(best_T));
-  res->iterations = it;
+  std::memcpy(res->T, h.best_T, sizeof(h.best_T));
+  res->iterations = run.iterations;
   res->num_inliers = n_inl;
-  res->best_iteration = best_it;
+  res->best_iteration = run.best_iteration;
   res->gpu_ms_total = ms;
   res->kernel_launches = ctx->launches - launches0;
   return CB_OK;

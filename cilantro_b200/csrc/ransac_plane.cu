@@ -17,7 +17,7 @@
 #include "host_solve.hpp"
 #include "launch.cuh"
 #include "plane_fit.hpp"
-#include "ransac_sampler.hpp"
+#include "ransac_loop.hpp"
 #include "reduce.cuh"
 #include "stats_kernels.cuh"
 #include <algorithm>
@@ -123,12 +123,6 @@ __global__ void plane_residual_kernel(const float* __restrict__ raw, size_t n, c
   }
 }
 
-// stable compaction: after the exclusive scan, point i is an inlier iff scan[i + 1] > scan[i]
-__global__ void inlier_scatter_kernel(const uint32_t* __restrict__ scan, size_t n, uint64_t* __restrict__ out) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    if (scan[i + 1] > scan[i]) out[scan[i]] = i;
-}
-
 // The moments of moments_kernel (count, sum (p - c), upper triangle of sum (p - c)(p - c)^T) over the points with
 // |n.p + d| <= thresh, the predicate that counted the hypothesis's inliers
 __global__ void __launch_bounds__(kReduceBlock) plane_moments_kernel(const float* __restrict__ raw, size_t n,
@@ -183,38 +177,6 @@ int score_planes(cb_context* ctx, const cb_cloud* cloud, const float4* d_planes,
 int fit_planes(cb_context* ctx, const cb_cloud* cloud, const uint32_t* d_idx, int H, int sample_size, float4* d_planes) {
   if (H == 0) return CB_OK;
   return launch(ctx, plane_fit_kernel, (H + 127) / 128, 128, 0, cloud->d_raw, d_idx, H, sample_size, d_planes);
-}
-
-// final residuals + stable compaction of the inliers; synchronises the stream
-int residuals_and_inliers(cb_context* ctx, const cb_cloud* cloud, const float* plane4, float thresh, float* residuals,
-                          uint64_t* inliers, size_t* num_inliers) {
-  const size_t n = cloud->n;
-  size_t k = 0;
-  if (n > 0) {
-    DeviceScope scope(ctx);
-    uint32_t* d_flags = nullptr;
-    float* d_res = nullptr;
-    uint64_t* d_inl = nullptr;
-    CB_TRY(scope.alloc(&d_flags, n + 2));
-    if (residuals) CB_TRY(scope.alloc(&d_res, n));
-    const float4 P = make_float4(plane4[0], plane4[1], plane4[2], plane4[3]);
-    const int blocks = grid_for(ctx, n + 1, 256);  // n + 1 items: the kernel also writes flags[n]
-    CB_TRY(launch(ctx, plane_residual_kernel, blocks, 256, 0, cloud->d_raw, n, P, thresh, d_res, d_flags));
-    CB_TRY(exclusive_scan_u32(ctx, d_flags, n + 1, 0u));
-    uint32_t cnt = 0;
-    CB_CUDA(cudaMemcpyAsync(&cnt, d_flags + n, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    if (residuals) CB_CUDA(cudaMemcpyAsync(residuals, d_res, n * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    k = cnt;
-    if (inliers && k > 0) {
-      CB_TRY(scope.alloc(&d_inl, k));
-      CB_TRY(launch(ctx, inlier_scatter_kernel, blocks, 256, 0, d_flags, n, d_inl));
-      CB_CUDA(cudaMemcpyAsync(inliers, d_inl, k * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-      CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    }
-  }
-  if (num_inliers) *num_inliers = k;
-  return CB_OK;
 }
 
 // moments of the points within thresh of the plane about the pivot c (synchronises the stream)
@@ -284,6 +246,40 @@ struct Events {
   }
 };
 
+// The plane model of ransac_loop: the samples are fitted (plane_fit_kernel) and scored on the device, and the planes
+// come back with the counts. ev.e[0..2] bracket each batch's fit and scoring.
+struct PlaneHypotheses {
+  cb_context* ctx;
+  const cb_cloud* cloud;
+  float thresh;
+  uint32_t* d_idx;
+  float4* d_planes;
+  uint32_t* d_counts;
+  Events ev;
+  std::vector<float> h_planes = std::vector<float>(4 * (size_t)kMaxBatch);
+  float best[4];
+  double ms_fit = 0.0, ms_score = 0.0;
+
+  int fit(const uint32_t* idx, size_t nb, size_t sample_size) {
+    CB_CUDA(cudaEventRecord(ev.e[0], ctx->stream));
+    CB_CUDA(cudaMemcpyAsync(d_idx, idx, 3 * nb * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    CB_TRY(fit_planes(ctx, cloud, d_idx, (int)nb, (int)sample_size, d_planes));
+    CB_CUDA(cudaEventRecord(ev.e[1], ctx->stream));
+    return CB_OK;
+  }
+  int score(size_t nb, uint32_t* counts) {
+    CB_TRY(score_planes(ctx, cloud, d_planes, (int)nb, thresh, d_counts));
+    CB_CUDA(cudaEventRecord(ev.e[2], ctx->stream));
+    CB_CUDA(cudaMemcpyAsync(counts, d_counts, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaMemcpyAsync(h_planes.data(), d_planes, nb * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
+    CB_CUDA(cudaStreamSynchronize(ctx->stream));
+    ms_fit += ev.ms(0, 1);
+    ms_score += ev.ms(1, 2);
+    return CB_OK;
+  }
+  void keep(size_t b) { std::memcpy(best, &h_planes[4 * b], sizeof(best)); }
+};
+
 }  // namespace
 
 extern "C" {
@@ -313,7 +309,17 @@ int cb_plane_residuals(cb_context* ctx, const cb_cloud* cloud, const float* plan
                        uint64_t* inliers, size_t* num_inliers) {
   CB_TRY(check_cloud(ctx, cloud));
   CB_CHECK(plane4, CB_ERR_INVALID, "null argument");
-  return residuals_and_inliers(ctx, cloud, plane4, thresh, residuals, inliers, num_inliers);
+  const size_t n = cloud->n;
+  DeviceScope scope(ctx);
+  uint32_t* d_flags = nullptr;
+  float* d_res = nullptr;
+  CB_TRY(scope.alloc(&d_flags, n + 2));
+  if (residuals) CB_TRY(scope.alloc(&d_res, n));
+  const float4 P = make_float4(plane4[0], plane4[1], plane4[2], plane4[3]);
+  if (n)  // n + 1 items: the kernel also writes flags[n]
+    CB_TRY(launch(ctx, plane_residual_kernel, grid_for(ctx, n + 1, 256), 256, 0, cloud->d_raw, n, P, thresh, d_res,
+                  d_flags));
+  return ransac_inliers(ctx, d_flags, d_res, n, 0, residuals, inliers, num_inliers);
 }
 
 int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_t inlier_count_thresh,
@@ -323,74 +329,28 @@ int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_
   CB_CHECK(res, CB_ERR_INVALID, "null argument");
   CB_CHECK(ctx->world == 1, CB_ERR_UNSUPPORTED, "cb_ransac_plane runs per process; shard hypotheses with cb_plane_score");
   const uint64_t launches0 = ctx->launches;
-  const size_t n = cloud->n;
-  size_t sample_size = 3;                                 // ransac_hyperplane_estimator.hpp:18 (points.rows())
-  if (n < sample_size) sample_size = n;                   // ransac_base.hpp:67
-  if (inlier_count_thresh > n) inlier_count_thresh = n;   // :68
-  RansacSampler sampler(n, seed);                         // :72-73 with the seed injected
-
-  const float nan = std::numeric_limits<float>::quiet_NaN();
-  float best[4] = {nan, nan, nan, nan};
-  size_t best_count = 0, best_it = 0, it = 0;
-  bool have_best = false, done = false;
-  double ms_fit = 0.0, ms_score = 0.0, ms_re = 0.0, ms_final = 0.0;
-
-  Events ev;
-  CB_TRY(ev.create());
+  RansacSampler sampler(cloud->n, seed);
+  PlaneHypotheses h{ctx, cloud, thresh};
+  std::fill(h.best, h.best + 4, std::numeric_limits<float>::quiet_NaN());
+  CB_TRY(h.ev.create());
+  Events& ev = h.ev;
   ScopedEvents total;
   CB_TRY(total.create());
   DeviceScope scope(ctx);
-  uint32_t* d_idx = nullptr;
-  float4* d_planes = nullptr;
-  uint32_t* d_counts = nullptr;
-  CB_TRY(scope.alloc(&d_idx, 3 * (size_t)kMaxBatch));
-  CB_TRY(scope.alloc(&d_planes, kMaxBatch));
-  CB_TRY(scope.alloc(&d_counts, kMaxBatch));
-  std::vector<uint32_t> h_idx(3 * (size_t)kMaxBatch, 0u), h_counts(kMaxBatch);
-  std::vector<float> h_planes(4 * (size_t)kMaxBatch);
+  CB_TRY(scope.alloc(&h.d_idx, 3 * (size_t)kMaxBatch));
+  CB_TRY(scope.alloc(&h.d_planes, kMaxBatch));
+  CB_TRY(scope.alloc(&h.d_counts, kMaxBatch));
   CB_CUDA(cudaEventRecord(total.e0, ctx->stream));
-  size_t batch = kFirstBatch;
-  // Batches grow geometrically: an early exit wastes at most as many hypotheses as already ran, and a run without
-  // an early exit soon scores full batches.
-  while (!done && it < max_iter) {
-    const size_t nb = std::min(batch, max_iter - it);
-    batch = std::min<size_t>(2 * batch, kMaxBatch);
-    for (size_t b = 0; b < nb; b++) sampler.next(sample_size, &h_idx[3 * b]);  // :83-91
-    CB_CUDA(cudaEventRecord(ev.e[0], ctx->stream));
-    CB_CUDA(cudaMemcpyAsync(d_idx, h_idx.data(), 3 * nb * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-    CB_TRY(fit_planes(ctx, cloud, d_idx, (int)nb, (int)sample_size, d_planes));  // :94
-    CB_CUDA(cudaEventRecord(ev.e[1], ctx->stream));
-    CB_TRY(score_planes(ctx, cloud, d_planes, (int)nb, thresh, d_counts));  // :95-101
-    CB_CUDA(cudaEventRecord(ev.e[2], ctx->stream));
-    CB_CUDA(cudaMemcpyAsync(h_counts.data(), d_counts, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaMemcpyAsync(h_planes.data(), d_planes, nb * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
-    CB_CUDA(cudaStreamSynchronize(ctx->stream));
-    ms_fit += ev.ms(0, 1);
-    ms_score += ev.ms(1, 2);
-    // sequential semantics over the batch (:103-114)
-    for (size_t b = 0; b < nb; b++) {
-      it++;
-      const size_t cnt = h_counts[b];
-      if (cnt < sample_size) continue;  // :104
-      if (cnt > best_count) {           // :107 (model_inliers_ starts empty)
-        best_count = cnt;
-        std::memcpy(best, &h_planes[4 * b], sizeof(best));
-        best_it = it - 1;
-        have_best = true;
-      }
-      if (best_count >= inlier_count_thresh) {  // :114
-        done = true;
-        break;
-      }
-    }
-  }
+  RansacRun run;
+  CB_TRY(ransac_loop(sampler, inlier_count_thresh, max_iter, kFirstBatch, kMaxBatch, h, &run));
   // No hypothesis ever reached sample_size inliers: the reference's model is an uninitialised Eigen::Hyperplane;
   // NaN stands in for it, with or without re-estimation.
   float plane[4];
-  std::memcpy(plane, best, sizeof(plane));
-  if (re_estimate && have_best) {  // :118-120
+  std::memcpy(plane, h.best, sizeof(plane));
+  double ms_re = 0.0;
+  if (re_estimate && run.have_best) {  // :118-120
     CB_CUDA(cudaEventRecord(ev.e[3], ctx->stream));
-    CB_TRY(reestimate(ctx, cloud, best, thresh, best_count, plane));
+    CB_TRY(reestimate(ctx, cloud, h.best, thresh, run.best_count, plane));
     CB_CUDA(cudaEventRecord(ev.e[4], ctx->stream));
     CB_CUDA(cudaEventSynchronize(ev.e[4]));
     ms_re = ev.ms(3, 4);
@@ -398,23 +358,22 @@ int cb_ransac_plane(cb_context* ctx, const cb_cloud* cloud, uint32_t seed, size_
   // the model's residuals and inliers (:95-101 for the kept hypothesis, :121-127 after re-estimation)
   size_t n_inl = 0;
   CB_CUDA(cudaEventRecord(ev.e[3], ctx->stream));
-  CB_TRY(residuals_and_inliers(ctx, cloud, plane, thresh, residuals, inliers, &n_inl));
+  CB_TRY(cb_plane_residuals(ctx, cloud, plane, thresh, residuals, inliers, &n_inl));
   CB_CUDA(cudaEventRecord(ev.e[4], ctx->stream));
   CB_CUDA(cudaEventRecord(total.e1, ctx->stream));
   CB_CUDA(cudaEventSynchronize(total.e1));
-  ms_final = ev.ms(3, 4);
   float ms = 0.f;
   CB_CUDA(cudaEventElapsedTime(&ms, total.e0, total.e1));
   std::memcpy(res->plane, plane, sizeof(plane));
-  std::memcpy(res->hyp_plane, best, sizeof(best));
-  res->iterations = it;
-  res->best_iteration = best_it;
+  std::memcpy(res->hyp_plane, h.best, sizeof(h.best));
+  res->iterations = run.iterations;
+  res->best_iteration = run.best_iteration;
   res->num_inliers = n_inl;
   res->gpu_ms_total = ms;
-  res->gpu_ms_fit = ms_fit;
-  res->gpu_ms_score = ms_score;
+  res->gpu_ms_fit = h.ms_fit;
+  res->gpu_ms_score = h.ms_score;
   res->gpu_ms_reestimate = ms_re;
-  res->gpu_ms_final = ms_final;
+  res->gpu_ms_final = ev.ms(3, 4);
   res->kernel_launches = ctx->launches - launches0;
   return CB_OK;
 }

@@ -1531,78 +1531,115 @@ template <template <class> class DistAdaptor = KDTreeDistanceAdaptors::L2, typen
           typename ClusterIndexT = size_t>
 using KMeansXf = KMeans<float, b200::kDynamic, DistAdaptor, PointIndexT, ClusterIndexT>;
 
-// ---- RigidTransformRANSACEstimator3f<> ----------------------------------------------------------------
-template <typename IndexT = size_t>
-class RigidTransformRANSACEstimator3f {
+namespace b200 {
+// RandomSampleConsensusBase (model_estimation/ransac_base.hpp:10-192) over one device call: the parameters, estimate()
+// and the results. Derived::run(inliers, residuals) makes the call for the members' parameters, sets model_ and
+// iterations_, and returns the number of inliers. Derived's sample size is 3; the seed of the sampler is injected with
+// setRandomSeed (the reference draws it from std::random_device, :73).
+template <class Derived, class ModelT, typename IndexT>
+class RansacEstimator {
 public:
-  using Model = RigidTransform3f;
+  using Model = ModelT;
+  using ResidualScalar = float;
   using ResidualVector = std::vector<float>;
+  using Index = IndexT;
   using IndexVector = std::vector<IndexT>;
 
-  RigidTransformRANSACEstimator3f(const ConstVectorSetMatrixMap3f& dst, const ConstVectorSetMatrixMap3f& src)
-      : n_(dst.cols()), dst_(dst), src_(src) {
-    defaults();
+  size_t getSampleSize() const { return sample_size_; }
+  size_t getTargetInlierCount() const { return target_; }
+  Derived& setTargetInlierCount(size_t c) { target_ = c; return self(); }
+  size_t getMaxNumberOfIterations() const { return max_iter_; }
+  Derived& setMaxNumberOfIterations(size_t m) { max_iter_ = m; return self(); }
+  float getMaxInlierResidual() const { return thresh_; }
+  Derived& setMaxInlierResidual(float t) { thresh_ = t; return self(); }
+  bool getReEstimationStep() const { return re_estimate_; }
+  Derived& setReEstimationStep(bool b) { re_estimate_ = b; return self(); }
+  Derived& setRandomSeed(uint32_t s) { seed_ = s; return self(); }
+
+  Derived& estimate() {
+    if (n_ < sample_size_) sample_size_ = n_;  // :67
+    if (target_ > n_) target_ = n_;            // :68
+    std::vector<uint64_t> inl(n_);
+    residuals_.resize(n_);
+    const size_t k = self().run(inl.data(), residuals_.data());
+    inliers_.assign(inl.begin(), inl.begin() + k);
+    return self();
   }
+  Derived& estimate(float max_residual, size_t target_inlier_count, size_t max_iter) {  // :133-139
+    thresh_ = max_residual;
+    target_ = target_inlier_count;
+    max_iter_ = max_iter;
+    return estimate();
+  }
+
+  const Derived& getEstimationResults(Model& model, ResidualVector& residuals, IndexVector& inliers) const {
+    model = model_;
+    residuals = residuals_;
+    inliers = inliers_;
+    return self();
+  }
+  const Model& getModel() const { return model_; }
+  const Derived& getModel(Model& m) const { m = model_; return self(); }
+  const ResidualVector& getModelResiduals() const { return residuals_; }
+  const Derived& getModelResiduals(ResidualVector& r) const { r = residuals_; return self(); }
+  const IndexVector& getModelInliers() const { return inliers_; }
+  const Derived& getModelInliers(IndexVector& i) const { i = inliers_; return self(); }
+  bool targetInlierCountAchieved() const { return inliers_.size() >= target_; }
+  size_t getNumberOfPerformedIterations() const { return iterations_; }
+  size_t getNumberOfInliers() const { return inliers_.size(); }
+
+protected:
+  // the reference estimators' defaults: target n/2 + n%2, 100 iterations, re-estimation on
+  RansacEstimator(size_t n, float thresh) : n_(n), target_(n / 2 + n % 2), thresh_(thresh), seed_(random_seed()) {}
+
+  size_t n_, sample_size_ = 3, target_, max_iter_ = 100, iterations_ = 0;
+  float thresh_;
+  bool re_estimate_ = true;
+  uint32_t seed_;
+  Model model_;
+  ResidualVector residuals_;
+  IndexVector inliers_;
+
+private:
+  Derived& self() { return *static_cast<Derived*>(this); }
+  const Derived& self() const { return *static_cast<const Derived*>(this); }
+};
+}  // namespace b200
+
+// ---- RigidTransformRANSACEstimator3f<> ----------------------------------------------------------------
+// TransformRANSACEstimator<RigidTransform3f> (model_estimation/ransac_transform_estimator.hpp): threshold 0.01.
+template <typename IndexT = size_t>
+class RigidTransformRANSACEstimator3f
+    : public b200::RansacEstimator<RigidTransformRANSACEstimator3f<IndexT>, RigidTransform3f, IndexT> {
+  using Base = b200::RansacEstimator<RigidTransformRANSACEstimator3f<IndexT>, RigidTransform3f, IndexT>;
+  friend Base;
+
+public:
+  RigidTransformRANSACEstimator3f(const ConstVectorSetMatrixMap3f& dst, const ConstVectorSetMatrixMap3f& src)
+      : Base(dst.cols(), 0.01f), dst_(dst), src_(src) {}
   template <class CorrespondencesT>
   RigidTransformRANSACEstimator3f(const ConstVectorSetMatrixMap3f& dst, const ConstVectorSetMatrixMap3f& src,
                                   const CorrespondencesT& corr)
-      : n_(corr.size()), dst_g_(gather(dst, corr, true)), src_g_(gather(src, corr, false)), dst_(dst_g_), src_(src_g_) {
-    defaults();
-  }
+      : Base(corr.size(), 0.01f), dst_g_(gather(dst, corr, true)), src_g_(gather(src, corr, false)), dst_(dst_g_),
+        src_(src_g_) {}
 
   // (dst, src, dst_ind, src_ind): pair k = (dst point dst_ind[k], src point src_ind[k])
   // (model_estimation/ransac_transform_estimator.hpp:46-59)
   template <typename IdxT>
   RigidTransformRANSACEstimator3f(const ConstVectorSetMatrixMap3f& dst, const ConstVectorSetMatrixMap3f& src,
                                   const std::vector<IdxT>& dst_ind, const std::vector<IdxT>& src_ind)
-      : n_(dst_ind.size()), dst_g_(gather_ind(dst, dst_ind, dst_ind.size())), src_g_(gather_ind(src, src_ind, dst_ind.size())),
-        dst_(dst_g_), src_(src_g_) {
-    defaults();
-  }
-
-  // RandomSampleConsensusBase setters (model_estimation/ransac_base.hpp:29-62)
-  RigidTransformRANSACEstimator3f& setMaxInlierResidual(float t) { thresh_ = t; return *this; }
-  RigidTransformRANSACEstimator3f& setTargetInlierCount(size_t c) { target_ = c; return *this; }
-  RigidTransformRANSACEstimator3f& setMaxNumberOfIterations(size_t n) { max_iter_ = n; return *this; }
-  RigidTransformRANSACEstimator3f& setReEstimationStep(bool b) { re_estimate_ = b; return *this; }
-  RigidTransformRANSACEstimator3f& setRandomSeed(uint32_t s) { seed_ = s; return *this; }  // injected (SURVEY F8)
-  float getMaxInlierResidual() const { return thresh_; }
-  size_t getTargetInlierCount() const { return target_; }
-  size_t getMaxNumberOfIterations() const { return max_iter_; }
-  bool getReEstimationStep() const { return re_estimate_; }
-
-  RigidTransformRANSACEstimator3f& estimate() {
-    cb_ransac_result r;
-    std::vector<uint64_t> inl(n_);
-    residuals_.resize(n_);
-    b200::check(cb_ransac_rigid(b200::Context::get(), dst_.h, src_.h, seed_, target_, max_iter_, thresh_,
-                                re_estimate_ ? 1 : 0, &r, inl.data(), residuals_.data()),
-                "cb_ransac_rigid");
-    model_ = RigidTransform3f(r.T);
-    iterations_ = r.iterations;
-    inliers_.assign(inl.begin(), inl.begin() + r.num_inliers);
-    return *this;
-  }
-  RigidTransformRANSACEstimator3f& estimate(float max_residual, size_t target_inlier_count, size_t max_iter) {
-    thresh_ = max_residual;
-    target_ = target_inlier_count;
-    max_iter_ = max_iter;
-    return estimate();
-  }
-  const Model& getModel() const { return model_; }
-  const ResidualVector& getModelResiduals() const { return residuals_; }
-  const IndexVector& getModelInliers() const { return inliers_; }
-  bool targetInlierCountAchieved() const { return inliers_.size() >= target_; }
-  size_t getNumberOfPerformedIterations() const { return iterations_; }
-  size_t getNumberOfInliers() const { return inliers_.size(); }
+      : Base(dst_ind.size(), 0.01f), dst_g_(gather_ind(dst, dst_ind, dst_ind.size())),
+        src_g_(gather_ind(src, src_ind, dst_ind.size())), dst_(dst_g_), src_(src_g_) {}
 
 private:
-  void defaults() {  // ransac_transform_estimator.hpp:27
-    target_ = n_ / 2 + n_ % 2;
-    max_iter_ = 100;
-    thresh_ = 0.01f;
-    re_estimate_ = true;
-    seed_ = b200::random_seed();
+  size_t run(uint64_t* inliers, float* residuals) {
+    cb_ransac_result r;
+    b200::check(cb_ransac_rigid(b200::Context::get(), dst_.h, src_.h, this->seed_, this->target_, this->max_iter_,
+                                this->thresh_, this->re_estimate_ ? 1 : 0, &r, inliers, residuals),
+                "cb_ransac_rigid");
+    this->model_ = RigidTransform3f(r.T);
+    this->iterations_ = r.iterations;
+    return r.num_inliers;
   }
   template <class CorrespondencesT>
   static VectorSet3f gather(const ConstVectorSetMatrixMap3f& pts, const CorrespondencesT& corr, bool first) {
@@ -1616,16 +1653,8 @@ private:
     for (size_t i = 0; i < count; i++) out.setCol(i, pts.col((size_t)ind[i]));
     return out;
   }
-  size_t n_;
   VectorSet3f dst_g_, src_g_;
   b200::CloudHandle dst_, src_;
-  size_t target_, max_iter_, iterations_ = 0;
-  float thresh_;
-  bool re_estimate_;
-  uint32_t seed_;
-  Model model_;
-  ResidualVector residuals_;
-  IndexVector inliers_;
 };
 
 // ---- PrincipalComponentAnalysis3f -----------------------------------------------------------------------

@@ -39,50 +39,19 @@ private:
 };
 
 // HyperplaneRANSACEstimator<float, 3, IndexT> (ransac_hyperplane_estimator.hpp:9-112) with the surface of
-// RandomSampleConsensusBase (ransac_base.hpp:10-187). Sample size 3 (setSampleSize is not offered); the seed of the
-// sampler is injected with setRandomSeed (the reference draws it from std::random_device).
+// RandomSampleConsensusBase (b200::RansacEstimator): threshold 0.1; setSampleSize is not offered.
 template <typename IndexT = size_t>
-class HyperplaneRANSACEstimator3f {
+class HyperplaneRANSACEstimator3f
+    : public b200::RansacEstimator<HyperplaneRANSACEstimator3f<IndexT>, Hyperplane3f, IndexT> {
+  using Base = b200::RansacEstimator<HyperplaneRANSACEstimator3f<IndexT>, Hyperplane3f, IndexT>;
+  friend Base;
+
 public:
-  using Model = Hyperplane3f;
-  using ResidualScalar = float;
-  using ResidualVector = std::vector<float>;
-  using Index = IndexT;
-  using IndexVector = std::vector<IndexT>;
+  using typename Base::IndexVector;
+  using typename Base::ResidualVector;
 
   HyperplaneRANSACEstimator3f(const ConstVectorSetMatrixMap3f& points)
-      : n_(points.cols()), points_(points), cloud_(points), target_(n_ / 2 + n_ % 2), seed_(b200::random_seed()) {}
-
-  size_t getSampleSize() const { return 3; }
-  size_t getTargetInlierCount() const { return target_; }
-  HyperplaneRANSACEstimator3f& setTargetInlierCount(size_t c) { target_ = c; return *this; }
-  size_t getMaxNumberOfIterations() const { return max_iter_; }
-  HyperplaneRANSACEstimator3f& setMaxNumberOfIterations(size_t m) { max_iter_ = m; return *this; }
-  float getMaxInlierResidual() const { return thresh_; }
-  HyperplaneRANSACEstimator3f& setMaxInlierResidual(float t) { thresh_ = t; return *this; }
-  bool getReEstimationStep() const { return re_estimate_; }
-  HyperplaneRANSACEstimator3f& setReEstimationStep(bool b) { re_estimate_ = b; return *this; }
-  HyperplaneRANSACEstimator3f& setRandomSeed(uint32_t s) { seed_ = s; return *this; }
-
-  HyperplaneRANSACEstimator3f& estimate() {
-    if (target_ > n_) target_ = n_;  // ransac_base.hpp:68
-    cb_ransac_plane_result r;
-    std::vector<uint64_t> inl(n_);
-    residuals_.resize(n_);
-    b200::check(cb_ransac_plane(b200::Context::get(), cloud_.h, seed_, target_, max_iter_, thresh_, re_estimate_ ? 1 : 0,
-                                &r, inl.data(), residuals_.data()),
-                "cb_ransac_plane");
-    model_ = Hyperplane3f(r.plane);
-    iterations_ = r.iterations;
-    inliers_.assign(inl.begin(), inl.begin() + r.num_inliers);
-    return *this;
-  }
-  HyperplaneRANSACEstimator3f& estimate(float max_residual, size_t target_inlier_count, size_t max_iter) {  // :133-140
-    thresh_ = max_residual;
-    target_ = target_inlier_count;
-    max_iter_ = max_iter;
-    return estimate();
-  }
+      : Base(points.cols(), 0.1f), points_(points), cloud_(points) {}
 
   // estimateModel (:21-42): the PCA plane of all points / of the listed points
   HyperplaneRANSACEstimator3f& estimateModel(Hyperplane3f& model) {
@@ -99,9 +68,9 @@ public:
   }
   // computeResiduals (:44-62)
   HyperplaneRANSACEstimator3f& computeResiduals(const Hyperplane3f& model, ResidualVector& residuals) {
-    residuals.resize(n_);
-    b200::check(cb_plane_residuals(b200::Context::get(), cloud_.h, model.coeffs().data(), thresh_, residuals.data(),
-                                   nullptr, nullptr),
+    residuals.resize(this->n_);
+    b200::check(cb_plane_residuals(b200::Context::get(), cloud_.h, model.coeffs().data(), this->thresh_,
+                                   residuals.data(), nullptr, nullptr),
                 "cb_plane_residuals");
     return *this;
   }
@@ -110,42 +79,26 @@ public:
     computeResiduals(model, r);
     return r;
   }
-  size_t getDataPointsCount() const { return n_; }
-
-  const HyperplaneRANSACEstimator3f& getEstimationResults(Model& model, ResidualVector& residuals,
-                                                          IndexVector& inliers) const {
-    model = model_;
-    residuals = residuals_;
-    inliers = inliers_;
-    return *this;
-  }
-  const Model& getModel() const { return model_; }
-  const HyperplaneRANSACEstimator3f& getModel(Model& m) const { m = model_; return *this; }
-  const ResidualVector& getModelResiduals() const { return residuals_; }
-  const HyperplaneRANSACEstimator3f& getModelResiduals(ResidualVector& r) const { r = residuals_; return *this; }
-  const IndexVector& getModelInliers() const { return inliers_; }
-  const HyperplaneRANSACEstimator3f& getModelInliers(IndexVector& i) const { i = inliers_; return *this; }
-  bool targetInlierCountAchieved() const { return inliers_.size() >= target_; }
-  size_t getNumberOfPerformedIterations() const { return iterations_; }
-  size_t getNumberOfInliers() const { return inliers_.size(); }
+  size_t getDataPointsCount() const { return this->n_; }
 
 private:
+  size_t run(uint64_t* inliers, float* residuals) {
+    cb_ransac_plane_result r;
+    b200::check(cb_ransac_plane(b200::Context::get(), cloud_.h, this->seed_, this->target_, this->max_iter_,
+                                this->thresh_, this->re_estimate_ ? 1 : 0, &r, inliers, residuals),
+                "cb_ransac_plane");
+    this->model_ = Hyperplane3f(r.plane);
+    this->iterations_ = r.iterations;
+    return r.num_inliers;
+  }
   // estimate_params_ (:96-110): normal = the last eigenvector column, offset = -(normal . mean)
   static Hyperplane3f pca_plane(const PrincipalComponentAnalysis3f& pca) {
     const auto& V = pca.getEigenVectors();
     const Vector3f n(V[2], V[5], V[8]), m = pca.getDataMean();
     return Hyperplane3f(n, -(n[0] * m[0] + (n[1] * m[1] + n[2] * m[2])));
   }
-  size_t n_;
   ConstVectorSetMatrixMap3f points_;
   b200::CloudHandle cloud_;
-  size_t target_, max_iter_ = 100, iterations_ = 0;  // ransac_hyperplane_estimator.hpp:18
-  float thresh_ = 0.1f;
-  bool re_estimate_ = true;
-  uint32_t seed_;
-  Model model_;
-  ResidualVector residuals_;
-  IndexVector inliers_;
 };
 
 template <typename IndexT = size_t>

@@ -21,6 +21,21 @@ def test_reference_examples_through_cpp_shims(cb, tmp_path):
     assert "all C++ shim checks passed" in out
 
 
+RANSAC_CLAMPS = os.path.join(ROOT, "tests", "cpp", "test_ransac_clamps.cpp")
+
+
+def test_ransac_surface_compiles_without_eigen():
+    r = cxx.syntax(RANSAC_CLAMPS)
+    assert r.returncode == 0, r.stderr
+
+
+@pytest.mark.gpu
+def test_ransac_estimators_clamp_like_the_reference(cb, tmp_path):
+    """Both RANSAC drop-ins report the sample size and target clamped to the data size after estimate()."""
+    out = cxx.run(cxx.build(RANSAC_CLAMPS, str(tmp_path / "test_ransac_clamps")))
+    assert "all RANSAC clamp checks passed" in out
+
+
 def test_eigen_adapters_type_check(tmp_path):
     """The `#if __has_include(<Eigen/Dense>)` adapters (VectorSet / ConstVectorSetMatrixMap / RigidTransform <-> Eigen).
     Eigen3 is absent from this image: they are compiled against tests/cpp/eigen_stub (a minimal stand-in with Eigen's
