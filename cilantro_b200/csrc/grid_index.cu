@@ -22,6 +22,17 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kMaxDim = 1024;        // cells per axis (bounds the cell_coord rounding error, nn_search.cuh)
 constexpr double kTargetOcc = 2.0;   // points per non-empty cell aimed for
+// widest extent of the finite coordinates along one axis that the grid searches exactly (FLT_MAX - 2^105)
+constexpr double kMaxSpan = (double)FLT_MAX - 0x1p105;
+
+// Origin of one axis: one cell below the extent [mn, mx], unless that would put mx more than kMaxSpan above it or the
+// origin itself below -FLT_MAX; then it is raised (never above mn). cell_coord computes x - origin in fp32, so this keeps
+// it finite for every point of the cloud, and a query for which it overflows is then more than 2^104 from every point
+// along that axis: its d2 is Inf and it has no neighbour to miss. Clouds inside +-1e38 keep mn - h bit for bit.
+float grid_origin(float mn, float mx, double h) {
+  const double o = std::max({(double)mn - h, (double)mx - kMaxSpan, -(double)FLT_MAX});
+  return (float)o;
+}
 
 __device__ __forceinline__ int float_to_ordered(float f) {
   int i = __float_as_int(f);
@@ -46,13 +57,12 @@ __global__ void bbox_init_kernel(int* bb) {
 __global__ void bbox_kernel(const float* __restrict__ raw, size_t n, int* bb) {
   float mn[3] = {3.0e38f, 3.0e38f, 3.0e38f}, mx[3] = {-3.0e38f, -3.0e38f, -3.0e38f};
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v[3] = {raw[3 * i], raw[3 * i + 1], raw[3 * i + 2]};
+    if (!finite_point(v[0], v[1], v[2])) continue;  // never a candidate: not part of the extent
 #pragma unroll
     for (int a = 0; a < 3; a++) {
-      float v = raw[3 * i + a];
-      if (v == v && fabsf(v) < 3.0e38f) {  // ignore NaN / Inf coordinates for the extent
-        mn[a] = fminf(mn[a], v);
-        mx[a] = fmaxf(mx[a], v);
-      }
+      mn[a] = fminf(mn[a], v[a]);
+      mx[a] = fmaxf(mx[a], v[a]);
     }
   }
 #pragma unroll
@@ -384,6 +394,8 @@ int ensure_index(cb_cloud* c) {
   CB_TRY(points_bbox(ctx, c->d_raw, n, mn, mx));
   double ext[3] = {(double)mx[0] - mn[0], (double)mx[1] - mn[1], (double)mx[2] - mn[2]};
   const double max_ext = std::max({ext[0], ext[1], ext[2], 1e-30});
+  CB_CHECK(max_ext <= kMaxSpan, CB_ERR_UNSUPPORTED,
+           "the finite coordinates of the cloud span more than FLT_MAX - 2^105 along an axis: x - origin would overflow");
 
   // 2. cell edge: start from a cube-root density guess, then shrink while the non-empty cells are
   //    over-full (surface-like clouds fill few cells).
@@ -421,9 +433,9 @@ int ensure_index(cb_cloud* c) {
       if (ok && tot <= cell_cap) break;
       h *= 1.26;
     }
-    gp.ox = (float)((double)mn[0] - h);
-    gp.oy = (float)((double)mn[1] - h);
-    gp.oz = (float)((double)mn[2] - h);
+    gp.ox = grid_origin(mn[0], mx[0], h);
+    gp.oy = grid_origin(mn[1], mx[1], h);
+    gp.oz = grid_origin(mn[2], mx[2], h);
     gp.inv_h = (float)(1.0 / h);
     gp.nx = dims[0];
     gp.ny = dims[1];

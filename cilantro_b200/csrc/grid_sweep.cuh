@@ -17,8 +17,7 @@ template <class BoundFn, class ScanFn, class ResetFn>
 __device__ __forceinline__ void grid_sweep(const GridView& g, float qx, float qy, float qz, BoundFn bound,
                                            ScanFn scan, ResetFn reset, uint32_t k_needed) {
   if (g.n == 0) return;
-  // a NaN / Inf query is at no finite distance from anything: no candidate can pass d2 < bound
-  if (!(fabsf(qx) + fabsf(qy) + fabsf(qz) < 3.0e38f)) return;
+  if (!finite_point(qx, qy, qz)) return;
   const QueryCell c = query_cell(g, qx, qy, qz);
   const float hs2 = g.hs2;
   int row_budget = kFarRowBudget;

@@ -34,8 +34,6 @@ constexpr uint32_t kUndecided = 0, kRep = 1, kNonRep = 2;
 // registers (left to itself it aims higher, at 32 registers, and spills).
 constexpr int kSweepBlocksPerSm = 8;
 
-__device__ __forceinline__ bool finite3(float x, float y, float z) { return fabsf(x) + fabsf(y) + fabsf(z) < 3.0e38f; }
-
 // packed xyz -> float4 seeds; active ids 0..n-1
 __global__ void init_seeds_kernel(const float* __restrict__ xyz, uint32_t n, float4* __restrict__ seeds,
                                   uint32_t* __restrict__ active) {
@@ -116,7 +114,7 @@ __global__ void key_xy_kernel(const float4* __restrict__ seeds, const uint32_t* 
 __device__ __forceinline__ bool group_start(const float4* __restrict__ seeds, const uint32_t* __restrict__ vals,
                                             uint32_t k) {
   const float4 s = seeds[vals[k]];
-  if (k == 0 || !finite3(s.x, s.y, s.z)) return true;
+  if (k == 0 || !finite_point(s.x, s.y, s.z)) return true;
   const float4 t = seeds[vals[k - 1]];
   return __float_as_uint(s.x) != __float_as_uint(t.x) || __float_as_uint(s.y) != __float_as_uint(t.y) ||
          __float_as_uint(s.z) != __float_as_uint(t.z);
@@ -152,7 +150,7 @@ __global__ void group_kernel(const float4* __restrict__ seeds, const uint32_t* _
 __global__ void state_init_kernel(const float* __restrict__ head_xyz, uint32_t ng, uint32_t* __restrict__ state) {
   for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += gridDim.x * blockDim.x) {
     const float* h = head_xyz + 3 * (size_t)g;
-    state[g] = finite3(h[0], h[1], h[2]) ? kUndecided : kRep;
+    state[g] = finite_point(h[0], h[1], h[2]) ? kUndecided : kRep;
   }
 }
 

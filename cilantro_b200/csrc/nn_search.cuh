@@ -40,6 +40,15 @@ inline Rigid rigid_from_t12(const float* T12) {
   return r;
 }
 
+// The one finiteness rule of the grid: a point with a NaN or Inf coordinate is at no finite distance from anything
+// (every d2 it takes part in is NaN or Inf, which fails d2 < bound), so it is never searched, never a candidate and
+// left out of the grid's extent. Every finite point is searched, up to +-FLT_MAX.
+// The quarter-weighted sum is at most 0.75 FLT_MAX for finite coordinates (no overflow) and Inf or NaN otherwise; one
+// chain of adds and one compare, as cheap as the sum of magnitudes it replaces on the per-query paths.
+__host__ __device__ __forceinline__ bool finite_point(float x, float y, float z) {
+  return 0.25f * fabsf(x) + (0.25f * fabsf(y) + 0.25f * fabsf(z)) < INFINITY;
+}
+
 __device__ __forceinline__ float sum3(float a0, float a1, float a2) { return __fadd_rn(a0, __fadd_rn(a1, a2)); }
 
 __device__ __forceinline__ void rotate_rigid(const Rigid& T, float x, float y, float z, float& qx, float& qy,
@@ -193,8 +202,7 @@ template <bool kExact>
 __device__ __forceinline__ Best grid_nearest_impl(const GridView& g, float qx, float qy, float qz, float max_d2) {
   Best best = no_best(max_d2);
   if (g.n == 0) return best;
-  // a NaN / Inf query is at no finite distance from anything: no candidate can pass d2 < best
-  if (!(fabsf(qx) + fabsf(qy) + fabsf(qz) < 3.0e38f)) return best;
+  if (!finite_point(qx, qy, qz)) return best;
 
   const QueryCell c = query_cell(g, qx, qy, qz);
   const int cx = c.cx, cy = c.cy, cz = c.cz;
